@@ -15,6 +15,9 @@ two half_joins, accumulable reduce, compaction).
           Rust reference cannot be built here) on the box's host cores
 
 `--impl reference` times that CPU implementation alone on the same config.
+`--dump-outputs DIR` writes the output corrections of the last timed step as
+DIR/out_<field>.npy (float64, rows in sorted order; the inputs are seeded, so
+two builds can be compared output for output).
 Multi-GPU (torchrun, one rank per GPU): key-sharded arrangements, NCCL
 all-to-all per exchange point, weak scaling (SF and batch grow with N).
 """
@@ -28,6 +31,7 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
+sys.dont_write_bytecode = True  # the benchmark writes nothing into the tree it runs from
 
 SEED = 7
 ORDERS_PER_BATCH_PER_GPU = 10_000  # ~100K update rows (2 order rows + ~8 lineitem rows per replaced order)
@@ -246,9 +250,9 @@ def best_oracle(B, sf_total, per_batch, n_warm, n_steps, keep_outputs_of_first=F
 def measured_peak():
     try:
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        return float(p["hbm_gbs"]), "measured"
+        return float(p["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured)"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet HBM3 bandwidth (MEASURED_PEAKS.json absent)"
 
 
 # ------------------------------------------------------- the CPU reference
@@ -299,9 +303,29 @@ def workload_config(sf_per_gpu, n):
         "orders_replaced_per_batch": ORDERS_PER_BATCH_PER_GPU * n,
         "parallelism": f"key-hash sharded x{n}; exchange rounds over NVLink peer memory (one scatter + one gather kernel,"
         " no host wait), NCCL all-to-all for hydration chunks" if n > 1 else "1 GPU",
-        "l2": "inputs_larger_than_l2 (arrangements >= 5 GB/GPU vs 126 MB L2)",
+        "l2": "inputs_larger_than_l2 (arrangements >= 5 GB/GPU vs 50 MB L2)",
         "plan": "customer>>orders[custkey]>>lineitem[orderkey]; orders>>customer>>lineitem; lineitem>>orders[orderkey]>>customer",
     }
+
+
+def dump_outputs(out_dir, rows):
+    """The output corrections of one timestamp (all ranks' rows) as one float64 array per field, rows sorted
+    by every field so that the order the device wrote them in does not matter.  The i128 SUM is
+    sum_hi * 2^64 + sum_lo, exact while it stays below 2^53 in magnitude."""
+    import numpy as np
+
+    rows = np.sort(rows, order=["key", "time", "diff", "count", "sum_hi", "sum_lo", "flags"])
+    os.makedirs(out_dir, exist_ok=True)
+    fields = {
+        "key": rows["key"],
+        "count": rows["count"],
+        "sum": rows["sum_hi"].astype(np.float64) * 2.0**64 + rows["sum_lo"].astype(np.float64),
+        "flags": rows["flags"],
+        "time": rows["time"],
+        "diff": rows["diff"],
+    }
+    for name, a in fields.items():
+        np.save(os.path.join(out_dir, f"out_{name}.npy"), np.asarray(a, dtype=np.float64))
 
 
 class stdout_to_stderr:
@@ -561,42 +585,16 @@ def run_ours(args, rank, world, local_rank):
     exact = [kv for kv in ranked if kv[1]["bytes"] > 0 and "map_rows" not in kv[0]]
     with_bytes = exact or [kv for kv in ranked if kv[1]["bytes"] > 0]
     dom_name, dom = with_bytes[0] if with_bytes else ranked[0]
-    peak, peak_kind = measured_peak()
+    peak, peak_source = measured_peak()
     achieved = dom["bytes"] / (dom["ms"] / 1000.0) / 1e9 if dom["ms"] > 0 else 0.0
-    # DRAM traffic of the dominant kernel from the committed `ncu --set full` capture
-    # (profiles/, same command line): mean of the captured launches, bytes per launch
-    traffic = None
-    try:
-        import csv
-
-        tag = "fused" if "fused" in dom_name else ("probe" if "probe" in dom_name else None)
-        cands = [os.path.join(ROOT, "profiles", f"{r}_ncu_full_{tag}_raw.csv") for r in ("r02c", "r02")]
-        path = next((c for c in cands if os.path.exists(c)), cands[-1])
-        if tag and world == 1 and os.path.exists(path):
-            rows = list(csv.reader(open(path)))
-            hdr, units = rows[0], rows[1]
-            tot = []
-            for r in rows[2:]:
-                b = 0.0
-                for col in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                    i = hdr.index(col)
-                    mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}.get(units[i], 1.0)
-                    b += float(r[i].replace(",", "")) * mult
-                tot.append(b)
-            traffic = sum(tot) / len(tot) if tot else None
-    except Exception:
-        traffic = None
     roofline = {
         "bound": "hbm",
         "kernel": dom_name,
         "achieved": achieved,
         "peak": peak,
-        "peak_source": f"MEASURED_PEAKS.json hbm_gbs ({peak_kind})",
+        "peak_source": peak_source,
         "unit": "GB/s",
         "frac": achieved / peak,
-        "traffic": traffic,
-        "traffic_source": "NOT measured in this run: mean DRAM bytes per launch of the committed ncu --set full capture of"
-        f" the same command (profiles/{os.path.basename(path)})" if traffic else None,
         "launches_per_step": dom["launches"] / n_prof,
         "avg_launch_us": 1000.0 * dom["ms"] / max(1, dom["launches"]),
         "algorithmic_bytes_per_launch": dom["bytes"] / max(1, dom["launches"]),
@@ -641,7 +639,7 @@ def run_ours(args, rank, world, local_rank):
     # and at N=1 also as the reported CPU baseline -- a bounded sample of the same workload)
     want_oracle = not args.no_cpu_baseline
     gathered = timed_out
-    if dist is not None and want_oracle:
+    if dist is not None and (want_oracle or args.dump_outputs):
         nn = torch.tensor([len(timed_out)], dtype=torch.int64, device="cuda")
         ns = [torch.zeros_like(nn) for _ in range(world)]
         dist.all_gather(ns, nn)
@@ -687,6 +685,8 @@ def run_ours(args, rank, world, local_rank):
         }
     elif rank == 0:
         line["parity"] = None
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, gathered[gathered["time"] == t_first + first_timed + n_timed - 1])
     if rank == 0:
         print(json.dumps(line), flush=True)
     if dist is not None:
@@ -704,7 +704,11 @@ def main():
     ap.add_argument("--sf-multi", type=float, default=12.5, help="scale factor per GPU at N > 1 (SF=100 at N=8, configs[4])")
     ap.add_argument("--cpu-batches", type=int, default=20)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the output corrections of the last timed step as DIR/out_<field>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(3, args.warmup)
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

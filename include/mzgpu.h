@@ -1,5 +1,5 @@
 /*
- * mzgpu.h — C ABI of the B200-native differential-dataflow operator core.
+ * mzgpu.h — C ABI of the H100-native differential-dataflow operator core.
  *
  * This is the drop-in boundary for Materialize's compute-layer hot path
  * (SURVEY.md §8b).  Every entry point replaces one piece of the Rust trait

@@ -1,7 +1,7 @@
-"""materialize_b200 — a B200-native differential-dataflow operator core.
+"""materialize_b200 — an H100-native differential-dataflow operator core.
 
 The hot path of Materialize's compute layer (update consolidation, arrangement
-build/merge, delta/linear join, accumulable reduce) as hand-written sm_100a CUDA
+build/merge, delta/linear join, accumulable reduce) as hand-written sm_90a CUDA
 behind the C ABI of include/mzgpu.h.  See DESIGN.md and INTEGRATION.md.
 
 Importing this package loads libmzgpu.so and raises if it is missing: there is

@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(HERE, "libmzgpu.so")
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "(nvcc, sm_100a). materialize_b200 has no CPU fallback."
+        "(nvcc, sm_90a). materialize_b200 has no CPU fallback."
     )
 
 lib = C.CDLL(LIB_PATH)

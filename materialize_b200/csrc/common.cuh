@@ -1,5 +1,5 @@
 // common.cuh — context, device memory, row traits and block-level primitives
-// shared by every kernel file of libmzgpu (sm_100a only).
+// shared by every kernel file of libmzgpu (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -24,7 +24,7 @@ struct mzgpu_ctx {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev = nullptr;
   cudaEvent_t ev_block = nullptr;  // MZGPU_BLOCKING_SYNC=1: host waits block on this event (no spinning)
-  int num_sms = 148;
+  int num_sms = 132;
   bool sticky = false;  // a CUDA/NCCL failure (or a deferred device-side report) happened: every later call fails
   int32_t sticky_code = MZGPU_E_CUDA;  // ... with this status
   std::string last_error;
@@ -78,8 +78,7 @@ struct mzgpu_ctx {
   // stream waits for the side stream the first time it touches such a batch
   cudaStream_t main_stream = nullptr, side_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_side = nullptr;
-  bool use_side = true;   // spine merges of R32 arrangements run beside the operators (MZGPU_SIDE_STREAM=0: main stream);
-                          // measured on the Q3 step: 212 -> 267 M rows/s (profiles/r02b_*)
+  bool use_side = true;   // spine merges of R32 arrangements run beside the operators (MZGPU_SIDE_STREAM=0: main stream)
   u64 side_seq = 0;    // merges issued on the side stream so far
   u64 joined_seq = 0;  // the main stream has waited for merges <= this
   // per-kernel profiling (mzgpu_profile_enable)
@@ -125,18 +124,17 @@ struct mzgpu_ctx {
   u64 mid_hits = 0, mid_misses = 0;
   size_t mid_block = (size_t)8 << 20;  // MZGPU_MID_BLOCK_MB (0: off)
 };
-// Blocks of at least this size bypass the driver's stream-ordered pool on reuse: measured on B200
-// (tools/diag_bulk.py cfg4, profiles/r02_diag_cfg4_before.log), cudaMallocAsync of 3-8 GB blocks cost
-// 0.2 s -> 1.9 s -> 4.3 s of HOST time per 100M-row reduce call although every block had been freed in
-// stream order before (20 ms of kernels per call).  The update-batch path (blocks of a few hundred MB
-// at most) allocates in microseconds and stays on the pool.
+// Blocks of at least this size bypass the driver's stream-ordered pool on reuse: cudaMallocAsync of
+// multi-GB blocks can cost host time that grows from call to call (tools/diag_bulk.py cfg4 shows it for
+// the 100M-row reduce) although every block was freed in stream order before.  The update-batch path
+// (blocks of a few hundred MB at most) allocates in microseconds and stays on the pool.  The cache holds
+// at most half of the H100's 80 GB; an allocation that fails hands every cached block back first.
 #define MZ_BIG_BLOCK ((size_t)512 << 20)
-#define MZ_BIG_CACHE_MAX ((size_t)96 << 30)
+#define MZ_BIG_CACHE_MAX ((size_t)40 << 30)
 // Mid-size blocks: with several workers an operator's scratch is sized by what the worker COULD receive
 // (a reduce activation at 2 GPUs allocates and frees ~600 MB in blocks of 30-200 MB for ~10 K actual rows),
-// and the driver's pool took 0.4-10 ms of host time per timestamp for them (profiles/r02b_diag_n2.log: all
-// of it inside the reduce activation's cudaMallocAsync / cudaFreeAsync calls, worse while NVML is polled).
-#define MZ_MID_CACHE_MAX ((size_t)24 << 30)
+// and the driver's pool spends host time on every such cudaMallocAsync / cudaFreeAsync on the hot path.
+#define MZ_MID_CACHE_MAX ((size_t)8 << 30)
 // the side stream has just been made to wait for the main stream: what the main stream's order covers, the
 // side stream's order covers now
 static inline void mz_mid_forked(mzgpu_ctx* ctx) {

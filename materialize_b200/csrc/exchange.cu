@@ -202,8 +202,7 @@ __global__ void __launch_bounds__(XT) k_p2p_scatter(const __grid_constant__ P2PJ
   __shared__ u32 s_last;
   // P2P_IT rows per thread and round: the keys of a round are loaded together, one range per destination is
   // reserved for all of them with a single global atomic, then the rows go out -- the per-round chain (key
-  // load, reservation, stores) is paid once per 1024 rows instead of once per 256 (25 us per launch for an
-  // 80 K-row buffer on 29 CTAs before: profiles/r02b_check_n1_n2_block_cache.log)
+  // load, reservation, stores) is paid once per 1024 rows instead of once per 256
   constexpr int P2P_IT = 4;
   for (u64 i0 = (u64)blockIdx.x * XT * P2P_IT; i0 < n; i0 += (u64)gridDim.x * XT * P2P_IT) {
     __syncthreads();

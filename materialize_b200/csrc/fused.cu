@@ -412,7 +412,7 @@ __device__ __forceinline__ void msd_warp_buckets2(const FusedArgs& a, FusedCtl* 
     // bitonic network over positions p = r*32 + lane, ordered by (hi, lo, idx): idx makes real
     // elements distinct (and puts the padding last among equal keys).  The (k, j) stages are
     // LOOPS: fully unrolled the network is ~2K instructions that every warp runs through once,
-    // and the kernel stalled on instruction fetch (profiles/r02b: 22-55 % "no_instructions").
+    // and the kernel stalls on instruction fetch.
     // Stages with j >= 32 exchange whole register rows (static pairs), the others shuffle.
     auto greater = [&](u64 h1, u64 l1, u32 i1, u64 h2, u64 l2, u32 i2) -> bool {
       if (KW == 2) return h1 > h2 || (h1 == h2 && (l1 > l2 || (l1 == l2 && i1 > i2)));
@@ -1564,9 +1564,9 @@ static int fused_fast_mode() {
   return fast;
 }
 
-// Measured (tools/merge_bench.py, profiles/r02_merge_bench_*.log): two sorted 20K / 80K-row batches merge
-// faster as a sort of A ++ B on the fast MSD path (44 / 59 us vs 52 / 65 us), from 2 x 160K rows on the
-// merge-path form wins (79 vs 93 us; 161 vs 245 us at 2 x 500K).
+// Two sorted update-batch-sized inputs merge faster as a sort of A ++ B on the fast MSD path; from a few
+// hundred thousand rows each the merge-path form wins (tools/merge_bench.py times both sides of the switch;
+// MZGPU_MERGE_SORT_MAX moves it).
 constexpr long long MERGE_SORT_MAX_DEFAULT = 1ll << 18;
 static u32 fused_merge_sort_max() {
   static long long v = -1;
@@ -1709,7 +1709,7 @@ int32_t fused_t(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* res) {
   // ordinary spine merges there are plain launches, mergepath.cu) takes at most one CTA slot per SM, so
   // that it can be co-resident with the operators' launches on the main stream (a cooperative launch
   // starts when its whole grid fits).  Main-stream launches use the whole resident capacity:
-  // (64 registers per thread: four CTAs per SM are resident, 592 on a B200; the bucket phase
+  // (64 registers per thread: four CTAs per SM are resident, 528 on an H100; the bucket phase
   // wants one warp per bucket, and a 160K-row merge has 4096 of them)
   const bool on_side = ctx->side_stream != nullptr && ctx->stream == ctx->side_stream;
   a.max_g = on_side ? (u32)ctx->num_sms : (u32)max_ctas;

@@ -1039,8 +1039,8 @@ extern "C" int32_t mzgpu_builder_done(mzgpu_builder* b, mzgpu_desc desc, mzgpu_b
 }
 
 static bool mz_merge_kernels_on() {
-  // on by default (validated: the GPU suite and the bench's per-step parity check pass either way,
-  // profiles/r02b_*); MZGPU_MERGE_KERNELS=0 runs R32 merges in the fused cooperative kernel instead
+  // on by default (the GPU suite and the bench's per-step parity check pass either way);
+  // MZGPU_MERGE_KERNELS=0 runs R32 merges in the fused cooperative kernel instead
   static const bool on = getenv("MZGPU_MERGE_KERNELS") == nullptr || atoi(getenv("MZGPU_MERGE_KERNELS")) != 0;
   return on;
 }

@@ -103,7 +103,7 @@ __device__ __forceinline__ void for_each_match(const TraceView& tv, u64 key, u64
 // A tile is expanded by the whole CTA.  The reference's half_join walks a cursor per key; a
 // thread per probe row doing the same serialises on memory latency (a key with rows in three
 // batches = a dozen dependent DRAM round trips, and the rest of the CTA waits at the scan
-// barrier: profiles/r02b: 56 % barrier stall, 60 us per launch for 14K probe rows).  Here:
+// barrier).  Here:
 //   1. thread per probe row: first slot of every batch (independent loads), hits counted;
 //   2. block scans give every hit its place in the tile's hit list (thread-major, batch order)
 //      and the tile's CANDIDATE list (the rows of every hit run, concatenated);
@@ -470,8 +470,7 @@ __global__ void __launch_bounds__(PT, 3) k_probe_chains(const __grid_constant__ 
   // The chains of a launch differ in size by an order of magnitude (the lineitem path of a Q3 step
   // carries four times the rows of the orders path, the customer path none): the resident CTAs are
   // shared out in proportion to the chains' tile counts (host bounds), not equally -- an equal split
-  // left the longest chain running four tiles deep on a third of the machine (profiles/r02: 44-55 us
-  // per launch at 20 % of the warp slots).  A chain's tiles are handed out by ticket to whichever of
+  // leaves the longest chain running four tiles deep on a third of the machine.  A chain's tiles are handed out by ticket to whichever of
   // its CTAs is free, so the look-back never waits for a CTA that has not started.
   if (blockIdx.x >= m.ctas[blockIdx.y]) return;
   const ProbeChain& ch = m.chain[blockIdx.y];

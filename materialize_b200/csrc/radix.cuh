@@ -41,8 +41,8 @@ __device__ __forceinline__ void rs_store(u32* p, u32 v) {
 
 // lanes of the warp whose 8-bit digit equals this lane's: eight ballots.  (The
 // hardware MATCH.ANY runs on the address-divergence unit at a small fraction of
-// the ballot rate: with ~30 distinct digits per warp it was the pipe that bound
-// the whole pass, profiles/r01_ncu_full_onesweep_raw.csv: pipe_adu 72 %.)
+// the ballot rate: with ~30 distinct digits per warp it becomes the pipe that
+// bounds the whole pass.)
 template <bool BALLOT>
 __device__ __forceinline__ u32 match_digit(u32 d) {
   if (!BALLOT) return __match_any_sync(0xffffffffu, d);

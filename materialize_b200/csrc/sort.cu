@@ -6,7 +6,7 @@
 //   Chunker::push_into `permutation.sort()`  src/timely-util/src/columnar/batcher.rs:74-79
 //   ColumnationChunker::form_chunk            src/timely-util/src/columnation.rs:477-488
 //
-// B200 design (HBM-bound integer work, no tensor-core path):
+// H100 design (HBM-bound integer work, no tensor-core path):
 //   1. one pass over the rows finds min/max of every key word, so constant and
 //      narrow words cost no radix passes (times are usually one value, keys a
 //      few dozen bits);

@@ -1,6 +1,6 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle on
 the same seeded inputs, bit-exact, plus size-independent properties at large
-sizes.  Run with `pytest -m gpu` on a B200."""
+sizes.  Run with `pytest -m gpu` on an H100."""
 import json
 import os
 
