@@ -151,6 +151,97 @@ def main():
     case(f"cfg4 reduce COUNT/SUM n={n4} zipf0.9 keys={nk}", n4, lambda: harness.gen_cfg4(ctx, 3, n4, cdf), run4, reps=2)
     if res["cases"] and "cfg4" in res["cases"][-1]["case"]:
         res["cases"][-1]["groups_out"] = run4.out
+
+    # ---- config 4 with several aggregate columns per key (mzgpu_reduce_lanes_*): an int64 column
+    # (val1) and a float64 column (val2) generated from the same seed, R40 rows.  Each variant runs on
+    # a context of its own, so device_bytes_peak is that variant's.
+    def lanes_of(k):
+        cols = [mz.accum_lane(mz.AGG_COUNT_SUM_I64, 1), mz.accum_lane(mz.AGG_COUNT_SUM_F64, 2)]
+        return (cols * 4)[:k]
+
+    def r40_cfg4(c, seed, n, first=0, t=0, diff=1):
+        a = harness.gen_cfg4(c, seed, n, cdf, first=first, t=t, diff=diff).download()
+        f = harness.gen_cfg4(c, seed, n, cdf, as_f64=True, first=first, t=t, diff=diff).download()
+        r = np.zeros(n, dtype=mz.R40)
+        r["key"], r["val1"], r["val2"], r["time"], r["diff"] = a["key"], a["val"], f["val"], a["time"], a["diff"]
+        return r
+
+    def lanes_case(name, n_rows, build, run):
+        if args.only and args.only not in name:
+            return
+        c = mz.Context(0)
+        run(c, build(c))  # warm-up
+        state = build(c)
+        c.sync()
+        t0 = time.perf_counter()
+        run(c, state)
+        c.sync()
+        secs = time.perf_counter() - t0
+        state = build(c)
+        c.profile(True)
+        c.profile_report()
+        run(c, state)
+        table = kernel_table(c, peak)
+        c.profile(False)
+        res["cases"].append(
+            {"case": name, "rows": n_rows, "seconds": secs, "rows_per_sec": n_rows / secs, "kernels": table[:10],
+             "device_bytes_peak": c.stats()["device_bytes_peak"]}
+        )
+        del state
+        c.close()  # its cached blocks go back before the next variant measures its peak
+        print(name, f"{n_rows / secs / 1e6:.1f} M rows/s", file=sys.stderr, flush=True)
+
+    # the bulk seal holds the exploded rows, their sorted copy, the consolidated batch and the segment
+    # sums at once (about 5 x the row width per input row): next to this script's other buffers, 2 lanes
+    # (128-byte rows) run at 50 M rows and 4 lanes (224 bytes) at 25 M
+    for k, n in ((2, n4 // 2), (4, n4 // 4)):
+        name = f"cfg4 bulk reduce lanes={k} n={n} zipf0.9 keys={nk} R40"
+        host = r40_cfg4(ctx, 3, n) if not args.only or args.only in name else None
+        lanes_case(
+            name,
+            n,
+            lambda c, host=host: mz.DeviceRows(c, 40).upload(host),
+            lambda c, d, k=k: mz.ReduceLanes(c, lanes_of(k), 40).step_dev(d, 1),
+        )
+        del host
+
+    # incremental regime: 1M-row batches, half of each batch retracting rows of the batch before; one
+    # 4-lane operator against four one-lane operators on the same batches
+    nb, per = 20 // (2 if args.quick else 1), 1_000_000 // scale
+    batches = {}
+
+    def inc_batches(c):
+        if not batches:
+            prev = None
+            for b in range(nb):
+                fresh = r40_cfg4(c, 5, per // 2, first=b * (per // 2), t=b, diff=1)
+                if prev is not None:
+                    back = prev.copy()
+                    back["time"], back["diff"] = b, -1
+                    fresh = np.concatenate([fresh, back])
+                batches[b] = fresh
+                prev = fresh[: per // 2]
+        return [mz.DeviceRows(c, 40).upload(batches[b]) for b in range(nb)]
+
+    def run_inc(c, bufs, ops_lanes):
+        ops = [mz.ReduceLanes(c, ls, 40) for ls in ops_lanes]
+        outs = [mz.DeviceRows(c, op.out_row_bytes) for op in ops]
+        for b, d in enumerate(bufs):
+            for op, o in zip(ops, outs):
+                op.step_dev(d, b + 1, o)
+
+    lanes_case(
+        f"cfg4 incremental lanes=4, one operator, {nb}x{per} R40",
+        nb * per,
+        inc_batches,
+        lambda c, bufs: run_inc(c, bufs, [lanes_of(4)]),
+    )
+    lanes_case(
+        f"cfg4 incremental lanes=4, four one-lane operators, {nb}x{per} R40",
+        nb * per,
+        inc_batches,
+        lambda c, bufs: run_inc(c, bufs, [[l] for l in lanes_of(4)]),
+    )
     txt = json.dumps(res, indent=1)
     if args.out:
         open(args.out, "w").write(txt)

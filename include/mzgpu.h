@@ -87,8 +87,11 @@ typedef struct mzgpu_r40 {
   int64_t diff;
 } mzgpu_r40;
 
-/* Accumulable-reduce update: key -> ((), time, (Vec<Accum>, Diff)) with one
- * accumulated column (src/compute/src/render/reduce.rs:1313-1334,1861-1903).
+/* Accumulable-reduce update: key -> ((), time, (Vec<Accum>, Diff))
+ * (src/compute/src/render/reduce.rs:1313-1334,1861-1903).  This struct is the
+ * one-lane row (mzgpu_reduce_new, or mzgpu_reduce_lanes_new with one lane); an
+ * operator with C lanes repeats the six lane words C times (see
+ * mzgpu_reduce_lanes_new for the table of widths).
  *   total     = Diff component of the pair
  *   non_nulls = Accum::*.non_nulls
  *   acc       = Accum::*.accum as i128 (lo/hi), wrapping
@@ -107,7 +110,9 @@ typedef struct mzgpu_racc {
 } mzgpu_racc;
 
 /* Reduce output update: (key, finalized aggregates), time, diff (+1/-1)
- * (finalize_accum, src/compute/src/render/reduce.rs:1671-1835).
+ * (finalize_accum, src/compute/src/render/reduce.rs:1671-1835).  This struct is
+ * the one-lane row; with C lanes the (count, sum_lo, sum_hi) triple repeats C
+ * times and flag bits 2l / 2l+1 belong to lane l.
  *   count  = COUNT(col)            = Int64(non_nulls)
  *   sum_lo/sum_hi = SUM(int64)     = i128 (numeric from i128);
  *                   SUM(f64)       = f64 bits in sum_lo, sum_hi = 0
@@ -193,8 +198,10 @@ typedef struct mzgpu_closure {
 #define MZGPU_HALFJOIN_LE 0
 #define MZGPU_HALFJOIN_LT 1
 
-/* Aggregate descriptor for the accumulable reduce (AccumulablePlan,
- * src/compute-types/src/plan/reduce.rs:146-158).  One accumulated column. */
+/* Aggregate kinds of the reduce operator.  MZGPU_AGG_COUNT_SUM_* accumulate one
+ * value column with mzgpu_reduce_new, and are the lane kinds of
+ * mzgpu_reduce_lanes_new, which accumulates up to eight columns in one
+ * arrangement (AccumulablePlan, src/compute-types/src/plan/reduce.rs:146-158). */
 #define MZGPU_AGG_COUNT_SUM_I64 0 /* COUNT(val), SUM(val) with val: int64   */
 #define MZGPU_AGG_COUNT_SUM_F64 1 /* COUNT(val), SUM(val) with val: float64 */
 /* ReducePlan::Distinct (build_distinct, src/compute/src/render/reduce.rs:264-334): the
@@ -547,6 +554,63 @@ int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_
 int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out);
 /* The input arrangement (for sharing / inspection). Borrowed. */
 mzgpu_spine* mzgpu_reduce_input_trace(mzgpu_reduce* r);
+
+/* ---- accumulable reduce over several value columns ("lanes") in one arrangement
+ * (build_accumulable over AccumulablePlan::simple_aggrs / full_aggrs, reduce.rs:1261-1471:
+ * every input row explodes into one Accum per aggregate, arranged once, and reduce_abelian
+ * emits one output row per key holding every finalized aggregate).  Lane l yields
+ * COUNT(col_l) and SUM(col_l) exactly as the one-column kinds do; AVG is SUM / COUNT
+ * downstream, and count(*) is any lane's count (NULLs are outside the fixed-width subset).
+ *
+ * A lane picks its column from the input row: field.src is MZGPU_SRC_VAL1 (R32 `val`, R40
+ * `val1`) or MZGPU_SRC_VAL2 (R40 `val2`), field.shift / field.bits the bit-field
+ * (dst_shift unused).  An I64 lane reads the field, sign-extended when sign_extend != 0
+ * (a 64-bit field is the i64 itself); an F64 lane must pick a whole word (shift 0, bits 64). */
+#define MZGPU_MAX_ACCUM_LANES 8
+typedef struct mzgpu_accum_lane {
+  int32_t kind;         /* MZGPU_AGG_COUNT_SUM_I64 or MZGPU_AGG_COUNT_SUM_F64 */
+  uint32_t sign_extend; /* I64 lanes: sign-extend the bit-field                */
+  mzgpu_field field;
+} mzgpu_accum_lane;
+/* Row widths.  The lane count rounds up to a class C in {1, 2, 4, 8}; the class's unused
+ * lanes are zero.  Arrangement row: key, time, total, C x (non_nulls, acc_lo, acc_hi,
+ * pos_infs, neg_infs, nans), padded to 16 bytes.  Output row: key, C x (count, sum_lo,
+ * sum_hi), flags, time, diff, padded to 16 bytes (widths chosen so that no output width
+ * equals an arrangement width: the generic kernels know a row by its width alone).
+ *     C   arrangement          output
+ *     1    80 B (mzgpu_racc)    64 B (mzgpu_rout)
+ *     2   128 B                 96 B
+ *     4   224 B                144 B
+ *     8   416 B                240 B
+ * Flags: bit 2l = lane l's SUM is NULL (total > 0 and the lane's accumulation is zero),
+ * bit 2l+1 = lane l has net-zero records with a non-zero accumulation (the per-aggregate
+ * AccumulableErrorCheck, reduce.rs:1418-1429).  A key has an output row while its whole
+ * accumulated diff (total and every lane) is non-zero; a change in any lane retracts and
+ * re-emits the whole row.  Output rows of C >= 2 are plain buffer rows:
+ * mzgpu_buf_consolidate on them returns MZGPU_E_UNSUPPORTED (they leave the operator
+ * consolidated).  The arrangement widths are accepted by batchers, builders and spines. */
+#define MZGPU_ROW_RACC2 128
+#define MZGPU_ROW_RACC4 224
+#define MZGPU_ROW_RACC8 416
+#define MZGPU_ROW_ROUT2 96
+#define MZGPU_ROW_ROUT4 144
+#define MZGPU_ROW_ROUT8 240
+/* The arrangement and output row widths for n_lanes (1..8); MZGPU_E_INVALID otherwise. */
+int32_t mzgpu_reduce_lanes_row_bytes(uint32_t n_lanes, uint32_t* arr_row_bytes, uint32_t* out_row_bytes);
+/* in_row_bytes: 32 (R32) or 40 (R40), the rows the join operators emit.  A malformed
+ * descriptor (kind, VAL2 on R32 input, a zero-width or out-of-range field, an F64 lane not
+ * picking a whole word, n_lanes of 0 or above 8) is MZGPU_E_INVALID before any launch.
+ * The handle is freed with mzgpu_reduce_free; mzgpu_reduce_input_trace returns its
+ * arrangement. */
+int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                               uint32_t n_lanes, mzgpu_reduce** out);
+/* One activation, with the protocol of mzgpu_reduce_accumulable[_buf]: `rows` are n input
+ * rows of in_row_bytes with times in [previous upper, upper); the output corrections
+ * (rows of the class's output width) are appended to `out`, consolidated.  After a failed
+ * activation the operator reports that status from then on. */
+int32_t mzgpu_reduce_lanes(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                           mzgpu_buf* out);
+int32_t mzgpu_reduce_lanes_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out);
 
 /* ------------------------------ f1 (first step): Row keys as fixed-width words */
 /* A `Row` orders by byte length first, then by its bytes (RowRef::cmp,

@@ -34,6 +34,8 @@ from .api import (  # noqa: F401
     LinearJoin,
     MzGpuError,
     ReduceAccumulable,
+    ReduceLanes,
+    accum_lane,
     Spine,
     TopK,
     half_join,

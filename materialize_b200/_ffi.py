@@ -51,19 +51,64 @@ ROUT = np.dtype(
         ("_pad", "<i8"),
     ]
 )
+# The lanes operator (mzgpu_reduce_lanes_new): the lane count rounds up to a class C in
+# {1, 2, 4, 8}; rows hold C lanes (unused ones zero).  Class 1 has the RACC / ROUT bytes.  The pad
+# words are fields, so that copies of these arrays keep every byte.
+ACCUM_LANE = np.dtype(
+    [("non_nulls", "<i8"), ("acc_lo", "<u8"), ("acc_hi", "<i8"), ("pos_infs", "<i8"), ("neg_infs", "<i8"), ("nans", "<i8")]
+)
+OUT_LANE = np.dtype([("count", "<i8"), ("sum_lo", "<u8"), ("sum_hi", "<i8")])
+LANE_CLASSES = (1, 2, 4, 8)
+# class -> (arrangement row bytes, output row bytes), as in include/mzgpu.h
+LANE_ROW_BYTES = {1: (80, 64), 2: (128, 96), 4: (224, 144), 8: (416, 240)}
+
+
+def lane_class(n_lanes):
+    return next(c for c in LANE_CLASSES if c >= n_lanes)
+
+
+RACC_LANES = {
+    c: np.dtype(
+        {
+            "names": ["key", "time", "total", "lanes", "_pad"],
+            "formats": ["<u8", "<u8", "<i8", (ACCUM_LANE, (c,)), "<i8"],
+            "offsets": [0, 8, 16, 24, 24 + 48 * c],
+            "itemsize": LANE_ROW_BYTES[c][0],
+        }
+    )
+    for c in LANE_CLASSES
+}
+ROUT_LANES = {
+    c: np.dtype(
+        {
+            "names": ["key", "lanes", "flags", "time", "diff", "_pad"],
+            "formats": ["<u8", (OUT_LANE, (c,)), "<u8", "<u8", "<i8", ("<i8", (LANE_ROW_BYTES[c][1] - 32 - 24 * c) // 8)],
+            "offsets": [0, 8, 8 + 24 * c, 16 + 24 * c, 24 + 24 * c, 32 + 24 * c],
+            "itemsize": LANE_ROW_BYTES[c][1],
+        }
+    )
+    for c in LANE_CLASSES
+}
 DTYPES = {16: R16, 32: R32, 40: R40, 80: RACC, 64: ROUT}
+DTYPES.update({LANE_ROW_BYTES[c][0]: RACC_LANES[c] for c in LANE_CLASSES[1:]})
+DTYPES.update({LANE_ROW_BYTES[c][1]: ROUT_LANES[c] for c in LANE_CLASSES[1:]})
 
 MEM_HOST, MEM_DEVICE = 0, 1
 FRONTIER_EMPTY = 2**64 - 1
 OK, E_INVALID, E_CUDA, E_CAPACITY, E_UNSUPPORTED, E_NCCL, E_FRONTIER = 0, -1, -2, -3, -4, -5, -6
 HALFJOIN_LE, HALFJOIN_LT = 0, 1
 AGG_COUNT_SUM_I64, AGG_COUNT_SUM_F64, AGG_DISTINCT, AGG_THRESHOLD, AGG_MIN, AGG_MAX, AGG_TOPK = 0, 1, 2, 3, 4, 5, 6
+MAX_ACCUM_LANES = 8
 COMM_ID_BYTES = 128
 P2P_HANDLE_BYTES = 64
 
 
 class Field(C.Structure):
     _fields_ = [("src", C.c_uint8), ("shift", C.c_uint8), ("bits", C.c_uint8), ("dst_shift", C.c_uint8)]
+
+
+class AccumLane(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("sign_extend", C.c_uint32), ("field", Field)]
 
 
 class Filter(C.Structure):
@@ -194,6 +239,10 @@ SIGNATURES = {
     "mzgpu_reduce_free": (None, [vp]),
     "mzgpu_reduce_accumulable": (i32, [vp, vp, u64, i32, u64, vp]),
     "mzgpu_reduce_input_trace": (vp, [vp]),
+    "mzgpu_reduce_lanes_row_bytes": (i32, [u32, PU32, PU32]),
+    "mzgpu_reduce_lanes_new": (i32, [vp, u32, vp, u32, PV]),
+    "mzgpu_reduce_lanes": (i32, [vp, vp, u64, i32, u64, vp]),
+    "mzgpu_reduce_lanes_buf": (i32, [vp, vp, u64, vp]),
     "mzgpu_comm_unique_id": (i32, [C.POINTER(C.c_uint8)]),
     "mzgpu_comm_init": (i32, [vp, C.POINTER(C.c_uint8)]),
     "mzgpu_exchange": (i32, [vp, vp, vp]),

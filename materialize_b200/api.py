@@ -588,6 +588,53 @@ class ReduceAccumulable:
         return Spine(self.ctx, 80, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
 
 
+def accum_lane(kind, src=SRC_VAL1, shift=0, bits=64, sign_extend=False):
+    """One lane of ReduceLanes: COUNT and SUM of the bit-field `bits` wide at `shift` of value word
+    `src` (1 = val / val1, 2 = val2); an I64 field is sign-extended when `sign_extend`."""
+    return (int(kind), int(src), int(shift), int(bits), bool(sign_extend))
+
+
+class ReduceLanes:
+    """COUNT / SUM of several value columns per key in one arrangement (mzgpu_reduce_lanes_new).
+    `lanes` is a list of accum_lane(...) tuples; input rows are R32 (in_row_bytes=32) or R40 (40).
+    Output rows have the dtype ROUT_LANES[class] (lane l in ["lanes"][:, l])."""
+
+    def __init__(self, ctx, lanes, in_row_bytes=32):
+        self.ctx = ctx
+        self.n_lanes = len(lanes)
+        self.in_row_bytes = in_row_bytes
+        arr = (F.AccumLane * max(1, len(lanes)))()
+        for i, (kind, src, shift, bits, sx) in enumerate(lanes):
+            arr[i].kind = kind
+            arr[i].sign_extend = 1 if sx else 0
+            arr[i].field = F.Field(src, shift, bits, 0)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_reduce_lanes_new(ctx.h, in_row_bytes, arr, len(lanes), C.byref(h)))
+        self.h = h
+        self.lane_class = F.lane_class(self.n_lanes)
+        self.arr_row_bytes, self.out_row_bytes = F.LANE_ROW_BYTES[self.lane_class]
+
+    def step(self, rows, upper):
+        rows = np.ascontiguousarray(rows)
+        out = DeviceRows(self.ctx, self.out_row_bytes)
+        self.ctx.check(F.lib.mzgpu_reduce_lanes(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h))
+        return out.download().view(F.ROUT_LANES[self.lane_class])
+
+    def step_dev(self, dev_rows, upper, out=None):
+        """One activation over device-resident rows; corrections are appended to `out` on the device."""
+        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
+        self.ctx.check(F.lib.mzgpu_reduce_lanes_buf(self.h, dev_rows.h, upper, out.h))
+        return out
+
+    def input_trace(self):
+        return Spine(self.ctx, self.arr_row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_reduce_free(self.h)
+            self.h = None
+
+
 class TopK(ReduceAccumulable):
     """TopK per key over (key, value) rows (BasicTopKPlan, src/compute/src/render/top_k.rs:215-248,
     521-673): `limit` < 0 or None = no limit; stepped like every other reduce kind."""

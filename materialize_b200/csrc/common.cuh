@@ -524,23 +524,62 @@ template <>
 struct RowT<64> {  // mzgpu_rout (key, count, sum_lo, sum_hi, flags, time | diff, pad)
   static constexpr int NW = 8, NK = 6, ND = 2, TW = 5, DK = 5;
 };
+// Multi-lane accumulable arrangement rows (mzgpu_reduce_lanes_new): key, time | total, then
+// C lanes of (non_nulls, acc_lo, acc_hi, pos_infs, neg_infs, nans), padded to 16 bytes.
+template <>
+struct RowT<128> {  // C = 2
+  static constexpr int NW = 16, NK = 2, ND = 14, TW = 1, DK = 1;
+};
+template <>
+struct RowT<224> {  // C = 4
+  static constexpr int NW = 28, NK = 2, ND = 26, TW = 1, DK = 1;
+};
+template <>
+struct RowT<416> {  // C = 8
+  static constexpr int NW = 52, NK = 2, ND = 50, TW = 1, DK = 1;
+};
 // DK = number of leading "data" words (key words before the time word): two
 // rows with equal DK words are the same (key, val).
+//
+// Every width has exactly one meaning, because the generic kernels (sort, consolidate, merge,
+// index) pick the diff arithmetic from the width alone.  The lanes operator's output rows for
+// C >= 2 (96, 144 and 240 bytes, LaneRows below) were given widths that no arrangement row uses,
+// and deliberately have no RowT: mzgpu_buf_consolidate on them returns MZGPU_E_UNSUPPORTED
+// instead of summing the wrong words.
 
-// Semigroup::plus_equals on the diff words.  ND == 8 is the accumulable diff:
-// words 2,3 (acc_lo, acc_hi) form an i128 (src/compute/src/render/reduce.rs:1940-2041).
+// Row widths of the accumulable reduce with lane class C (1, 2, 4 or 8 lanes): the arrangement
+// row (RowT above) and the output row (key, C x (count, sum_lo, sum_hi), flags, time, diff, pad).
+// C = 1 is mzgpu_racc / mzgpu_rout.  The output widths skip 80 and 128 and 224 (see above).
+template <int C>
+struct LaneRows {
+  static constexpr int ARR_NW = C == 1 ? 10 : (C == 2 ? 16 : (C == 4 ? 28 : 52));
+  static constexpr int OUT_NW = C == 1 ? 8 : (C == 2 ? 12 : (C == 4 ? 18 : 30));
+  static constexpr int OUT_TW = 3 * C + 2;  // time word of an output row (the diff follows)
+};
+static inline int mz_lane_class(uint32_t n_lanes) { return n_lanes <= 1 ? 1 : (n_lanes <= 2 ? 2 : (n_lanes <= 4 ? 4 : 8)); }
+static inline int mz_lane_arr_bytes(int c) { return c == 1 ? 80 : (c == 2 ? 128 : (c == 4 ? 224 : 416)); }
+static inline int mz_lane_out_bytes(int c) { return c == 1 ? 64 : (c == 2 ? 96 : (c == 4 ? 144 : 240)); }
+
+// Semigroup::plus_equals on the diff words.  ND >= 8 is the accumulable diff: word 0 is the
+// total, lane l spans words 1+6l .. 6+6l, and its words 1,2 (acc_lo, acc_hi) form an i128
+// (src/compute/src/render/reduce.rs:1940-2041).  ND == 8 is one lane plus a pad word.
 template <int ND>
 __host__ __device__ __forceinline__ void diff_add(u64* a, const u64* b) {
-  if (ND == 8) {
+  if (ND >= 8) {
     a[0] += b[0];
-    a[1] += b[1];
-    u64 lo = a[2] + b[2];
-    u64 carry = lo < a[2] ? 1 : 0;
-    a[2] = lo;
-    a[3] = a[3] + b[3] + carry;
-    a[4] += b[4];
-    a[5] += b[5];
-    a[6] += b[6];
+#pragma unroll
+    for (int l = 0; l < (ND - 1) / 6; ++l) {
+      u64* x = a + 1 + 6 * l;
+      const u64* y = b + 1 + 6 * l;
+      x[0] += y[0];
+      u64 lo = x[1] + y[1];
+      u64 carry = lo < x[1] ? 1 : 0;
+      x[1] = lo;
+      x[2] = x[2] + y[2] + carry;
+      x[3] += y[3];
+      x[4] += y[4];
+      x[5] += y[5];
+    }
   } else {
     a[0] += b[0];  // ND == 2 is (diff, pad): pad stays 0
   }
@@ -548,8 +587,34 @@ __host__ __device__ __forceinline__ void diff_add(u64* a, const u64* b) {
 template <int ND>
 __host__ __device__ __forceinline__ bool diff_is_zero(const u64* a) {
   if (ND == 8) return (a[0] | a[1] | a[2] | a[3] | a[4] | a[5] | a[6]) == 0;
+  if (ND > 8) {
+    u64 x = 0;
+#pragma unroll
+    for (int w = 0; w < ND; ++w) x |= a[w];  // pad words stay zero
+    return x == 0;
+  }
   return a[0] == 0;
 }
+#ifdef __CUDACC__
+// diff_add into global or shared memory by atomics, for the multi-lane diffs (ND > 8); the
+// atomic that wraps a lane's acc_lo carries into its acc_hi
+template <int ND>
+__device__ __forceinline__ void atomic_lanes_add(u64* __restrict__ acc, const u64* d) {
+  if (d[0]) atomicAdd((unsigned long long*)&acc[0], (unsigned long long)d[0]);
+#pragma unroll
+  for (int l = 0; l < (ND - 1) / 6; ++l) {
+    u64* x = acc + 1 + 6 * l;
+    const u64* y = d + 1 + 6 * l;
+    if (y[0]) atomicAdd((unsigned long long*)&x[0], (unsigned long long)y[0]);
+    const u64 old = atomicAdd((unsigned long long*)&x[1], (unsigned long long)y[1]);
+    const u64 hi = y[2] + ((old + y[1]) < old ? 1 : 0);
+    if (hi) atomicAdd((unsigned long long*)&x[2], (unsigned long long)hi);
+    if (y[3]) atomicAdd((unsigned long long*)&x[3], (unsigned long long)y[3]);
+    if (y[4]) atomicAdd((unsigned long long*)&x[4], (unsigned long long)y[4]);
+    if (y[5]) atomicAdd((unsigned long long*)&x[5], (unsigned long long)y[5]);
+  }
+}
+#endif
 
 // ----------------------------------------------------------- device helpers
 #ifdef __CUDACC__
@@ -935,6 +1000,15 @@ int32_t mz_map_rows_dev(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const mzgpu_cl
 
 // reduce.cu
 int32_t mz_explode(mzgpu_ctx* ctx, const u64* d_r32, DLen n, u64 n_ub, int agg_kind, u64* d_racc);
+// the lanes operator's explode_one: R32 / R40 rows -> one arrangement row of class C each
+struct LaneSet {
+  mzgpu_accum_lane lane[MZGPU_MAX_ACCUM_LANES];
+  u32 n;         // lanes in use; the class's other lanes stay zero
+  u32 in_words;  // 4 (R32) or 5 (R40)
+  u32 f64_mask;  // bit l: lane l is MZGPU_AGG_COUNT_SUM_F64
+};
+int32_t mz_explode_lanes(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
+                         u64* d_arr);
 struct TopKParams {
   i64 limit;  // < 0: none
   u64 offset;
@@ -943,11 +1017,13 @@ struct TopKParams {
 int32_t mz_reduce_minmax_async(mzgpu_ctx* ctx, const u64* d_batch_rows, DLen n, u64 n_ub,
                                const TraceView& prior, int agg_kind, const TopKParams& tp, u64* d_out,
                                u64 out_cap, u64* d_out_len);
-int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, const u64* d_batch_rows, DLen n, u64 n_ub,
-                                    const TraceView& prior, int agg_kind, u64* d_out, u64 out_cap,
-                                    u64* d_out_len);
-int32_t mz_reduce_corrections(mzgpu_ctx* ctx, const u64* d_batch_rows, u64 n, const TraceView& prior,
-                              int agg_kind, DevMem* out, u64* n_out);
+// `c` is the lane class (1 for every mzgpu_reduce_new kind); for c >= 2 the lanes' kinds come
+// from `ls` (f64_mask, n) and agg_kind is unused
+int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, DLen n, u64 n_ub,
+                                    const TraceView& prior, int agg_kind, const LaneSet* ls, u64* d_out,
+                                    u64 out_cap, u64* d_out_len);
+int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
+                              int agg_kind, const LaneSet* ls, DevMem* out, u64* n_out);
 
 // correction.cu (time-major rows: (time, key, val | diff))
 // column.cu (columnar wire format, f4)

@@ -55,6 +55,8 @@ __device__ __forceinline__ void atomic_diff_add(u64* __restrict__ acc, const u64
     if (d[4]) atomicAdd((unsigned long long*)&acc[4], (unsigned long long)d[4]);
     if (d[5]) atomicAdd((unsigned long long*)&acc[5], (unsigned long long)d[5]);
     if (d[6]) atomicAdd((unsigned long long*)&acc[6], (unsigned long long)d[6]);
+  } else if (ND > 8) {
+    atomic_lanes_add<ND>(acc, d);
   } else {
     atomicAdd((unsigned long long*)&acc[0], (unsigned long long)d[0]);
   }
@@ -190,6 +192,9 @@ int32_t gather_t(mzgpu_ctx* ctx, const u64* rows, const u32* perm, u64 n, u64* o
     case 40: return CALL(40);                                         \
     case 80: return CALL(80);                                         \
     case 64: return CALL(64);                                         \
+    case 128: return CALL(128);                                       \
+    case 224: return CALL(224);                                       \
+    case 416: return CALL(416);                                       \
     default:                                                          \
       MZ_SET_ERR(ctx, "unsupported row width %d", rb);                \
       return MZGPU_E_UNSUPPORTED;                                     \

@@ -662,7 +662,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
   u32 bb = 0;  // log2(buckets)
   // (the fast path takes up to 32768 buckets -- a million rows; without it the exact path's 4096)
   const u32 bb_max = a.fast != 0 ? 15u : 12u;
-  while (bb < bb_max && ((u64)(ND == 8 ? 12 : 48) << bb) < n) ++bb;
+  while (bb < bb_max && ((u64)(ND >= 8 ? 12 : 48) << bb) < n) ++bb;
   const u32 NB = 1u << bb;
   u32 G = gdim;
   {
@@ -974,7 +974,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
       __shared__ u64 s_wlb;
       msd_warp_buckets<RB, WR>(a, ctl, sm.scan.base, NB, c, G, na, since, s_wcnt, &s_wlb);
       msd_done = true;
-    } else if (s_max_unit <= LOCAL_MAX) {
+    } else if (ND <= 8 && s_max_unit <= LOCAL_MAX) {  // (its shared sums hold at most 8 diff words)
       for (u64 i = gtid; i < n; i += gstride) {
         const u64 p = (u64)sm.scan.base[a.v1[i]] + a.v0[i];
         a.m_lo[p] = a.k0[i];
@@ -1409,6 +1409,8 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
         if (d[4]) atomicAdd((unsigned long long*)&acc[4], (unsigned long long)d[4]);
         if (d[5]) atomicAdd((unsigned long long*)&acc[5], (unsigned long long)d[5]);
         if (d[6]) atomicAdd((unsigned long long*)&acc[6], (unsigned long long)d[6]);
+      } else if (ND > 8) {
+        atomic_lanes_add<ND>(acc, d);
       } else {
         atomicAdd((unsigned long long*)&acc[0], (unsigned long long)d[0]);
       }
@@ -1534,7 +1536,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
 }
 
 template <int RB>
-__global__ void __launch_bounds__(FT, (RB == 80 ? 2 : 4)) k_fused_consolidate(const FusedArgs a) {
+__global__ void __launch_bounds__(FT, (RB >= 80 ? 2 : 4)) k_fused_consolidate(const FusedArgs a) {
   fused_body<RB>(a, blockIdx.x, gridDim.x);
 }
 
@@ -1549,7 +1551,7 @@ struct FusedMany {
   FusedArgs job[FUSED_MANY_MAX];
 };
 template <int RB>
-__global__ void __launch_bounds__(FT, (RB == 80 ? 2 : 4)) k_fused_many(const __grid_constant__ FusedMany m) {
+__global__ void __launch_bounds__(FT, (RB >= 80 ? 2 : 4)) k_fused_many(const __grid_constant__ FusedMany m) {
   u32 j = 0;
   while (j + 1 < m.k && blockIdx.x >= m.start[j + 1]) ++j;
   fused_body<RB>(m.job[j], blockIdx.x - m.start[j], m.start[j + 1] - m.start[j]);
@@ -1617,7 +1619,7 @@ int32_t fused_prepare(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* res, int sl
   {
     const u64 n_max = cap < MSD_FAST_MAX_ROWS ? cap : MSD_FAST_MAX_ROWS;
     u32 bb = 0;
-    while (bb < 15 && ((u64)(ND == 8 ? 12 : 48) << bb) < n_max) ++bb;
+    while (bb < 15 && ((u64)(ND >= 8 ? 12 : 48) << bb) < n_max) ++bb;
     const u64 regions = ((u64)1 << bb) * 128;
     if (regions > mcap) mcap = regions;
   }
@@ -1865,6 +1867,9 @@ int32_t mz_fused_flush(mzgpu_ctx* ctx) {
     case 40: st = fused_launch_many<40>(ctx, k, d->args, d->want, d->bytes); break;
     case 80: st = fused_launch_many<80>(ctx, k, d->args, d->want, d->bytes); break;
     case 64: st = fused_launch_many<64>(ctx, k, d->args, d->want, d->bytes); break;
+    case 128: st = fused_launch_many<128>(ctx, k, d->args, d->want, d->bytes); break;
+    case 224: st = fused_launch_many<224>(ctx, k, d->args, d->want, d->bytes); break;
+    case 416: st = fused_launch_many<416>(ctx, k, d->args, d->want, d->bytes); break;
     default: st = MZGPU_E_UNSUPPORTED; break;
   }
   for (int j = 0; j < k; ++j) d->scratch[j].release();  // stream ordered: after the launch
@@ -1893,6 +1898,9 @@ int32_t mz_fused_defer(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* out) {
     case 40: st = fused_defer_t<40>(ctx, d, job, out); break;
     case 80: st = fused_defer_t<80>(ctx, d, job, out); break;
     case 64: st = fused_defer_t<64>(ctx, d, job, out); break;
+    case 128: st = fused_defer_t<128>(ctx, d, job, out); break;
+    case 224: st = fused_defer_t<224>(ctx, d, job, out); break;
+    case 416: st = fused_defer_t<416>(ctx, d, job, out); break;
     default:
       MZ_SET_ERR(ctx, "fused: unsupported row width %d", job.rb);
       return MZGPU_E_UNSUPPORTED;
@@ -1922,6 +1930,9 @@ int32_t mz_fused_consolidate_many(mzgpu_ctx* ctx, int k, const FusedJob* jobs, F
     case 40: return fused_many_t<40>(ctx, k, jobs, outs);
     case 80: return fused_many_t<80>(ctx, k, jobs, outs);
     case 64: return fused_many_t<64>(ctx, k, jobs, outs);
+    case 128: return fused_many_t<128>(ctx, k, jobs, outs);
+    case 224: return fused_many_t<224>(ctx, k, jobs, outs);
+    case 416: return fused_many_t<416>(ctx, k, jobs, outs);
     default:
       MZ_SET_ERR(ctx, "fused: unsupported row width %d", jobs[0].rb);
       return MZGPU_E_UNSUPPORTED;
@@ -1935,6 +1946,9 @@ int32_t mz_fused_consolidate(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* res)
     case 40: return fused_t<40>(ctx, job, res);
     case 80: return fused_t<80>(ctx, job, res);
     case 64: return fused_t<64>(ctx, job, res);
+    case 128: return fused_t<128>(ctx, job, res);
+    case 224: return fused_t<224>(ctx, job, res);
+    case 416: return fused_t<416>(ctx, job, res);
     default:
       MZ_SET_ERR(ctx, "fused: unsupported row width %d", job.rb);
       return MZGPU_E_UNSUPPORTED;

@@ -421,7 +421,11 @@ static int32_t validate_closure(mzgpu_ctx* ctx, const mzgpu_closure* c) {
   return MZGPU_OK;
 }
 
-static bool valid_row_bytes(uint32_t rb) { return rb == 16 || rb == 32 || rb == 40 || rb == 80 || rb == 64; }
+// arrangement rows: R32, and the accumulable rows of every lane class (RACC = class 1)
+static bool arrangement_row_bytes(uint32_t rb) { return rb == 32 || rb == 80 || rb == 128 || rb == 224 || rb == 416; }
+static bool valid_row_bytes(uint32_t rb) {
+  return rb == 16 || rb == 40 || rb == 64 || arrangement_row_bytes(rb) || rb == 96 || rb == 144 || rb == 240;
+}
 
 // ------------------------------------------------------ device-side append
 // dst[base ...] = src[0 .. n), new length left in *out_len; every size may live
@@ -885,7 +889,7 @@ static int32_t make_empty_batch(mzgpu_ctx* ctx, uint32_t rb, mzgpu_desc desc, mz
 extern "C" int32_t mzgpu_batch_build(mzgpu_ctx* ctx, uint32_t row_bytes, const void* rows, uint64_t n,
                                      int32_t mem, mzgpu_desc desc, mzgpu_batch** out) {
   MZ_CHECK_CTX(ctx);
-  if (out == nullptr || (rows == nullptr && n) || (row_bytes != 32 && row_bytes != 80)) return MZGPU_E_INVALID;
+  if (out == nullptr || (rows == nullptr && n) || !arrangement_row_bytes(row_bytes)) return MZGPU_E_INVALID;
   if (n == 0) return make_empty_batch(ctx, row_bytes, desc, out);
   DevMem in;
   const void* d_in = rows;
@@ -995,7 +999,7 @@ struct mzgpu_builder {
 extern "C" int32_t mzgpu_builder_new(mzgpu_ctx* ctx, uint32_t row_bytes, uint64_t capacity_rows,
                                      mzgpu_builder** out) {
   MZ_CHECK_CTX(ctx);
-  if (out == nullptr || (row_bytes != 32 && row_bytes != 80)) return MZGPU_E_INVALID;
+  if (out == nullptr || !arrangement_row_bytes(row_bytes)) return MZGPU_E_INVALID;
   std::unique_ptr<mzgpu_builder> b(new mzgpu_builder());
   b->ctx = ctx;
   b->rb = row_bytes;
@@ -1420,7 +1424,7 @@ static int32_t batcher_seal_many(int k, mzgpu_batcher* const* bs, u64 upper, mzg
 
 extern "C" int32_t mzgpu_batcher_new(mzgpu_ctx* ctx, uint32_t row_bytes, mzgpu_batcher** out) {
   MZ_CHECK_CTX(ctx);
-  if (out == nullptr || (row_bytes != 32 && row_bytes != 80)) return MZGPU_E_INVALID;
+  if (out == nullptr || !arrangement_row_bytes(row_bytes)) return MZGPU_E_INVALID;
   mzgpu_batcher* b = new mzgpu_batcher();
   b->ctx = ctx;
   b->rb = row_bytes;
@@ -1765,7 +1769,7 @@ static int32_t spine_take_err(mzgpu_spine* s) {
 extern "C" int32_t mzgpu_spine_new(mzgpu_ctx* ctx, uint32_t row_bytes, uint32_t effort,
                                    mzgpu_spine** out) {
   MZ_CHECK_CTX(ctx);
-  if (out == nullptr || (row_bytes != 32 && row_bytes != 80)) return MZGPU_E_INVALID;
+  if (out == nullptr || !arrangement_row_bytes(row_bytes)) return MZGPU_E_INVALID;
   mzgpu_spine* s = new mzgpu_spine();
   s->ctx = ctx;
   s->rb = row_bytes;
@@ -2495,6 +2499,9 @@ struct mzgpu_reduce {
   mzgpu_ctx* ctx;
   int agg_kind;
   TopKParams topk = {-1, 0, 0};
+  // mzgpu_reduce_lanes_new: lane class (1, 2, 4, 8) and descriptors; 0 for every other operator
+  int lane_class = 0;
+  LaneSet lanes = {};
   mzgpu_batcher* batcher = nullptr;
   mzgpu_spine* input = nullptr;
   int32_t failed = MZGPU_OK;  // set when an activation failed after its seal (reduce_dev)
@@ -2561,8 +2568,12 @@ static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, 
       MZ_TRY(s.rows.alloc(ctx, n_ub * 32));
       MZ_CUDA(ctx, cudaMemcpyAsync(s.rows.p, d_rows, n_ub * 32, cudaMemcpyDeviceToDevice, ctx->stream));
     } else {
-      MZ_TRY(s.rows.alloc(ctx, n_ub * 80));
-      MZ_TRY(mz_explode(ctx, d_rows, n, n_ub, r->agg_kind, s.rows.as<u64>()));
+      const int c = r->lane_class;
+      MZ_TRY(s.rows.alloc(ctx, n_ub * (c ? mz_lane_arr_bytes(c) : 80)));
+      if (c)
+        MZ_TRY(mz_explode_lanes(ctx, c, d_rows, n, n_ub, r->lanes, s.rows.as<u64>()));
+      else
+        MZ_TRY(mz_explode(ctx, d_rows, n, n_ub, r->agg_kind, s.rows.as<u64>()));
     }
     if (n.p == nullptr) {
       s.len.set(ctx, n.imm);
@@ -2585,20 +2596,23 @@ static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, 
   TraceView tv;
   int32_t st = trace_view(ctx, prior, &tv);
   const u64 b_ub = batch->len_ub;
+  const int lc = r->lane_class ? r->lane_class : 1;
+  const u64 out_rb = (u64)mz_lane_out_bytes(lc);
+  const LaneSet* ls = r->lane_class ? &r->lanes : nullptr;
   if (st == MZGPU_OK && b_ub > 0) {
     if ((b_ub + 255) / 256 <= MZ_LB_TILES && per_row * b_ub <= MZ_BOUND_MAX_ROWS) {
       DevMem corr, cons;
       Lazy4 clen, flen;
       u64 ccap = 0;
-      st = corr.alloc(ctx, per_row * b_ub * 64);
+      st = corr.alloc(ctx, per_row * b_ub * out_rb);
       if (st == MZGPU_OK) st = clen.make_pending(ctx);
       if (st == MZGPU_OK) {
         if (minmax)
           st = mz_reduce_minmax_async(ctx, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv, r->agg_kind,
                                       r->topk, corr.as<u64>(), per_row * b_ub, clen.dptr());
         else
-          st = mz_reduce_corrections_async(ctx, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv, r->agg_kind,
-                                           corr.as<u64>(), per_row * b_ub, clen.dptr());
+          st = mz_reduce_corrections_async(ctx, lc, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv,
+                                           r->agg_kind, ls, corr.as<u64>(), per_row * b_ub, clen.dptr());
         clen.mark_written();
       }
       if (st == MZGPU_OK && !minmax) {
@@ -2622,11 +2636,17 @@ static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, 
         st = MZGPU_E_UNSUPPORTED;
       }
       if (st == MZGPU_OK)
-        st = mz_reduce_corrections(ctx, batch->rows.as<u64>(), batch->st.v[0], tv, r->agg_kind, &corr, &n_corr);
-      if (st == MZGPU_OK && n_corr)
-        st = consolidate_dev(ctx, 64, corr.p, dlen_imm(n_corr), n_corr, &cons, &ccap, &flen);
-      if (st == MZGPU_OK && n_corr)
-        st = buf_append_dev(out, cons.p, dlen_of(flen, 0), flen.known ? flen.v[0] : n_corr);
+        st = mz_reduce_corrections(ctx, lc, batch->rows.as<u64>(), batch->st.v[0], tv, r->agg_kind, ls, &corr,
+                                   &n_corr);
+      if (st == MZGPU_OK && n_corr && lc > 1) {
+        // consolidated by construction, as in the single-pass form (and no RowT for these widths)
+        st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
+      } else {
+        if (st == MZGPU_OK && n_corr)
+          st = consolidate_dev(ctx, 64, corr.p, dlen_imm(n_corr), n_corr, &cons, &ccap, &flen);
+        if (st == MZGPU_OK && n_corr)
+          st = buf_append_dev(out, cons.p, dlen_of(flen, 0), flen.known ? flen.v[0] : n_corr);
+      }
     }
   }
   // The seal above consumed the batcher's rows and advanced its frontier, so the batch joins the
@@ -2646,7 +2666,7 @@ static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, 
 
 extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_t n,
                                             int32_t mem, uint64_t upper, mzgpu_buf* out) {
-  if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64) return MZGPU_E_INVALID;
+  if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->lane_class) return MZGPU_E_INVALID;
   mzgpu_ctx* ctx = r->ctx;
   MZ_CHECK_CTX(ctx);
   ctx->stats.rows_in += n;
@@ -2661,9 +2681,99 @@ extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* ro
 }
 extern "C" int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
                                                 mzgpu_buf* out) {
-  if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64)
+  if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64 || r->lane_class)
     return MZGPU_E_INVALID;
   MZ_CHECK_CTX(r->ctx);
+  r->ctx->stats.rows_in += rows->ub;
+  return reduce_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out);
+}
+
+// ------------------------------------------------------- reduce over several value columns
+extern "C" int32_t mzgpu_reduce_lanes_row_bytes(uint32_t n_lanes, uint32_t* arr_row_bytes, uint32_t* out_row_bytes) {
+  if (n_lanes == 0 || n_lanes > MZGPU_MAX_ACCUM_LANES) return MZGPU_E_INVALID;
+  const int c = mz_lane_class(n_lanes);
+  if (arr_row_bytes != nullptr) *arr_row_bytes = (uint32_t)mz_lane_arr_bytes(c);
+  if (out_row_bytes != nullptr) *out_row_bytes = (uint32_t)mz_lane_out_bytes(c);
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                                          uint32_t n_lanes, mzgpu_reduce** out) {
+  MZ_CHECK_CTX(ctx);
+  if (out == nullptr || (lanes == nullptr && n_lanes) || (in_row_bytes != 32 && in_row_bytes != 40)) {
+    MZ_SET_ERR(ctx, "reduce_lanes: bad arguments (input rows of %u bytes)", in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  if (n_lanes == 0 || n_lanes > MZGPU_MAX_ACCUM_LANES) {
+    MZ_SET_ERR(ctx, "reduce_lanes: %u lanes (1..%d)", n_lanes, MZGPU_MAX_ACCUM_LANES);
+    return MZGPU_E_INVALID;
+  }
+  LaneSet ls = {};
+  for (uint32_t l = 0; l < n_lanes; ++l) {
+    const mzgpu_accum_lane& L = lanes[l];
+    const mzgpu_field& f = L.field;
+    const bool f64 = L.kind == MZGPU_AGG_COUNT_SUM_F64;
+    const char* bad = nullptr;
+    if (L.kind != MZGPU_AGG_COUNT_SUM_I64 && !f64)
+      bad = "kind is not COUNT_SUM_I64 / COUNT_SUM_F64";
+    else if (f.src != MZGPU_SRC_VAL1 && !(f.src == MZGPU_SRC_VAL2 && in_row_bytes == 40))
+      bad = "source word is not a value word of the input row";
+    else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
+      bad = "field is empty or out of range";
+    else if (f64 && (f.shift != 0 || f.bits != 64))
+      bad = "a float64 lane must pick a whole word";
+    if (bad != nullptr) {
+      MZ_SET_ERR(ctx, "reduce_lanes: lane %u: %s", l, bad);
+      return MZGPU_E_INVALID;
+    }
+    ls.lane[l] = L;
+    if (f64) ls.f64_mask |= 1u << l;
+  }
+  ls.n = n_lanes;
+  ls.in_words = in_row_bytes / 8;
+  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
+  r->ctx = ctx;
+  r->lane_class = mz_lane_class(n_lanes);
+  r->lanes = ls;
+  // class 1 runs the one-column kernels, which take the lane's kind as the aggregate kind
+  r->agg_kind = (ls.f64_mask & 1u) ? MZGPU_AGG_COUNT_SUM_F64 : MZGPU_AGG_COUNT_SUM_I64;
+  const uint32_t rb = (uint32_t)mz_lane_arr_bytes(r->lane_class);
+  MZ_TRY(mzgpu_batcher_new(ctx, rb, &r->batcher));
+  MZ_TRY(mzgpu_spine_new(ctx, rb, 1, &r->input));
+  *out = r.release();
+  return MZGPU_OK;
+}
+
+static bool lanes_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out) {
+  return r->lane_class != 0 && in_rb == r->lanes.in_words * 8 && out->rb == (uint32_t)mz_lane_out_bytes(r->lane_class);
+}
+extern "C" int32_t mzgpu_reduce_lanes(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                      mzgpu_buf* out) {
+  if (r == nullptr || out == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = r->ctx;
+  MZ_CHECK_CTX(ctx);
+  const uint32_t in_rb = r->lanes.in_words * 8;
+  if (!lanes_io_ok(r, in_rb, out)) {
+    MZ_SET_ERR(ctx, "reduce_lanes: output buffer of %u-byte rows", out->rb);
+    return MZGPU_E_INVALID;
+  }
+  ctx->stats.rows_in += n;
+  DevMem in;
+  const u64* d_rows = (const u64*)rows;
+  if (mem == MZGPU_MEM_HOST && n) {
+    MZ_TRY(in.alloc(ctx, n * in_rb));
+    MZ_TRY(copy_in(ctx, in.p, rows, n * in_rb, mem));
+    d_rows = in.as<u64>();
+  }
+  return reduce_dev(r, d_rows, dlen_imm(n), n, upper, out);
+}
+extern "C" int32_t mzgpu_reduce_lanes_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out) {
+  if (r == nullptr || rows == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(r->ctx);
+  if (!lanes_io_ok(r, rows->rb, out)) {
+    MZ_SET_ERR(r->ctx, "reduce_lanes: input rows of %u bytes / output rows of %u bytes", rows->rb, out->rb);
+    return MZGPU_E_INVALID;
+  }
   r->ctx->stats.rows_in += rows->ub;
   return reduce_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out);
 }

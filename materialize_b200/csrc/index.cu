@@ -166,6 +166,9 @@ int32_t mz_count_keys(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n, 
     case 32: MZ_LAUNCH(ctx, k_count_keys<4>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
     case 80: MZ_LAUNCH(ctx, k_count_keys<10>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
     case 64: MZ_LAUNCH(ctx, k_count_keys<8>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
+    case 128: MZ_LAUNCH(ctx, k_count_keys<16>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
+    case 224: MZ_LAUNCH(ctx, k_count_keys<28>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
+    case 416: MZ_LAUNCH(ctx, k_count_keys<52>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
     default: MZ_SET_ERR(ctx, "index: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
   }
   MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 24, d_count, 16, cudaMemcpyDeviceToHost, ctx->stream));
@@ -191,6 +194,9 @@ int32_t mz_build_index(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n,
     case 32: MZ_LAUNCH(ctx, k_build_index<4>, grid, 512, 0, r, n, t, slots - 1); break;
     case 80: MZ_LAUNCH(ctx, k_build_index<10>, grid, 512, 0, r, n, t, slots - 1); break;
     case 64: MZ_LAUNCH(ctx, k_build_index<8>, grid, 512, 0, r, n, t, slots - 1); break;
+    case 128: MZ_LAUNCH(ctx, k_build_index<16>, grid, 512, 0, r, n, t, slots - 1); break;
+    case 224: MZ_LAUNCH(ctx, k_build_index<28>, grid, 512, 0, r, n, t, slots - 1); break;
+    case 416: MZ_LAUNCH(ctx, k_build_index<52>, grid, 512, 0, r, n, t, slots - 1); break;
     default: MZ_SET_ERR(ctx, "index: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
   }
   return MZGPU_OK;
@@ -206,6 +212,9 @@ int32_t mz_seek_keys(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, DLen n, 
     case 32: MZ_LAUNCH(ctx, k_seek_keys<4>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
     case 80: MZ_LAUNCH(ctx, k_seek_keys<10>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
     case 64: MZ_LAUNCH(ctx, k_seek_keys<8>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
+    case 128: MZ_LAUNCH(ctx, k_seek_keys<16>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
+    case 224: MZ_LAUNCH(ctx, k_seek_keys<28>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
+    case 416: MZ_LAUNCH(ctx, k_seek_keys<52>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
     default: MZ_SET_ERR(ctx, "seek_keys: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
   }
   return MZGPU_OK;
@@ -226,12 +235,18 @@ int32_t mz_key_page(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n_row
     case 32: MZ_LAUNCH(ctx, k_key_heads_count<4>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
     case 80: MZ_LAUNCH(ctx, k_key_heads_count<10>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
     case 64: MZ_LAUNCH(ctx, k_key_heads_count<8>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
+    case 128: MZ_LAUNCH(ctx, k_key_heads_count<16>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
+    case 224: MZ_LAUNCH(ctx, k_key_heads_count<28>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
+    case 416: MZ_LAUNCH(ctx, k_key_heads_count<52>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
     default: MZ_SET_ERR(ctx, "key_page: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
   }
   MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, counts.as<u32>(), tiles, total.as<u64>());
   switch (row_bytes) {
     case 32: MZ_LAUNCH(ctx, k_key_heads_emit<4>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
     case 80: MZ_LAUNCH(ctx, k_key_heads_emit<10>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
+    case 128: MZ_LAUNCH(ctx, k_key_heads_emit<16>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
+    case 224: MZ_LAUNCH(ctx, k_key_heads_emit<28>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
+    case 416: MZ_LAUNCH(ctx, k_key_heads_emit<52>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
     default: MZ_LAUNCH(ctx, k_key_heads_emit<8>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
   }
   return MZGPU_OK;

@@ -76,7 +76,11 @@ __global__ void __launch_bounds__(MT) k_merge_tiles(const u64* __restrict__ A, u
   constexpr int NW = RowT<RB>::NW, NK = RowT<RB>::NK, TW = RowT<RB>::TW;
   constexpr int VT = MergeCfg<RB>::VT;
   constexpr u32 TILE = MergeCfg<RB>::TILE;
-  __shared__ __align__(16) u64 sm[TILE * NW];
+  // rows wider than RACC do not fit a tile in shared memory: only their sort keys are staged
+  // there (SW words per row), and the output copies each row from global memory
+  constexpr bool KEYS_ONLY = NW > 10;
+  constexpr int SW = KEYS_ONLY ? NK : NW;
+  __shared__ __align__(16) u64 sm[TILE * SW];
   const u64 t = blockIdx.x;
   const u64 diag0 = t * TILE;
   u64 diag1 = diag0 + TILE;
@@ -86,18 +90,23 @@ __global__ void __launch_bounds__(MT) k_merge_tiles(const u64* __restrict__ A, u
   const u32 ca = (u32)(a1 - a0), cb = (u32)(b1 - b0);
   // stage both ranges; times advanced on the way in
   for (u32 i = threadIdx.x; i < ca + cb; i += MT) {
-    u64 r[NW];
-    if (i < ca)
-      load_row<NW>(A, a0 + i, r);
-    else
-      load_row<NW>(B, b0 + (i - ca), r);
+    u64 r[SW];
+    if (KEYS_ONLY) {
+      const u64* g = i < ca ? A + (a0 + i) * NW : B + (b0 + (i - ca)) * NW;
+#pragma unroll
+      for (int w = 0; w < SW; ++w) r[w] = g[w];
+    } else if (i < ca) {
+      load_row<SW>(A, a0 + i, r);
+    } else {
+      load_row<SW>(B, b0 + (i - ca), r);
+    }
     if (TW >= 0) r[TW >= 0 ? TW : 0] = r[TW >= 0 ? TW : 0] < since ? since : r[TW >= 0 ? TW : 0];
 #pragma unroll
-    for (int w = 0; w < NW; ++w) sm[(u64)i * NW + w] = r[w];
+    for (int w = 0; w < SW; ++w) sm[(u64)i * SW + w] = r[w];
   }
   __syncthreads();
   const u64* sa = sm;
-  const u64* sb = sm + (u64)ca * NW;
+  const u64* sb = sm + (u64)ca * SW;
   // per-thread merge path inside the tile
   u32 d = threadIdx.x * VT;
   const u32 total = ca + cb;
@@ -106,7 +115,7 @@ __global__ void __launch_bounds__(MT) k_merge_tiles(const u64* __restrict__ A, u
   while (lo < hi) {
     u32 mid = (lo + hi) >> 1;
     u32 b = d - mid;
-    if (!keys_less<NK, -1>(sb + (u64)(b - 1) * NW, sa + (u64)mid * NW, 0))
+    if (!keys_less<NK, -1>(sb + (u64)(b - 1) * SW, sa + (u64)mid * SW, 0))
       lo = mid + 1;
     else
       hi = mid;
@@ -122,12 +131,22 @@ __global__ void __launch_bounds__(MT) k_merge_tiles(const u64* __restrict__ A, u
     else if (ib >= cb)
       take_a = true;
     else
-      take_a = !keys_less<NK, -1>(sb + (u64)ib * NW, sa + (u64)ia * NW, 0);
-    const u64* src = take_a ? sa + (u64)ia * NW : sb + (u64)ib * NW;
-    u64 r[NW];
+      take_a = !keys_less<NK, -1>(sb + (u64)ib * SW, sa + (u64)ia * SW, 0);
+    if (KEYS_ONLY) {
+      // keys (time advanced) from the tile, the rest of the row from global memory, word by word
+      const u64* k = take_a ? sa + (u64)ia * SW : sb + (u64)ib * SW;
+      const u64* g = take_a ? A + (a0 + ia) * NW : B + (b0 + ib) * NW;
+      u64* dst = out + (diag0 + o) * NW;
 #pragma unroll
-    for (int w = 0; w < NW; ++w) r[w] = src[w];
-    store_row<NW>(out, diag0 + o, r);
+      for (int w = 0; w < SW; ++w) dst[w] = k[w];
+      for (int w = SW; w < NW; ++w) dst[w] = g[w];
+    } else {
+      const u64* src = take_a ? sa + (u64)ia * SW : sb + (u64)ib * SW;
+      u64 r[NW];
+#pragma unroll
+      for (int w = 0; w < NW; ++w) r[w] = src[w];
+      store_row<NW>(out, diag0 + o, r);
+    }
     if (take_a)
       ++ia;
     else
@@ -245,6 +264,9 @@ int32_t mz_merge_consolidate(mzgpu_ctx* ctx, int row_bytes, const void* d_a, u64
     case 32: return merge_t<32>(ctx, a, na, b, nb, since, out, n_out);
     case 80: return merge_t<80>(ctx, a, na, b, nb, since, out, n_out);
     case 64: return merge_t<64>(ctx, a, na, b, nb, since, out, n_out);
+    case 128: return merge_t<128>(ctx, a, na, b, nb, since, out, n_out);
+    case 224: return merge_t<224>(ctx, a, na, b, nb, since, out, n_out);
+    case 416: return merge_t<416>(ctx, a, na, b, nb, since, out, n_out);
     default:
       MZ_SET_ERR(ctx, "merge: unsupported row width %d", row_bytes);
       return MZGPU_E_UNSUPPORTED;
@@ -258,6 +280,9 @@ int32_t mz_extract(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n, u64
     case 32: return extract_t<32>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
     case 80: return extract_t<80>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
     case 64: return extract_t<64>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
+    case 128: return extract_t<128>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
+    case 224: return extract_t<224>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
+    case 416: return extract_t<416>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
     default:
       MZ_SET_ERR(ctx, "extract: unsupported row width %d", row_bytes);
       return MZGPU_E_UNSUPPORTED;

@@ -97,6 +97,38 @@ __device__ __forceinline__ void mul_i128_i64(u64 lo, u64 hi, i64 d, u64* rlo, u6
   *rhi = __umul64hi(lo, dl) + hi * dl + lo * dh;
 }
 
+// One lane of explode_one (datum_to_accumulator, reduce.rs:1530-1669): the lane's six diff words
+// (non_nulls, acc_lo, acc_hi, pos_infs, neg_infs, nans) for value bits `v` and multiplicity `diff`.
+// k_explode below computes the same words for its one column inline: written through this helper
+// it compiles to a different register allocation, and the one-column kernel is kept as it was.
+__device__ __forceinline__ void explode_lane(u64 v, bool f64, i64 diff, u64* o) {
+  o[0] = (u64)diff;  // non_nulls
+  u64 alo, ahi;
+  u64 pinf = 0, ninf = 0, nan = 0;
+  if (f64) {
+    const double x = __longlong_as_double((long long)v);
+    const bool is_nan = isnan(x);
+    const bool is_pinf = isinf(x) && x > 0;
+    const bool is_ninf = isinf(x) && x < 0;
+    nan = is_nan ? (u64)diff : 0;
+    pinf = is_pinf ? (u64)diff : 0;
+    ninf = is_ninf ? (u64)diff : 0;
+    if (is_nan || is_pinf || is_ninf) {
+      alo = 0;
+      ahi = 0;
+    } else {
+      f64_to_i128_sat(x * 16777216.0, &alo, &ahi);
+    }
+  } else {
+    alo = v;
+    ahi = (i64)v < 0 ? ~0ull : 0ull;
+  }
+  mul_i128_i64(alo, ahi, diff, &o[1], &o[2]);
+  o[3] = pinf;
+  o[4] = ninf;
+  o[5] = nan;
+}
+
 __global__ void __launch_bounds__(RT) k_explode(const u64* __restrict__ rows, const DLen dn, int agg_kind,
                                                 u64* __restrict__ out) {
   const u64 n = dlen_get(dn);
@@ -145,48 +177,96 @@ __global__ void __launch_bounds__(RT) k_explode(const u64* __restrict__ rows, co
   }
 }
 
-// finalize_accum + error-check flag for one accumulated diff S (words 2..8 of a RACC row)
-__device__ __forceinline__ void finalize(const u64* S, int agg_kind, u64* o /* count, sum_lo, sum_hi, flags */) {
+// explode_one of the lanes operator: R32 / R40 rows, lane l reads its bit-field of val1 / val2
+template <int C>
+__global__ void __launch_bounds__(RT) k_explode_lanes(const u64* __restrict__ rows, const DLen dn,
+                                                      const __grid_constant__ LaneSet ls, u64* __restrict__ out) {
+  constexpr int NW = LaneRows<C>::ARR_NW;
+  const u64 n = dlen_get(dn);
+  const u32 iw = ls.in_words;
+  for (u64 i = (u64)blockIdx.x * RT + threadIdx.x; i < n; i += (u64)gridDim.x * RT) {
+    const u64* r = rows + i * iw;
+    const u64 key = r[0], v1 = r[1], v2 = iw == 5 ? r[2] : 0, t = r[iw - 2];
+    const i64 diff = (i64)r[iw - 1];
+    u64 o[NW];
+    o[0] = key;
+    o[1] = t;
+    o[2] = (u64)diff;  // total
+#pragma unroll
+    for (int l = 0; l < C; ++l) {
+      if ((u32)l < ls.n) {
+        const mzgpu_accum_lane& L = ls.lane[l];
+        u64 v = field_get(L.field, key, v1, v2);
+        if (L.sign_extend && L.field.bits < 64 && ((v >> (L.field.bits - 1)) & 1)) v |= ~0ull << L.field.bits;
+        explode_lane(v, L.kind == MZGPU_AGG_COUNT_SUM_F64, diff, &o[3 + 6 * l]);
+      } else {
+#pragma unroll
+        for (int w = 0; w < 6; ++w) o[3 + 6 * l + w] = 0;
+      }
+    }
+#pragma unroll
+    for (int w = 3 + 6 * C; w < NW; ++w) o[w] = 0;
+    store_row<NW>(out, i, o);
+  }
+}
+
+// finalize_accum + error-check flags for one accumulated diff S (the diff words of an arrangement
+// row: total, then C lanes).  o = C x (count, sum_lo, sum_hi), flags.  For C = 1 the kind is
+// agg_kind; for C >= 2 lane l is F64 if bit l of f64_mask is set, and lanes >= n_lanes (zero) get
+// no flags.
+template <int C>
+__device__ __forceinline__ void finalize(const u64* S, int agg_kind, u32 f64_mask, u32 n_lanes, u64* o) {
   const i64 total = (i64)S[0];
-  if (agg_kind == MZGPU_AGG_DISTINCT) {  // (key, ()) once; error flag for a negative multiplicity
+  if (C == 1 && agg_kind == MZGPU_AGG_DISTINCT) {  // (key, ()) once; error flag for a negative multiplicity
     o[0] = 1;
     o[1] = 0;
     o[2] = 0;
     o[3] = total < 0 ? 2 : 0;
     return;
   }
-  const bool accum_zero = (S[1] | S[2] | S[3] | S[4] | S[5] | S[6]) == 0;
   u64 flags = 0;
-  if (total > 0 && accum_zero) flags |= 1;
-  if (total == 0 && !accum_zero) flags |= 2;
-  o[0] = S[1];
-  if (agg_kind == MZGPU_AGG_COUNT_SUM_F64) {
-    const i64 pinf = (i64)S[4], ninf = (i64)S[5], nan = (i64)S[6];
-    u64 bits;
-    if (nan > 0 || (pinf > 0 && ninf > 0))
-      bits = 0x7ff8000000000000ull;
-    else if (pinf > 0)
-      bits = 0x7ff0000000000000ull;
-    else if (ninf > 0)
-      bits = 0xfff0000000000000ull;
-    else
-      bits = (u64)__double_as_longlong(i128_to_f64(S[2], S[3]) / 16777216.0);
-    o[1] = bits;
-    o[2] = 0;
-  } else {
-    o[1] = S[2];
-    o[2] = S[3];
+#pragma unroll
+  for (int l = 0; l < C; ++l) {
+    const u64* A = S + 1 + 6 * l;
+    u64* q = o + 3 * l;
+    const bool accum_zero = (A[0] | A[1] | A[2] | A[3] | A[4] | A[5]) == 0;
+    u64 lf = 0;
+    if (total > 0 && accum_zero) lf |= 1;
+    if (total == 0 && !accum_zero) lf |= 2;
+    if (C > 1 && (u32)l >= n_lanes) lf = 0;
+    q[0] = A[0];
+    const bool f64 = C == 1 ? agg_kind == MZGPU_AGG_COUNT_SUM_F64 : ((f64_mask >> l) & 1u) != 0;
+    if (f64) {
+      const i64 pinf = (i64)A[3], ninf = (i64)A[4], nan = (i64)A[5];
+      u64 bits;
+      if (nan > 0 || (pinf > 0 && ninf > 0))
+        bits = 0x7ff8000000000000ull;
+      else if (pinf > 0)
+        bits = 0x7ff0000000000000ull;
+      else if (ninf > 0)
+        bits = 0xfff0000000000000ull;
+      else
+        bits = (u64)__double_as_longlong(i128_to_f64(A[1], A[2]) / 16777216.0);
+      q[1] = bits;
+      q[2] = 0;
+    } else {
+      q[1] = A[1];
+      q[2] = A[2];
+    }
+    if (lf & 1) {
+      q[1] = 0;
+      q[2] = 0;
+    }
+    flags |= lf << (2 * l);
   }
-  if (flags & 1) {
-    o[1] = 0;
-    o[2] = 0;
-  }
-  o[3] = flags;
+  o[3 * C] = flags;
 }
 
 // sum of all prior updates of `key` (times before the new batch).  The first hash
 // slot of GROUP batches is fetched before any is inspected (independent loads).
+template <int C>
 __device__ __forceinline__ void prior_sum(const TraceView& tv, u64 key, u64* S) {
+  constexpr int NW = LaneRows<C>::ARR_NW, ND = NW - 2;
   const u64 h0 = mix64(key);
   constexpr int GROUP = 8;
   for (u32 b0 = 0; b0 < tv.n_batches; b0 += GROUP) {
@@ -214,12 +294,16 @@ __device__ __forceinline__ void prior_sum(const TraceView& tv, u64 key, u64* S) 
           const u32 len = (u32)(sl.y >> 44);
           const u64 bn = len != 0 ? first + len : bv_n(bv);
           for (u64 r = first; r < bn; ++r) {
-            const u64* row = bv.rows + r * 10;
+            const u64* row = bv.rows + r * NW;
             if (len == 0 && row[0] != key) break;
-            u64 d[8];
+            if (C == 1) {
+              u64 d[ND];
 #pragma unroll
-            for (int w = 0; w < 8; ++w) d[w] = row[2 + w];
-            diff_add<8>(S, d);
+              for (int w = 0; w < ND; ++w) d[w] = row[2 + w];
+              diff_add<ND>(S, d);
+            } else {
+              diff_add<ND>(S, row + 2);  // wide rows: word by word from memory
+            }
           }
           break;
         }
@@ -230,49 +314,70 @@ __device__ __forceinline__ void prior_sum(const TraceView& tv, u64 key, u64* S) 
   }
 }
 
-// The corrections of ONE key, out[pos .. pos + c), put into consolidated order (words 1..5:
-// count, sum_lo, sum_hi, flags, time; the key is the same).  A key's corrections are distinct rows
-// (-old and +new differ in their values, different times differ in the time word), and keys are
-// written in ascending order by construction, so with this the kernel's whole output is already
-// what consolidate() would return: the separate sort launch (40 us for a few hundred rows) is gone.
+// The corrections of ONE key, out[pos .. pos + c), put into consolidated order (the words after
+// the key up to the time: C x (count, sum_lo, sum_hi), flags, time; the key is the same).  A key's
+// corrections are distinct rows (-old and +new differ in their values, different times differ in
+// the time word), and keys are written in ascending order by construction, so with this the
+// kernel's whole output is already what consolidate() would return: the separate sort launch
+// (40 us for a few hundred rows) is gone.
+template <int C>
 __device__ __forceinline__ void sort_key_corrections(u64* __restrict__ out, u64 pos, u32 c) {
+  constexpr int OW = LaneRows<C>::OUT_NW, TWO = LaneRows<C>::OUT_TW;
   for (u32 x = 1; x < c; ++x) {
-    u64 r[8];
-    load_row<8>(out, pos + x, r);
+    u64 r[OW];
+    load_row<OW>(out, pos + x, r);
     u32 y = x;
     while (y > 0) {
-      u64 p[8];
-      load_row<8>(out, pos + y - 1, p);
+      u64 p[OW];
+      load_row<OW>(out, pos + y - 1, p);
       bool less = false;
 #pragma unroll
-      for (int w = 1; w <= 5; ++w) {
+      for (int w = 1; w <= TWO; ++w) {
         if (r[w] != p[w]) {
           less = r[w] < p[w];
           break;
         }
       }
       if (!less) break;
-      store_row<8>(out, pos + y, p);
+      store_row<OW>(out, pos + y, p);
       --y;
     }
-    if (y != x) store_row<8>(out, pos + y, r);
+    if (y != x) store_row<OW>(out, pos + y, r);
   }
+}
+
+// output row (key, finalized aggregates, time, diff, zero padding)
+template <int C>
+__device__ __forceinline__ void put_out_row(u64* __restrict__ out, u64 at, u64 key, const u64* v, u64 t, u64 diff) {
+  constexpr int OW = LaneRows<C>::OUT_NW, NV = 3 * C + 1;
+  u64 r[OW];
+  r[0] = key;
+#pragma unroll
+  for (int w = 0; w < NV; ++w) r[1 + w] = v[w];
+  r[1 + NV] = t;
+  r[2 + NV] = diff;
+#pragma unroll
+  for (int w = 3 + NV; w < OW; ++w) r[w] = 0;
+  store_row<OW>(out, at, r);
 }
 
 // Corrections of one changed key: rows [i, ...) of the new batch with this key,
 // given the key's prior accumulation S0.  Counts (and optionally writes at
 // out[pos...]) the (-old, +new) output rows.
+template <int C>
 __device__ __forceinline__ u32 walk_key(const u64* __restrict__ rows, u64 n, u64 i, u64 key, const u64* S0,
-                                        int agg_kind, bool do_write, u64* __restrict__ out, u64 pos) {
-  u64 S[8];
+                                        int agg_kind, u32 f64_mask, u32 n_lanes, bool do_write,
+                                        u64* __restrict__ out, u64 pos) {
+  constexpr int NW = LaneRows<C>::ARR_NW, ND = NW - 2, NV = 3 * C + 1;
+  u64 S[ND];
 #pragma unroll
-  for (int w = 0; w < 8; ++w) S[w] = S0[w];
-  if (agg_kind == MZGPU_AGG_THRESHOLD) {
+  for (int w = 0; w < ND; ++w) S[w] = S0[w];
+  if (C == 1 && agg_kind == MZGPU_AGG_THRESHOLD) {
     // output multiplicity = max(accumulated multiplicity, 0); one row per change, diff = the change
     i64 mult = (i64)S[0] > 0 ? (i64)S[0] : 0;
     u32 c = 0;
     for (u64 j = i; j < n; ++j) {
-      const u64* row = rows + j * 10;
+      const u64* row = rows + j * NW;
       if (row[0] != key) break;
       S[0] += row[2];
       const i64 m2 = (i64)S[0] > 0 ? (i64)S[0] : 0;
@@ -285,81 +390,92 @@ __device__ __forceinline__ u32 walk_key(const u64* __restrict__ rows, u64 n, u64
       }
       mult = m2;
     }
-    if (do_write && c > 1) sort_key_corrections(out, pos, c);
+    if (do_write && c > 1) sort_key_corrections<C>(out, pos, c);
     return c;
   }
-  bool had = !diff_is_zero<8>(S);
-  u64 oldv[4] = {0, 0, 0, 0};
-  if (had) finalize(S, agg_kind, oldv);
+  bool had = !diff_is_zero<ND>(S);
+  u64 oldv[NV];
+#pragma unroll
+  for (int w = 0; w < NV; ++w) oldv[w] = 0;
+  if (had) finalize<C>(S, agg_kind, f64_mask, n_lanes, oldv);
   u32 c = 0;
   for (u64 j = i; j < n; ++j) {
-    const u64* row = rows + j * 10;
+    const u64* row = rows + j * NW;
     if (row[0] != key) break;
-    u64 d[8];
+    if (C == 1) {
+      u64 d[ND];
 #pragma unroll
-    for (int w = 0; w < 8; ++w) d[w] = row[2 + w];
-    diff_add<8>(S, d);
+      for (int w = 0; w < ND; ++w) d[w] = row[2 + w];
+      diff_add<ND>(S, d);
+    } else {
+      diff_add<ND>(S, row + 2);
+    }
     const u64 t = row[1];
-    const bool has = !diff_is_zero<8>(S);
-    u64 newv[4] = {0, 0, 0, 0};
-    if (has) finalize(S, agg_kind, newv);
-    const bool same = had && has && oldv[0] == newv[0] && oldv[1] == newv[1] && oldv[2] == newv[2] &&
-                      oldv[3] == newv[3];
+    const bool has = !diff_is_zero<ND>(S);
+    u64 newv[NV];
+#pragma unroll
+    for (int w = 0; w < NV; ++w) newv[w] = 0;
+    if (has) finalize<C>(S, agg_kind, f64_mask, n_lanes, newv);
+    bool same = had && has;
+#pragma unroll
+    for (int w = 0; w < NV; ++w) same = same && oldv[w] == newv[w];
     if (!same) {
       if (had) {
-        if (do_write) {
-          u64 r[8] = {key, oldv[0], oldv[1], oldv[2], oldv[3], t, ~0ull, 0};
-          store_row<8>(out, pos + c, r);
-        }
+        if (do_write) put_out_row<C>(out, pos + c, key, oldv, t, ~0ull);
         ++c;
       }
       if (has) {
-        if (do_write) {
-          u64 r[8] = {key, newv[0], newv[1], newv[2], newv[3], t, 1, 0};
-          store_row<8>(out, pos + c, r);
-        }
+        if (do_write) put_out_row<C>(out, pos + c, key, newv, t, 1);
         ++c;
       }
     }
     had = has;
 #pragma unroll
-    for (int w = 0; w < 4; ++w) oldv[w] = newv[w];
+    for (int w = 0; w < NV; ++w) oldv[w] = newv[w];
   }
-  if (do_write && c > 1) sort_key_corrections(out, pos, c);
+  if (do_write && c > 1) sort_key_corrections<C>(out, pos, c);
   return c;
 }
 
-template <bool WRITE>
+template <int C, bool WRITE>
 __global__ void __launch_bounds__(RT) k_corrections(const u64* __restrict__ rows, u64 n,
                                                     const __grid_constant__ TraceView prior, int agg_kind,
+                                                    u32 f64_mask, u32 n_lanes,
                                                     u32* __restrict__ tile_counts,
                                                     const u32* __restrict__ tile_base,
                                                     u64* __restrict__ out) {
+  constexpr int NW = LaneRows<C>::ARR_NW, ND = NW - 2;
   __shared__ u32 sm[34];
   const u64 i = (u64)blockIdx.x * RT + threadIdx.x;
   u32 cnt = 0;
-  const bool head = i < n && (i == 0 || rows[(i - 1) * 10] != rows[i * 10]);
+  const bool head = i < n && (i == 0 || rows[(i - 1) * NW] != rows[i * NW]);
   u64 key = 0;
-  u64 S0[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  u64 S0[ND];
+#pragma unroll
+  for (int w = 0; w < ND; ++w) S0[w] = 0;
   if (head) {
-    key = rows[i * 10];
-    prior_sum(prior, key, S0);
-    cnt = walk_key(rows, n, i, key, S0, agg_kind, false, nullptr, 0);
+    key = rows[i * NW];
+    prior_sum<C>(prior, key, S0);
+    cnt = walk_key<C>(rows, n, i, key, S0, agg_kind, f64_mask, n_lanes, false, nullptr, 0);
   }
   u32 total;
   u32 ex = block_exclusive_scan(cnt, sm, &total);
   if (!WRITE) {
     if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
   } else {
-    if (head && cnt > 0) walk_key(rows, n, i, key, S0, agg_kind, true, out, (u64)tile_base[blockIdx.x] + ex);
+    if (head && cnt > 0)
+      walk_key<C>(rows, n, i, key, S0, agg_kind, f64_mask, n_lanes, true, out, (u64)tile_base[blockIdx.x] + ex);
   }
 }
 
 // single-pass form (sizes on the device, chained tiles): see probe.cu
+template <int C>
 __global__ void __launch_bounds__(RT) k_corrections_lb(const u64* __restrict__ rows, const DLen dn,
                                                        const __grid_constant__ TraceView prior, int agg_kind,
+                                                       u32 f64_mask, u32 n_lanes,
                                                        const LookBack lb, u64* __restrict__ out, u64 out_cap,
                                                        u64* __restrict__ out_len, u64* __restrict__ status) {
+  constexpr int NW = LaneRows<C>::ARR_NW, ND = NW - 2;
   __shared__ u32 sm[34];
   __shared__ u32 s_tile;
   __shared__ u64 s_b;
@@ -373,13 +489,15 @@ __global__ void __launch_bounds__(RT) k_corrections_lb(const u64* __restrict__ r
     }
     const u64 i = (u64)tile * RT + threadIdx.x;
     u32 cnt = 0;
-    const bool head = i < n && (i == 0 || rows[(i - 1) * 10] != rows[i * 10]);
+    const bool head = i < n && (i == 0 || rows[(i - 1) * NW] != rows[i * NW]);
     u64 key = 0;
-    u64 S0[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    u64 S0[ND];
+#pragma unroll
+    for (int w = 0; w < ND; ++w) S0[w] = 0;
     if (head) {
-      key = rows[i * 10];
-      prior_sum(prior, key, S0);
-      cnt = walk_key(rows, n, i, key, S0, agg_kind, false, nullptr, 0);
+      key = rows[i * NW];
+      prior_sum<C>(prior, key, S0);
+      cnt = walk_key<C>(rows, n, i, key, S0, agg_kind, f64_mask, n_lanes, false, nullptr, 0);
     }
     u32 total;
     const u32 ex = block_exclusive_scan(cnt, sm, &total);
@@ -389,7 +507,7 @@ __global__ void __launch_bounds__(RT) k_corrections_lb(const u64* __restrict__ r
       if (pos + cnt > out_cap)
         atomicMax((unsigned long long*)status, (unsigned long long)(pos + cnt));
       else
-        walk_key(rows, n, i, key, S0, agg_kind, true, out, pos);
+        walk_key<C>(rows, n, i, key, S0, agg_kind, f64_mask, n_lanes, true, out, pos);
     }
     if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *out_len = excl + total;
   }
@@ -903,41 +1021,77 @@ int32_t mz_explode(mzgpu_ctx* ctx, const u64* d_r32, DLen n, u64 n_ub, int agg_k
   return MZGPU_OK;
 }
 
-int32_t mz_reduce_corrections(mzgpu_ctx* ctx, const u64* d_batch_rows, u64 n, const TraceView& prior,
-                              int agg_kind, DevMem* out, u64* n_out) {
+int32_t mz_explode_lanes(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
+                         u64* d_arr) {
+  if (n_ub == 0) return MZGPU_OK;
+  u64 grid = (n_ub + RT - 1) / RT;
+  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (ls.in_words * 8 + mz_lane_arr_bytes(c)) : 0);
+  switch (c) {
+    case 1: MZ_LAUNCH(ctx, k_explode_lanes<1>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr); break;
+    case 2: MZ_LAUNCH(ctx, k_explode_lanes<2>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr); break;
+    case 4: MZ_LAUNCH(ctx, k_explode_lanes<4>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr); break;
+    case 8: MZ_LAUNCH(ctx, k_explode_lanes<8>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr); break;
+    default: MZ_SET_ERR(ctx, "explode: lane class %d", c); return MZGPU_E_INVALID;
+  }
+  return MZGPU_OK;
+}
+
+#define MZ_LANE_CLASSES(c, X)                                       \
+  switch (c) {                                                      \
+    case 1: X(1); break;                                            \
+    case 2: X(2); break;                                            \
+    case 4: X(4); break;                                            \
+    case 8: X(8); break;                                            \
+    default: MZ_SET_ERR(ctx, "reduce: lane class %d", c); return MZGPU_E_INVALID; \
+  }
+
+int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
+                              int agg_kind, const LaneSet* ls, DevMem* out, u64* n_out) {
   *n_out = 0;
   if (n == 0) return out->alloc(ctx, 16);
+  const u32 fm = ls != nullptr ? ls->f64_mask : 0, nl = ls != nullptr ? ls->n : 1;
   const u64 n_tiles = (n + RT - 1) / RT;
   DevMem tiles;
   MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
   u64* d_total = ctx->d_scratch + 30;
-  MZ_LAUNCH(ctx, (k_corrections<false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind,
-            tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
+#define COUNT(C)                                                                                             \
+  MZ_LAUNCH(ctx, (k_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, \
+            tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr)
+  MZ_LANE_CLASSES(c, COUNT)
+#undef COUNT
   MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
   MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 30, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
   MZ_SYNC(ctx);
   ctx->stats.d2h_bytes += 8;
   const u64 total = ctx->h_scratch[30];
-  MZ_TRY(out->alloc(ctx, total * 64));
+  MZ_TRY(out->alloc(ctx, total * mz_lane_out_bytes(c)));
   *n_out = total;
   if (total == 0) return MZGPU_OK;
-  MZ_LAUNCH(ctx, (k_corrections<true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind,
-            (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
+#define WRITE(C)                                                                                            \
+  MZ_LAUNCH(ctx, (k_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, \
+            (u32*)nullptr, tiles.as<u32>(), out->as<u64>())
+  MZ_LANE_CLASSES(c, WRITE)
+#undef WRITE
   return MZGPU_OK;
 }
 
 // Single-pass form: batch length read on the device; at most two output rows per
 // new (key, time) row, so capacity 2 * n_ub always suffices.
-int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, const u64* d_batch_rows, DLen n, u64 n_ub,
-                                    const TraceView& prior, int agg_kind, u64* d_out, u64 out_cap,
-                                    u64* d_out_len) {
+int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, DLen n, u64 n_ub,
+                                    const TraceView& prior, int agg_kind, const LaneSet* ls, u64* d_out,
+                                    u64 out_cap, u64* d_out_len) {
+  const u32 fm = ls != nullptr ? ls->f64_mask : 0, nl = ls != nullptr ? ls->n : 1;
   LookBack lb;
   MZ_TRY(mz_lookback_begin(ctx, (n_ub + RT - 1) / RT, &lb));
   u64 grid = (n_ub + RT - 1) / RT;
   if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
   if (grid == 0) grid = 1;
-  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (80 + 16 + 80 + 128) : 0);
-  MZ_LAUNCH(ctx, k_corrections_lb, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, lb, d_out, out_cap,
-            d_out_len, ctx->d_status);
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (2 * mz_lane_arr_bytes(c) + 16 + 2 * mz_lane_out_bytes(c)) : 0);
+#define LAUNCH(C)                                                                                         \
+  MZ_LAUNCH(ctx, k_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, lb, \
+            d_out, out_cap, d_out_len, ctx->d_status)
+  MZ_LANE_CLASSES(c, LAUNCH)
+#undef LAUNCH
   return MZGPU_OK;
 }

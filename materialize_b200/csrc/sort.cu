@@ -334,6 +334,9 @@ int32_t mz_sort_perm(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n, D
     case 40: return sort_perm_t<40>(ctx, r, n, perm_out);
     case 80: return sort_perm_t<80>(ctx, r, n, perm_out);
     case 64: return sort_perm_t<64>(ctx, r, n, perm_out);
+    case 128: return sort_perm_t<128>(ctx, r, n, perm_out);
+    case 224: return sort_perm_t<224>(ctx, r, n, perm_out);
+    case 416: return sort_perm_t<416>(ctx, r, n, perm_out);
     default:
       MZ_SET_ERR(ctx, "sort: unsupported row width %d", row_bytes);
       return MZGPU_E_UNSUPPORTED;

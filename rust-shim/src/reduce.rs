@@ -57,6 +57,33 @@ impl GpuReduce {
     /// src/compute/src/arrangement/manager.rs:55-73).
     pub fn input_trace(&self) -> *mut sys::Spine { unsafe { sys::mzgpu_reduce_input_trace(self.h) } }
 }
+/// `build_accumulable` over several aggregates (`AccumulablePlan::simple_aggrs`, reduce.rs:146-158 of
+/// src/compute-types/src/plan): one arrangement of `(Vec<Accum>, Diff)`, one output row per key with
+/// every lane's COUNT and SUM (`sys::mzgpu_reduce_lanes_new` documents the row layouts).  The input is
+/// R32 (`in_row_bytes` 32) or a join's R40 result (40); `distinct_aggrs` are not a lane kind and come
+/// back as an error, so the caller keeps the Rust operator for such plans.
+pub struct GpuReduceLanes { h: *mut sys::Reduce, pub arr_row_bytes: u32, pub out_row_bytes: u32 }
+
+impl GpuReduceLanes {
+    pub fn new(in_row_bytes: u32, lanes: &[sys::AccumLane]) -> Result<Self, (i32, String)> {
+        let (mut arr, mut out) = (0u32, 0u32);
+        let mut h = std::ptr::null_mut();
+        unsafe {
+            sys::check(worker_ctx(), sys::mzgpu_reduce_lanes_row_bytes(lanes.len() as u32, &mut arr, &mut out))?;
+            sys::check(worker_ctx(), sys::mzgpu_reduce_lanes_new(worker_ctx(), in_row_bytes, lanes.as_ptr(), lanes.len() as u32, &mut h))?;
+        }
+        Ok(GpuReduceLanes { h, arr_row_bytes: arr, out_row_bytes: out })
+    }
+    /// One activation over a device buffer of input rows; output rows (`out_row_bytes` wide) are appended to `out`.
+    pub fn step(&mut self, rows: *mut sys::Buf, upper: u64, out: *mut sys::Buf) -> Result<(), (i32, String)> {
+        unsafe { sys::check(worker_ctx(), sys::mzgpu_reduce_lanes_buf(self.h, rows, upper, out)) }
+    }
+    pub fn input_trace(&self) -> *mut sys::Spine { unsafe { sys::mzgpu_reduce_input_trace(self.h) } }
+}
+impl Drop for GpuReduceLanes {
+    fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
+}
+
 impl Drop for GpuReduce {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
 }

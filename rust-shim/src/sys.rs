@@ -47,6 +47,13 @@ pub const AGG_THRESHOLD: i32 = 3;
 pub const AGG_MIN: i32 = 4;
 pub const AGG_MAX: i32 = 5;
 pub const AGG_TOPK: i32 = 6;
+pub const MAX_ACCUM_LANES: usize = 8;
+/// A column pick (mzgpu_field): bits [shift, shift + bits) of word `src`.
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct Field { pub src: u8, pub shift: u8, pub bits: u8, pub dst_shift: u8 }
+/// One aggregate lane of the multi-column accumulable reduce (mzgpu_accum_lane).
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct AccumLane { pub kind: i32, pub sign_extend: u32, pub field: Field }
 pub const COMM_ID_BYTES: usize = 128;
 pub const P2P_HANDLE_BYTES: usize = 64;
 
@@ -158,6 +165,10 @@ extern "C" {
     pub fn mzgpu_topk_new(ctx: *mut Ctx, limit: i64, offset: u64, descending: i32, out: *mut *mut Reduce) -> i32;
     pub fn mzgpu_reduce_accumulable_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf) -> i32;
     pub fn mzgpu_reduce_input_trace(r: *mut Reduce) -> *mut Spine;
+    pub fn mzgpu_reduce_lanes_row_bytes(n_lanes: u32, arr_row_bytes: *mut u32, out_row_bytes: *mut u32) -> i32;
+    pub fn mzgpu_reduce_lanes_new(ctx: *mut Ctx, in_row_bytes: u32, lanes: *const AccumLane, n_lanes: u32, out: *mut *mut Reduce) -> i32;
+    pub fn mzgpu_reduce_lanes(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf) -> i32;
+    pub fn mzgpu_reduce_lanes_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf) -> i32;
     pub fn mzgpu_rowkey_pack(row_bytes: *const u8, len: u64, key_out: *mut u64) -> i32;
     pub fn mzgpu_rowkeys_pack(data: *const u8, offsets: *const u64, n: u64, keys_out: *mut u64, n_done: *mut u64) -> i32;
     pub fn mzgpu_rowkey_unpack(key: u64, row_bytes_out: *mut u8, len_out: *mut u64) -> i32;
