@@ -8,6 +8,7 @@
 
 #include <chrono>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/mzgpu.h"
@@ -72,13 +73,11 @@ struct mzgpu_ctx {
   std::vector<struct mzgpu_batch*> deferred_inputs;  // retained until the flush
   u64 defer_seq = 0, flushed_seq = 0;   // deferred jobs enqueued / launched
   int deferred_unlaunched = 0;          // jobs prepared by mz_fused_defer and not launched yet
-  bool defer_merges = true;             // spine merges wait for each other (MZGPU_DEFER_MERGES=0: launch at once)
   // ---- side stream: batch merges (spine maintenance) run here, concurrently with the
   // operators on the main stream; a batch produced here carries side_seq and the main
   // stream waits for the side stream the first time it touches such a batch
   cudaStream_t main_stream = nullptr, side_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_side = nullptr;
-  bool use_side = true;   // spine merges of R32 arrangements run beside the operators (MZGPU_SIDE_STREAM=0: main stream)
   u64 side_seq = 0;    // merges issued on the side stream so far
   u64 joined_seq = 0;  // the main stream has waited for merges <= this
   // per-kernel profiling (mzgpu_profile_enable)
@@ -546,6 +545,34 @@ struct RowT<416> {  // C = 8
 // C >= 2 (96, 144 and 240 bytes, LaneRows below) were given widths that no arrangement row uses,
 // and deliberately have no RowT: mzgpu_buf_consolidate on them returns MZGPU_E_UNSUPPORTED
 // instead of summing the wrong words.
+
+// The compile-time values a runtime row width (or lane class) is dispatched over; each set is named
+// once here and every entry point instantiates its kernels for exactly the members of its set.
+template <int... V>
+struct IntSet {
+  static constexpr const char* kind = "row width";
+  static constexpr bool has(int v) { return ((v == V) || ...); }
+};
+using RowWidths = IntSet<16, 32, 40, 64, 80, 128, 224, 416>;  // every RowT: sort, consolidate, fused
+using BatchWidths = IntSet<32, 64, 80, 128, 224, 416>;         // sorted batches: merge, extract, index
+using ExchangeWidths = IntSet<32, 80>;
+struct LaneClasses : IntSet<1, 2, 4, 8> {  // accumulable reduce with 1, 2, 4 or 8 lanes (LaneRows below)
+  static constexpr const char* kind = "lane class";
+};
+
+template <int... V, class F>
+int32_t mz_dispatch_in(IntSet<V...>, mzgpu_ctx* ctx, int value, const char* what, const char* kind, F&& f) {
+  int32_t st = MZGPU_OK;
+  if (((value == V && (st = f(std::integral_constant<int, V>()), true)) || ...)) return st;
+  MZ_SET_ERR(ctx, "%s: unsupported %s %d", what, kind, value);
+  return MZGPU_E_UNSUPPORTED;
+}
+// f(std::integral_constant<int, value>()) when `value` is a member of Set, and its status;
+// MZGPU_E_UNSUPPORTED (with "<what>: unsupported <Set::kind> <value>" as the last error) otherwise.
+template <class Set, class F>
+int32_t mz_dispatch(mzgpu_ctx* ctx, int value, const char* what, F&& f) {
+  return mz_dispatch_in(Set(), ctx, value, what, Set::kind, f);
+}
 
 // Row widths of the accumulable reduce with lane class C (1, 2, 4 or 8 lanes): the arrangement
 // row (RowT above) and the output row (key, C x (count, sum_lo, sum_hi), flags, time, diff, pad).

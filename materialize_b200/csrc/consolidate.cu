@@ -185,33 +185,18 @@ int32_t gather_t(mzgpu_ctx* ctx, const u64* rows, const u32* perm, u64 n, u64* o
 
 }  // namespace
 
-#define DISPATCH_RB(rb, CALL)                                         \
-  switch (rb) {                                                       \
-    case 16: return CALL(16);                                         \
-    case 32: return CALL(32);                                         \
-    case 40: return CALL(40);                                         \
-    case 80: return CALL(80);                                         \
-    case 64: return CALL(64);                                         \
-    case 128: return CALL(128);                                       \
-    case 224: return CALL(224);                                       \
-    case 416: return CALL(416);                                       \
-    default:                                                          \
-      MZ_SET_ERR(ctx, "unsupported row width %d", rb);                \
-      return MZGPU_E_UNSUPPORTED;                                     \
-  }
-
 int32_t mz_gather_rows(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, const u32* d_perm, u64 n,
                        void* d_out) {
-#define CALL(RB) gather_t<RB>(ctx, (const u64*)d_rows, d_perm, n, (u64*)d_out)
-  DISPATCH_RB(row_bytes, CALL)
-#undef CALL
+  return mz_dispatch<RowWidths>(ctx, row_bytes, "gather", [&](auto RB) {
+    return gather_t<RB>(ctx, (const u64*)d_rows, d_perm, n, (u64*)d_out);
+  });
 }
 
 int32_t mz_consolidate_sorted(mzgpu_ctx* ctx, int row_bytes, const void* d_sorted, u64 n, void* d_out,
                               u64* n_out) {
-#define CALL(RB) consolidate_sorted_t<RB>(ctx, (const u64*)d_sorted, n, (u64*)d_out, n_out)
-  DISPATCH_RB(row_bytes, CALL)
-#undef CALL
+  return mz_dispatch<RowWidths>(ctx, row_bytes, "consolidate", [&](auto RB) {
+    return consolidate_sorted_t<RB>(ctx, (const u64*)d_sorted, n, (u64*)d_out, n_out);
+  });
 }
 
 int32_t mz_sort_consolidate(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n, DevMem* out,

@@ -337,18 +337,13 @@ int32_t mz_partition(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, DLen n, 
   unsigned long long* cur = (unsigned long long*)d_cursors;
   u64 blocks = (n_ub + XT - 1) / XT;
   unsigned grid = (unsigned)(blocks < (u64)ctx->num_sms * 8 ? blocks : (u64)ctx->num_sms * 8);
-  switch (row_bytes) {
-    case 32: MZ_LAUNCH(ctx, k_part_count<4>, grid, XT, 0, r, n, peers, c); break;
-    case 80: MZ_LAUNCH(ctx, k_part_count<10>, grid, XT, 0, r, n, peers, c); break;
-    default: MZ_SET_ERR(ctx, "exchange: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
-  }
-  MZ_LAUNCH(ctx, k_part_offsets, 1, 32, 0, c, peers, cur);
-  switch (row_bytes) {
-    case 32: MZ_LAUNCH(ctx, k_part_scatter<4>, grid, XT, 0, r, n, peers, cur, (u64*)d_out); break;
-    case 80: MZ_LAUNCH(ctx, k_part_scatter<10>, grid, XT, 0, r, n, peers, cur, (u64*)d_out); break;
-    default: return MZGPU_E_UNSUPPORTED;
-  }
-  return MZGPU_OK;
+  return mz_dispatch<ExchangeWidths>(ctx, row_bytes, "exchange", [&](auto RB) {
+    constexpr int NW = RowT<RB>::NW;
+    MZ_LAUNCH(ctx, k_part_count<NW>, grid, XT, 0, r, n, peers, c);
+    MZ_LAUNCH(ctx, k_part_offsets, 1, 32, 0, c, peers, cur);
+    MZ_LAUNCH(ctx, k_part_scatter<NW>, grid, XT, 0, r, n, peers, cur, (u64*)d_out);
+    return MZGPU_OK;
+  });
 }
 
 // All buffers of one exchange round in three launches (count, offsets, scatter).
@@ -365,7 +360,7 @@ int32_t mz_partition_many(mzgpu_ctx* ctx, u32 k, const int* row_bytes, const voi
   memset(&jobs, 0, sizeof(jobs));
   u64 max_ub = 0;
   for (u32 j = 0; j < k; ++j) {
-    if (row_bytes[j] != 32 && row_bytes[j] != 80) {
+    if (!ExchangeWidths::has(row_bytes[j])) {
       MZ_SET_ERR(ctx, "exchange: unsupported row width %d", row_bytes[j]);
       return MZGPU_E_UNSUPPORTED;
     }

@@ -92,8 +92,8 @@ struct FusedArgs {
   u64* lb_keep;
   u32 max_g;     // CTAs that take part at most
   u32 merge;     // both inputs are sorted and consolidated: merge path instead of a sort
-  u32 fast;      // fast MSD path allowed (MZGPU_FUSED_FAST=0 turns it off: bisecting, A/B timing)
-  u32 merge_sort_max;  // a merge of at most this many rows runs as a sort of A ++ B (MZGPU_MERGE_SORT_MAX)
+  u32 fast;      // fast MSD path allowed (fused_prepare always sets it)
+  u32 merge_sort_max;  // a merge of at most this many rows runs as a sort of A ++ B (MERGE_SORT_MAX)
 };
 
 __device__ __forceinline__ u64 gtimer() {
@@ -1557,29 +1557,9 @@ __global__ void __launch_bounds__(FT, (RB >= 80 ? 2 : 4)) k_fused_many(const __g
   fused_body<RB>(m.job[j], blockIdx.x - m.start[j], m.start[j + 1] - m.start[j]);
 }
 
-static int fused_fast_mode() {
-  static int fast = -1;
-  if (fast < 0) {
-    const char* ev = getenv("MZGPU_FUSED_FAST");
-    fast = ev ? atoi(ev) : 1;
-  }
-  return fast;
-}
-
 // Two sorted update-batch-sized inputs merge faster as a sort of A ++ B on the fast MSD path; from a few
-// hundred thousand rows each the merge-path form wins (tools/merge_bench.py times both sides of the switch;
-// MZGPU_MERGE_SORT_MAX moves it).
-constexpr long long MERGE_SORT_MAX_DEFAULT = 1ll << 18;
-static u32 fused_merge_sort_max() {
-  static long long v = -1;
-  if (v < 0) {
-    const char* ev = getenv("MZGPU_MERGE_SORT_MAX");
-    v = ev ? atoll(ev) : (long long)MERGE_SORT_MAX_DEFAULT;
-    if (v > (long long)MSD_FAST_MAX_ROWS) v = (long long)MSD_FAST_MAX_ROWS;
-    if (v < 0) v = 0;
-  }
-  return (u32)v;
-}
+// hundred thousand rows each the merge-path form wins.
+constexpr u32 MERGE_SORT_MAX = 1u << 18;
 
 // Everything of a launch but the launch: buffers, control block, kernel arguments.
 // `slot` < 0: the context's single-job control blocks; otherwise job slot `slot` of a
@@ -1668,8 +1648,8 @@ int32_t fused_prepare(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* res, int sl
   a.table_cap = slots;
   a.res = res->st.dptr();
   a.kres = res->kst.dptr();
-  a.fast = fused_fast_mode() ? 1u : 0u;
-  a.merge_sort_max = fused_merge_sort_max();
+  a.fast = 1u;
+  a.merge_sort_max = MERGE_SORT_MAX;
   a.dbg = nullptr;
   if (ctx->profile && ctx->d_dbg != nullptr && ctx->dbg_next < MZ_DBG_RECORDS) {
     a.dbg = ctx->d_dbg + 32 * (size_t)ctx->dbg_next++;
@@ -1677,18 +1657,6 @@ int32_t fused_prepare(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* res, int sl
   }
   *want_out = (cap + 127) / 128 + 1;  // one CTA per MSD bucket (128..256 rows each), at least one per radix tile
   return MZGPU_OK;
-}
-
-static int fused_coop_mode() {
-  // A cooperative launch guarantees what the kernel's own grid barrier needs (all CTAs
-  // co-resident).  MZGPU_COOP=0 uses a plain launch instead (same grid, <= the resident
-  // capacity): only for measuring the launch-path difference.
-  static int coop = -1;
-  if (coop < 0) {
-    const char* ev = getenv("MZGPU_COOP");
-    coop = ev ? atoi(ev) : 1;
-  }
-  return coop;
 }
 
 template <int RB>
@@ -1727,13 +1695,8 @@ int32_t fused_t(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* res) {
     // mzgpu_profile_report substitutes the actual row count of profiled launches.
     MZ_BYTES(ctx, (job.na.p == nullptr && job.nb.p == nullptr) ? (job.na.imm + job.nb.imm) * RB * 4 : 0);
     ProfScope prof(ctx, "k_fused_consolidate");
-    cudaError_t e;
-    if (fused_coop_mode()) {
-      e = cudaLaunchCooperativeKernel((void*)k_fused_consolidate<RB>, dim3(grid), dim3(FT), kargs, 0, ctx->stream);
-    } else {
-      k_fused_consolidate<RB><<<grid, FT, 0, ctx->stream>>>(a);
-      e = cudaGetLastError();
-    }
+    const cudaError_t e =
+        cudaLaunchCooperativeKernel((void*)k_fused_consolidate<RB>, dim3(grid), dim3(FT), kargs, 0, ctx->stream);
     if (e != cudaSuccess) {
       MZ_SET_ERR(ctx, "cooperative launch failed: %s", cudaGetErrorString(e));
       ctx->sticky = true;
@@ -1789,13 +1752,8 @@ int32_t fused_launch_many(mzgpu_ctx* ctx, int k, const FusedArgs* args, const u6
   {
     MZ_BYTES(ctx, bytes);
     ProfScope prof(ctx, "k_fused_consolidate");  // one profile line for the operator, whatever the launch shape
-    cudaError_t e;
-    if (fused_coop_mode()) {
-      e = cudaLaunchCooperativeKernel((void*)k_fused_many<RB>, dim3(at), dim3(FT), kargs, 0, ctx->stream);
-    } else {
-      k_fused_many<RB><<<at, FT, 0, ctx->stream>>>(m);
-      e = cudaGetLastError();
-    }
+    const cudaError_t e =
+        cudaLaunchCooperativeKernel((void*)k_fused_many<RB>, dim3(at), dim3(FT), kargs, 0, ctx->stream);
     if (e != cudaSuccess) {
       MZ_SET_ERR(ctx, "cooperative launch failed: %s", cudaGetErrorString(e));
       ctx->sticky = true;
@@ -1860,18 +1818,9 @@ int32_t mz_fused_flush(mzgpu_ctx* ctx) {
   const int k = d->k;
   d->k = 0;  // whatever happens below, the jobs are not retried
   ctx->deferred_unlaunched = 0;
-  int32_t st;
-  switch (d->rb) {
-    case 16: st = fused_launch_many<16>(ctx, k, d->args, d->want, d->bytes); break;
-    case 32: st = fused_launch_many<32>(ctx, k, d->args, d->want, d->bytes); break;
-    case 40: st = fused_launch_many<40>(ctx, k, d->args, d->want, d->bytes); break;
-    case 80: st = fused_launch_many<80>(ctx, k, d->args, d->want, d->bytes); break;
-    case 64: st = fused_launch_many<64>(ctx, k, d->args, d->want, d->bytes); break;
-    case 128: st = fused_launch_many<128>(ctx, k, d->args, d->want, d->bytes); break;
-    case 224: st = fused_launch_many<224>(ctx, k, d->args, d->want, d->bytes); break;
-    case 416: st = fused_launch_many<416>(ctx, k, d->args, d->want, d->bytes); break;
-    default: st = MZGPU_E_UNSUPPORTED; break;
-  }
+  const int32_t st = mz_dispatch<RowWidths>(ctx, d->rb, "fused flush", [&](auto RB) {
+    return fused_launch_many<RB>(ctx, k, d->args, d->want, d->bytes);
+  });
   for (int j = 0; j < k; ++j) d->scratch[j].release();  // stream ordered: after the launch
   d->bytes = 0;
   mz_cnt_unpark(ctx);  // counter blocks freed while the jobs waited (their inputs' lengths)
@@ -1891,21 +1840,7 @@ int32_t mz_fused_defer(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* out) {
   if (ctx->fused_deferred == nullptr) ctx->fused_deferred = new FusedDeferred();
   FusedDeferred* d = (FusedDeferred*)ctx->fused_deferred;
   if (d->k > 0 && (d->rb != job.rb || d->k == FUSED_MANY_MAX)) MZ_TRY(mz_fused_flush(ctx));
-  int32_t st;
-  switch (job.rb) {
-    case 16: st = fused_defer_t<16>(ctx, d, job, out); break;
-    case 32: st = fused_defer_t<32>(ctx, d, job, out); break;
-    case 40: st = fused_defer_t<40>(ctx, d, job, out); break;
-    case 80: st = fused_defer_t<80>(ctx, d, job, out); break;
-    case 64: st = fused_defer_t<64>(ctx, d, job, out); break;
-    case 128: st = fused_defer_t<128>(ctx, d, job, out); break;
-    case 224: st = fused_defer_t<224>(ctx, d, job, out); break;
-    case 416: st = fused_defer_t<416>(ctx, d, job, out); break;
-    default:
-      MZ_SET_ERR(ctx, "fused: unsupported row width %d", job.rb);
-      return MZGPU_E_UNSUPPORTED;
-  }
-  if (st != MZGPU_OK) return st;
+  MZ_TRY(mz_dispatch<RowWidths>(ctx, job.rb, "fused", [&](auto RB) { return fused_defer_t<RB>(ctx, d, job, out); }));
   ctx->deferred_unlaunched = d->k;
   out->st.mark_written();
   out->kst.mark_written();
@@ -1924,33 +1859,9 @@ int32_t mz_fused_consolidate_many(mzgpu_ctx* ctx, int k, const FusedJob* jobs, F
       MZ_SET_ERR(ctx, "fused multi-job launch: mixed row widths %d / %d", jobs[0].rb, jobs[j].rb);
       return MZGPU_E_INVALID;
     }
-  switch (jobs[0].rb) {
-    case 16: return fused_many_t<16>(ctx, k, jobs, outs);
-    case 32: return fused_many_t<32>(ctx, k, jobs, outs);
-    case 40: return fused_many_t<40>(ctx, k, jobs, outs);
-    case 80: return fused_many_t<80>(ctx, k, jobs, outs);
-    case 64: return fused_many_t<64>(ctx, k, jobs, outs);
-    case 128: return fused_many_t<128>(ctx, k, jobs, outs);
-    case 224: return fused_many_t<224>(ctx, k, jobs, outs);
-    case 416: return fused_many_t<416>(ctx, k, jobs, outs);
-    default:
-      MZ_SET_ERR(ctx, "fused: unsupported row width %d", jobs[0].rb);
-      return MZGPU_E_UNSUPPORTED;
-  }
+  return mz_dispatch<RowWidths>(ctx, jobs[0].rb, "fused", [&](auto RB) { return fused_many_t<RB>(ctx, k, jobs, outs); });
 }
 
 int32_t mz_fused_consolidate(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* res) {
-  switch (job.rb) {
-    case 16: return fused_t<16>(ctx, job, res);
-    case 32: return fused_t<32>(ctx, job, res);
-    case 40: return fused_t<40>(ctx, job, res);
-    case 80: return fused_t<80>(ctx, job, res);
-    case 64: return fused_t<64>(ctx, job, res);
-    case 128: return fused_t<128>(ctx, job, res);
-    case 224: return fused_t<224>(ctx, job, res);
-    case 416: return fused_t<416>(ctx, job, res);
-    default:
-      MZ_SET_ERR(ctx, "fused: unsupported row width %d", job.rb);
-      return MZGPU_E_UNSUPPORTED;
-  }
+  return mz_dispatch<RowWidths>(ctx, job.rb, "fused", [&](auto RB) { return fused_t<RB>(ctx, job, res); });
 }

@@ -54,7 +54,6 @@ extern "C" int32_t mzgpu_ctx_create(int32_t device, int32_t worker_index, int32_
     MZ_CUDA(ctx, cudaMalloc(&ctx->d_fused_ctl[i], mz_fused_ctl_bytes()));
     MZ_CUDA(ctx, cudaMemset(ctx->d_fused_ctl[i], 0, mz_fused_ctl_bytes()));
   }
-  if (const char* e = getenv("MZGPU_DEFER_MERGES")) ctx->defer_merges = atoi(e) != 0;
   if (const char* e = getenv("MZGPU_MID_BLOCK_MB")) ctx->mid_block = (size_t)strtoull(e, nullptr, 10) << 20;
   for (int i = 0; i < 16; ++i) {
     MZ_CUDA(ctx, cudaMalloc(&ctx->d_fused_ctl_many[i], mz_fused_ctl_bytes()));
@@ -64,7 +63,6 @@ extern "C" int32_t mzgpu_ctx_create(int32_t device, int32_t worker_index, int32_
   MZ_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->side_stream, cudaStreamNonBlocking));
   MZ_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
   MZ_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_side, cudaEventDisableTiming));
-  if (const char* e = getenv("MZGPU_SIDE_STREAM")) ctx->use_side = atoi(e) != 0;
   // keep freed blocks cached in the stream-ordered pool
   cudaMemPool_t pool;
   MZ_CUDA(ctx, cudaDeviceGetDefaultMemPool(&pool, device));
@@ -421,11 +419,11 @@ static int32_t validate_closure(mzgpu_ctx* ctx, const mzgpu_closure* c) {
   return MZGPU_OK;
 }
 
-// arrangement rows: R32, and the accumulable rows of every lane class (RACC = class 1)
-static bool arrangement_row_bytes(uint32_t rb) { return rb == 32 || rb == 80 || rb == 128 || rb == 224 || rb == 416; }
-static bool valid_row_bytes(uint32_t rb) {
-  return rb == 16 || rb == 40 || rb == 64 || arrangement_row_bytes(rb) || rb == 96 || rb == 144 || rb == 240;
-}
+// arrangement rows: every sorted-batch width but the reduce's 64-byte output rows, i.e. R32 and the
+// accumulable rows of every lane class (RACC = class 1)
+static bool arrangement_row_bytes(uint32_t rb) { return rb != 64 && BatchWidths::has((int)rb); }
+// buffer rows: every RowT width, and the wide output rows of the lanes reduce (they have no RowT)
+static bool valid_row_bytes(uint32_t rb) { return RowWidths::has((int)rb) || rb == 96 || rb == 144 || rb == 240; }
 
 // ------------------------------------------------------ device-side append
 // dst[base ...] = src[0 .. n), new length left in *out_len; every size may live
@@ -1042,12 +1040,6 @@ extern "C" int32_t mzgpu_builder_done(mzgpu_builder* b, mzgpu_desc desc, mzgpu_b
   return st;
 }
 
-static bool mz_merge_kernels_on() {
-  // on by default (the GPU suite and the bench's per-step parity check pass either way);
-  // MZGPU_MERGE_KERNELS=0 runs R32 merges in the fused cooperative kernel instead
-  static const bool on = getenv("MZGPU_MERGE_KERNELS") == nullptr || atoi(getenv("MZGPU_MERGE_KERNELS")) != 0;
-  return on;
-}
 // Batch::Merger in one step: union, advance_by(since), consolidate, index.
 static int32_t merge_batches(mzgpu_batch* b1, mzgpu_batch* b2, u64 since, mzgpu_batch** out) {
   mzgpu_ctx* ctx = b1->ctx;
@@ -1060,8 +1052,8 @@ static int32_t merge_batches(mzgpu_batch* b1, mzgpu_batch* b2, u64 since, mzgpu_
   // max(time, since), for which 0 is the no-op
   const u64 adv = since == MZGPU_FRONTIER_EMPTY ? 0 : since;
   // R32 arrangements: the merge-path kernels (mergepath.cu) -- three ordinary launches, any size, no
-  // host wait, no cooperative launch (MZGPU_MERGE_KERNELS=0 switches them off)
-  if (mz_merge_kernels_on() && b1->rb == 32 && (b1->len_ub + b2->len_ub + 1023) / 1024 <= MZ_LB_TILES) {
+  // host wait, no cooperative launch
+  if (b1->rb == 32 && (b1->len_ub + b2->len_ub + 1023) / 1024 <= MZ_LB_TILES) {
     const u64 cap = b1->len_ub + b2->len_ub;
     FusedOut fo;
     MZ_TRY(mz_merge_r32_async(ctx, b1->rows.p, batch_dlen(b1), b2->rows.p, batch_dlen(b2), cap, adv, &fo));
@@ -1083,7 +1075,7 @@ static int32_t merge_batches(mzgpu_batch* b1, mzgpu_batch* b2, u64 since, mzgpu_
     job.want_index = true;
     job.merge = true;
     FusedOut fo;
-    if (ctx->defer_merges && ctx->stream == ctx->main_stream) {
+    if (ctx->stream == ctx->main_stream) {
       // The merges that the inserts of one timestamp trigger (one per arrangement, all alike)
       // are independent: they are prepared here and launched together, by the first reader of
       // any of their outputs (batch_ready) or the next counter read-back.
@@ -1601,7 +1593,7 @@ struct mzgpu_spine {
     if (b1->st.known && b2->st.known && b1->st.v[0] == 0 && b2->st.v[0] == 0) {
       mzgpu_desc d = {b1->desc.lower, b2->desc.upper, m.merge_since};
       st = make_empty_batch(ctx, rb, d, &out);
-    } else if (ctx->use_side && ctx->stream == ctx->main_stream && !ctx->profile && mz_merge_kernels_on() && rb == 32) {
+    } else if (ctx->stream == ctx->main_stream && !ctx->profile && rb == 32) {
       // Spine maintenance runs on the side stream, concurrently with the operators on the main
       // stream (the merge-path kernels are ordinary launches: they share the machine with the probes
       // and the reduce of the timestamp that triggered them).  The side stream first catches up with

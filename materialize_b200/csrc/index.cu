@@ -161,16 +161,10 @@ int32_t mz_count_keys(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n, 
   u64* d_count = ctx->d_scratch + 24;
   MZ_CUDA(ctx, cudaMemsetAsync(d_count, 0, 16, ctx->stream));
   unsigned grid = (unsigned)((n + 511) / 512);
-  const u64* r = (const u64*)d_rows;
-  switch (row_bytes) {
-    case 32: MZ_LAUNCH(ctx, k_count_keys<4>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
-    case 80: MZ_LAUNCH(ctx, k_count_keys<10>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
-    case 64: MZ_LAUNCH(ctx, k_count_keys<8>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
-    case 128: MZ_LAUNCH(ctx, k_count_keys<16>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
-    case 224: MZ_LAUNCH(ctx, k_count_keys<28>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
-    case 416: MZ_LAUNCH(ctx, k_count_keys<52>, grid, 512, 0, r, n, (unsigned long long*)d_count); break;
-    default: MZ_SET_ERR(ctx, "index: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
-  }
+  MZ_TRY(mz_dispatch<BatchWidths>(ctx, row_bytes, "index", [&](auto RB) {
+    MZ_LAUNCH(ctx, k_count_keys<RowT<RB>::NW>, grid, 512, 0, (const u64*)d_rows, n, (unsigned long long*)d_count);
+    return MZGPU_OK;
+  }));
   MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 24, d_count, 16, cudaMemcpyDeviceToHost, ctx->stream));
   MZ_SYNC(ctx);
   ctx->stats.d2h_bytes += 16;
@@ -188,18 +182,10 @@ int32_t mz_build_index(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n,
   MZ_CUDA(ctx, cudaMemsetAsync(table->p, 0, slots * sizeof(HashSlot), ctx->stream));
   if (n == 0) return MZGPU_OK;
   unsigned grid = (unsigned)((n + 511) / 512);
-  const u64* r = (const u64*)d_rows;
-  HashSlot* t = table->as<HashSlot>();
-  switch (row_bytes) {
-    case 32: MZ_LAUNCH(ctx, k_build_index<4>, grid, 512, 0, r, n, t, slots - 1); break;
-    case 80: MZ_LAUNCH(ctx, k_build_index<10>, grid, 512, 0, r, n, t, slots - 1); break;
-    case 64: MZ_LAUNCH(ctx, k_build_index<8>, grid, 512, 0, r, n, t, slots - 1); break;
-    case 128: MZ_LAUNCH(ctx, k_build_index<16>, grid, 512, 0, r, n, t, slots - 1); break;
-    case 224: MZ_LAUNCH(ctx, k_build_index<28>, grid, 512, 0, r, n, t, slots - 1); break;
-    case 416: MZ_LAUNCH(ctx, k_build_index<52>, grid, 512, 0, r, n, t, slots - 1); break;
-    default: MZ_SET_ERR(ctx, "index: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
-  }
-  return MZGPU_OK;
+  return mz_dispatch<BatchWidths>(ctx, row_bytes, "index", [&](auto RB) {
+    MZ_LAUNCH(ctx, k_build_index<RowT<RB>::NW>, grid, 512, 0, (const u64*)d_rows, n, table->as<HashSlot>(), slots - 1);
+    return MZGPU_OK;
+  });
 }
 
 // a8: batched seek_key.  d_probe: n_probe keys (device); d_out: n_probe x {key, first, len}.
@@ -207,17 +193,10 @@ int32_t mz_seek_keys(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, DLen n, 
                      u64* d_out) {
   if (n_probe == 0) return MZGPU_OK;
   unsigned grid = (unsigned)((n_probe + 255) / 256);
-  const u64* r = (const u64*)d_rows;
-  switch (row_bytes) {
-    case 32: MZ_LAUNCH(ctx, k_seek_keys<4>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
-    case 80: MZ_LAUNCH(ctx, k_seek_keys<10>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
-    case 64: MZ_LAUNCH(ctx, k_seek_keys<8>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
-    case 128: MZ_LAUNCH(ctx, k_seek_keys<16>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
-    case 224: MZ_LAUNCH(ctx, k_seek_keys<28>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
-    case 416: MZ_LAUNCH(ctx, k_seek_keys<52>, grid, 256, 0, r, n, d_probe, n_probe, d_out); break;
-    default: MZ_SET_ERR(ctx, "seek_keys: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
-  }
-  return MZGPU_OK;
+  return mz_dispatch<BatchWidths>(ctx, row_bytes, "seek_keys", [&](auto RB) {
+    MZ_LAUNCH(ctx, k_seek_keys<RowT<RB>::NW>, grid, 256, 0, (const u64*)d_rows, n, d_probe, n_probe, d_out);
+    return MZGPU_OK;
+  });
 }
 
 // a8: step_key paging.  n_rows is exact (the caller resolved the batch); d_out: max_keys x {key, first, len}.
@@ -231,23 +210,12 @@ int32_t mz_key_page(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n_row
   MZ_TRY(total.alloc(ctx, 16));
   const u64* r = (const u64*)d_rows;
   const DLen dn = dlen_imm(n_rows);
-  switch (row_bytes) {
-    case 32: MZ_LAUNCH(ctx, k_key_heads_count<4>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
-    case 80: MZ_LAUNCH(ctx, k_key_heads_count<10>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
-    case 64: MZ_LAUNCH(ctx, k_key_heads_count<8>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
-    case 128: MZ_LAUNCH(ctx, k_key_heads_count<16>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
-    case 224: MZ_LAUNCH(ctx, k_key_heads_count<28>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
-    case 416: MZ_LAUNCH(ctx, k_key_heads_count<52>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>()); break;
-    default: MZ_SET_ERR(ctx, "key_page: unsupported row width %d", row_bytes); return MZGPU_E_UNSUPPORTED;
-  }
-  MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, counts.as<u32>(), tiles, total.as<u64>());
-  switch (row_bytes) {
-    case 32: MZ_LAUNCH(ctx, k_key_heads_emit<4>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
-    case 80: MZ_LAUNCH(ctx, k_key_heads_emit<10>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
-    case 128: MZ_LAUNCH(ctx, k_key_heads_emit<16>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
-    case 224: MZ_LAUNCH(ctx, k_key_heads_emit<28>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
-    case 416: MZ_LAUNCH(ctx, k_key_heads_emit<52>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
-    default: MZ_LAUNCH(ctx, k_key_heads_emit<8>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys, d_out); break;
-  }
-  return MZGPU_OK;
+  return mz_dispatch<BatchWidths>(ctx, row_bytes, "key_page", [&](auto RB) {
+    constexpr int NW = RowT<RB>::NW;
+    MZ_LAUNCH(ctx, k_key_heads_count<NW>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>());
+    MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, counts.as<u32>(), tiles, total.as<u64>());
+    MZ_LAUNCH(ctx, k_key_heads_emit<NW>, (unsigned)tiles, 256, 0, r, dn, counts.as<u32>(), first_ordinal, max_keys,
+              d_out);
+    return MZGPU_OK;
+  });
 }

@@ -258,33 +258,14 @@ int32_t extract_t(mzgpu_ctx* ctx, const u64* rows, u64 n, u64 upper, DevMem* shi
 
 int32_t mz_merge_consolidate(mzgpu_ctx* ctx, int row_bytes, const void* d_a, u64 na, const void* d_b,
                              u64 nb, u64 since, DevMem* out, u64* n_out) {
-  const u64* a = (const u64*)d_a;
-  const u64* b = (const u64*)d_b;
-  switch (row_bytes) {
-    case 32: return merge_t<32>(ctx, a, na, b, nb, since, out, n_out);
-    case 80: return merge_t<80>(ctx, a, na, b, nb, since, out, n_out);
-    case 64: return merge_t<64>(ctx, a, na, b, nb, since, out, n_out);
-    case 128: return merge_t<128>(ctx, a, na, b, nb, since, out, n_out);
-    case 224: return merge_t<224>(ctx, a, na, b, nb, since, out, n_out);
-    case 416: return merge_t<416>(ctx, a, na, b, nb, since, out, n_out);
-    default:
-      MZ_SET_ERR(ctx, "merge: unsupported row width %d", row_bytes);
-      return MZGPU_E_UNSUPPORTED;
-  }
+  return mz_dispatch<BatchWidths>(ctx, row_bytes, "merge", [&](auto RB) {
+    return merge_t<RB>(ctx, (const u64*)d_a, na, (const u64*)d_b, nb, since, out, n_out);
+  });
 }
 
 int32_t mz_extract(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n, u64 upper, DevMem* ship,
                    u64* n_ship, DevMem* keep, u64* n_keep, u64* min_keep_time) {
-  const u64* r = (const u64*)d_rows;
-  switch (row_bytes) {
-    case 32: return extract_t<32>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
-    case 80: return extract_t<80>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
-    case 64: return extract_t<64>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
-    case 128: return extract_t<128>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
-    case 224: return extract_t<224>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
-    case 416: return extract_t<416>(ctx, r, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
-    default:
-      MZ_SET_ERR(ctx, "extract: unsupported row width %d", row_bytes);
-      return MZGPU_E_UNSUPPORTED;
-  }
+  return mz_dispatch<BatchWidths>(ctx, row_bytes, "extract", [&](auto RB) {
+    return extract_t<RB>(ctx, (const u64*)d_rows, n, upper, ship, n_ship, keep, n_keep, min_keep_time);
+  });
 }

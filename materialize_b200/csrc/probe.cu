@@ -828,12 +828,11 @@ int32_t mz_probe_async_many(mzgpu_ctx* ctx, int k, const ProbeJobHost* jobs) {
     chain_tiles[c] = tiles;
   }
   // all chains of a launch run side by side: the resident CTAs (3 per SM) are shared out in proportion
-  // to the chains' tiles (MZGPU_PROBE_SHARE=0: equally, the round-1 split, for A/B runs)
-  static const bool prop = getenv("MZGPU_PROBE_SHARE") == nullptr || atoi(getenv("MZGPU_PROBE_SHARE")) != 0;
+  // to the chains' tiles
   const u64 resident = (u64)ctx->num_sms * 3;
   max_grid = 1;
   for (int c = 0; c < nc; ++c) {
-    u64 g = prop && total_tiles > 0 ? (resident * chain_tiles[c] + total_tiles - 1) / total_tiles : (resident + nc - 1) / (u64)nc;
+    u64 g = total_tiles > 0 ? (resident * chain_tiles[c] + total_tiles - 1) / total_tiles : 1;
     if (g > chain_tiles[c]) g = chain_tiles[c];  // one CTA per tile at most
     if (g == 0) g = 1;                            // (an empty chain still has its length word to write)
     m.ctas[c] = (u32)g;

@@ -43,9 +43,7 @@ __device__ __forceinline__ void rs_store(u32* p, u32 v) {
 // hardware MATCH.ANY runs on the address-divergence unit at a small fraction of
 // the ballot rate: with ~30 distinct digits per warp it becomes the pipe that
 // bounds the whole pass.)
-template <bool BALLOT>
 __device__ __forceinline__ u32 match_digit(u32 d) {
-  if (!BALLOT) return __match_any_sync(0xffffffffu, d);
   u32 m = 0xffffffffu;
 #pragma unroll
   for (int b = 0; b < 8; ++b) {
@@ -86,7 +84,7 @@ __device__ __forceinline__ void rs_mbar_wait(u64* bar, u32 parity) {
       : "memory");
 }
 
-template <int ITEMS, int THREADS = RS_THREADS, bool BALLOT = true, bool TMA_LOAD = false>
+template <int ITEMS, int THREADS = RS_THREADS, bool TMA_LOAD = false>
 __device__ __forceinline__ void rs_tile_pass(RsSmemT<ITEMS, THREADS>& s, u32 tile, const u64* kin,
                                              const u32* vin, u64* kout,
                                              u32* vout, u64 n, int shift,
@@ -134,12 +132,12 @@ __device__ __forceinline__ void rs_tile_pass(RsSmemT<ITEMS, THREADS>& s, u32 til
       val[j] = ok ? vin[base + idx] : 0u;
     }
   }
-  // stable in-warp ranking with match_any / popc (warp-shuffle histograms)
+  // stable in-warp ranking with match_digit / popc (warp-shuffle histograms)
   const u32 lt_mask = (1u << lane) - 1;
 #pragma unroll
   for (int j = 0; j < ITEMS; ++j) {
     u32 d = (u32)((key[j] >> shift) & 255);
-    u32 m = match_digit<BALLOT>(d);
+    u32 m = match_digit(d);
     u32 leader = __ffs(m) - 1;
     u32 old = 0;
     if (lane == leader) {

@@ -1027,24 +1027,11 @@ int32_t mz_explode_lanes(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u64 n
   u64 grid = (n_ub + RT - 1) / RT;
   if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * (ls.in_words * 8 + mz_lane_arr_bytes(c)) : 0);
-  switch (c) {
-    case 1: MZ_LAUNCH(ctx, k_explode_lanes<1>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr); break;
-    case 2: MZ_LAUNCH(ctx, k_explode_lanes<2>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr); break;
-    case 4: MZ_LAUNCH(ctx, k_explode_lanes<4>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr); break;
-    case 8: MZ_LAUNCH(ctx, k_explode_lanes<8>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr); break;
-    default: MZ_SET_ERR(ctx, "explode: lane class %d", c); return MZGPU_E_INVALID;
-  }
-  return MZGPU_OK;
+  return mz_dispatch<LaneClasses>(ctx, c, "explode", [&](auto C) {
+    MZ_LAUNCH(ctx, k_explode_lanes<C>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr);
+    return MZGPU_OK;
+  });
 }
-
-#define MZ_LANE_CLASSES(c, X)                                       \
-  switch (c) {                                                      \
-    case 1: X(1); break;                                            \
-    case 2: X(2); break;                                            \
-    case 4: X(4); break;                                            \
-    case 8: X(8); break;                                            \
-    default: MZ_SET_ERR(ctx, "reduce: lane class %d", c); return MZGPU_E_INVALID; \
-  }
 
 int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
                               int agg_kind, const LaneSet* ls, DevMem* out, u64* n_out) {
@@ -1055,11 +1042,11 @@ int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u6
   DevMem tiles;
   MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
   u64* d_total = ctx->d_scratch + 30;
-#define COUNT(C)                                                                                             \
-  MZ_LAUNCH(ctx, (k_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, \
-            tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr)
-  MZ_LANE_CLASSES(c, COUNT)
-#undef COUNT
+  MZ_TRY(mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
+    MZ_LAUNCH(ctx, (k_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
+              tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
+    return MZGPU_OK;
+  }));
   MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
   MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 30, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
   MZ_SYNC(ctx);
@@ -1068,12 +1055,11 @@ int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u6
   MZ_TRY(out->alloc(ctx, total * mz_lane_out_bytes(c)));
   *n_out = total;
   if (total == 0) return MZGPU_OK;
-#define WRITE(C)                                                                                            \
-  MZ_LAUNCH(ctx, (k_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, \
-            (u32*)nullptr, tiles.as<u32>(), out->as<u64>())
-  MZ_LANE_CLASSES(c, WRITE)
-#undef WRITE
-  return MZGPU_OK;
+  return mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
+    MZ_LAUNCH(ctx, (k_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
+              (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
+    return MZGPU_OK;
+  });
 }
 
 // Single-pass form: batch length read on the device; at most two output rows per
@@ -1088,10 +1074,9 @@ int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_ro
   if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
   if (grid == 0) grid = 1;
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * (2 * mz_lane_arr_bytes(c) + 16 + 2 * mz_lane_out_bytes(c)) : 0);
-#define LAUNCH(C)                                                                                         \
-  MZ_LAUNCH(ctx, k_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, lb, \
-            d_out, out_cap, d_out_len, ctx->d_status)
-  MZ_LANE_CLASSES(c, LAUNCH)
-#undef LAUNCH
-  return MZGPU_OK;
+  return mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
+    MZ_LAUNCH(ctx, k_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, lb, d_out,
+              out_cap, d_out_len, ctx->d_status);
+    return MZGPU_OK;
+  });
 }

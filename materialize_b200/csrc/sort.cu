@@ -24,11 +24,9 @@
 
 namespace {
 
-// tile shape variants of the pass kernel (MZGPU_RS_VARIANT selects; default 0)
-struct RsVariant {
-  int items, threads;
-};
-static const RsVariant RS_VARIANTS[] = {{16, 256}, {16, 512}, {24, 256}, {12, 512}, {20, 384}, {16, 256}, {24, 256}, {14, 256}, {10, 256}};
+// tile shape of the pass kernel: RS_ITEMS keys per thread, RS_THREADS threads, RS_MINB CTAs per SM
+constexpr int RS_ITEMS = 16;
+constexpr int RS_MINB = 3;
 
 struct ChunkPlan {
   int nwords;
@@ -129,7 +127,7 @@ __global__ void __launch_bounds__(256) k_rs_scan_hist(u32* __restrict__ ghist, i
 }
 
 // ------------------------------------------------------------ onesweep pass
-template <int ITEMS, int THREADS, bool BALLOT, int MINB>
+template <int ITEMS, int THREADS, int MINB>
 __global__ void __launch_bounds__(THREADS, MINB) k_rs_onesweep(
     const u64* __restrict__ kin, const u32* __restrict__ vin, u64* __restrict__ kout,
     u32* __restrict__ vout, u64 n, int shift, const u32* __restrict__ gbase,
@@ -141,26 +139,23 @@ __global__ void __launch_bounds__(THREADS, MINB) k_rs_onesweep(
   // which is what makes the look-back deadlock-free
   if (threadIdx.x == 0) s.tile = atomicAdd(tile_counter, 1u);
   __syncthreads();
-  // (MZGPU_RS_TMA=0 at build time of the variant table would select plain loads; the bulk path is
-  // the default: see rs_tile_pass)
-  rs_tile_pass<ITEMS, THREADS, BALLOT, true>(s, s.tile, kin, vin, kout, vout, n, shift, gbase, tile_state);
+  rs_tile_pass<ITEMS, THREADS, true>(s, s.tile, kin, vin, kout, vout, n, shift, gbase, tile_state);
 }
 
-template <int ITEMS, int THREADS, bool BALLOT = true, int MINB = (THREADS >= 512 ? 1 : (ITEMS > 16 ? 2 : 3))>
 static int32_t launch_onesweep(mzgpu_ctx* ctx, const u64* kin, const u32* vin, u64* kout, u32* vout, u64 n,
                                int shift, const u32* gbase, u32* state, u32* counter) {
-  typedef RsSmemT<ITEMS, THREADS> Smem;
+  typedef RsSmemT<RS_ITEMS, RS_THREADS> Smem;
   static bool attr_set = false;
   if (!attr_set) {
-    MZ_CUDA(ctx, cudaFuncSetAttribute(k_rs_onesweep<ITEMS, THREADS, BALLOT, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)sizeof(Smem)));
+    MZ_CUDA(ctx, cudaFuncSetAttribute(k_rs_onesweep<RS_ITEMS, RS_THREADS, RS_MINB>,
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem)));
     attr_set = true;
   }
-  const u64 n_tiles = (n + (u64)ITEMS * THREADS - 1) / ((u64)ITEMS * THREADS);
+  const u64 n_tiles = (n + (u64)RS_ITEMS * RS_THREADS - 1) / ((u64)RS_ITEMS * RS_THREADS);
   MZ_BYTES(ctx, n * 24);  // read key+idx (12 B), write key+idx (12 B)
   {
     ProfScope _prof(ctx, "k_rs_onesweep");
-    k_rs_onesweep<ITEMS, THREADS, BALLOT, MINB><<<(unsigned)n_tiles, THREADS, sizeof(Smem), ctx->stream>>>(
+    k_rs_onesweep<RS_ITEMS, RS_THREADS, RS_MINB><<<(unsigned)n_tiles, RS_THREADS, sizeof(Smem), ctx->stream>>>(
         kin, vin, kout, vout, n, shift, gbase, state, counter);
   }
   ctx->stats.kernel_launches++;
@@ -185,13 +180,7 @@ int32_t radix_sort_pairs(mzgpu_ctx* ctx, u64* ka, u32* va, u64* kb, u32* vb, u64
   *k_res = ka;
   *v_res = va;
   if (npass == 0 || n <= 1) return MZGPU_OK;
-  static int variant = -1;
-  if (variant < 0) {
-    const char* e = getenv("MZGPU_RS_VARIANT");
-    variant = e ? atoi(e) : 0;
-    if (variant < 0 || variant >= (int)(sizeof(RS_VARIANTS) / sizeof(RS_VARIANTS[0]))) variant = 0;
-  }
-  const u64 tile = (u64)RS_VARIANTS[variant].items * RS_VARIANTS[variant].threads;
+  const u64 tile = (u64)RS_ITEMS * RS_THREADS;
   const u64 n_tiles = (n + tile - 1) / tile;
   DevMem hist, state, counters;
   MZ_TRY(hist.alloc(ctx, (size_t)npass * 256 * 4));
@@ -214,17 +203,7 @@ int32_t radix_sort_pairs(mzgpu_ctx* ctx, u64* ka, u32* va, u64* kb, u32* vb, u64
     const u32* gb = hist.as<u32>() + p * 256;
     u32* stp = state.as<u32>() + (size_t)p * n_tiles * 256;
     u32* cnt = counters.as<u32>() + p;
-    switch (variant) {
-      case 1: MZ_TRY((launch_onesweep<16, 512>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;
-      case 2: MZ_TRY((launch_onesweep<24, 256>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;
-      case 3: MZ_TRY((launch_onesweep<12, 512>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;
-      case 4: MZ_TRY((launch_onesweep<20, 384>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;
-      case 5: MZ_TRY((launch_onesweep<16, 256, false>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;  // MATCH.ANY
-      case 6: MZ_TRY((launch_onesweep<24, 256, false>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;
-      case 7: MZ_TRY((launch_onesweep<14, 256, true, 4>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;
-      case 8: MZ_TRY((launch_onesweep<10, 256, true, 5>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;
-      default: MZ_TRY((launch_onesweep<16, 256>(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt))); break;
-    }
+    MZ_TRY(launch_onesweep(ctx, kin, vin, kout, vout, n, 8 * p, gb, stp, cnt));
     std::swap(kin, kout);
     std::swap(vin, vout);
   }
@@ -327,18 +306,6 @@ int32_t sort_perm_t(mzgpu_ctx* ctx, const u64* d_rows, u64 n, DevMem* perm_out) 
 }  // namespace
 
 int32_t mz_sort_perm(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, u64 n, DevMem* perm_out) {
-  const u64* r = (const u64*)d_rows;
-  switch (row_bytes) {
-    case 16: return sort_perm_t<16>(ctx, r, n, perm_out);
-    case 32: return sort_perm_t<32>(ctx, r, n, perm_out);
-    case 40: return sort_perm_t<40>(ctx, r, n, perm_out);
-    case 80: return sort_perm_t<80>(ctx, r, n, perm_out);
-    case 64: return sort_perm_t<64>(ctx, r, n, perm_out);
-    case 128: return sort_perm_t<128>(ctx, r, n, perm_out);
-    case 224: return sort_perm_t<224>(ctx, r, n, perm_out);
-    case 416: return sort_perm_t<416>(ctx, r, n, perm_out);
-    default:
-      MZ_SET_ERR(ctx, "sort: unsupported row width %d", row_bytes);
-      return MZGPU_E_UNSUPPORTED;
-  }
+  return mz_dispatch<RowWidths>(ctx, row_bytes, "sort",
+                                [&](auto RB) { return sort_perm_t<RB>(ctx, (const u64*)d_rows, n, perm_out); });
 }

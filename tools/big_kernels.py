@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Bulk-regime kernel timings (BASELINE configs 1 and 2 sizes) for tuning: live CUDA-event
-time and algorithmic GB/s per kernel.  Env MZGPU_RS_VARIANT selects the radix tile shape."""
+time and algorithmic GB/s per kernel."""
 import json
 import os
 import sys
@@ -13,7 +13,7 @@ from materialize_b200 import harness  # noqa: E402
 ctx = mz.Context(0)
 peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
 which = sys.argv[1] if len(sys.argv) > 1 else "both"
-out = {"variant": os.environ.get("MZGPU_RS_VARIANT", "0")}
+out = {}
 
 
 def table():

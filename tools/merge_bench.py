@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Batch merges at update-batch-to-spine sizes: device time of mzgpu_batch_merge for two sorted,
 consolidated R32 batches of n/2 rows each (the merges a spine schedules while the Q3 workload steps).
-Run on a GPU box; MZGPU_MERGE_SORT_MAX=<rows> moves the point where a merge stops being run as a sort."""
+Run on a GPU box."""
 import os
 import sys
 
@@ -13,7 +13,6 @@ import materialize_b200 as mz  # noqa: E402
 
 ctx = mz.Context(0)
 rng = np.random.default_rng(1)
-print("MZGPU_MERGE_SORT_MAX =", os.environ.get("MZGPU_MERGE_SORT_MAX", "(default)"))
 for n in (40_000, 160_000, 320_000, 640_000, 1_000_000, 1_280_000, 2_560_000):
     halves = []
     for h in range(2):
