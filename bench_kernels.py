@@ -159,6 +159,13 @@ def main():
         cols = [mz.accum_lane(mz.AGG_COUNT_SUM_I64, 1), mz.accum_lane(mz.AGG_COUNT_SUM_F64, 2)]
         return (cols * 4)[:k]
 
+    # COUNT(DISTINCT) / SUM(DISTINCT) next to the plain columns: the two plain lanes of lanes_of(2), a
+    # distinct lane over val1 (nearly every value new) and one over its low 12 bits, sign-extended (values
+    # repeat within a key)
+    def distinct_lanes():
+        d = mz.AGG_COUNT_SUM_I64 | mz.ACCUM_DISTINCT
+        return lanes_of(2) + [mz.accum_lane(d, 1), mz.accum_lane(d, 1, 0, 12, True)]
+
     def r40_cfg4(c, seed, n, first=0, t=0, diff=1):
         a = harness.gen_cfg4(c, seed, n, cdf, first=first, t=t, diff=diff).download()
         f = harness.gen_cfg4(c, seed, n, cdf, as_f64=True, first=first, t=t, diff=diff).download()
@@ -173,10 +180,12 @@ def main():
         run(c, build(c))  # warm-up
         state = build(c)
         c.sync()
+        syncs0 = c.stats()["host_syncs"]
         t0 = time.perf_counter()
         run(c, state)
         c.sync()
         secs = time.perf_counter() - t0
+        syncs = c.stats()["host_syncs"] - syncs0  # host waits of the timed run, its closing sync included
         state = build(c)
         c.profile(True)
         c.profile_report()
@@ -185,7 +194,7 @@ def main():
         c.profile(False)
         res["cases"].append(
             {"case": name, "rows": n_rows, "seconds": secs, "rows_per_sec": n_rows / secs, "kernels": table[:10],
-             "device_bytes_peak": c.stats()["device_bytes_peak"]}
+             "device_bytes_peak": c.stats()["device_bytes_peak"], "host_syncs": syncs}
         )
         del state
         c.close()  # its cached blocks go back before the next variant measures its peak
@@ -204,6 +213,15 @@ def main():
             lambda c, d, k=k: mz.ReduceLanes(c, lanes_of(k), 40).step_dev(d, 1),
         )
         del host
+    name = f"cfg4 bulk reduce lanes=4 (2 plain + 2 distinct) n={n4 // 4} zipf0.9 keys={nk} R40"
+    host = r40_cfg4(ctx, 3, n4 // 4) if not args.only or args.only in name else None
+    lanes_case(
+        name,
+        n4 // 4,
+        lambda c, host=host: mz.DeviceRows(c, 40).upload(host),
+        lambda c, d: mz.ReduceLanes(c, distinct_lanes(), 40).step_dev(d, 1),
+    )
+    del host
 
     # incremental regime: 1M-row batches, half of each batch retracting rows of the batch before; one
     # 4-lane operator against four one-lane operators on the same batches
@@ -235,6 +253,12 @@ def main():
         nb * per,
         inc_batches,
         lambda c, bufs: run_inc(c, bufs, [lanes_of(4)]),
+    )
+    lanes_case(
+        f"cfg4 incremental lanes=4 (2 plain + 2 distinct), one operator, {nb}x{per} R40",
+        nb * per,
+        inc_batches,
+        lambda c, bufs: run_inc(c, bufs, [distinct_lanes()]),
     )
     lanes_case(
         f"cfg4 incremental lanes=4, four one-lane operators, {nb}x{per} R40",

@@ -568,10 +568,28 @@ mzgpu_spine* mzgpu_reduce_input_trace(mzgpu_reduce* r);
  * (a 64-bit field is the i64 itself); an F64 lane must pick a whole word (shift 0, bits 64). */
 #define MZGPU_MAX_ACCUM_LANES 8
 typedef struct mzgpu_accum_lane {
-  int32_t kind;         /* MZGPU_AGG_COUNT_SUM_I64 or MZGPU_AGG_COUNT_SUM_F64 */
+  int32_t kind;         /* MZGPU_AGG_COUNT_SUM_I64 or MZGPU_AGG_COUNT_SUM_F64, optionally | MZGPU_ACCUM_DISTINCT */
   uint32_t sign_extend; /* I64 lanes: sign-extend the bit-field                */
   mzgpu_field field;
 } mzgpu_accum_lane;
+/* OR'd into mzgpu_accum_lane.kind: the lane is COUNT(DISTINCT col) / SUM(DISTINCT col)
+ * (AccumulablePlan::distinct_aggrs, src/compute-types/src/plan/reduce.rs:146-158; rendered by
+ * build_accumulable, src/compute/src/render/reduce.rs:1338-1373).  Values are distinct by the lane's
+ * i64 datum (after bit-field extraction and sign extension).  The operator keeps one more
+ * arrangement per distinct lane, of R32 rows (group key, value, time, diff) keyed by the group key
+ * (mzgpu_reduce_lanes_distinct_trace), and a (key, value) pair is present while its accumulated
+ * multiplicity is non-zero -- a negative multiplicity counts as present, as in the reference, which
+ * checks for errors only at the final arrangement.  Each change of presence adds one row to the
+ * main arrangement: total = +-1 and only this lane's Accum, that of the value.  So a key's total
+ * word is (number of plain lanes > 0 ? sum of the key's input diffs : 0) + the number of present
+ * pairs over all distinct lanes, and that total decides the key's NULL-SUM and error flags as for
+ * any lane.  Lane widths and classes do not change: a distinct lane is one lane of the class.
+ *
+ * MZGPU_AGG_COUNT_SUM_F64 | MZGPU_ACCUM_DISTINCT is MZGPU_E_UNSUPPORTED: whether the reference's
+ * Row arrangement treats -0.0 / +0.0, and NaNs with different payloads, as one value depends on
+ * the Row ordering versus Datum equality (src/repr/src/row.rs:1878-1881 and the tests near
+ * :3768-3800), and nothing pins that here.  Any other bit in `kind` is MZGPU_E_INVALID. */
+#define MZGPU_ACCUM_DISTINCT 0x100
 /* Row widths.  The lane count rounds up to a class C in {1, 2, 4, 8}; the class's unused
  * lanes are zero.  Arrangement row: key, time, total, C x (non_nulls, acc_lo, acc_hi,
  * pos_infs, neg_infs, nans), padded to 16 bytes.  Output row: key, C x (count, sum_lo,
@@ -611,6 +629,10 @@ int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgp
 int32_t mzgpu_reduce_lanes(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
                            mzgpu_buf* out);
 int32_t mzgpu_reduce_lanes_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out);
+/* The pair arrangement of distinct lane `lane` (R32 rows: group key, value, time, diff; the
+ * reference's "Arranged Accumulable Distinct"), borrowed like mzgpu_reduce_input_trace; NULL for a
+ * lane without MZGPU_ACCUM_DISTINCT, a lane index out of range, or another operator. */
+mzgpu_spine* mzgpu_reduce_lanes_distinct_trace(mzgpu_reduce* r, uint32_t lane);
 
 /* ------------------------------ f1 (first step): Row keys as fixed-width words */
 /* A `Row` orders by byte length first, then by its bytes (RowRef::cmp,

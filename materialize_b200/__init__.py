@@ -9,6 +9,7 @@ no CPU fallback.
 """
 from . import _ffi  # noqa: F401  (loads the CUDA library; raises if absent)
 from .api import (  # noqa: F401
+    ACCUM_DISTINCT,
     AGG_COUNT_SUM_F64,
     AGG_DISTINCT,
     AGG_THRESHOLD,

@@ -99,6 +99,7 @@ OK, E_INVALID, E_CUDA, E_CAPACITY, E_UNSUPPORTED, E_NCCL, E_FRONTIER = 0, -1, -2
 HALFJOIN_LE, HALFJOIN_LT = 0, 1
 AGG_COUNT_SUM_I64, AGG_COUNT_SUM_F64, AGG_DISTINCT, AGG_THRESHOLD, AGG_MIN, AGG_MAX, AGG_TOPK = 0, 1, 2, 3, 4, 5, 6
 MAX_ACCUM_LANES = 8
+ACCUM_DISTINCT = 0x100  # OR'd into a lane's kind: COUNT(DISTINCT col) / SUM(DISTINCT col)
 COMM_ID_BYTES = 128
 P2P_HANDLE_BYTES = 64
 
@@ -243,6 +244,7 @@ SIGNATURES = {
     "mzgpu_reduce_lanes_new": (i32, [vp, u32, vp, u32, PV]),
     "mzgpu_reduce_lanes": (i32, [vp, vp, u64, i32, u64, vp]),
     "mzgpu_reduce_lanes_buf": (i32, [vp, vp, u64, vp]),
+    "mzgpu_reduce_lanes_distinct_trace": (vp, [vp, u32]),
     "mzgpu_comm_unique_id": (i32, [C.POINTER(C.c_uint8)]),
     "mzgpu_comm_init": (i32, [vp, C.POINTER(C.c_uint8)]),
     "mzgpu_exchange": (i32, [vp, vp, vp]),

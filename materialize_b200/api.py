@@ -20,6 +20,7 @@ import numpy as np
 
 from . import _ffi as F
 from ._ffi import (  # noqa: F401  (re-exported)
+    ACCUM_DISTINCT,
     AGG_COUNT_SUM_F64,
     AGG_DISTINCT,
     AGG_THRESHOLD,
@@ -590,7 +591,8 @@ class ReduceAccumulable:
 
 def accum_lane(kind, src=SRC_VAL1, shift=0, bits=64, sign_extend=False):
     """One lane of ReduceLanes: COUNT and SUM of the bit-field `bits` wide at `shift` of value word
-    `src` (1 = val / val1, 2 = val2); an I64 field is sign-extended when `sign_extend`."""
+    `src` (1 = val / val1, 2 = val2); an I64 field is sign-extended when `sign_extend`.  A kind of
+    AGG_COUNT_SUM_I64 | ACCUM_DISTINCT makes the lane COUNT(DISTINCT col) / SUM(DISTINCT col)."""
     return (int(kind), int(src), int(shift), int(bits), bool(sign_extend))
 
 
@@ -628,6 +630,11 @@ class ReduceLanes:
 
     def input_trace(self):
         return Spine(self.ctx, self.arr_row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+
+    def distinct_trace(self, lane):
+        """The (key, value) pair arrangement (R32 rows) of distinct lane `lane`; None for any other lane."""
+        h = F.lib.mzgpu_reduce_lanes_distinct_trace(self.h, lane)
+        return Spine(self.ctx, 32, _borrowed=h) if h else None
 
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:

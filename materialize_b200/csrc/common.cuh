@@ -1033,9 +1033,28 @@ struct LaneSet {
   u32 n;         // lanes in use; the class's other lanes stay zero
   u32 in_words;  // 4 (R32) or 5 (R40)
   u32 f64_mask;  // bit l: lane l is MZGPU_AGG_COUNT_SUM_F64
+  u32 distinct_mask;  // bit l: lane l carries MZGPU_ACCUM_DISTINCT (its words stay zero in the explode)
 };
 int32_t mz_explode_lanes(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
                          u64* d_arr);
+// the distinct lanes' pair rows: for the j-th set bit l of ls.distinct_mask, d_pairs[j] receives the R32
+// rows (key, lane l's value, time, diff) of the input, and *d_lens[j] the row count unless d_lens[j] is
+// nullptr (one launch)
+int32_t mz_distinct_pairs(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
+                          u64* const* d_pairs, u64* const* d_lens);
+// Presence changes of the distinct lanes' new pair batches (one launch per MZ_LB_TILES tiles): one class-c
+// arrangement row per change of a (key, value) pair between zero and non-zero accumulated multiplicity,
+// appended at d_out (capacity out_cap rows, at least the pair batches' total length); the row count is
+// left in len->v[*len_word] on the device.
+struct DistinctJobHost {
+  const u64* rows;  // the new pair batch (R32, sorted and consolidated)
+  DLen n;
+  u64 n_ub;
+  u32 lane;               // lane index in the class row
+  const TraceView* prior;  // the pair arrangement's earlier batches
+};
+int32_t mz_distinct_presence(mzgpu_ctx* ctx, int c, int k, const DistinctJobHost* jobs, u64* d_out, u64 out_cap,
+                             Lazy4* len, int* len_word);
 struct TopKParams {
   i64 limit;  // < 0: none
   u64 offset;

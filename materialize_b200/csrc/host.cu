@@ -2496,11 +2496,21 @@ struct mzgpu_reduce {
   LaneSet lanes = {};
   mzgpu_batcher* batcher = nullptr;
   mzgpu_spine* input = nullptr;
+  // distinct lanes (MZGPU_ACCUM_DISTINCT), in lane order: the lane index, and the batcher and R32 pair
+  // arrangement of its (key, value) pairs
+  int n_distinct = 0;
+  u32 distinct_lane[MZGPU_MAX_ACCUM_LANES] = {};
+  mzgpu_batcher* pair_batcher[MZGPU_MAX_ACCUM_LANES] = {};
+  mzgpu_spine* pairs[MZGPU_MAX_ACCUM_LANES] = {};
   int32_t failed = MZGPU_OK;  // set when an activation failed after its seal (reduce_dev)
   std::string failed_msg;
   ~mzgpu_reduce() {
     delete batcher;
     delete input;
+    for (int j = 0; j < n_distinct; ++j) {
+      delete pair_batcher[j];
+      delete pairs[j];
+    }
   }
 };
 
@@ -2535,6 +2545,62 @@ extern "C" int32_t mzgpu_topk_new(mzgpu_ctx* ctx, int64_t limit, uint64_t offset
 extern "C" void mzgpu_reduce_free(mzgpu_reduce* r) { delete r; }
 extern "C" mzgpu_spine* mzgpu_reduce_input_trace(mzgpu_reduce* r) { return r ? r->input : nullptr; }
 
+// The distinct lanes' part of an activation (build_accumulable's distinct_aggrs, reduce.rs:1338-1373): the
+// input's (key, value) pairs of every distinct lane (one launch), the pair batchers sealed at `upper` (shared
+// cooperative launches), and the presence changes of the new pair batches (one launch) pushed into the main
+// batcher as one more stash segment.  pair_new receives the sealed pair batches (the caller inserts them);
+// *sealed is set once the pair batchers' frontiers may have moved.
+static int32_t distinct_step(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper,
+                             mzgpu_batch** pair_new, bool* sealed) {
+  mzgpu_ctx* ctx = r->ctx;
+  const int d = r->n_distinct;
+  if (n_ub) {
+    Seg segs[MZGPU_MAX_ACCUM_LANES];
+    u64* outs[MZGPU_MAX_ACCUM_LANES] = {};
+    u64* lens[MZGPU_MAX_ACCUM_LANES] = {};
+    for (int j = 0; j < d; ++j) {
+      MZ_TRY(segs[j].rows.alloc(ctx, n_ub * 32));
+      outs[j] = segs[j].rows.as<u64>();
+      if (n.p == nullptr) {
+        segs[j].len.set(ctx, n.imm);
+      } else {
+        MZ_TRY(segs[j].len.make_pending(ctx));
+        lens[j] = segs[j].len.dptr();
+      }
+      segs[j].ub = n.p == nullptr ? n.imm : n_ub;
+    }
+    MZ_TRY(mz_distinct_pairs(ctx, d_rows, n, n_ub, r->lanes, outs, lens));
+    for (int j = 0; j < d; ++j) {
+      if (n.p != nullptr) segs[j].len.mark_written();
+      MZ_TRY(batcher_push_seg(r->pair_batcher[j], std::move(segs[j])));
+    }
+  }
+  *sealed = true;
+  MZ_TRY(batcher_seal_many(d, r->pair_batcher, upper, pair_new));
+  std::vector<TraceView> tvs((size_t)d);
+  std::vector<mzgpu_batch*> prior;
+  DistinctJobHost jobs[MZGPU_MAX_ACCUM_LANES];
+  u64 cap = 0;
+  for (int j = 0; j < d; ++j) {
+    prior.clear();
+    r->pairs[j]->all_batches(prior);
+    MZ_TRY(trace_view(ctx, prior, &tvs[(size_t)j]));
+    const mzgpu_batch* b = pair_new[j];
+    jobs[j] = DistinctJobHost{b->rows.as<u64>(), batch_dlen(b), b->len_ub, r->distinct_lane[j], &tvs[(size_t)j]};
+    cap += b->len_ub;
+  }
+  if (cap == 0) return MZGPU_OK;
+  // at most one presence change per new pair row
+  Seg s;
+  const int c = r->lane_class;
+  MZ_TRY(s.rows.alloc(ctx, cap * mz_lane_arr_bytes(c)));
+  MZ_TRY(mz_distinct_presence(ctx, c, d, jobs, s.rows.as<u64>(), cap, &s.len, &s.word));
+  s.ub = cap;
+  return batcher_push_seg(r->batcher, std::move(s));
+}
+
+static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                           bool minmax, u64 per_row);
 static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out) {
   mzgpu_ctx* ctx = r->ctx;
   if (r->failed != MZGPU_OK) {  // an earlier activation lost its corrections: the operator is dead, not the worker
@@ -2544,6 +2610,8 @@ static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, 
   // batches sealed by earlier activations are merge-eligible now; their lengths
   // have reached the host with whatever the caller read since (no extra wait)
   MZ_TRY(mzgpu_spine_set_physical_compaction(r->input, r->input->upper));
+  for (int j = 0; j < r->n_distinct; ++j)
+    MZ_TRY(mzgpu_spine_set_physical_compaction(r->pairs[j], r->pairs[j]->upper));
   // explode_one: values move into the diff; the exploded rows become a stash segment
   // MIN / MAX / TopK keep the (key, value) rows themselves
   const bool minmax =
@@ -2554,7 +2622,40 @@ static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, 
     const u64 w = r->topk.limit >= 0 && r->topk.limit < 32 ? (u64)r->topk.limit : 32;
     per_row = 2 * w + 2;
   }
-  if (n_ub) {
+  // Distinct lanes first.  Their pair batches join the pair arrangements at the end whatever happens in
+  // between, and a failure once a pair batcher may have been sealed kills the operator, as one after the
+  // main seal does.
+  mzgpu_batch* pair_new[MZGPU_MAX_ACCUM_LANES] = {};
+  bool pairs_sealed = false;
+  auto finish_pairs = [&](int32_t st) -> int32_t {
+    for (int j = 0; j < r->n_distinct; ++j) {
+      if (pair_new[j] == nullptr) continue;
+      int32_t ins = MZGPU_OK;
+      if (pair_new[j]->desc.lower != pair_new[j]->desc.upper) ins = mzgpu_spine_insert(r->pairs[j], pair_new[j]);
+      mzgpu_batch_release(pair_new[j]);
+      pair_new[j] = nullptr;
+      if (st == MZGPU_OK) st = ins;
+    }
+    if (st != MZGPU_OK && pairs_sealed && !ctx->sticky && r->failed == MZGPU_OK) {
+      r->failed = st;
+      r->failed_msg = ctx->last_error;
+    }
+    return st;
+  };
+  if (r->n_distinct) {
+    const int32_t ds = distinct_step(r, d_rows, n, n_ub, upper, pair_new, &pairs_sealed);
+    if (ds != MZGPU_OK) return finish_pairs(ds);
+  }
+  return finish_pairs(reduce_main(r, d_rows, n, n_ub, upper, out, minmax, per_row));
+}
+
+// explode -> arrange -> reduce_abelian of one activation (after the distinct lanes' part)
+static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                           bool minmax, u64 per_row) {
+  mzgpu_ctx* ctx = r->ctx;
+  // a lanes operator whose lanes are all distinct has no plain explode
+  const bool plain = r->lane_class == 0 || r->lanes.distinct_mask != (1u << r->lanes.n) - 1;
+  if (n_ub && plain) {
     Seg s;
     if (minmax) {
       MZ_TRY(s.rows.alloc(ctx, n_ub * 32));
@@ -2704,10 +2805,12 @@ extern "C" int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes,
   for (uint32_t l = 0; l < n_lanes; ++l) {
     const mzgpu_accum_lane& L = lanes[l];
     const mzgpu_field& f = L.field;
-    const bool f64 = L.kind == MZGPU_AGG_COUNT_SUM_F64;
+    const int32_t base = L.kind & ~MZGPU_ACCUM_DISTINCT;
+    const bool distinct = (L.kind & MZGPU_ACCUM_DISTINCT) != 0;
+    const bool f64 = base == MZGPU_AGG_COUNT_SUM_F64;
     const char* bad = nullptr;
-    if (L.kind != MZGPU_AGG_COUNT_SUM_I64 && !f64)
-      bad = "kind is not COUNT_SUM_I64 / COUNT_SUM_F64";
+    if (base != MZGPU_AGG_COUNT_SUM_I64 && !f64)
+      bad = "kind is not COUNT_SUM_I64 / COUNT_SUM_F64, optionally | MZGPU_ACCUM_DISTINCT";
     else if (f.src != MZGPU_SRC_VAL1 && !(f.src == MZGPU_SRC_VAL2 && in_row_bytes == 40))
       bad = "source word is not a value word of the input row";
     else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
@@ -2718,8 +2821,14 @@ extern "C" int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes,
       MZ_SET_ERR(ctx, "reduce_lanes: lane %u: %s", l, bad);
       return MZGPU_E_INVALID;
     }
+    if (distinct && f64) {
+      MZ_SET_ERR(ctx, "reduce_lanes: lane %u: DISTINCT over float64 is not supported (which floats the "
+                      "reference's Row arrangement treats as one value is not pinned)", l);
+      return MZGPU_E_UNSUPPORTED;
+    }
     ls.lane[l] = L;
     if (f64) ls.f64_mask |= 1u << l;
+    if (distinct) ls.distinct_mask |= 1u << l;
   }
   ls.n = n_lanes;
   ls.in_words = in_row_bytes / 8;
@@ -2727,13 +2836,28 @@ extern "C" int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes,
   r->ctx = ctx;
   r->lane_class = mz_lane_class(n_lanes);
   r->lanes = ls;
-  // class 1 runs the one-column kernels, which take the lane's kind as the aggregate kind
+  // class 1 runs the one-column kernels, which take the lane's kind (without the DISTINCT bit) as the
+  // aggregate kind
   r->agg_kind = (ls.f64_mask & 1u) ? MZGPU_AGG_COUNT_SUM_F64 : MZGPU_AGG_COUNT_SUM_I64;
   const uint32_t rb = (uint32_t)mz_lane_arr_bytes(r->lane_class);
   MZ_TRY(mzgpu_batcher_new(ctx, rb, &r->batcher));
   MZ_TRY(mzgpu_spine_new(ctx, rb, 1, &r->input));
+  for (uint32_t l = 0; l < n_lanes; ++l) {
+    if (((ls.distinct_mask >> l) & 1u) == 0) continue;
+    const int j = r->n_distinct++;
+    r->distinct_lane[j] = l;
+    MZ_TRY(mzgpu_batcher_new(ctx, 32, &r->pair_batcher[j]));
+    MZ_TRY(mzgpu_spine_new(ctx, 32, 1, &r->pairs[j]));
+  }
   *out = r.release();
   return MZGPU_OK;
+}
+
+extern "C" mzgpu_spine* mzgpu_reduce_lanes_distinct_trace(mzgpu_reduce* r, uint32_t lane) {
+  if (r == nullptr) return nullptr;
+  for (int j = 0; j < r->n_distinct; ++j)
+    if (r->distinct_lane[j] == lane) return r->pairs[j];
+  return nullptr;
 }
 
 static bool lanes_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out) {

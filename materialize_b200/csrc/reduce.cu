@@ -16,6 +16,8 @@
 // times in order, emitting (-old, +new) output rows whenever the finalized
 // aggregate changes.  All arithmetic is integer (i64 / i128 with carries), so
 // results do not depend on summation order and match the reference bit for bit.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace {
@@ -177,6 +179,13 @@ __global__ void __launch_bounds__(RT) k_explode(const u64* __restrict__ rows, co
   }
 }
 
+// a lane's value: the bit-field of its source word, sign-extended when asked
+__device__ __forceinline__ u64 lane_value(const mzgpu_accum_lane& L, u64 key, u64 v1, u64 v2) {
+  u64 v = field_get(L.field, key, v1, v2);
+  if (L.sign_extend && L.field.bits < 64 && ((v >> (L.field.bits - 1)) & 1)) v |= ~0ull << L.field.bits;
+  return v;
+}
+
 // explode_one of the lanes operator: R32 / R40 rows, lane l reads its bit-field of val1 / val2
 template <int C>
 __global__ void __launch_bounds__(RT) k_explode_lanes(const u64* __restrict__ rows, const DLen dn,
@@ -194,11 +203,9 @@ __global__ void __launch_bounds__(RT) k_explode_lanes(const u64* __restrict__ ro
     o[2] = (u64)diff;  // total
 #pragma unroll
     for (int l = 0; l < C; ++l) {
-      if ((u32)l < ls.n) {
+      if ((u32)l < ls.n && ((ls.distinct_mask >> l) & 1u) == 0) {  // distinct lanes: mz_distinct_presence
         const mzgpu_accum_lane& L = ls.lane[l];
-        u64 v = field_get(L.field, key, v1, v2);
-        if (L.sign_extend && L.field.bits < 64 && ((v >> (L.field.bits - 1)) & 1)) v |= ~0ull << L.field.bits;
-        explode_lane(v, L.kind == MZGPU_AGG_COUNT_SUM_F64, diff, &o[3 + 6 * l]);
+        explode_lane(lane_value(L, key, v1, v2), L.kind == MZGPU_AGG_COUNT_SUM_F64, diff, &o[3 + 6 * l]);
       } else {
 #pragma unroll
         for (int w = 0; w < 6; ++w) o[3 + 6 * l + w] = 0;
@@ -993,7 +1000,247 @@ __global__ void __launch_bounds__(RT) k_minmax_lb(const u64* __restrict__ rows, 
   }
 }
 
+// ------------------------------------------------------------ distinct lanes
+// COUNT(DISTINCT x) / SUM(DISTINCT x) (build_accumulable's distinct_aggrs, reduce.rs:1338-1373): the input is
+// mapped to ((key, value), ()) and arranged per lane ("Arranged Accumulable Distinct"); reduce_abelian emits
+// ((key, value), +1) while the pair's accumulated multiplicity is non-zero, and explode_one turns each such
+// output update into a diff vector with total = its diff and only this lane's Accum (that of the value).
+// Here the pair arrangement is an R32 spine keyed by the group key, and k_distinct_presence emits those
+// exploded rows for one new pair batch directly: one thread per (key, value) run of the batch.
+
+struct PairMap {
+  u64* out[MZGPU_MAX_ACCUM_LANES];  // R32 rows per distinct lane
+  u64* len[MZGPU_MAX_ACCUM_LANES];  // where to write their row count, the input's (nullptr: known on the host)
+  u32 lane[MZGPU_MAX_ACCUM_LANES];
+  u32 k;
+};
+__global__ void __launch_bounds__(RT) k_distinct_pairs(const u64* __restrict__ rows, const DLen dn,
+                                                       const __grid_constant__ LaneSet ls,
+                                                       const __grid_constant__ PairMap pm) {
+  const u64 n = dlen_get(dn);
+  const u32 iw = ls.in_words;
+  if (blockIdx.x == 0 && threadIdx.x < pm.k && pm.len[threadIdx.x] != nullptr) *pm.len[threadIdx.x] = n;
+  for (u64 i = (u64)blockIdx.x * RT + threadIdx.x; i < n; i += (u64)gridDim.x * RT) {
+    const u64* r = rows + i * iw;
+    const u64 key = r[0], v1 = r[1], v2 = iw == 5 ? r[2] : 0;
+    u64 o[4] = {key, 0, r[iw - 2], r[iw - 1]};
+    for (u32 j = 0; j < pm.k; ++j) {
+      o[1] = lane_value(ls.lane[pm.lane[j]], key, v1, v2);
+      store_row<4>(pm.out[j], i, o);
+    }
+  }
+}
+
+// accumulated multiplicity of (key, val) over the prior batches of a pair arrangement: the key's rows come
+// from the hash index (as mm_runs finds them), the value's rows inside them by binary search (R32 rows are
+// sorted by (key, val, time))
+__device__ __forceinline__ i64 pair_prior(const TraceView& tv, u64 key, u64 val) {
+  i64 m = 0;
+  const u64 h0 = mix64(key);
+  for (u32 b = 0; b < tv.n_batches; ++b) {
+    const BatchView& bv = tv.b[b];
+    const u64 mask = bv_mask(bv);
+    u64 h = h0 & mask;
+    while (true) {
+      const ulonglong2 sl = *reinterpret_cast<const ulonglong2*>(&bv.table[h]);
+      if (sl.y == 0) break;
+      if (sl.x == key) {
+        const u64 first = (sl.y & MZ_SLOT_ROW_MASK) - 1;
+        const u32 len = (u32)(sl.y >> 44);
+        const u64 end = len != 0 ? first + len : bv_n(bv);  // (run length not recorded: the rows after it)
+        u64 lo = first, hi = end;
+        while (lo < hi) {  // first row with (key, val) >= (key, val)
+          const u64 mid = (lo + hi) >> 1;
+          const u64* x = bv.rows + mid * 4;
+          if (x[0] < key || (x[0] == key && x[1] < val))
+            lo = mid + 1;
+          else
+            hi = mid;
+        }
+        for (u64 r = lo; r < end; ++r) {
+          const u64* x = bv.rows + r * 4;
+          if (x[0] != key || x[1] != val) break;
+          m += (i64)x[3];
+        }
+        break;
+      }
+      h = (h + 1) & mask;
+    }
+  }
+  return m;
+}
+
+// The run of (key, val) at rows [i, ...) of the new pair batch, in time order on top of the prior
+// multiplicity m: one class-C row (key, time, total = +-1, lane `lane` = the value's Accum times +-1) per
+// change between zero and non-zero.  Returns the count; writes at out[pos ...] if do_write.
+template <int C>
+__device__ __forceinline__ u32 presence_walk(const u64* __restrict__ rows, u64 n, u64 i, u32 lane, i64 m,
+                                             bool do_write, u64* __restrict__ out, u64 pos) {
+  constexpr int NW = LaneRows<C>::ARR_NW;
+  const u64 key = rows[i * 4], val = rows[i * 4 + 1];
+  u32 c = 0;
+  for (u64 j = i; j < n; ++j) {
+    const u64* row = rows + j * 4;
+    if (row[0] != key || row[1] != val) break;
+    const bool was = m != 0;
+    m += (i64)row[3];
+    if (was == (m != 0)) continue;
+    if (do_write) {
+      const i64 s = was ? -1 : 1;
+      u64 o[NW];
+      o[0] = key;
+      o[1] = row[2];
+      o[2] = (u64)s;
+#pragma unroll
+      for (int l = 0; l < C; ++l) {
+        if ((u32)l == lane) {
+          explode_lane(val, false, s, &o[3 + 6 * l]);
+        } else {
+#pragma unroll
+          for (int w = 0; w < 6; ++w) o[3 + 6 * l + w] = 0;
+        }
+      }
+#pragma unroll
+      for (int w = 3 + 6 * C; w < NW; ++w) o[w] = 0;
+      store_row<NW>(out, pos + c, o);
+    }
+    ++c;
+  }
+  return c;
+}
+
+// The new pair batches of every distinct lane of an activation in one launch.  As in k_probe_chains, the
+// tiles of the jobs are numbered one after the other (from the batch lengths on the device) and one
+// look-back runs over all of them, so the rows of job q follow those of job q - 1.  A launch covers the
+// tiles [tile0, tile0 + MZ_LB_TILES); the next launch continues at out_base = this launch's *out_len.
+constexpr int DISTINCT_MAX = MZGPU_MAX_ACCUM_LANES;
+struct DistinctJob {
+  const u64* rows;
+  DLen dn;
+  u32 lane;
+  TraceView prior;
+};
+struct DistinctMany {
+  u32 k;
+  DistinctJob job[DISTINCT_MAX];
+};
+static_assert(sizeof(DistinctMany) <= 32000, "kernel parameter space");
+
+template <int C>
+__global__ void __launch_bounds__(RT) k_distinct_presence(const __grid_constant__ DistinctMany m, u64 tile0,
+                                                          const LookBack lb, const DLen out_base,
+                                                          u64* __restrict__ out, u64 out_cap,
+                                                          u64* __restrict__ out_len, u64* __restrict__ status) {
+  __shared__ u32 sm[34];
+  __shared__ u32 s_tile;
+  __shared__ u64 s_b;
+  u64 nj[DISTINCT_MAX], tiles_before[DISTINCT_MAX + 1];
+  tiles_before[0] = 0;
+#pragma unroll
+  for (int q = 0; q < DISTINCT_MAX; ++q) {
+    nj[q] = (u32)q < m.k ? dlen_get(m.job[q].dn) : 0;
+    tiles_before[q + 1] = tiles_before[q] + (nj[q] + RT - 1) / RT;
+  }
+  const u64 n_tiles = tiles_before[DISTINCT_MAX];
+  const u64 tile_end = n_tiles < tile0 + MZ_LB_TILES ? n_tiles : tile0 + MZ_LB_TILES;
+  const u64 base0 = dlen_get(out_base);
+  while (true) {
+    const u32 lt = lb_next_tile(lb, &s_tile);
+    const u64 tile = tile0 + lt;
+    if (tile >= tile_end) {
+      if (lt == 0 && threadIdx.x == 0) *out_len = base0;  // no tile in this launch's range
+      break;
+    }
+    u32 q = 0;
+    while (q + 1 < m.k && tile >= tiles_before[q + 1]) ++q;
+    const DistinctJob& J = m.job[q];
+    const u64* rows = J.rows;
+    const u64 n = nj[q];
+    const u64 i = (tile - tiles_before[q]) * RT + threadIdx.x;
+    const bool head =
+        i < n && (i == 0 || rows[(i - 1) * 4] != rows[i * 4] || rows[(i - 1) * 4 + 1] != rows[i * 4 + 1]);
+    u32 cnt = 0;
+    i64 m0 = 0;
+    if (head) {
+      m0 = pair_prior(J.prior, rows[i * 4], rows[i * 4 + 1]);
+      cnt = presence_walk<C>(rows, n, i, J.lane, m0, false, nullptr, 0);
+    }
+    u32 total;
+    const u32 ex = block_exclusive_scan(cnt, sm, &total);
+    const u64 excl = lb_exclusive_prefix(lb, lt, (u64)total, &s_b);
+    if (head && cnt > 0) {
+      const u64 pos = base0 + excl + ex;
+      if (pos + cnt > out_cap)
+        atomicMax((unsigned long long*)status, (unsigned long long)(pos + cnt));
+      else
+        presence_walk<C>(rows, n, i, J.lane, m0, true, out, pos);
+    }
+    if (tile == tile_end - 1 && threadIdx.x == 0) *out_len = base0 + excl + total;
+  }
+}
+
 }  // namespace
+
+int32_t mz_distinct_pairs(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
+                          u64* const* d_pairs, u64* const* d_lens) {
+  PairMap pm;
+  memset(&pm, 0, sizeof(pm));
+  for (u32 l = 0; l < ls.n; ++l) {
+    if (((ls.distinct_mask >> l) & 1u) == 0) continue;
+    pm.out[pm.k] = d_pairs[pm.k];
+    pm.len[pm.k] = d_lens[pm.k];
+    pm.lane[pm.k] = l;
+    pm.k++;
+  }
+  u64 grid = (n_ub + RT - 1) / RT;
+  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  if (grid == 0) grid = 1;  // (the lengths are written even for no rows)
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (ls.in_words * 8 + 32 * pm.k) : 0);
+  MZ_LAUNCH(ctx, k_distinct_pairs, (unsigned)grid, RT, 0, d_rows, n, ls, pm);
+  return MZGPU_OK;
+}
+
+int32_t mz_distinct_presence(mzgpu_ctx* ctx, int c, int k, const DistinctJobHost* jobs, u64* d_out, u64 out_cap,
+                             Lazy4* len, int* len_word) {
+  if (k <= 0 || k > DISTINCT_MAX) {
+    MZ_SET_ERR(ctx, "distinct presence: %d jobs (1..%d)", k, DISTINCT_MAX);
+    return MZGPU_E_INVALID;
+  }
+  static thread_local DistinctMany m;  // large: kept off the stack
+  memset(&m, 0, sizeof(m));
+  m.k = (u32)k;
+  u64 tiles = 0, bytes = 0;
+  for (int j = 0; j < k; ++j) {
+    m.job[j].rows = jobs[j].rows;
+    m.job[j].dn = jobs[j].n;
+    m.job[j].lane = jobs[j].lane;
+    m.job[j].prior = *jobs[j].prior;
+    tiles += (jobs[j].n_ub + RT - 1) / RT;
+    if (jobs[j].n.p == nullptr) bytes += jobs[j].n.imm * (32 + 16 * jobs[j].prior->n_batches + mz_lane_arr_bytes(c));
+  }
+  MZ_TRY(len->make_pending(ctx));
+  // one launch per MZ_LB_TILES tiles (the look-back state's size); each continues where the one before
+  // stopped, with the running length alternating between two words of `len`
+  const u64 launches = tiles > MZ_LB_TILES ? (tiles + MZ_LB_TILES - 1) / MZ_LB_TILES : 1;
+  for (u64 x = 0; x < launches; ++x) {
+    const u64 t0 = x * MZ_LB_TILES, lt = std::min<u64>(tiles - std::min(tiles, t0), MZ_LB_TILES);
+    LookBack lb;
+    MZ_TRY(mz_lookback_begin(ctx, lt, &lb));
+    u64 grid = std::min<u64>(lt, (u64)ctx->num_sms * 8);
+    if (grid == 0) grid = 1;
+    const DLen base = x == 0 ? dlen_imm(0) : DLen{len->dptr() + ((x - 1) & 1), 0};
+    u64* out_len = len->dptr() + (x & 1);
+    MZ_BYTES(ctx, x == 0 ? bytes : 0);
+    MZ_TRY(mz_dispatch<LaneClasses>(ctx, c, "distinct presence", [&](auto C) {
+      MZ_LAUNCH(ctx, k_distinct_presence<C>, (unsigned)grid, RT, 0, m, t0, lb, base, d_out, out_cap, out_len,
+                ctx->d_status);
+      return MZGPU_OK;
+    }));
+  }
+  len->mark_written();
+  *len_word = (int)((launches - 1) & 1);
+  return MZGPU_OK;
+}
 
 // MIN / MAX / TopK corrections of a sealed R32 batch against the prior R32 arrangement.
 // MIN / MAX: at most two output rows per distinct (key, time), capacity 2 * n_ub suffices;

@@ -60,8 +60,9 @@ impl GpuReduce {
 /// `build_accumulable` over several aggregates (`AccumulablePlan::simple_aggrs`, reduce.rs:146-158 of
 /// src/compute-types/src/plan): one arrangement of `(Vec<Accum>, Diff)`, one output row per key with
 /// every lane's COUNT and SUM (`sys::mzgpu_reduce_lanes_new` documents the row layouts).  The input is
-/// R32 (`in_row_bytes` 32) or a join's R40 result (40); `distinct_aggrs` are not a lane kind and come
-/// back as an error, so the caller keeps the Rust operator for such plans.
+/// R32 (`in_row_bytes` 32) or a join's R40 result (40).  An int64 lane whose kind carries
+/// `sys::ACCUM_DISTINCT` is one of the plan's `distinct_aggrs`; a float64 distinct lane comes back as
+/// `MZGPU_E_UNSUPPORTED`, so the caller keeps the Rust operator for such plans.
 pub struct GpuReduceLanes { h: *mut sys::Reduce, pub arr_row_bytes: u32, pub out_row_bytes: u32 }
 
 impl GpuReduceLanes {
@@ -79,6 +80,11 @@ impl GpuReduceLanes {
         unsafe { sys::check(worker_ctx(), sys::mzgpu_reduce_lanes_buf(self.h, rows, upper, out)) }
     }
     pub fn input_trace(&self) -> *mut sys::Spine { unsafe { sys::mzgpu_reduce_input_trace(self.h) } }
+    /// The (key, value) pair arrangement of distinct lane `lane` ("Arranged Accumulable Distinct"); null
+    /// for any other lane.
+    pub fn distinct_trace(&self, lane: u32) -> *mut sys::Spine {
+        unsafe { sys::mzgpu_reduce_lanes_distinct_trace(self.h, lane) }
+    }
 }
 impl Drop for GpuReduceLanes {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }

@@ -48,6 +48,8 @@ pub const AGG_MIN: i32 = 4;
 pub const AGG_MAX: i32 = 5;
 pub const AGG_TOPK: i32 = 6;
 pub const MAX_ACCUM_LANES: usize = 8;
+/// OR'd into `AccumLane::kind`: the lane is COUNT(DISTINCT col) / SUM(DISTINCT col) (int64 lanes only).
+pub const ACCUM_DISTINCT: i32 = 0x100;
 /// A column pick (mzgpu_field): bits [shift, shift + bits) of word `src`.
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)]
 pub struct Field { pub src: u8, pub shift: u8, pub bits: u8, pub dst_shift: u8 }
@@ -169,6 +171,7 @@ extern "C" {
     pub fn mzgpu_reduce_lanes_new(ctx: *mut Ctx, in_row_bytes: u32, lanes: *const AccumLane, n_lanes: u32, out: *mut *mut Reduce) -> i32;
     pub fn mzgpu_reduce_lanes(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf) -> i32;
     pub fn mzgpu_reduce_lanes_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf) -> i32;
+    pub fn mzgpu_reduce_lanes_distinct_trace(r: *mut Reduce, lane: u32) -> *mut Spine;
     pub fn mzgpu_rowkey_pack(row_bytes: *const u8, len: u64, key_out: *mut u64) -> i32;
     pub fn mzgpu_rowkeys_pack(data: *const u8, offsets: *const u64, n: u64, keys_out: *mut u64, n_done: *mut u64) -> i32;
     pub fn mzgpu_rowkey_unpack(key: u64, row_bytes_out: *mut u8, len_out: *mut u64) -> i32;
