@@ -397,6 +397,13 @@ int32_t mzgpu_batch_key_page(mzgpu_batch* b, uint64_t first_ordinal, uint64_t ma
  * step_val / map_times over one or several consecutive key runs -- into caller memory
  * (rows of the batch's row width). */
 int32_t mzgpu_batch_rows(mzgpu_batch* b, uint64_t first, uint64_t len, void* rows, int32_t mem);
+/* The batch's hash index, for tests and diagnostics (read-only): *n_slots table slots of 16
+ * bytes {key, meta} into `slots` (in `mem` space; MZGPU_E_CAPACITY with the three counts set if
+ * cap_slots < *n_slots), the distinct keys, and the longest key run (saturating at 1024).  A slot
+ * with meta == 0 is empty; otherwise meta bits [0, 44) hold the key's first row + 1 and bits
+ * [44, 64) its run length, or 0 where the builder left the run to the reader. */
+int32_t mzgpu_batch_index_export(mzgpu_batch* b, void* slots, uint64_t cap_slots, int32_t mem, uint64_t* n_slots,
+                                 uint64_t* n_keys, uint64_t* longest_run);
 
 /* ---- a5: Builder::{with_capacity, push, done} (src/timely-util/src/operator.rs:634-677;
  * OrdValBuilder): chunks of updates are pushed in order, `done` seals them into a batch

@@ -272,6 +272,7 @@ SIGNATURES = {
     "mzgpu_batch_seek_keys": (i32, [vp, vp, u64, i32, vp]),
     "mzgpu_batch_key_page": (i32, [vp, u64, u64, i32, vp, PU64]),
     "mzgpu_batch_rows": (i32, [vp, u64, u64, vp, i32]),
+    "mzgpu_batch_index_export": (i32, [vp, vp, u64, i32, PU64, PU64, PU64]),
     "mzgpu_builder_new": (i32, [vp, u32, u64, PV]),
     "mzgpu_builder_free": (None, [vp]),
     "mzgpu_builder_push": (i32, [vp, vp, u64, i32]),
@@ -295,6 +296,7 @@ SIGNATURES = {
 COLUMN_U64X4, COLUMN_U64X2, COLUMN_ROWROW = 0, 1, 2
 
 KEY_RUN = np.dtype([("key", "<u8"), ("first", "<u8"), ("len", "<u8")])
+HASH_SLOT = np.dtype([("key", "<u8"), ("meta", "<u8")])
 ARRANGEMENT_SIZE = np.dtype([("size_bytes", "<u8"), ("capacity_bytes", "<u8"), ("allocations", "<u8"), ("batches", "<u8"), ("updates", "<u8")])
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -270,6 +270,21 @@ class Batch:
         self.ctx.check(F.lib.mzgpu_batch_rows(self.h, first, length, _ptr(out), F.MEM_HOST))
         return out
 
+    def index(self):
+        """The hash index, for tests and diagnostics: (slots as HASH_SLOT records, distinct keys,
+        longest key run saturating at 1024)."""
+        n_slots, n_keys, longest = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        st = F.lib.mzgpu_batch_index_export(self.h, None, 0, F.MEM_HOST, C.byref(n_slots), C.byref(n_keys), C.byref(longest))
+        if st not in (F.OK, F.E_CAPACITY):
+            self.ctx.check(st)
+        slots = np.zeros(n_slots.value, dtype=F.HASH_SLOT)
+        self.ctx.check(
+            F.lib.mzgpu_batch_index_export(
+                self.h, _ptr(slots), len(slots), F.MEM_HOST, C.byref(n_slots), C.byref(n_keys), C.byref(longest)
+            )
+        )
+        return slots, n_keys.value, longest.value
+
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:
             F.lib.mzgpu_batch_release(self.h)

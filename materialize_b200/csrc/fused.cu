@@ -956,12 +956,14 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
     const u32 NU = (NB + 7) / 8;
     constexpr u32 LOCAL_MAX = ND == 8 ? 256u : MSD_LOCAL_MAX;
     if (a.dbg != nullptr && c == 0 && tid == 0) {
-      a.dbg[21] = s_max_bucket <= WCAP ? 1 : (s_max_unit <= LOCAL_MAX ? 2 : 3);
+      a.dbg[21] = s_max_bucket <= WCAP ? 1 : (ND <= 8 && s_max_unit <= LOCAL_MAX ? 2 : 3);
       a.dbg[22] = s_max_bucket;
       a.dbg[23] = NB;
     }
     if (s_max_bucket <= WCAP) {
-      // every bucket fits a warp
+      // every bucket fits a warp.  Unreachable while fused_prepare sets `fast`: this exact path then
+      // runs only after the fast path overflowed, i.e. some bucket of the same NB buckets held more
+      // than WCAP rows, and the recount above finds that bucket again.
       for (u64 i = gtid; i < n; i += gstride) {
         const u64 p = (u64)sm.scan.base[a.v1[i]] + a.v0[i];
         a.m_lo[p] = a.k0[i];

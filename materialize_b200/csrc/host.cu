@@ -987,6 +987,19 @@ extern "C" int32_t mzgpu_batch_rows(mzgpu_batch* b, uint64_t first, uint64_t len
   }
   return copy_out(b->ctx, rows, (const char*)b->rows.p + first * b->rb, len * b->rb, mem);
 }
+extern "C" int32_t mzgpu_batch_index_export(mzgpu_batch* b, void* slots, uint64_t cap_slots, int32_t mem,
+                                            uint64_t* n_slots, uint64_t* n_keys, uint64_t* longest_run) {
+  if (b == nullptr || (cap_slots && slots == nullptr)) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(b->ctx);
+  MZ_TRY(batch_ready(b));
+  MZ_TRY(batch_resolve(b));
+  const u64 ns = b->st.v[1] + 1;
+  if (n_slots) *n_slots = ns;
+  if (n_keys) *n_keys = b->st.v[2];
+  if (longest_run) *longest_run = b->st.v[3];
+  if (cap_slots < ns) return MZGPU_E_CAPACITY;
+  return copy_out(b->ctx, slots, b->table.p, ns * sizeof(HashSlot), mem);
+}
 
 // ---- a5: Builder::{push, done}
 struct mzgpu_builder {

@@ -473,8 +473,8 @@ struct CursorList {
 // ------------------------------------------------------ batch merger (a7)
 // Batch::Merger for OrdValBatch: merge keys -> vals -> (time,diff) lists with
 // time.advance_by(since) (= max for totally ordered u64 times,
-// src/repr/src/timestamp.rs:486-495), consolidate each (key,val) history, drop
-// empty vals and keys.  `b1.upper == b2.lower`.
+// src/repr/src/timestamp.rs:486-495; advance_by of the empty antichain leaves a time
+// alone), consolidate each (key,val) history, drop empty vals and keys.  `b1.upper == b2.lower`.
 template <class R>
 std::shared_ptr<Batch<R>> merge_batches(const Batch<R>& b1, const Batch<R>& b2, u64 since) {
   std::vector<R> out;
@@ -486,7 +486,7 @@ std::shared_ptr<Batch<R>> merge_batches(const Batch<R>& b1, const Batch<R>& b2, 
     hist.clear();
     auto push = [&](const R& r) {
       R x = r;
-      if (Tr<R>::time(x) < since) Tr<R>::set_time(x, since);
+      if (since != FRONTIER_EMPTY && Tr<R>::time(x) < since) Tr<R>::set_time(x, since);
       hist.push_back(x);
     };
     if (a) a->map_times(push);

@@ -86,6 +86,8 @@ extern "C" {
     pub fn mzgpu_batch_seek_keys(b: *mut Batch, keys: *const u64, n: u64, mem: i32, runs: *mut KeyRun) -> i32;
     pub fn mzgpu_batch_key_page(b: *mut Batch, first_ordinal: u64, max_keys: u64, mem: i32, runs: *mut KeyRun, n_out: *mut u64) -> i32;
     pub fn mzgpu_batch_rows(b: *mut Batch, first: u64, len: u64, rows: *mut c_void, mem: i32) -> i32;
+    pub fn mzgpu_batch_index_export(b: *mut Batch, slots: *mut c_void, cap_slots: u64, mem: i32, n_slots: *mut u64,
+                                    n_keys: *mut u64, longest_run: *mut u64) -> i32;
     // a6, a14: spine
     pub fn mzgpu_spine_new(ctx: *mut Ctx, row_bytes: u32, effort: u32, out: *mut *mut Spine) -> i32;
     pub fn mzgpu_spine_free(s: *mut Spine);
