@@ -266,6 +266,37 @@ def main():
         inc_batches,
         lambda c, bufs: run_inc(c, bufs, [[l] for l in lanes_of(4)]),
     )
+    # HAVING inside the operator: the same 4-lane incremental run without and with a two-predicate filter
+    # (COUNT(val1) >= 2 AND SUM(val1) > 0), alternating on one context; the best of three rounds each
+    name = f"cfg4 incremental lanes=4, without / with a two-predicate HAVING, {nb}x{per} R40"
+    if not args.only or args.only in name:
+        hv = mz.having([mz.h_count(0), mz.h_int(2), mz.h_cmp("ge")], [mz.h_sum(2), mz.h_num(0), mz.h_cmp("gt")])
+        c = mz.Context(0)
+
+        def run_having(bufs, having):
+            op = mz.ReduceLanes(c, lanes_of(4), 40, having=having)
+            out = mz.DeviceRows(c, op.out_row_bytes)
+            for b, d in enumerate(bufs):
+                op.step_dev(d, b + 1, out)
+            return len(out)
+
+        best, rows_out = {"without": None, "with": None}, {}
+        for rnd in range(4):  # round 0 warms up
+            for label, having in (("without", None), ("with", hv)):
+                bufs = inc_batches(c)
+                c.sync()
+                t0 = time.perf_counter()
+                rows_out[label] = run_having(bufs, having)
+                c.sync()
+                dt = time.perf_counter() - t0
+                if rnd > 0:
+                    best[label] = dt if best[label] is None else min(best[label], dt)
+        res["cases"].append(
+            {"case": name, "rows": nb * per, "seconds_without": best["without"], "seconds_with": best["with"],
+             "output_rows_without": rows_out["without"], "output_rows_with": rows_out["with"]}
+        )
+        c.close()
+        print(name, f"{best['without']:.4f} s / {best['with']:.4f} s", file=sys.stderr, flush=True)
     txt = json.dumps(res, indent=1)
     if args.out:
         open(args.out, "w").write(txt)

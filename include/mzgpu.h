@@ -641,6 +641,104 @@ int32_t mzgpu_reduce_lanes_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
  * lane without MZGPU_ACCUM_DISTINCT, a lane index out of range, or another operator. */
 mzgpu_spine* mzgpu_reduce_lanes_distinct_trace(mzgpu_reduce* r, uint32_t lane);
 
+/* ---- HAVING: the filter half of the reduce's fused mfp_after (render_reduce hands every reduce an
+ * mfp_after, src/compute/src/render/reduce.rs:64-78; build_accumulable applies it to (key, finalized
+ * aggregates) in its ReduceAccumulable closure, :1384-1409 and evaluate_mfp_after :1474-1499, and reports
+ * its errors in AccumulableErrorCheck, :1452-1464).
+ *
+ * A filter is up to MZGPU_HAVING_MAX_PREDICATES predicates, evaluated in order as
+ * SafeMfpPlan::evaluate_inner does (src/expr/src/linear.rs:1680-1700): the first predicate that is not
+ * TRUE (FALSE or NULL) drops the row and later predicates are not evaluated; an error stops evaluation
+ * with that error.  A predicate is a postfix program over typed values:
+ *   INT   i64: a bit-field of the output key (optionally sign-extended, integer_to_bigint(#0{a}); a
+ *         64-bit field is the i64 itself), a
+ *         lane's COUNT, or an integer constant.  "int32" when it is a key field of at most 32 bits
+ *         (sign-extended, or fewer than 32 bits), an integer constant in i32 range, or the result of
+ *         a 32-bit operation.
+ *   NUM   i128: the SUM of an int64 lane (numeric), or an i128 constant.
+ *   FLOAT f64: the SUM of a float64 lane, or a constant.
+ *   BOOL
+ * A SUM is NULL when its lane's NULL flag (bit 2l) is set; a COUNT is never NULL.
+ * Arithmetic is on INT only and carries its SQL width (arg = 32 or 64; a 32-bit operation takes int32
+ * operands): add/sub/mul give NumericFieldOverflow when the result leaves the width
+ * (src/expr/src/scalar/func.rs:107, 117, 690, 700, 904, 914); div truncates, a zero divisor gives
+ * DivisionByZero and MIN / -1 Int32OutOfRange / Int64OutOfRange (func.rs:1037-1059).  Both operands
+ * are evaluated; the first operand's error wins over the second's, and an error over a NULL, which
+ * propagates (the eager argument unpacking of src/repr/src/scalar.rs:2126-2160).
+ * Comparisons (arg = MZGPU_CMP_*, signed) take INT / INT, NUM / NUM, INT / NUM (the INT widened
+ * exactly) or FLOAT / FLOAT, which compare as OrderedFloat (Datum::Float64, src/repr/src/scalar.rs:99:
+ * NaN equals NaN and is above everything, -0.0 equals +0.0); a NULL operand gives NULL.
+ * AND / OR / NOT are three-valued with the error rules of the variadic And / Or
+ * (src/expr/src/scalar/func/variadic.rs:74-99, 1147-1170): for AND a FALSE operand wins over an
+ * error, otherwise the larger error wins, otherwise NULL wins over TRUE; OR mirrors it with TRUE.
+ *
+ * Errors (in the order of the EvalError variants, src/expr/src/scalar.rs:1724-1740, which And's
+ * std::cmp::max compares) are written into flag bits 16-18 of the output row
+ * (MZGPU_ROUT_HAVING_ERR_SHIFT): this project carries errors as row flags, not in a separate error
+ * collection.  A key has an output row at time t while its accumulated diff is non-zero (as without a
+ * filter) AND it carries a lane error flag (bit 2l+1), or its predicates raised an error, or every
+ * predicate is TRUE: error rows are never filtered away.  Corrections stay the (-old, +new) changes of
+ * that visible row.  The map and project parts of mfp_after stay with the caller: the row layout does
+ * not change, and a mapped column (SUM(b) + 1) is computed downstream; a map expression a predicate
+ * reads (COUNT(b) + 1) is written inline in the predicate. */
+#define MZGPU_HAVING_MAX_PREDICATES 4
+#define MZGPU_HAVING_MAX_OPS 16 /* per predicate */
+#define MZGPU_HAVING_MAX_CONSTS 8
+#define MZGPU_HAVING_MAX_STACK 8
+/* opcodes (mzgpu_having_op.code) */
+#define MZGPU_HOP_KEY 1   /* push INT: bits [shift, shift + bits) of the key, sign-extended if sign_extend */
+#define MZGPU_HOP_COUNT 2 /* push INT: COUNT of lane `arg` */
+#define MZGPU_HOP_SUM 3   /* push SUM of lane `arg`: NUM (int64 lane) or FLOAT (float64 lane), NULL by flag 2l */
+#define MZGPU_HOP_INT 4   /* push INT constant consts[konst] (in i64 range) */
+#define MZGPU_HOP_NUM 5   /* push NUM constant consts[konst] */
+#define MZGPU_HOP_FLOAT 6 /* push FLOAT constant: the f64 bits in consts[konst].lo */
+#define MZGPU_HOP_ADD 7   /* INT, INT -> INT at width arg (32 or 64) */
+#define MZGPU_HOP_SUB 8
+#define MZGPU_HOP_MUL 9
+#define MZGPU_HOP_DIV 10
+#define MZGPU_HOP_CMP 11 /* arg = MZGPU_CMP_*: -> BOOL */
+#define MZGPU_HOP_AND 12 /* BOOL, BOOL -> BOOL */
+#define MZGPU_HOP_OR 13
+#define MZGPU_HOP_NOT 14 /* BOOL -> BOOL */
+/* the predicate error in flag bits 16-18 of an output row */
+#define MZGPU_ROUT_HAVING_ERR_SHIFT 16
+#define MZGPU_HAVING_ERR_DIVISION_BY_ZERO 1
+#define MZGPU_HAVING_ERR_NUMERIC_FIELD_OVERFLOW 2
+#define MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE 3
+#define MZGPU_HAVING_ERR_INT64_OUT_OF_RANGE 4
+typedef struct mzgpu_having_op {
+  uint8_t code;        /* MZGPU_HOP_* */
+  uint8_t arg;         /* COUNT / SUM: lane; arithmetic: width 32 / 64; CMP: MZGPU_CMP_* */
+  uint8_t shift;       /* KEY: right shift of the key word */
+  uint8_t bits;        /* KEY: field width 1..64 */
+  uint8_t sign_extend; /* KEY: sign-extend the field */
+  uint8_t konst;       /* INT / NUM / FLOAT: constant index */
+  uint8_t _pad[2];
+} mzgpu_having_op;
+typedef struct mzgpu_having_const {
+  uint64_t lo, hi; /* INT / NUM: i128 two's complement; FLOAT: lo = the f64 bits, hi = 0 */
+} mzgpu_having_const;
+typedef struct mzgpu_having {
+  uint32_t n_predicates; /* 0..MZGPU_HAVING_MAX_PREDICATES (0: no filter) */
+  uint32_t n_consts;
+  uint32_t n_ops[MZGPU_HAVING_MAX_PREDICATES];
+  mzgpu_having_op ops[MZGPU_HAVING_MAX_PREDICATES][MZGPU_HAVING_MAX_OPS];
+  mzgpu_having_const consts[MZGPU_HAVING_MAX_CONSTS];
+} mzgpu_having;
+/* mzgpu_reduce_lanes_new with a HAVING filter.  having == NULL, or n_predicates == 0, is exactly
+ * mzgpu_reduce_lanes_new.  The lanes are checked first, as mzgpu_reduce_lanes_new does; the program is
+ * then checked on the host, before any launch, and a program that fails leaves no operator behind (*out
+ * is not written) and the context usable:
+ * MZGPU_E_INVALID for a malformed one (unknown opcode, an empty predicate or more than
+ * MZGPU_HAVING_MAX_OPS ops, stack underflow or a depth above MZGPU_HAVING_MAX_STACK, a lane >= n_lanes,
+ * a bad key field, a bad width or compare op, a constant index >= n_consts, an INT constant outside
+ * i64, an operand of the wrong type, a 32-bit operation on a value that is not int32, or a predicate
+ * that does not leave exactly one BOOL); MZGPU_E_UNSUPPORTED for a well-formed program outside the
+ * subset (arithmetic on a NUM or FLOAT, FLOAT compared with INT / NUM, BOOL compared with BOOL), so
+ * that the caller keeps its own path at render time. */
+int32_t mzgpu_reduce_lanes_new_having(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                                      uint32_t n_lanes, const mzgpu_having* having, mzgpu_reduce** out);
+
 /* ------------------------------ f1 (first step): Row keys as fixed-width words */
 /* A `Row` orders by byte length first, then by its bytes (RowRef::cmp,
  * src/repr/src/row.rs:704-722; the arrangement key order of RowRowSpine,

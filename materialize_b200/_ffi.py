@@ -112,6 +112,36 @@ class AccumLane(C.Structure):
     _fields_ = [("kind", C.c_int32), ("sign_extend", C.c_uint32), ("field", Field)]
 
 
+# HAVING programs of the lanes operator (mzgpu_having, include/mzgpu.h)
+HAVING_MAX_PREDICATES, HAVING_MAX_OPS, HAVING_MAX_CONSTS, HAVING_MAX_STACK = 4, 16, 8, 8
+HOP_KEY, HOP_COUNT, HOP_SUM, HOP_INT, HOP_NUM, HOP_FLOAT = 1, 2, 3, 4, 5, 6
+HOP_ADD, HOP_SUB, HOP_MUL, HOP_DIV, HOP_CMP, HOP_AND, HOP_OR, HOP_NOT = 7, 8, 9, 10, 11, 12, 13, 14
+# ROUT_LANES flags: bit 2l = lane l's SUM is NULL, bit 2l+1 = lane l's net-zero error; bits 16-18 = the
+# HAVING program's error
+ROUT_HAVING_ERR_SHIFT = 16
+HAVING_ERR_DIVISION_BY_ZERO, HAVING_ERR_NUMERIC_FIELD_OVERFLOW = 1, 2
+HAVING_ERR_INT32_OUT_OF_RANGE, HAVING_ERR_INT64_OUT_OF_RANGE = 3, 4
+
+
+class HavingOp(C.Structure):
+    _fields_ = [("code", C.c_uint8), ("arg", C.c_uint8), ("shift", C.c_uint8), ("bits", C.c_uint8),
+                ("sign_extend", C.c_uint8), ("konst", C.c_uint8), ("_pad", C.c_uint8 * 2)]
+
+
+class HavingConst(C.Structure):
+    _fields_ = [("lo", C.c_uint64), ("hi", C.c_uint64)]
+
+
+class Having(C.Structure):
+    _fields_ = [
+        ("n_predicates", C.c_uint32),
+        ("n_consts", C.c_uint32),
+        ("n_ops", C.c_uint32 * HAVING_MAX_PREDICATES),
+        ("ops", (HavingOp * HAVING_MAX_OPS) * HAVING_MAX_PREDICATES),
+        ("consts", HavingConst * HAVING_MAX_CONSTS),
+    ]
+
+
 class Filter(C.Structure):
     _fields_ = [("field", Field), ("op", C.c_uint32), ("rhs", C.c_uint64)]
 
@@ -245,6 +275,7 @@ SIGNATURES = {
     "mzgpu_reduce_lanes": (i32, [vp, vp, u64, i32, u64, vp]),
     "mzgpu_reduce_lanes_buf": (i32, [vp, vp, u64, vp]),
     "mzgpu_reduce_lanes_distinct_trace": (vp, [vp, u32]),
+    "mzgpu_reduce_lanes_new_having": (i32, [vp, u32, vp, u32, C.POINTER(Having), PV]),
     "mzgpu_comm_unique_id": (i32, [C.POINTER(C.c_uint8)]),
     "mzgpu_comm_init": (i32, [vp, C.POINTER(C.c_uint8)]),
     "mzgpu_exchange": (i32, [vp, vp, vp]),

@@ -35,6 +35,11 @@ from ._ffi import (  # noqa: F401  (re-exported)
     R40,
     RACC,
     ROUT,
+    ROUT_HAVING_ERR_SHIFT,
+    HAVING_ERR_DIVISION_BY_ZERO,
+    HAVING_ERR_NUMERIC_FIELD_OVERFLOW,
+    HAVING_ERR_INT32_OUT_OF_RANGE,
+    HAVING_ERR_INT64_OUT_OF_RANGE,
     Closure,
     MzGpuError,
 )
@@ -611,12 +616,110 @@ def accum_lane(kind, src=SRC_VAL1, shift=0, bits=64, sign_extend=False):
     return (int(kind), int(src), int(shift), int(bits), bool(sign_extend))
 
 
+# HAVING ops (mzgpu_having_op): one constructor per opcode.  An op is (code, arg, shift, bits,
+# sign_extend, constant value or None); having() builds the descriptor and its constant pool.
+def h_key(shift=0, bits=64, sign_extend=False):
+    """INT: bits [shift, shift + bits) of the output key, sign-extended when asked."""
+    return (F.HOP_KEY, 0, int(shift), int(bits), 1 if sign_extend else 0, None)
+
+
+def h_count(lane):
+    """INT: COUNT of `lane`."""
+    return (F.HOP_COUNT, int(lane), 0, 0, 0, None)
+
+
+def h_sum(lane):
+    """NUM (int64 lane) or FLOAT (float64 lane): SUM of `lane`; NULL when its NULL flag is set."""
+    return (F.HOP_SUM, int(lane), 0, 0, 0, None)
+
+
+def h_int(v):
+    return (F.HOP_INT, 0, 0, 0, 0, int(v))
+
+
+def h_num(v):
+    return (F.HOP_NUM, 0, 0, 0, 0, int(v))
+
+
+def h_float(x):
+    return (F.HOP_FLOAT, 0, 0, 0, 0, float(x))
+
+
+def h_add(width=64):
+    return (F.HOP_ADD, int(width), 0, 0, 0, None)
+
+
+def h_sub(width=64):
+    return (F.HOP_SUB, int(width), 0, 0, 0, None)
+
+
+def h_mul(width=64):
+    return (F.HOP_MUL, int(width), 0, 0, 0, None)
+
+
+def h_div(width=64):
+    return (F.HOP_DIV, int(width), 0, 0, 0, None)
+
+
+def h_cmp(op):
+    """op: "eq", "ne", "lt", "le", "gt" or "ge" (signed, or OrderedFloat for FLOAT)."""
+    return (F.HOP_CMP, _CMP[op], 0, 0, 0, None)
+
+
+def h_and():
+    return (F.HOP_AND, 0, 0, 0, 0, None)
+
+
+def h_or():
+    return (F.HOP_OR, 0, 0, 0, 0, None)
+
+
+def h_not():
+    return (F.HOP_NOT, 0, 0, 0, 0, None)
+
+
+def having(*predicates):
+    """The mzgpu_having of a list of predicates, each a list of h_*() ops in postfix order.  A program past the
+    descriptor's limits (predicates, ops per predicate, distinct constants) raises MzGpuError(E_INVALID), as
+    the library does for a descriptor it cannot hold."""
+    if len(predicates) > F.HAVING_MAX_PREDICATES:
+        raise MzGpuError(F.E_INVALID, f"having: {len(predicates)} predicates (at most {F.HAVING_MAX_PREDICATES})")
+    for p, ops in enumerate(predicates):
+        if len(ops) > F.HAVING_MAX_OPS:
+            raise MzGpuError(F.E_INVALID, f"having: predicate {p} has {len(ops)} ops (at most {F.HAVING_MAX_OPS})")
+    hv = F.Having()
+    hv.n_predicates = len(predicates)
+    pool = []
+    for p, ops in enumerate(predicates):
+        hv.n_ops[p] = len(ops)
+        for i, (code, arg, shift, bits, sx, value) in enumerate(ops):
+            o = hv.ops[p][i]
+            o.code, o.arg, o.shift, o.bits, o.sign_extend = code, arg, shift, bits, sx
+            if value is None:
+                continue
+            if code == F.HOP_FLOAT:
+                words = (int(np.float64(value).view(np.uint64)), 0)
+            else:
+                words = (value & (2**64 - 1), (value >> 64) & (2**64 - 1))
+            if words not in pool:
+                if len(pool) == F.HAVING_MAX_CONSTS:
+                    raise MzGpuError(F.E_INVALID, f"having: more than {F.HAVING_MAX_CONSTS} distinct constants")
+                pool.append(words)
+            o.konst = pool.index(words)
+    hv.n_consts = len(pool)
+    for k, (lo, hi) in enumerate(pool):
+        hv.consts[k].lo, hv.consts[k].hi = lo, hi
+    return hv
+
+
 class ReduceLanes:
     """COUNT / SUM of several value columns per key in one arrangement (mzgpu_reduce_lanes_new).
     `lanes` is a list of accum_lane(...) tuples; input rows are R32 (in_row_bytes=32) or R40 (40).
-    Output rows have the dtype ROUT_LANES[class] (lane l in ["lanes"][:, l])."""
+    Output rows have the dtype ROUT_LANES[class] (lane l in ["lanes"][:, l]).  `having`: a HAVING
+    filter, having(...) or an F.Having (mzgpu_reduce_lanes_new_having); its errors are in bits
+    16-18 of "flags" (ROUT_HAVING_ERR_SHIFT)."""
 
-    def __init__(self, ctx, lanes, in_row_bytes=32):
+    def __init__(self, ctx, lanes, in_row_bytes=32, having=None):
         self.ctx = ctx
         self.n_lanes = len(lanes)
         self.in_row_bytes = in_row_bytes
@@ -626,7 +729,10 @@ class ReduceLanes:
             arr[i].sign_extend = 1 if sx else 0
             arr[i].field = F.Field(src, shift, bits, 0)
         h = C.c_void_p()
-        ctx.check(F.lib.mzgpu_reduce_lanes_new(ctx.h, in_row_bytes, arr, len(lanes), C.byref(h)))
+        if having is None:
+            ctx.check(F.lib.mzgpu_reduce_lanes_new(ctx.h, in_row_bytes, arr, len(lanes), C.byref(h)))
+        else:
+            ctx.check(F.lib.mzgpu_reduce_lanes_new_having(ctx.h, in_row_bytes, arr, len(lanes), C.byref(having), C.byref(h)))
         self.h = h
         self.lane_class = F.lane_class(self.n_lanes)
         self.arr_row_bytes, self.out_row_bytes = F.LANE_ROW_BYTES[self.lane_class]

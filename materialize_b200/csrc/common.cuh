@@ -1064,12 +1064,14 @@ int32_t mz_reduce_minmax_async(mzgpu_ctx* ctx, const u64* d_batch_rows, DLen n, 
                                const TraceView& prior, int agg_kind, const TopKParams& tp, u64* d_out,
                                u64 out_cap, u64* d_out_len);
 // `c` is the lane class (1 for every mzgpu_reduce_new kind); for c >= 2 the lanes' kinds come
-// from `ls` (f64_mask, n) and agg_kind is unused
+// from `ls` (f64_mask, n) and agg_kind is unused.  `hv`: the lanes operator's HAVING program
+// (validated, at least one predicate), run by the filtered kernels; nullptr runs the unfiltered ones.
 int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, DLen n, u64 n_ub,
                                     const TraceView& prior, int agg_kind, const LaneSet* ls, u64* d_out,
-                                    u64 out_cap, u64* d_out_len);
+                                    u64 out_cap, u64* d_out_len, const mzgpu_having* hv = nullptr);
 int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
-                              int agg_kind, const LaneSet* ls, DevMem* out, u64* n_out);
+                              int agg_kind, const LaneSet* ls, DevMem* out, u64* n_out,
+                              const mzgpu_having* hv = nullptr);
 
 // correction.cu (time-major rows: (time, key, val | diff))
 // column.cu (columnar wire format, f4)

@@ -2515,6 +2515,9 @@ struct mzgpu_reduce {
   u32 distinct_lane[MZGPU_MAX_ACCUM_LANES] = {};
   mzgpu_batcher* pair_batcher[MZGPU_MAX_ACCUM_LANES] = {};
   mzgpu_spine* pairs[MZGPU_MAX_ACCUM_LANES] = {};
+  // mzgpu_reduce_lanes_new_having: the validated HAVING program, run by the corrections kernels
+  bool has_having = false;
+  mzgpu_having having = {};
   int32_t failed = MZGPU_OK;  // set when an activation failed after its seal (reduce_dev)
   std::string failed_msg;
   ~mzgpu_reduce() {
@@ -2705,6 +2708,7 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
   const int lc = r->lane_class ? r->lane_class : 1;
   const u64 out_rb = (u64)mz_lane_out_bytes(lc);
   const LaneSet* ls = r->lane_class ? &r->lanes : nullptr;
+  const mzgpu_having* hv = r->has_having ? &r->having : nullptr;
   if (st == MZGPU_OK && b_ub > 0) {
     if ((b_ub + 255) / 256 <= MZ_LB_TILES && per_row * b_ub <= MZ_BOUND_MAX_ROWS) {
       DevMem corr, cons;
@@ -2718,7 +2722,7 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
                                       r->topk, corr.as<u64>(), per_row * b_ub, clen.dptr());
         else
           st = mz_reduce_corrections_async(ctx, lc, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv,
-                                           r->agg_kind, ls, corr.as<u64>(), per_row * b_ub, clen.dptr());
+                                           r->agg_kind, ls, corr.as<u64>(), per_row * b_ub, clen.dptr(), hv);
         clen.mark_written();
       }
       if (st == MZGPU_OK && !minmax) {
@@ -2743,7 +2747,7 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
       }
       if (st == MZGPU_OK)
         st = mz_reduce_corrections(ctx, lc, batch->rows.as<u64>(), batch->st.v[0], tv, r->agg_kind, ls, &corr,
-                                   &n_corr);
+                                   &n_corr, hv);
       if (st == MZGPU_OK && n_corr && lc > 1) {
         // consolidated by construction, as in the single-pass form (and no RowT for these widths)
         st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
@@ -2863,6 +2867,121 @@ extern "C" int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes,
     MZ_TRY(mzgpu_spine_new(ctx, 32, 1, &r->pairs[j]));
   }
   *out = r.release();
+  return MZGPU_OK;
+}
+
+// The HAVING program's checks (include/mzgpu.h): a type per stack slot, simulated op by op.
+// MZGPU_E_INVALID for a malformed program, MZGPU_E_UNSUPPORTED for a well-formed one outside the subset.
+static int32_t validate_having(mzgpu_ctx* ctx, const mzgpu_having& h, const LaneSet& ls) {
+  enum Ty { INT32, INT64, NUM, FLOAT, BOOL };
+  auto bad = [&](int32_t st, uint32_t p, uint32_t i, const char* why) {
+    MZ_SET_ERR(ctx, "reduce_lanes having: predicate %u, op %u: %s", p, i, why);
+    return st;
+  };
+  if (h.n_predicates > MZGPU_HAVING_MAX_PREDICATES || h.n_consts > MZGPU_HAVING_MAX_CONSTS) {
+    MZ_SET_ERR(ctx, "reduce_lanes having: %u predicates (0..%d), %u constants (0..%d)", h.n_predicates,
+               MZGPU_HAVING_MAX_PREDICATES, h.n_consts, MZGPU_HAVING_MAX_CONSTS);
+    return MZGPU_E_INVALID;
+  }
+  int32_t unsupported = MZGPU_OK;  // reported once the whole program is known to be well-formed
+  const char* unsupported_why = nullptr;
+  uint32_t up = 0, ui = 0;
+  auto outside = [&](uint32_t p, uint32_t i, const char* why) {
+    if (unsupported == MZGPU_OK) {
+      unsupported = MZGPU_E_UNSUPPORTED;
+      unsupported_why = why;
+      up = p;
+      ui = i;
+    }
+  };
+  for (uint32_t p = 0; p < h.n_predicates; ++p) {
+    const uint32_t n_ops = h.n_ops[p];
+    if (n_ops == 0 || n_ops > MZGPU_HAVING_MAX_OPS) return bad(MZGPU_E_INVALID, p, 0, "op count (1..16)");
+    Ty ty[MZGPU_HAVING_MAX_STACK];
+    int sp = 0;
+    for (uint32_t i = 0; i < n_ops; ++i) {
+      const mzgpu_having_op& o = h.ops[p][i];
+      const uint32_t code = o.code;
+      if (code >= MZGPU_HOP_KEY && code <= MZGPU_HOP_FLOAT) {
+        if (sp == MZGPU_HAVING_MAX_STACK) return bad(MZGPU_E_INVALID, p, i, "stack overflow (depth 8)");
+        Ty t;
+        if (code == MZGPU_HOP_KEY) {
+          if (o.bits == 0 || o.bits > 64 || (uint32_t)o.shift + o.bits > 64 || o.sign_extend > 1)
+            return bad(MZGPU_E_INVALID, p, i, "key field is empty or out of range");
+          t = (o.bits < 32 || (o.bits == 32 && o.sign_extend)) ? INT32 : INT64;
+        } else if (code == MZGPU_HOP_COUNT || code == MZGPU_HOP_SUM) {
+          if (o.arg >= ls.n) return bad(MZGPU_E_INVALID, p, i, "lane out of range");
+          t = code == MZGPU_HOP_COUNT ? INT64 : (((ls.f64_mask >> o.arg) & 1u) ? FLOAT : NUM);
+        } else {
+          if (o.konst >= h.n_consts) return bad(MZGPU_E_INVALID, p, i, "constant index out of range");
+          const mzgpu_having_const& k = h.consts[o.konst];
+          const bool fits64 = k.hi == ((int64_t)k.lo < 0 ? ~0ull : 0ull);
+          if (code == MZGPU_HOP_INT) {
+            if (!fits64) return bad(MZGPU_E_INVALID, p, i, "INT constant outside i64");
+            const int64_t v = (int64_t)k.lo;
+            t = v >= INT32_MIN && v <= INT32_MAX ? INT32 : INT64;
+          } else if (code == MZGPU_HOP_FLOAT) {
+            if (k.hi != 0) return bad(MZGPU_E_INVALID, p, i, "FLOAT constant with a non-zero high word");
+            t = FLOAT;
+          } else {
+            t = NUM;
+          }
+        }
+        ty[sp++] = t;
+        continue;
+      }
+      if (code == MZGPU_HOP_NOT) {
+        if (sp < 1) return bad(MZGPU_E_INVALID, p, i, "stack underflow");
+        if (ty[sp - 1] != BOOL) return bad(MZGPU_E_INVALID, p, i, "NOT of a non-BOOL");
+        continue;
+      }
+      if (code < MZGPU_HOP_ADD || code > MZGPU_HOP_OR) return bad(MZGPU_E_INVALID, p, i, "unknown opcode");
+      if (sp < 2) return bad(MZGPU_E_INVALID, p, i, "stack underflow");
+      const Ty a = ty[sp - 2], b = ty[sp - 1];
+      --sp;
+      const bool ia = a == INT32 || a == INT64, ib = b == INT32 || b == INT64;
+      if (code == MZGPU_HOP_AND || code == MZGPU_HOP_OR) {
+        if (a != BOOL || b != BOOL) return bad(MZGPU_E_INVALID, p, i, "AND / OR of a non-BOOL");
+      } else if (code == MZGPU_HOP_CMP) {
+        if (o.arg > MZGPU_CMP_GE) return bad(MZGPU_E_INVALID, p, i, "unknown compare op");
+        if ((a == BOOL) != (b == BOOL)) return bad(MZGPU_E_INVALID, p, i, "BOOL compared with a value");
+        if (a == BOOL) outside(p, i, "BOOL comparisons");
+        else if ((a == FLOAT) != (b == FLOAT)) outside(p, i, "FLOAT compared with INT / NUM");
+        ty[sp - 1] = BOOL;
+      } else {
+        if (o.arg != 32 && o.arg != 64) return bad(MZGPU_E_INVALID, p, i, "width is not 32 or 64");
+        if (a == BOOL || b == BOOL) return bad(MZGPU_E_INVALID, p, i, "arithmetic on a BOOL");
+        if (!ia || !ib) {
+          outside(p, i, "arithmetic on a NUM or FLOAT");
+          ty[sp - 1] = a;
+        } else if (o.arg == 32 && (a != INT32 || b != INT32)) {
+          return bad(MZGPU_E_INVALID, p, i, "32-bit operation on an operand that is not int32");
+        } else {
+          ty[sp - 1] = o.arg == 32 ? INT32 : INT64;
+        }
+      }
+    }
+    if (sp != 1 || ty[0] != BOOL) return bad(MZGPU_E_INVALID, p, n_ops, "the predicate does not leave one BOOL");
+  }
+  if (unsupported != MZGPU_OK) return bad(unsupported, up, ui, unsupported_why);
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_reduce_lanes_new_having(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                                                 uint32_t n_lanes, const mzgpu_having* having, mzgpu_reduce** out) {
+  MZ_CHECK_CTX(ctx);
+  mzgpu_reduce* r = nullptr;
+  MZ_TRY(mzgpu_reduce_lanes_new(ctx, in_row_bytes, lanes, n_lanes, &r));
+  if (having != nullptr && having->n_predicates != 0) {
+    const int32_t st = validate_having(ctx, *having, r->lanes);
+    if (st != MZGPU_OK) {
+      mzgpu_reduce_free(r);
+      return st;
+    }
+    r->has_having = true;
+    r->having = *having;
+  }
+  *out = r;
   return MZGPU_OK;
 }
 

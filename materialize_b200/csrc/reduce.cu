@@ -269,6 +269,173 @@ __device__ __forceinline__ void finalize(const u64* S, int agg_kind, u32 f64_mas
   o[3 * C] = flags;
 }
 
+// ---------------------------------------------------------------- HAVING (mfp_after's filter)
+// The predicate program of include/mzgpu.h (mzgpu_having), checked on the host (host.cu:
+// validate_having), run on one finalized row.  Every thread of a warp reads the same ops from the
+// parameter bank.  A stack value is (lo, hi): the i128 of an INT (sign-extended) or a NUM, the f64
+// bits of a FLOAT (fl), 0 / 1 of a BOOL; st is HV_VAL, HV_NULL or HV_NULL + e for error e
+// (MZGPU_HAVING_ERR_*, ordered as the EvalError variants, so the larger st is the larger error).
+constexpr u32 HV_VAL = 0, HV_NULL = 1;
+
+// OrderedFloat (Datum::Float64): NaN equals NaN and is above everything; -0.0 equals +0.0
+__device__ __forceinline__ int hv_cmp3(u64 alo, u64 ahi, u64 blo, u64 bhi, bool fl) {
+  if (fl) {
+    const double a = __longlong_as_double((long long)alo), b = __longlong_as_double((long long)blo);
+    const bool an = isnan(a), bn = isnan(b);
+    if (an || bn) return an && bn ? 0 : (an ? 1 : -1);
+    return a < b ? -1 : (a > b ? 1 : 0);
+  }
+  if (ahi != bhi) return (i64)ahi < (i64)bhi ? -1 : 1;
+  return alo < blo ? -1 : (alo > blo ? 1 : 0);
+}
+
+// checked i64 arithmetic at SQL width w: add / sub / mul_int32 / 64 -> NumericFieldOverflow
+// (src/expr/src/scalar/func.rs:107, 117, 690, 700, 904, 914); div_int32 / 64 truncates, DivisionByZero,
+// MIN / -1 -> Int32OutOfRange / Int64OutOfRange (func.rs:1037-1059).  A 32-bit operation has int32
+// operands (host-checked), so its exact result is the i64 one.  Returns 0 or the error.
+__device__ __forceinline__ u32 hv_arith(int code, int w, i64 a, i64 b, i64* r) {
+  i64 x;
+  bool ovf = false;
+  if (code == MZGPU_HOP_ADD) {
+    x = (i64)((u64)a + (u64)b);
+    ovf = ((a ^ x) & (b ^ x)) < 0;
+  } else if (code == MZGPU_HOP_SUB) {
+    x = (i64)((u64)a - (u64)b);
+    ovf = ((a ^ b) & (a ^ x)) < 0;
+  } else if (code == MZGPU_HOP_MUL) {
+    x = (i64)((u64)a * (u64)b);
+    ovf = __mul64hi((long long)a, (long long)b) != (x >> 63);
+  } else {
+    if (b == 0) return MZGPU_HAVING_ERR_DIVISION_BY_ZERO;
+    if (b == -1 && a == (w == 32 ? (i64)(-2147483647 - 1) : (i64)0x8000000000000000ull))
+      return w == 32 ? MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE : MZGPU_HAVING_ERR_INT64_OUT_OF_RANGE;
+    x = a / b;
+  }
+  if (w == 32 && x != (i64)(int)x) ovf = true;
+  if (ovf) return MZGPU_HAVING_ERR_NUMERIC_FIELD_OVERFLOW;
+  *r = x;
+  return 0;
+}
+
+// The predicates on one finalized row v = C x (count, sum_lo, sum_hi), flags.  Returns the error
+// (1..4) of the first predicate that raised one, 8 if every predicate is TRUE, 0 if one is FALSE or
+// NULL (SafeMfpPlan::evaluate_inner, src/expr/src/linear.rs:1680-1700).
+template <int C>
+__device__ __forceinline__ u32 having_eval(const mzgpu_having& hv, u64 key, const u64* v, u32 f64_mask) {
+  constexpr int D = MZGPU_HAVING_MAX_STACK;
+  u64 lo[D], hi[D];
+  u32 st[D];
+  bool fl[D];
+  for (u32 p = 0; p < hv.n_predicates; ++p) {
+    int sp = 0;
+    for (u32 i = 0; i < hv.n_ops[p]; ++i) {
+      const mzgpu_having_op o = hv.ops[p][i];
+      const u32 code = o.code;
+      if (code <= MZGPU_HOP_FLOAT) {  // push
+        u64 a = 0, b = 0;
+        u32 s = HV_VAL;
+        bool f = false;
+        if (code == MZGPU_HOP_KEY) {
+          a = key >> o.shift;
+          if (o.bits < 64) {
+            a &= (1ull << o.bits) - 1;
+            if (o.sign_extend && ((a >> (o.bits - 1)) & 1)) a |= ~0ull << o.bits;
+          }
+          b = (i64)a < 0 ? ~0ull : 0;
+        } else if (code == MZGPU_HOP_COUNT || code == MZGPU_HOP_SUM) {
+#pragma unroll
+          for (int l = 0; l < C; ++l) {  // (a select, not an index: v stays in registers)
+            if ((u32)l != o.arg) continue;
+            if (code == MZGPU_HOP_COUNT) {
+              a = v[3 * l];
+              b = (i64)a < 0 ? ~0ull : 0;
+            } else {
+              a = v[3 * l + 1];
+              b = v[3 * l + 2];
+              f = ((f64_mask >> l) & 1u) != 0;
+              if ((v[3 * C] >> (2 * l)) & 1) s = HV_NULL;
+            }
+          }
+        } else {
+          a = hv.consts[o.konst].lo;
+          b = hv.consts[o.konst].hi;
+          f = code == MZGPU_HOP_FLOAT;
+        }
+        lo[sp] = a;
+        hi[sp] = b;
+        st[sp] = s;
+        fl[sp] = f;
+        ++sp;
+        continue;
+      }
+      if (code == MZGPU_HOP_NOT) {
+        if (st[sp - 1] == HV_VAL) lo[sp - 1] ^= 1;
+        continue;
+      }
+      --sp;
+      const int x = sp - 1, y = sp;  // x = the first operand and the result
+      const u32 sx = st[x], sy = st[y];
+      if (code == MZGPU_HOP_AND || code == MZGPU_HOP_OR) {
+        // variadic And / Or (src/expr/src/scalar/func/variadic.rs:74-99, 1147-1170)
+        const u64 dom = code == MZGPU_HOP_AND ? 0 : 1;
+        if ((sx == HV_VAL && lo[x] == dom) || (sy == HV_VAL && lo[y] == dom)) {
+          lo[x] = dom;
+          st[x] = HV_VAL;
+        } else {
+          st[x] = sx > sy ? sx : sy;  // the larger error, else NULL, else both are the other value
+        }
+        continue;
+      }
+      if (sx > HV_NULL || sy > HV_NULL) {  // the first operand's error, else the second's
+        st[x] = sx > HV_NULL ? sx : sy;
+        continue;
+      }
+      if (sx == HV_NULL || sy == HV_NULL) {
+        st[x] = HV_NULL;
+        continue;
+      }
+      if (code == MZGPU_HOP_CMP) {
+        const int c3 = hv_cmp3(lo[x], hi[x], lo[y], hi[y], fl[x]);
+        bool r;
+        switch (o.arg) {
+          case MZGPU_CMP_EQ: r = c3 == 0; break;
+          case MZGPU_CMP_NE: r = c3 != 0; break;
+          case MZGPU_CMP_LT: r = c3 < 0; break;
+          case MZGPU_CMP_LE: r = c3 <= 0; break;
+          case MZGPU_CMP_GT: r = c3 > 0; break;
+          default: r = c3 >= 0; break;
+        }
+        lo[x] = r ? 1 : 0;
+        hi[x] = 0;
+        fl[x] = false;
+        continue;
+      }
+      i64 r = 0;
+      const u32 e = hv_arith((int)code, o.arg, (i64)lo[x], (i64)lo[y], &r);
+      if (e != 0) {
+        st[x] = HV_NULL + e;
+      } else {
+        lo[x] = (u64)r;
+        hi[x] = r < 0 ? ~0ull : 0;
+      }
+    }
+    // one BOOL is left (host-checked)
+    if (st[0] > HV_NULL) return st[0] - HV_NULL;
+    if (st[0] == HV_NULL || lo[0] == 0) return 0;
+  }
+  return 8;
+}
+
+// Run the filter on a finalized row of a non-zero accumulation: its error goes into flag bits 16-18;
+// returns whether the row is visible (a lane error flag, a predicate error, or every predicate TRUE).
+template <int C>
+__device__ __forceinline__ bool having_apply(const mzgpu_having& hv, u64 key, u64* v, u32 f64_mask) {
+  const u32 r = having_eval<C>(hv, key, v, f64_mask);
+  const u64 err = r & 7;
+  v[3 * C] |= err << MZGPU_ROUT_HAVING_ERR_SHIFT;
+  return err != 0 || (r & 8) != 0 || (v[3 * C] & 0xAAAAull) != 0;
+}
+
 // sum of all prior updates of `key` (times before the new batch).  The first hash
 // slot of GROUP batches is fetched before any is inspected (independent loads).
 template <int C>
@@ -370,11 +537,12 @@ __device__ __forceinline__ void put_out_row(u64* __restrict__ out, u64 at, u64 k
 
 // Corrections of one changed key: rows [i, ...) of the new batch with this key,
 // given the key's prior accumulation S0.  Counts (and optionally writes at
-// out[pos...]) the (-old, +new) output rows.
-template <int C>
+// out[pos...]) the (-old, +new) output rows.  With HV the row exists only while the
+// HAVING program `hv` lets it through (having_apply), and carries the program's error.
+template <int C, bool HV = false>
 __device__ __forceinline__ u32 walk_key(const u64* __restrict__ rows, u64 n, u64 i, u64 key, const u64* S0,
                                         int agg_kind, u32 f64_mask, u32 n_lanes, bool do_write,
-                                        u64* __restrict__ out, u64 pos) {
+                                        u64* __restrict__ out, u64 pos, const mzgpu_having* hv = nullptr) {
   constexpr int NW = LaneRows<C>::ARR_NW, ND = NW - 2, NV = 3 * C + 1;
   u64 S[ND];
 #pragma unroll
@@ -405,6 +573,9 @@ __device__ __forceinline__ u32 walk_key(const u64* __restrict__ rows, u64 n, u64
 #pragma unroll
   for (int w = 0; w < NV; ++w) oldv[w] = 0;
   if (had) finalize<C>(S, agg_kind, f64_mask, n_lanes, oldv);
+  if constexpr (HV) {
+    if (had) had = having_apply<C>(*hv, key, oldv, f64_mask);
+  }
   u32 c = 0;
   for (u64 j = i; j < n; ++j) {
     const u64* row = rows + j * NW;
@@ -418,11 +589,14 @@ __device__ __forceinline__ u32 walk_key(const u64* __restrict__ rows, u64 n, u64
       diff_add<ND>(S, row + 2);
     }
     const u64 t = row[1];
-    const bool has = !diff_is_zero<ND>(S);
+    bool has = !diff_is_zero<ND>(S);
     u64 newv[NV];
 #pragma unroll
     for (int w = 0; w < NV; ++w) newv[w] = 0;
     if (has) finalize<C>(S, agg_kind, f64_mask, n_lanes, newv);
+    if constexpr (HV) {
+      if (has) has = having_apply<C>(*hv, key, newv, f64_mask);
+    }
     bool same = had && has;
 #pragma unroll
     for (int w = 0; w < NV; ++w) same = same && oldv[w] == newv[w];
@@ -519,6 +693,91 @@ __global__ void __launch_bounds__(RT) k_corrections_lb(const u64* __restrict__ r
     if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *out_len = excl + total;
   }
 }
+
+// The two forms above with a HAVING program (mzgpu_reduce_lanes_new_having).  They are separate kernels
+// so that the unfiltered ones keep their code; the bounds are the same (at most two rows per new
+// (key, time)), and sort_key_corrections keeps the output consolidated.
+template <int C, bool WRITE>
+__global__ void __launch_bounds__(RT) k_corrections_having(const u64* __restrict__ rows, u64 n,
+                                                           const __grid_constant__ TraceView prior, u32 f64_mask,
+                                                           u32 n_lanes, const __grid_constant__ mzgpu_having hv,
+                                                           u32* __restrict__ tile_counts,
+                                                           const u32* __restrict__ tile_base,
+                                                           u64* __restrict__ out) {
+  constexpr int NW = LaneRows<C>::ARR_NW, ND = NW - 2;
+  // (the lanes operator: for C = 1 finalize takes lane 0's kind as the aggregate kind)
+  const int agg_kind = (f64_mask & 1u) ? MZGPU_AGG_COUNT_SUM_F64 : MZGPU_AGG_COUNT_SUM_I64;
+  __shared__ u32 sm[34];
+  const u64 i = (u64)blockIdx.x * RT + threadIdx.x;
+  u32 cnt = 0;
+  const bool head = i < n && (i == 0 || rows[(i - 1) * NW] != rows[i * NW]);
+  u64 key = 0;
+  u64 S0[ND];
+#pragma unroll
+  for (int w = 0; w < ND; ++w) S0[w] = 0;
+  if (head) {
+    key = rows[i * NW];
+    prior_sum<C>(prior, key, S0);
+    cnt = walk_key<C, true>(rows, n, i, key, S0, agg_kind, f64_mask, n_lanes, false, nullptr, 0, &hv);
+  }
+  u32 total;
+  u32 ex = block_exclusive_scan(cnt, sm, &total);
+  if (!WRITE) {
+    if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
+  } else {
+    if (head && cnt > 0)
+      walk_key<C, true>(rows, n, i, key, S0, agg_kind, f64_mask, n_lanes, true, out,
+                        (u64)tile_base[blockIdx.x] + ex, &hv);
+  }
+}
+
+template <int C>
+__global__ void __launch_bounds__(RT) k_corrections_lb_having(const u64* __restrict__ rows, const DLen dn,
+                                                              const __grid_constant__ TraceView prior, u32 f64_mask,
+                                                              u32 n_lanes, const __grid_constant__ mzgpu_having hv,
+                                                              const LookBack lb, u64* __restrict__ out, u64 out_cap,
+                                                              u64* __restrict__ out_len, u64* __restrict__ status) {
+  constexpr int NW = LaneRows<C>::ARR_NW, ND = NW - 2;
+  const int agg_kind = (f64_mask & 1u) ? MZGPU_AGG_COUNT_SUM_F64 : MZGPU_AGG_COUNT_SUM_I64;
+  __shared__ u32 sm[34];
+  __shared__ u32 s_tile;
+  __shared__ u64 s_b;
+  const u64 n = dlen_get(dn);
+  const u64 n_tiles = (n + RT - 1) / RT;
+  while (true) {
+    const u32 tile = lb_next_tile(lb, &s_tile);
+    if ((u64)tile >= n_tiles) {
+      if (n_tiles == 0 && tile == 0 && threadIdx.x == 0) *out_len = 0;
+      break;
+    }
+    const u64 i = (u64)tile * RT + threadIdx.x;
+    u32 cnt = 0;
+    const bool head = i < n && (i == 0 || rows[(i - 1) * NW] != rows[i * NW]);
+    u64 key = 0;
+    u64 S0[ND];
+#pragma unroll
+    for (int w = 0; w < ND; ++w) S0[w] = 0;
+    if (head) {
+      key = rows[i * NW];
+      prior_sum<C>(prior, key, S0);
+      cnt = walk_key<C, true>(rows, n, i, key, S0, agg_kind, f64_mask, n_lanes, false, nullptr, 0, &hv);
+    }
+    u32 total;
+    const u32 ex = block_exclusive_scan(cnt, sm, &total);
+    const u64 excl = lb_exclusive_prefix(lb, tile, (u64)total, &s_b);
+    if (head && cnt > 0) {
+      const u64 pos = excl + ex;
+      if (pos + cnt > out_cap)
+        atomicMax((unsigned long long*)status, (unsigned long long)(pos + cnt));
+      else
+        walk_key<C, true>(rows, n, i, key, S0, agg_kind, f64_mask, n_lanes, true, out, pos, &hv);
+    }
+    if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *out_len = excl + total;
+  }
+}
+// the largest parameter block of the two (k_corrections_lb_having) within the classic 4 KB
+static_assert(sizeof(TraceView) + sizeof(mzgpu_having) + sizeof(LookBack) + sizeof(DLen) + 6 * sizeof(u64) <= 4096,
+              "k_corrections_lb_having parameters");
 
 // ------------------------------------------------------------------ MIN / MAX
 // Result of the hierarchical reduce (reduce.rs:1050-1135): per key the live
@@ -1281,7 +1540,7 @@ int32_t mz_explode_lanes(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u64 n
 }
 
 int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
-                              int agg_kind, const LaneSet* ls, DevMem* out, u64* n_out) {
+                              int agg_kind, const LaneSet* ls, DevMem* out, u64* n_out, const mzgpu_having* hv) {
   *n_out = 0;
   if (n == 0) return out->alloc(ctx, 16);
   const u32 fm = ls != nullptr ? ls->f64_mask : 0, nl = ls != nullptr ? ls->n : 1;
@@ -1290,8 +1549,12 @@ int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u6
   MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
   u64* d_total = ctx->d_scratch + 30;
   MZ_TRY(mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
-    MZ_LAUNCH(ctx, (k_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
-              tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
+    if (hv != nullptr)
+      MZ_LAUNCH(ctx, (k_corrections_having<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, fm, nl, *hv,
+                tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
+    else
+      MZ_LAUNCH(ctx, (k_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
+                tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
     return MZGPU_OK;
   }));
   MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
@@ -1303,8 +1566,12 @@ int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u6
   *n_out = total;
   if (total == 0) return MZGPU_OK;
   return mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
-    MZ_LAUNCH(ctx, (k_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
-              (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
+    if (hv != nullptr)
+      MZ_LAUNCH(ctx, (k_corrections_having<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, fm, nl, *hv,
+                (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
+    else
+      MZ_LAUNCH(ctx, (k_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
+                (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
     return MZGPU_OK;
   });
 }
@@ -1313,7 +1580,7 @@ int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u6
 // new (key, time) row, so capacity 2 * n_ub always suffices.
 int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, DLen n, u64 n_ub,
                                     const TraceView& prior, int agg_kind, const LaneSet* ls, u64* d_out,
-                                    u64 out_cap, u64* d_out_len) {
+                                    u64 out_cap, u64* d_out_len, const mzgpu_having* hv) {
   const u32 fm = ls != nullptr ? ls->f64_mask : 0, nl = ls != nullptr ? ls->n : 1;
   LookBack lb;
   MZ_TRY(mz_lookback_begin(ctx, (n_ub + RT - 1) / RT, &lb));
@@ -1322,8 +1589,12 @@ int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_ro
   if (grid == 0) grid = 1;
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * (2 * mz_lane_arr_bytes(c) + 16 + 2 * mz_lane_out_bytes(c)) : 0);
   return mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
-    MZ_LAUNCH(ctx, k_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, lb, d_out,
-              out_cap, d_out_len, ctx->d_status);
+    if (hv != nullptr)
+      MZ_LAUNCH(ctx, k_corrections_lb_having<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, fm, nl, *hv, lb,
+                d_out, out_cap, d_out_len, ctx->d_status);
+    else
+      MZ_LAUNCH(ctx, k_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, lb, d_out,
+                out_cap, d_out_len, ctx->d_status);
     return MZGPU_OK;
   });
 }

@@ -75,6 +75,19 @@ impl GpuReduceLanes {
         }
         Ok(GpuReduceLanes { h, arr_row_bytes: arr, out_row_bytes: out })
     }
+    /// The same with the filter half of the reduce's `mfp_after` (`sys::Having`, INTEGRATION.md maps a
+    /// `SafeMfpPlan`'s predicates to it).  A program outside the device subset comes back as
+    /// `MZGPU_E_UNSUPPORTED`: the caller keeps the Rust operator for that plan.
+    pub fn new_having(in_row_bytes: u32, lanes: &[sys::AccumLane], having: &sys::Having) -> Result<Self, (i32, String)> {
+        let (mut arr, mut out) = (0u32, 0u32);
+        let mut h = std::ptr::null_mut();
+        unsafe {
+            sys::check(worker_ctx(), sys::mzgpu_reduce_lanes_row_bytes(lanes.len() as u32, &mut arr, &mut out))?;
+            sys::check(worker_ctx(), sys::mzgpu_reduce_lanes_new_having(worker_ctx(), in_row_bytes, lanes.as_ptr(),
+                                                                       lanes.len() as u32, having, &mut h))?;
+        }
+        Ok(GpuReduceLanes { h, arr_row_bytes: arr, out_row_bytes: out })
+    }
     /// One activation over a device buffer of input rows; output rows (`out_row_bytes` wide) are appended to `out`.
     pub fn step(&mut self, rows: *mut sys::Buf, upper: u64, out: *mut sys::Buf) -> Result<(), (i32, String)> {
         unsafe { sys::check(worker_ctx(), sys::mzgpu_reduce_lanes_buf(self.h, rows, upper, out)) }

@@ -56,6 +56,29 @@ pub struct Field { pub src: u8, pub shift: u8, pub bits: u8, pub dst_shift: u8 }
 /// One aggregate lane of the multi-column accumulable reduce (mzgpu_accum_lane).
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)]
 pub struct AccumLane { pub kind: i32, pub sign_extend: u32, pub field: Field }
+/// HAVING: the filter half of a reduce's mfp_after (mzgpu_having; include/mzgpu.h has the semantics).
+pub const HAVING_MAX_PREDICATES: usize = 4;
+pub const HAVING_MAX_OPS: usize = 16;
+pub const HAVING_MAX_CONSTS: usize = 8;
+pub const HOP_KEY: u8 = 1; pub const HOP_COUNT: u8 = 2; pub const HOP_SUM: u8 = 3;
+pub const HOP_INT: u8 = 4; pub const HOP_NUM: u8 = 5; pub const HOP_FLOAT: u8 = 6;
+pub const HOP_ADD: u8 = 7; pub const HOP_SUB: u8 = 8; pub const HOP_MUL: u8 = 9; pub const HOP_DIV: u8 = 10;
+pub const HOP_CMP: u8 = 11; pub const HOP_AND: u8 = 12; pub const HOP_OR: u8 = 13; pub const HOP_NOT: u8 = 14;
+/// Output-row flag bits 16-18: the predicate error (1 DivisionByZero, 2 NumericFieldOverflow,
+/// 3 Int32OutOfRange, 4 Int64OutOfRange).
+pub const ROUT_HAVING_ERR_SHIFT: u32 = 16;
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct HavingOp { pub code: u8, pub arg: u8, pub shift: u8, pub bits: u8, pub sign_extend: u8, pub konst: u8, pub _pad: [u8; 2] }
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct HavingConst { pub lo: u64, pub hi: u64 }
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct Having {
+    pub n_predicates: u32,
+    pub n_consts: u32,
+    pub n_ops: [u32; HAVING_MAX_PREDICATES],
+    pub ops: [[HavingOp; HAVING_MAX_OPS]; HAVING_MAX_PREDICATES],
+    pub consts: [HavingConst; HAVING_MAX_CONSTS],
+}
 pub const COMM_ID_BYTES: usize = 128;
 pub const P2P_HANDLE_BYTES: usize = 64;
 
@@ -174,6 +197,7 @@ extern "C" {
     pub fn mzgpu_reduce_lanes(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf) -> i32;
     pub fn mzgpu_reduce_lanes_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf) -> i32;
     pub fn mzgpu_reduce_lanes_distinct_trace(r: *mut Reduce, lane: u32) -> *mut Spine;
+    pub fn mzgpu_reduce_lanes_new_having(ctx: *mut Ctx, in_row_bytes: u32, lanes: *const AccumLane, n_lanes: u32, having: *const Having, out: *mut *mut Reduce) -> i32;
     pub fn mzgpu_rowkey_pack(row_bytes: *const u8, len: u64, key_out: *mut u64) -> i32;
     pub fn mzgpu_rowkeys_pack(data: *const u8, offsets: *const u64, n: u64, keys_out: *mut u64, n_done: *mut u64) -> i32;
     pub fn mzgpu_rowkey_unpack(key: u64, row_bytes_out: *mut u8, len_out: *mut u64) -> i32;
