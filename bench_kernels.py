@@ -297,6 +297,105 @@ def main():
         )
         c.close()
         print(name, f"{best['without']:.4f} s / {best['with']:.4f} s", file=sys.stderr, flush=True)
+
+    # Monotonic MIN / MAX: cfg 4's incremental regime made insert-only, 4 unsigned lanes (MIN / MAX of val1
+    # and of val2's bits).  One monotonic operator against four MIN / MAX operators, which take R32
+    # (key, value) projections made before the timed region; alternating on one context, best of two rounds
+    # after a warm-up.  The four operators walk every live value of a hot key once per batch, so the
+    # comparison runs over the first `nb_cmp` batches; the monotonic operator alone then runs all nb.
+    name = f"cfg4 incremental insert-only MIN/MAX lanes=4, monotonic vs four MIN/MAX operators, {nb}x{per} R40"
+    if not args.only or args.only in name:
+        nb_cmp = min(nb, 5)
+        c = mz.Context(0)
+        ins = [r40_cfg4(c, 7, per, first=b * per, t=b, diff=1) for b in range(nb)]
+        mono_lanes = [mz.accum_lane(mz.AGG_MIN, 1), mz.accum_lane(mz.AGG_MAX, 1), mz.accum_lane(mz.AGG_MIN, 2),
+                      mz.accum_lane(mz.AGG_MAX, 2)]
+        kinds = [(mz.AGG_MIN, "val1"), (mz.AGG_MAX, "val1"), (mz.AGG_MIN, "val2"), (mz.AGG_MAX, "val2")]
+
+        def proj(r, col):
+            p = np.zeros(len(r), dtype=mz.R32)
+            p["key"], p["val"], p["time"], p["diff"] = r["key"], r[col], r["time"], r["diff"]
+            return p
+
+        def collect(coll, rows, vals):
+            for k, v, d in zip(rows["key"].tolist(), vals, rows["diff"].tolist()):
+                coll[(k, v)] = coll.get((k, v), 0) + d
+
+        def run_mono(k):
+            cm = mz.Context(0)  # one context per leg: its own device_bytes_peak
+            bufs = [mz.DeviceRows(cm, 40).upload(ins[b]) for b in range(k)]
+            op = mz.ReduceMonotonic(cm, mono_lanes, 40)
+            out, errs = mz.DeviceRows(cm, op.out_row_bytes), mz.DeviceRows(cm, 16)
+            cm.sync()
+            t0 = time.perf_counter()
+            for b, d in enumerate(bufs):
+                op.step_dev(d, b + 1, out, errs)
+            cm.sync()
+            dt = time.perf_counter() - t0
+            r = (dt, out.download(), len(errs), len(op.input_trace().export()), cm.stats()["device_bytes_peak"])
+            del op, out, errs, bufs
+            cm.close()
+            return r
+
+        def run_four(k):
+            from materialize_b200 import _ffi as F
+
+            cf = mz.Context(0)
+            bufs = [[mz.DeviceRows(cf, 32).upload(proj(ins[b], col)) for b in range(k)] for _, col in kinds]
+            ops = [mz.ReduceAccumulable(cf, kind) for kind, _ in kinds]
+            outs = [mz.DeviceRows(cf, 64) for _ in kinds]
+            cf.sync()
+            t0 = time.perf_counter()
+            for b in range(k):
+                for j in range(4):
+                    ops[j].step_dev(bufs[j][b], b + 1, outs[j])
+            cf.sync()
+            dt = time.perf_counter() - t0
+            r = (dt, [o.download() for o in outs], sum(len(mz.Spine(cf, 32, _borrowed=F.lib.mzgpu_reduce_input_trace(op.h)).export()) for op in ops),
+                 cf.stats()["device_bytes_peak"])
+            del ops, outs, bufs
+            cf.close()
+            return r
+
+        best = {"mono": None, "four": None}
+        for rnd in range(3):  # round 0 warms up
+            dm, mout, n_err, marr, peak_m = run_mono(nb_cmp)
+            df, fouts, farr, peak_f = run_four(nb_cmp)
+            if rnd > 0:
+                best["mono"] = dm if best["mono"] is None else min(best["mono"], dm)
+                best["four"] = df if best["four"] is None else min(best["four"], df)
+        agree = n_err == 0
+        for j in range(4):
+            cm_, cf_ = {}, {}
+            collect(cm_, mout, mout["vals"][:, j].tolist())
+            collect(cf_, fouts[j], fouts[j]["sum_lo"].tolist())
+            agree = agree and {k: d for k, d in cm_.items() if d} == {k: d for k, d in cf_.items() if d}
+        dm_all, _, _, marr_all, peak_all = run_mono(nb)
+        res["cases"].append(
+            {"case": name, "rows": nb_cmp * per, "batches_compared": nb_cmp,
+             "seconds_monotonic": best["mono"], "seconds_four_minmax": best["four"], "outputs_agree": agree,
+             "arrangement_rows_monotonic": marr, "arrangement_bytes_monotonic": 48 * marr,
+             "arrangement_rows_four_minmax": farr, "arrangement_bytes_four_minmax": 32 * farr,
+             "device_bytes_peak_monotonic": peak_m, "device_bytes_peak_four_minmax": peak_f,
+             "monotonic_all_batches": {"batches": nb, "seconds": dm_all, "arrangement_rows": marr_all,
+                                       "device_bytes_peak": peak_all}}
+        )
+        print(name, f"{best['mono']:.4f} s / {best['four']:.4f} s, agree={agree}, all {nb}: {dm_all:.4f} s",
+              file=sys.stderr, flush=True)
+        del ins
+        c.close()
+
+    name = f"bulk monotonic MIN/MAX lanes=4 n={n4} zipf0.9 keys={nk} R40"
+    host = r40_cfg4(ctx, 3, n4) if not args.only or args.only in name else None
+    lanes_case(
+        name,
+        n4,
+        lambda c, host=host: mz.DeviceRows(c, 40).upload(host),
+        lambda c, d: mz.ReduceMonotonic(c, [mz.accum_lane(mz.AGG_MIN, 1), mz.accum_lane(mz.AGG_MAX, 1),
+                                            mz.accum_lane(mz.AGG_MIN, 2), mz.accum_lane(mz.AGG_MAX, 2)],
+                                        40).step_dev(d, 1),
+    )
+    del host
     txt = json.dumps(res, indent=1)
     if args.out:
         open(args.out, "w").write(txt)

@@ -739,6 +739,74 @@ typedef struct mzgpu_having {
 int32_t mzgpu_reduce_lanes_new_having(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
                                       uint32_t n_lanes, const mzgpu_having* having, mzgpu_reduce** out);
 
+/* ---- monotonic MIN / MAX reduce: several MIN / MAX columns per key kept in the arrangement's diff
+ * (HierarchicalPlan::Monotonic, src/compute-types/src/plan/reduce.rs:160-250, which the planner picks for
+ * append-only inputs; rendered by build_monotonic, src/compute/src/render/reduce.rs:1138-1253).
+ *
+ * One activation:
+ *   1. must_consolidate != 0: the rows are consolidated by (key, the lanes' values, time) first
+ *      (consolidate_named_if): every value bit no lane reads is cleared, then equal rows fold, so a
+ *      +1 / -1 pair at one time cancels.
+ *   2. ensure_monotonic (src/timely-util/src/operator.rs:425-456): a row is kept iff its diff > 0.
+ *      Every other row, diff == 0 included, is one error at its time: `errs` receives R16 rows
+ *      (key = time, diff = rows rejected at that time), consolidated.  Rejected rows reach no key.
+ *   3. A kept row's lane values become the diff, one Min / Max per lane; its multiplicity does not
+ *      matter.  The arrangement keeps per (key, time) the per-lane extremum, and a key never leaves it
+ *      once a row of it was kept (IsZero is always false).
+ *   4. Output: per key, (key, the lanes' MIN / MAX) -- (-old, +new) whenever the accumulated values
+ *      change, +new alone for the key's first kept row.
+ *
+ * Lanes reuse mzgpu_accum_lane: kind = MZGPU_AGG_MIN or MZGPU_AGG_MAX, field as for the lanes reduce
+ * (src MZGPU_SRC_VAL1, or MZGPU_SRC_VAL2 of R40 input; shift, bits).  Unlike the accumulable lanes, where
+ * a 64-bit field is always the i64, sign_extend chooses the ORDER here:
+ *   sign_extend != 0: an int64 aggregate (MinInt16/32/64, MaxInt*, Date, Timestamp): the field
+ *                     sign-extended, compared signed;
+ *   sign_extend == 0: unsigned order (MinUInt*, MaxUInt*, MzTimestamp, Bool).
+ * Output values are the natural values: the i64 bits of a signed lane, the u64 of an unsigned one.
+ * NULLs are outside the fixed-width subset: every kept row carries a value for every lane.
+ *
+ * Lane word encoding in the arrangement (what mzgpu_reduce_input_trace exports): word = value
+ * ^ 2^63 for a signed lane, complemented on top of that for MIN, so every lane accumulates as an
+ * unsigned MAX and zero is the identity.  The same xor decodes a word.
+ *
+ * Row widths (lane count rounds up to a class of 4 or 8; unused lanes are zero):
+ *     lanes   arrangement                                   output
+ *     1-4      48 B: key, time | 4 lane words                56 B: key, 4 values, time, diff
+ *     5-8     112 B: key, time | 8 lane words, 4 zero words  88 B: key, 8 values, time, diff
+ * The output rows have no generic meaning: mzgpu_buf_consolidate on them returns MZGPU_E_UNSUPPORTED
+ * (they leave the operator consolidated).  The arrangement widths are accepted by batchers, builders and
+ * spines, and accumulate there by the per-word max.
+ *
+ * Not supported: float64 MIN / MAX (OrderedFloat ties -0.0 with +0.0, and NaNs with different payloads,
+ * so which bits survive would depend on arrival order), MonotonicTop1Plan / MonotonicTopKPlan, HAVING on
+ * this operator, and COUNT / SUM in the same operator (a MonotonicPlan holds MIN / MAX-type functions
+ * only). */
+/* OR'd into a MIN / MAX lane's kind: the column is float64.  Always MZGPU_E_UNSUPPORTED (see above), so
+ * that a caller describing such a plan keeps its own path. */
+#define MZGPU_MONO_F64 0x200
+#define MZGPU_ROW_RMONO4 48
+#define MZGPU_ROW_RMONO8 112
+#define MZGPU_ROW_MONO_OUT4 56
+#define MZGPU_ROW_MONO_OUT8 88
+/* The arrangement and output row widths for n_lanes (1..8); MZGPU_E_INVALID otherwise. */
+int32_t mzgpu_reduce_monotonic_row_bytes(uint32_t n_lanes, uint32_t* arr_row_bytes, uint32_t* out_row_bytes);
+/* in_row_bytes: 32 (R32) or 40 (R40); n_lanes 1..8.  Checked on the host before any launch:
+ * MZGPU_E_INVALID for a malformed descriptor (a kind other than MIN / MAX, a COUNT / SUM kind, any flag bit
+ * but MZGPU_MONO_F64, VAL2 on R32 input, a zero-width or out-of-range field, n_lanes of 0 or above 8);
+ * then MZGPU_E_UNSUPPORTED for a float64 lane.  A failure leaves no operator behind (*out is not written)
+ * and the context usable.  The handle is freed with mzgpu_reduce_free; mzgpu_reduce_input_trace returns its
+ * arrangement. */
+int32_t mzgpu_reduce_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                                   uint32_t n_lanes, int32_t must_consolidate, mzgpu_reduce** out);
+/* One activation, with the protocol of mzgpu_reduce_lanes[_buf]: `rows` are n input rows of
+ * in_row_bytes with times in [previous upper, upper); the corrections (rows of the class's output width)
+ * are appended to `out`, consolidated, and the errors (R16) to `errs` (required).  After a failed
+ * activation the operator reports that status from then on. */
+int32_t mzgpu_reduce_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                               mzgpu_buf* out, mzgpu_buf* errs);
+int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                   mzgpu_buf* errs);
+
 /* ------------------------------ f1 (first step): Row keys as fixed-width words */
 /* A `Row` orders by byte length first, then by its bytes (RowRef::cmp,
  * src/repr/src/row.rs:704-722; the arrangement key order of RowRowSpine,

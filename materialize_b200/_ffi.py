@@ -89,9 +89,27 @@ ROUT_LANES = {
     )
     for c in LANE_CLASSES
 }
+# The monotonic MIN / MAX reduce (mzgpu_reduce_monotonic_new): the lane count rounds up to a class of 4 or
+# 8.  Arrangement rows hold the encoded lane words (value ^ 2^63 for a signed lane, complemented for MIN);
+# output rows hold the values.
+MONO_CLASSES = (4, 8)
+MONO_ROW_BYTES = {4: (48, 56), 8: (112, 88)}
+
+
+def mono_class(n_lanes):
+    return 4 if n_lanes <= 4 else 8
+
+
+RMONO = {
+    4: np.dtype([("key", "<u8"), ("time", "<u8"), ("lanes", "<u8", (4,))]),
+    8: np.dtype([("key", "<u8"), ("time", "<u8"), ("lanes", "<u8", (8,)), ("_pad", "<u8", (4,))]),
+}
+MONO_OUT = {c: np.dtype([("key", "<u8"), ("vals", "<u8", (c,)), ("time", "<u8"), ("diff", "<i8")]) for c in MONO_CLASSES}
 DTYPES = {16: R16, 32: R32, 40: R40, 80: RACC, 64: ROUT}
 DTYPES.update({LANE_ROW_BYTES[c][0]: RACC_LANES[c] for c in LANE_CLASSES[1:]})
 DTYPES.update({LANE_ROW_BYTES[c][1]: ROUT_LANES[c] for c in LANE_CLASSES[1:]})
+DTYPES.update({MONO_ROW_BYTES[c][0]: RMONO[c] for c in MONO_CLASSES})
+DTYPES.update({MONO_ROW_BYTES[c][1]: MONO_OUT[c] for c in MONO_CLASSES})
 
 MEM_HOST, MEM_DEVICE = 0, 1
 FRONTIER_EMPTY = 2**64 - 1
@@ -100,6 +118,7 @@ HALFJOIN_LE, HALFJOIN_LT = 0, 1
 AGG_COUNT_SUM_I64, AGG_COUNT_SUM_F64, AGG_DISTINCT, AGG_THRESHOLD, AGG_MIN, AGG_MAX, AGG_TOPK = 0, 1, 2, 3, 4, 5, 6
 MAX_ACCUM_LANES = 8
 ACCUM_DISTINCT = 0x100  # OR'd into a lane's kind: COUNT(DISTINCT col) / SUM(DISTINCT col)
+MONO_F64 = 0x200  # OR'd into a monotonic MIN / MAX lane's kind: a float64 column (always E_UNSUPPORTED)
 COMM_ID_BYTES = 128
 P2P_HANDLE_BYTES = 64
 
@@ -276,6 +295,10 @@ SIGNATURES = {
     "mzgpu_reduce_lanes_buf": (i32, [vp, vp, u64, vp]),
     "mzgpu_reduce_lanes_distinct_trace": (vp, [vp, u32]),
     "mzgpu_reduce_lanes_new_having": (i32, [vp, u32, vp, u32, C.POINTER(Having), PV]),
+    "mzgpu_reduce_monotonic_row_bytes": (i32, [u32, PU32, PU32]),
+    "mzgpu_reduce_monotonic_new": (i32, [vp, u32, vp, u32, i32, PV]),
+    "mzgpu_reduce_monotonic": (i32, [vp, vp, u64, i32, u64, vp, vp]),
+    "mzgpu_reduce_monotonic_buf": (i32, [vp, vp, u64, vp, vp]),
     "mzgpu_comm_unique_id": (i32, [C.POINTER(C.c_uint8)]),
     "mzgpu_comm_init": (i32, [vp, C.POINTER(C.c_uint8)]),
     "mzgpu_exchange": (i32, [vp, vp, vp]),

@@ -21,6 +21,9 @@ import numpy as np
 from . import _ffi as F
 from ._ffi import (  # noqa: F401  (re-exported)
     ACCUM_DISTINCT,
+    MONO_F64,
+    MONO_OUT,
+    RMONO,
     AGG_COUNT_SUM_F64,
     AGG_DISTINCT,
     AGG_THRESHOLD,
@@ -612,7 +615,8 @@ class ReduceAccumulable:
 def accum_lane(kind, src=SRC_VAL1, shift=0, bits=64, sign_extend=False):
     """One lane of ReduceLanes: COUNT and SUM of the bit-field `bits` wide at `shift` of value word
     `src` (1 = val / val1, 2 = val2); an I64 field is sign-extended when `sign_extend`.  A kind of
-    AGG_COUNT_SUM_I64 | ACCUM_DISTINCT makes the lane COUNT(DISTINCT col) / SUM(DISTINCT col)."""
+    AGG_COUNT_SUM_I64 | ACCUM_DISTINCT makes the lane COUNT(DISTINCT col) / SUM(DISTINCT col).  For
+    ReduceMonotonic the kind is AGG_MIN or AGG_MAX and `sign_extend` chooses signed order."""
     return (int(kind), int(src), int(shift), int(bits), bool(sign_extend))
 
 
@@ -756,6 +760,51 @@ class ReduceLanes:
         """The (key, value) pair arrangement (R32 rows) of distinct lane `lane`; None for any other lane."""
         h = F.lib.mzgpu_reduce_lanes_distinct_trace(self.h, lane)
         return Spine(self.ctx, 32, _borrowed=h) if h else None
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_reduce_free(self.h)
+            self.h = None
+
+
+class ReduceMonotonic:
+    """MIN / MAX of several value columns per key over append-only input (mzgpu_reduce_monotonic_new,
+    build_monotonic).  `lanes` are accum_lane(AGG_MIN | AGG_MAX, ...) tuples; sign_extend=True makes a lane
+    an int64 aggregate (signed order), False an unsigned one.  Input rows are R32 (in_row_bytes=32) or R40
+    (40).  step() returns (corrections, errors): corrections of dtype MONO_OUT[class] (lane l in
+    ["vals"][:, l]), errors R16 rows (key = time, diff = rows with diff <= 0 at that time)."""
+
+    def __init__(self, ctx, lanes, in_row_bytes=32, must_consolidate=False):
+        self.ctx = ctx
+        self.n_lanes = len(lanes)
+        self.in_row_bytes = in_row_bytes
+        arr = (F.AccumLane * max(1, len(lanes)))()
+        for i, (kind, src, shift, bits, sx) in enumerate(lanes):
+            arr[i].kind = kind
+            arr[i].sign_extend = 1 if sx else 0
+            arr[i].field = F.Field(src, shift, bits, 0)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_reduce_monotonic_new(ctx.h, in_row_bytes, arr, len(lanes), 1 if must_consolidate else 0,
+                                                   C.byref(h)))
+        self.h = h
+        self.lane_class = F.mono_class(self.n_lanes)
+        self.arr_row_bytes, self.out_row_bytes = F.MONO_ROW_BYTES[self.lane_class]
+
+    def step(self, rows, upper):
+        rows = np.ascontiguousarray(rows)
+        out, errs = DeviceRows(self.ctx, self.out_row_bytes), DeviceRows(self.ctx, 16)
+        self.ctx.check(F.lib.mzgpu_reduce_monotonic(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
+        return out.download(), errs.download()
+
+    def step_dev(self, dev_rows, upper, out=None, errs=None):
+        """One activation over device-resident rows; corrections and errors are appended on the device."""
+        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
+        errs = errs if errs is not None else DeviceRows(self.ctx, 16)
+        self.ctx.check(F.lib.mzgpu_reduce_monotonic_buf(self.h, dev_rows.h, upper, out.h, errs.h))
+        return out, errs
+
+    def input_trace(self):
+        return Spine(self.ctx, self.arr_row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
 
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:

@@ -500,51 +500,65 @@ int32_t mz_lookback_begin_at(mzgpu_ctx* ctx, u64 at, u64 max_tiles, LookBack* lb
 
 // ---------------------------------------------------------------- row traits
 // A row is NW 64-bit words: NK sort-key words first (compared as unsigned, in
-// order), then the diff words.  TW = index of the time word (or -1).
+// order), then the diff words.  TW = index of the time word (or -1).  SG = the
+// diff's semigroup: MZ_SG_SUM (differences that add, and vanish at zero) or
+// MZ_SG_MAX (the monotonic reduce: per-word unsigned max, never zero).
+enum : int { MZ_SG_SUM = 0, MZ_SG_MAX = 1 };
 template <int RB>
 struct RowT;
 template <>
 struct RowT<16> {  // mzgpu_r16 (key | diff)
-  static constexpr int NW = 2, NK = 1, ND = 1, TW = -1, DK = 1;
+  static constexpr int NW = 2, NK = 1, ND = 1, TW = -1, DK = 1, SG = MZ_SG_SUM;
 };
 template <>
 struct RowT<32> {  // mzgpu_r32 (key, val, time | diff)
-  static constexpr int NW = 4, NK = 3, ND = 1, TW = 2, DK = 2;
+  static constexpr int NW = 4, NK = 3, ND = 1, TW = 2, DK = 2, SG = MZ_SG_SUM;
 };
 template <>
 struct RowT<40> {  // mzgpu_r40 (key, val1, val2, time | diff)
-  static constexpr int NW = 5, NK = 4, ND = 1, TW = 3, DK = 3;
+  static constexpr int NW = 5, NK = 4, ND = 1, TW = 3, DK = 3, SG = MZ_SG_SUM;
 };
 template <>
 struct RowT<80> {  // mzgpu_racc (key, time | total, non_nulls, acc_lo, acc_hi, pinf, ninf, nan, pad)
-  static constexpr int NW = 10, NK = 2, ND = 8, TW = 1, DK = 1;
+  static constexpr int NW = 10, NK = 2, ND = 8, TW = 1, DK = 1, SG = MZ_SG_SUM;
 };
 template <>
 struct RowT<64> {  // mzgpu_rout (key, count, sum_lo, sum_hi, flags, time | diff, pad)
-  static constexpr int NW = 8, NK = 6, ND = 2, TW = 5, DK = 5;
+  static constexpr int NW = 8, NK = 6, ND = 2, TW = 5, DK = 5, SG = MZ_SG_SUM;
 };
 // Multi-lane accumulable arrangement rows (mzgpu_reduce_lanes_new): key, time | total, then
 // C lanes of (non_nulls, acc_lo, acc_hi, pos_infs, neg_infs, nans), padded to 16 bytes.
 template <>
 struct RowT<128> {  // C = 2
-  static constexpr int NW = 16, NK = 2, ND = 14, TW = 1, DK = 1;
+  static constexpr int NW = 16, NK = 2, ND = 14, TW = 1, DK = 1, SG = MZ_SG_SUM;
 };
 template <>
 struct RowT<224> {  // C = 4
-  static constexpr int NW = 28, NK = 2, ND = 26, TW = 1, DK = 1;
+  static constexpr int NW = 28, NK = 2, ND = 26, TW = 1, DK = 1, SG = MZ_SG_SUM;
 };
 template <>
 struct RowT<416> {  // C = 8
-  static constexpr int NW = 52, NK = 2, ND = 50, TW = 1, DK = 1;
+  static constexpr int NW = 52, NK = 2, ND = 50, TW = 1, DK = 1, SG = MZ_SG_SUM;
+};
+// Monotonic MIN / MAX arrangement rows (mzgpu_reduce_monotonic_new): key, time | one encoded lane
+// word per lane (MonoRows below), the class's unused lanes and the pad words zero.
+template <>
+struct RowT<48> {  // 1-4 lanes
+  static constexpr int NW = 6, NK = 2, ND = 4, TW = 1, DK = 1, SG = MZ_SG_MAX;
+};
+template <>
+struct RowT<112> {  // 5-8 lanes, 4 pad words
+  static constexpr int NW = 14, NK = 2, ND = 12, TW = 1, DK = 1, SG = MZ_SG_MAX;
 };
 // DK = number of leading "data" words (key words before the time word): two
 // rows with equal DK words are the same (key, val).
 //
 // Every width has exactly one meaning, because the generic kernels (sort, consolidate, merge,
 // index) pick the diff arithmetic from the width alone.  The lanes operator's output rows for
-// C >= 2 (96, 144 and 240 bytes, LaneRows below) were given widths that no arrangement row uses,
-// and deliberately have no RowT: mzgpu_buf_consolidate on them returns MZGPU_E_UNSUPPORTED
-// instead of summing the wrong words.
+// C >= 2 (96, 144 and 240 bytes, LaneRows below) and the monotonic operator's output rows (56 and
+// 88 bytes, MonoRows below) were given widths that no arrangement row uses, and deliberately have
+// no RowT: mzgpu_buf_consolidate on them returns MZGPU_E_UNSUPPORTED instead of summing the wrong
+// words.
 
 // The compile-time values a runtime row width (or lane class) is dispatched over; each set is named
 // once here and every entry point instantiates its kernels for exactly the members of its set.
@@ -553,8 +567,8 @@ struct IntSet {
   static constexpr const char* kind = "row width";
   static constexpr bool has(int v) { return ((v == V) || ...); }
 };
-using RowWidths = IntSet<16, 32, 40, 64, 80, 128, 224, 416>;  // every RowT: sort, consolidate, fused
-using BatchWidths = IntSet<32, 64, 80, 128, 224, 416>;         // sorted batches: merge, extract, index
+using RowWidths = IntSet<16, 32, 40, 64, 80, 128, 224, 416, 48, 112>;  // every RowT: sort, consolidate, fused
+using BatchWidths = IntSet<32, 64, 80, 128, 224, 416, 48, 112>;         // sorted batches: merge, extract, index
 using ExchangeWidths = IntSet<32, 80>;
 struct LaneClasses : IntSet<1, 2, 4, 8> {  // accumulable reduce with 1, 2, 4 or 8 lanes (LaneRows below)
   static constexpr const char* kind = "lane class";
@@ -587,12 +601,32 @@ static inline int mz_lane_class(uint32_t n_lanes) { return n_lanes <= 1 ? 1 : (n
 static inline int mz_lane_arr_bytes(int c) { return c == 1 ? 80 : (c == 2 ? 128 : (c == 4 ? 224 : 416)); }
 static inline int mz_lane_out_bytes(int c) { return c == 1 ? 64 : (c == 2 ? 96 : (c == 4 ? 144 : 240)); }
 
-// Semigroup::plus_equals on the diff words.  ND >= 8 is the accumulable diff: word 0 is the
+// Monotonic MIN / MAX reduce (mzgpu_reduce_monotonic_new) with lane class C (4: 1-4 lanes, 8: 5-8
+// lanes): the arrangement row (RowT<48> / RowT<112>) and the output row (key, C values, time, diff).
+template <int C>
+struct MonoRows {
+  static constexpr int ARR_NW = C == 4 ? 6 : 14;
+  static constexpr int OUT_NW = C + 3;
+};
+struct MonoClasses : IntSet<4, 8> {
+  static constexpr const char* kind = "monotonic lane class";
+};
+static inline int mz_mono_class(uint32_t n_lanes) { return n_lanes <= 4 ? 4 : 8; }
+static inline int mz_mono_arr_bytes(int c) { return c == 4 ? 48 : 112; }
+static inline int mz_mono_out_bytes(int c) { return c == 4 ? 56 : 88; }
+
+// Semigroup::plus_equals on the diff words, by the row's semigroup SG.
+// MZ_SG_SUM: ND >= 8 is the accumulable diff: word 0 is the
 // total, lane l spans words 1+6l .. 6+6l, and its words 1,2 (acc_lo, acc_hi) form an i128
 // (src/compute/src/render/reduce.rs:1940-2041).  ND == 8 is one lane plus a pad word.
-template <int ND>
+// MZ_SG_MAX: the monotonic reduce's Vec<ReductionMonoid> (reduce.rs:2193-2233), every lane
+// encoded as an unsigned max (MonoRows): per-word max, zero the identity.
+template <int ND, int SG = MZ_SG_SUM>
 __host__ __device__ __forceinline__ void diff_add(u64* a, const u64* b) {
-  if (ND >= 8) {
+  if (SG == MZ_SG_MAX) {
+#pragma unroll
+    for (int w = 0; w < ND; ++w) a[w] = b[w] > a[w] ? b[w] : a[w];
+  } else if (ND >= 8) {
     a[0] += b[0];
 #pragma unroll
     for (int l = 0; l < (ND - 1) / 6; ++l) {
@@ -611,8 +645,10 @@ __host__ __device__ __forceinline__ void diff_add(u64* a, const u64* b) {
     a[0] += b[0];  // ND == 2 is (diff, pad): pad stays 0
   }
 }
-template <int ND>
+// IsZero: MZ_SG_MAX is never zero (reduce.rs:2235-2244), so a key stays once a row was accepted
+template <int ND, int SG = MZ_SG_SUM>
 __host__ __device__ __forceinline__ bool diff_is_zero(const u64* a) {
+  if (SG == MZ_SG_MAX) return false;
   if (ND == 8) return (a[0] | a[1] | a[2] | a[3] | a[4] | a[5] | a[6]) == 0;
   if (ND > 8) {
     u64 x = 0;
@@ -640,6 +676,13 @@ __device__ __forceinline__ void atomic_lanes_add(u64* __restrict__ acc, const u6
     if (y[4]) atomicAdd((unsigned long long*)&x[4], (unsigned long long)y[4]);
     if (y[5]) atomicAdd((unsigned long long*)&x[5], (unsigned long long)y[5]);
   }
+}
+// diff_add of MZ_SG_MAX rows by atomics (zero-initialised accumulators: zero is the identity)
+template <int ND>
+__device__ __forceinline__ void atomic_diff_max(u64* __restrict__ acc, const u64* d) {
+#pragma unroll
+  for (int w = 0; w < ND; ++w)
+    if (d[w]) atomicMax((unsigned long long*)&acc[w], (unsigned long long)d[w]);
 }
 #endif
 
@@ -1072,6 +1115,24 @@ int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_ro
 int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
                               int agg_kind, const LaneSet* ls, DevMem* out, u64* n_out,
                               const mzgpu_having* hv = nullptr);
+// the monotonic MIN / MAX reduce (mzgpu_reduce_monotonic_new): lane l's arrangement word is its value ^ xm[l]
+// (2^63 for a signed lane, then all ones for MIN), so every lane accumulates as an unsigned max
+struct MonoXor {
+  u64 xm[MZGPU_MAX_ACCUM_LANES];
+  u32 n;  // lanes in use; the class's other lanes stay zero
+};
+// rows with diff > 0 -> class-c arrangement rows at d_arr, every other row -> an R16 (time, +1) row at
+// d_errs; their counts are left in d_cnt[0] and d_cnt[1] (two words of a counter block, zeroed here)
+int32_t mz_monotonic_explode(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
+                             const MonoXor& mx, u64* d_arr, u64* d_errs, u64* d_cnt);
+// the R32 / R40 rows with value word 1 masked by m1 and word 2 (R40) by m2
+int32_t mz_monotonic_mask(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, u32 in_words, u64 m1, u64 m2,
+                          u64* d_out);
+int32_t mz_monotonic_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, DLen n, u64 n_ub,
+                                       const TraceView& prior, const MonoXor& mx, u64* d_out, u64 out_cap,
+                                       u64* d_out_len);
+int32_t mz_monotonic_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
+                                 const MonoXor& mx, DevMem* out, u64* n_out);
 
 // correction.cu (time-major rows: (time, key, val | diff))
 // column.cu (columnar wire format, f4)

@@ -42,9 +42,11 @@ __global__ void __launch_bounds__(CT) k_heads(const u64* __restrict__ rows, u64 
   if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
 }
 
-template <int ND>
+template <int ND, int SG>
 __device__ __forceinline__ void atomic_diff_add(u64* __restrict__ acc, const u64* d) {
-  if (ND == 8) {
+  if (SG == MZ_SG_MAX) {
+    atomic_diff_max<ND>(acc, d);
+  } else if (ND == 8) {
     if (d[0]) atomicAdd((unsigned long long*)&acc[0], (unsigned long long)d[0]);
     if (d[1]) atomicAdd((unsigned long long*)&acc[1], (unsigned long long)d[1]);
     // 128-bit add: the atomic that wraps the low word carries into the high word
@@ -67,6 +69,7 @@ __global__ void __launch_bounds__(CT) k_segsum(const u64* __restrict__ rows, u64
                                                const u32* __restrict__ tile_base,
                                                u64* __restrict__ seg_sums,
                                                u32* __restrict__ seg_first) {
+  constexpr int SG = RowT<NW * 8>::SG;
   __shared__ u32 sm[34];
   const u64 i = (u64)blockIdx.x * CT + threadIdx.x;
   const u32 lane = lane_id();
@@ -88,14 +91,14 @@ __global__ void __launch_bounds__(CT) k_segsum(const u64* __restrict__ rows, u64
     u64 o[ND];
 #pragma unroll
     for (int w = 0; w < ND; ++w) o[w] = __shfl_up_sync(0xffffffffu, d[w], off);
-    if (lane >= (u32)off && oseg == seg) diff_add<ND>(d, o);
+    if (lane >= (u32)off && oseg == seg) diff_add<ND, SG>(d, o);
   }
   u32 nseg = __shfl_down_sync(0xffffffffu, seg, 1);
   bool tail = valid && (lane == 31 || nseg != seg);
-  if (tail) atomic_diff_add<ND>(seg_sums + (u64)seg * ND, d);
+  if (tail) atomic_diff_add<ND, SG>(seg_sums + (u64)seg * ND, d);
 }
 
-template <int ND>
+template <int ND, int SG>
 __global__ void __launch_bounds__(CT) k_nz(const u64* __restrict__ seg_sums,
                                            const u64* __restrict__ n_seg_ptr,
                                            u32* __restrict__ tile_counts) {
@@ -103,7 +106,7 @@ __global__ void __launch_bounds__(CT) k_nz(const u64* __restrict__ seg_sums,
   const u64 S = *n_seg_ptr;
   u64 s = (u64)blockIdx.x * CT + threadIdx.x;
   u32 flag = 0;
-  if (s < S) flag = diff_is_zero<ND>(seg_sums + s * ND) ? 0u : 1u;
+  if (s < S) flag = diff_is_zero<ND, SG>(seg_sums + s * ND) ? 0u : 1u;
   u32 total;
   block_exclusive_scan(flag, sm, &total);
   if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
@@ -116,11 +119,12 @@ __global__ void __launch_bounds__(CT) k_emit(const u64* __restrict__ rows,
                                              const u64* __restrict__ n_seg_ptr,
                                              const u32* __restrict__ tile_base,
                                              u64* __restrict__ out) {
+  constexpr int SG = RowT<NW * 8>::SG;
   __shared__ u32 sm[34];
   const u64 S = *n_seg_ptr;
   u64 s = (u64)blockIdx.x * CT + threadIdx.x;
   u32 flag = 0;
-  if (s < S) flag = diff_is_zero<ND>(seg_sums + s * ND) ? 0u : 1u;
+  if (s < S) flag = diff_is_zero<ND, SG>(seg_sums + s * ND) ? 0u : 1u;
   u32 total;
   u32 ex = block_exclusive_scan(flag, sm, &total);
   if (flag) {
@@ -163,7 +167,7 @@ int32_t consolidate_sorted_t(mzgpu_ctx* ctx, const u64* rows, u64 n, u64* out, u
   MZ_BYTES(ctx, n * (NW * 8 + 4));
   MZ_LAUNCH(ctx, (k_segsum<NW, NK, ND>), (unsigned)n_tiles, CT, 0, rows, n, tiles.as<u32>(),
             seg_sums.as<u64>(), seg_first.as<u32>());
-  MZ_LAUNCH(ctx, (k_nz<ND>), (unsigned)n_tiles, CT, 0, seg_sums.as<u64>(), d_nseg, tiles.as<u32>());
+  MZ_LAUNCH(ctx, (k_nz<ND, RowT<RB>::SG>), (unsigned)n_tiles, CT, 0, seg_sums.as<u64>(), d_nseg, tiles.as<u32>());
   MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_nout);
   MZ_LAUNCH(ctx, (k_emit<NW, NK, ND>), (unsigned)n_tiles, CT, 0, rows, seg_sums.as<u64>(),
             seg_first.as<u32>(), d_nseg, tiles.as<u32>(), out);

@@ -175,6 +175,7 @@ __device__ __forceinline__ void msd_warp_buckets(const FusedArgs& a, FusedCtl* c
                                                  u32 G, u64 na, u64 since, u64* s_cnt /* 8 + 1 words */,
                                                  u64* s_lb) {
   constexpr int NW = RowT<RB>::NW, NK = RowT<RB>::NK, ND = RowT<RB>::ND, TW = RowT<RB>::TW;
+  constexpr int SG = RowT<RB>::SG;
   const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const u64 upper = a.upper;
   LookBack lbs;
@@ -294,9 +295,9 @@ __device__ __forceinline__ void msd_warp_buckets(const FusedArgs& a, FusedCtl* c
         u64 o[ND];
 #pragma unroll
         for (int w = 0; w < ND; ++w) o[w] = __shfl_up_sync(0xffffffffu, d[r][w], off);
-        if ((int)lane - off >= start_eff) diff_add<ND>(d[r], o);
+        if ((int)lane - off >= start_eff) diff_add<ND, SG>(d[r], o);
       }
-      if (my_start < 0) diff_add<ND>(d[r], carry);  // my segment started in an earlier row
+      if (my_start < 0) diff_add<ND, SG>(d[r], carry);  // my segment started in an earlier row
 #pragma unroll
       for (int w = 0; w < ND; ++w) carry[w] = __shfl_sync(0xffffffffu, d[r][w], 31);
     }
@@ -316,7 +317,7 @@ __device__ __forceinline__ void msd_warp_buckets(const FusedArgs& a, FusedCtl* c
       }
       const bool tail = p < m && (p == m - 1 || nhead);
       cls[r] = 0;
-      if (tail && !diff_is_zero<ND>(d[r]))
+      if (tail && !diff_is_zero<ND, SG>(d[r]))
         cls[r] = (TW < 0 || upper == MZGPU_FRONTIER_EMPTY || tt[r] < upper) ? 1u : 2u;
       const u32 ms = __ballot_sync(0xffffffffu, cls[r] == 1u), mk = __ballot_sync(0xffffffffu, cls[r] == 2u);
       const u32 lt = (1u << lane) - 1;
@@ -376,6 +377,7 @@ __device__ __forceinline__ void msd_warp_buckets2(const FusedArgs& a, FusedCtl* 
                                                   u64 since, u64 mask, bool inline_index, u64* s_cnt, u64* s_lb,
                                                   u64* s_keys /* [FT/32][32*R] */, u32* s_stat /* [2] */) {
   constexpr int NW = RowT<RB>::NW, NK = RowT<RB>::NK, ND = RowT<RB>::ND, TW = RowT<RB>::TW;
+  constexpr int SG = RowT<RB>::SG;
   constexpr u32 CAP = 32u * R;
   const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const u64 upper = a.upper;
@@ -513,9 +515,9 @@ __device__ __forceinline__ void msd_warp_buckets2(const FusedArgs& a, FusedCtl* 
         u64 o[ND];
 #pragma unroll
         for (int w = 0; w < ND; ++w) o[w] = __shfl_up_sync(0xffffffffu, d[r][w], off);
-        if ((int)lane - off >= start_eff) diff_add<ND>(d[r], o);
+        if ((int)lane - off >= start_eff) diff_add<ND, SG>(d[r], o);
       }
-      if (my_start < 0) diff_add<ND>(d[r], carry);
+      if (my_start < 0) diff_add<ND, SG>(d[r], carry);
 #pragma unroll
       for (int w = 0; w < ND; ++w) carry[w] = __shfl_sync(0xffffffffu, d[r][w], 31);
     }
@@ -535,7 +537,7 @@ __device__ __forceinline__ void msd_warp_buckets2(const FusedArgs& a, FusedCtl* 
       }
       const bool tail = p < m && (p == m - 1 || nhead);
       cls[r] = 0;
-      if (tail && !diff_is_zero<ND>(d[r]))
+      if (tail && !diff_is_zero<ND, SG>(d[r]))
         cls[r] = (TW < 0 || upper == MZGPU_FRONTIER_EMPTY || tt[r] < upper) ? 1u : 2u;
       const u32 ms = __ballot_sync(0xffffffffu, cls[r] == 1u), mk = __ballot_sync(0xffffffffu, cls[r] == 2u);
       const u32 lt = (1u << lane) - 1;
@@ -640,6 +642,7 @@ union FusedSmem {
 template <int RB>
 __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, const u32 gdim) {
   constexpr int NW = RowT<RB>::NW, NK = RowT<RB>::NK, ND = RowT<RB>::ND, TW = RowT<RB>::TW;
+  constexpr int SG = RowT<RB>::SG;
   __shared__ FusedSmem sm;
   __shared__ u32 sm_scan[34];
   __shared__ int s_nwords, s_nrounds, s_word[6], s_shift[6], s_round[6], s_rbits[MAX_ROUNDS];
@@ -956,7 +959,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
     const u32 NU = (NB + 7) / 8;
     constexpr u32 LOCAL_MAX = ND == 8 ? 256u : MSD_LOCAL_MAX;
     if (a.dbg != nullptr && c == 0 && tid == 0) {
-      a.dbg[21] = s_max_bucket <= WCAP ? 1 : (ND <= 8 && s_max_unit <= LOCAL_MAX ? 2 : 3);
+      a.dbg[21] = s_max_bucket <= WCAP ? 1 : (ND <= 8 && SG == MZ_SG_SUM && s_max_unit <= LOCAL_MAX ? 2 : 3);
       a.dbg[22] = s_max_bucket;
       a.dbg[23] = NB;
     }
@@ -976,7 +979,8 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
       __shared__ u64 s_wlb;
       msd_warp_buckets<RB, WR>(a, ctl, sm.scan.base, NB, c, G, na, since, s_wcnt, &s_wlb);
       msd_done = true;
-    } else if (ND <= 8 && s_max_unit <= LOCAL_MAX) {  // (its shared sums hold at most 8 diff words)
+    } else if (ND <= 8 && SG == MZ_SG_SUM && s_max_unit <= LOCAL_MAX) {  // (its shared sums hold at most 8
+      // summed diff words; monotonic rows take the LSD path, as the wide accumulable rows do)
       for (u64 i = gtid; i < n; i += gstride) {
         const u64 p = (u64)sm.scan.base[a.v1[i]] + a.v0[i];
         a.m_lo[p] = a.k0[i];
@@ -1078,7 +1082,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
             u64 o[ND];
 #pragma unroll
             for (int w = 0; w < ND; ++w) o[w] = __shfl_up_sync(0xffffffffu, d[w], off);
-            if (lane >= (u32)off && oseg == seg) diff_add<ND>(d, o);
+            if (lane >= (u32)off && oseg == seg) diff_add<ND, SG>(d, o);
           }
           const u32 nxt = __shfl_down_sync(0xffffffffu, seg, 1);
           if (valid && (lane == 31 || nxt != seg)) {
@@ -1126,7 +1130,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
 #pragma unroll
                 for (int w = 1; w < ND; ++w) d[w] = 0;
               }
-              if (!diff_is_zero<ND>(d)) {
+              if (!diff_is_zero<ND, SG>(d)) {
                 load_in(sm.msd.idx[j], r);
 #pragma unroll
                 for (int w = 0; w < ND; ++w) r[NK + w] = d[w];
@@ -1397,12 +1401,14 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
       u64 o[ND];
 #pragma unroll
       for (int w = 0; w < ND; ++w) o[w] = __shfl_up_sync(0xffffffffu, d[w], off);
-      if (lane >= (u32)off && oseg == seg) diff_add<ND>(d, o);
+      if (lane >= (u32)off && oseg == seg) diff_add<ND, SG>(d, o);
     }
     u32 nseg = __shfl_down_sync(0xffffffffu, seg, 1);
     if (valid && (lane == 31 || nseg != seg)) {
       u64* acc = a.seg_sums + (u64)seg * ND;
-      if (ND == 8) {
+      if (SG == MZ_SG_MAX) {
+        atomic_diff_max<ND>(acc, d);
+      } else if (ND == 8) {
         if (d[0]) atomicAdd((unsigned long long*)&acc[0], (unsigned long long)d[0]);
         if (d[1]) atomicAdd((unsigned long long*)&acc[1], (unsigned long long)d[1]);
         u64 old = atomicAdd((unsigned long long*)&acc[2], (unsigned long long)d[2]);
@@ -1429,7 +1435,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
   auto seg_class = [&](u64 s, u64* d) -> u32 {  // 0 dropped, 1 ship, 2 keep
 #pragma unroll
     for (int w = 0; w < ND; ++w) d[w] = *(volatile u64*)&a.seg_sums[s * ND + w];
-    if (diff_is_zero<ND>(d)) return 0u;
+    if (diff_is_zero<ND, SG>(d)) return 0u;
     if (TW < 0 || upper == MZGPU_FRONTIER_EMPTY) return 1u;
     const u64 t = a.sorted[(u64)a.seg_first[s] * NW + (TW >= 0 ? TW : 0)];
     return t < upper ? 1u : 2u;

@@ -419,11 +419,13 @@ static int32_t validate_closure(mzgpu_ctx* ctx, const mzgpu_closure* c) {
   return MZGPU_OK;
 }
 
-// arrangement rows: every sorted-batch width but the reduce's 64-byte output rows, i.e. R32 and the
-// accumulable rows of every lane class (RACC = class 1)
+// arrangement rows: every sorted-batch width but the reduce's 64-byte output rows, i.e. R32, the
+// accumulable rows of every lane class (RACC = class 1) and the monotonic reduce's rows
 static bool arrangement_row_bytes(uint32_t rb) { return rb != 64 && BatchWidths::has((int)rb); }
-// buffer rows: every RowT width, and the wide output rows of the lanes reduce (they have no RowT)
-static bool valid_row_bytes(uint32_t rb) { return RowWidths::has((int)rb) || rb == 96 || rb == 144 || rb == 240; }
+// buffer rows: every RowT width, and the output rows of the lanes and monotonic reduces (they have no RowT)
+static bool valid_row_bytes(uint32_t rb) {
+  return RowWidths::has((int)rb) || rb == 96 || rb == 144 || rb == 240 || rb == 56 || rb == 88;
+}
 
 // ------------------------------------------------------ device-side append
 // dst[base ...] = src[0 .. n), new length left in *out_len; every size may live
@@ -2518,6 +2520,12 @@ struct mzgpu_reduce {
   // mzgpu_reduce_lanes_new_having: the validated HAVING program, run by the corrections kernels
   bool has_having = false;
   mzgpu_having having = {};
+  // mzgpu_reduce_monotonic_new: lane class (4, 8; 0 for every other operator), the lanes' encodings, and
+  // consolidate_named_if's flag with the value bits the lanes read
+  int mono_class = 0;
+  MonoXor mono = {};
+  bool must_consolidate = false;
+  u64 mono_mask[2] = {0, 0};
   int32_t failed = MZGPU_OK;  // set when an activation failed after its seal (reduce_dev)
   std::string failed_msg;
   ~mzgpu_reduce() {
@@ -2776,7 +2784,8 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
 
 extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_t n,
                                             int32_t mem, uint64_t upper, mzgpu_buf* out) {
-  if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->lane_class) return MZGPU_E_INVALID;
+  if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->lane_class || r->mono_class)
+    return MZGPU_E_INVALID;
   mzgpu_ctx* ctx = r->ctx;
   MZ_CHECK_CTX(ctx);
   ctx->stats.rows_in += n;
@@ -2791,7 +2800,8 @@ extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* ro
 }
 extern "C" int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
                                                 mzgpu_buf* out) {
-  if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64 || r->lane_class)
+  if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64 || r->lane_class ||
+      r->mono_class)
     return MZGPU_E_INVALID;
   MZ_CHECK_CTX(r->ctx);
   r->ctx->stats.rows_in += rows->ub;
@@ -3024,6 +3034,196 @@ extern "C" int32_t mzgpu_reduce_lanes_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint
   }
   r->ctx->stats.rows_in += rows->ub;
   return reduce_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out);
+}
+
+// ------------------------------------------------------- monotonic MIN / MAX reduce
+extern "C" int32_t mzgpu_reduce_monotonic_row_bytes(uint32_t n_lanes, uint32_t* arr_row_bytes,
+                                                    uint32_t* out_row_bytes) {
+  if (n_lanes == 0 || n_lanes > MZGPU_MAX_ACCUM_LANES) return MZGPU_E_INVALID;
+  const int c = mz_mono_class(n_lanes);
+  if (arr_row_bytes != nullptr) *arr_row_bytes = (uint32_t)mz_mono_arr_bytes(c);
+  if (out_row_bytes != nullptr) *out_row_bytes = (uint32_t)mz_mono_out_bytes(c);
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_reduce_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                                              uint32_t n_lanes, int32_t must_consolidate, mzgpu_reduce** out) {
+  MZ_CHECK_CTX(ctx);
+  if (out == nullptr || (lanes == nullptr && n_lanes) || (in_row_bytes != 32 && in_row_bytes != 40)) {
+    MZ_SET_ERR(ctx, "reduce_monotonic: bad arguments (input rows of %u bytes)", in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  if (n_lanes == 0 || n_lanes > MZGPU_MAX_ACCUM_LANES) {
+    MZ_SET_ERR(ctx, "reduce_monotonic: %u lanes (1..%d)", n_lanes, MZGPU_MAX_ACCUM_LANES);
+    return MZGPU_E_INVALID;
+  }
+  LaneSet ls = {};
+  MonoXor mx = {};
+  u64 mask[2] = {0, 0};
+  int unsupported = -1;  // the first float64 lane, reported once every lane is known to be well-formed
+  for (uint32_t l = 0; l < n_lanes; ++l) {
+    const mzgpu_accum_lane& L = lanes[l];
+    const mzgpu_field& f = L.field;
+    const int32_t base = L.kind & ~MZGPU_MONO_F64;
+    const char* bad = nullptr;
+    if (base != MZGPU_AGG_MIN && base != MZGPU_AGG_MAX)
+      bad = "kind is not MZGPU_AGG_MIN / MZGPU_AGG_MAX, optionally | MZGPU_MONO_F64";
+    else if (f.src != MZGPU_SRC_VAL1 && !(f.src == MZGPU_SRC_VAL2 && in_row_bytes == 40))
+      bad = "source word is not a value word of the input row";
+    else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
+      bad = "field is empty or out of range";
+    if (bad != nullptr) {
+      MZ_SET_ERR(ctx, "reduce_monotonic: lane %u: %s", l, bad);
+      return MZGPU_E_INVALID;
+    }
+    if ((L.kind & MZGPU_MONO_F64) != 0 && unsupported < 0) unsupported = (int)l;
+    ls.lane[l] = L;
+    mx.xm[l] = (L.sign_extend ? 1ull << 63 : 0) ^ (base == MZGPU_AGG_MIN ? ~0ull : 0);
+    mask[f.src == MZGPU_SRC_VAL2 ? 1 : 0] |= (f.bits == 64 ? ~0ull : ((1ull << f.bits) - 1)) << f.shift;
+  }
+  if (unsupported >= 0) {
+    MZ_SET_ERR(ctx, "reduce_monotonic: lane %d: float64 MIN / MAX is not supported (OrderedFloat ties -0.0 with "
+                    "+0.0 and NaN payloads, so the surviving bits would depend on arrival order)", unsupported);
+    return MZGPU_E_UNSUPPORTED;
+  }
+  ls.n = n_lanes;
+  ls.in_words = in_row_bytes / 8;
+  mx.n = n_lanes;
+  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
+  r->ctx = ctx;
+  r->agg_kind = -1;
+  r->mono_class = mz_mono_class(n_lanes);
+  r->lanes = ls;
+  r->mono = mx;
+  r->must_consolidate = must_consolidate != 0;
+  r->mono_mask[0] = mask[0];
+  r->mono_mask[1] = mask[1];
+  const uint32_t rb = (uint32_t)mz_mono_arr_bytes(r->mono_class);
+  MZ_TRY(mzgpu_batcher_new(ctx, rb, &r->batcher));
+  MZ_TRY(mzgpu_spine_new(ctx, rb, 1, &r->input));
+  *out = r.release();
+  return MZGPU_OK;
+}
+
+// One activation of build_monotonic: [consolidate ->] ensure_monotonic + explode -> arrange -> corrections.
+static int32_t monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                             mzgpu_buf* errs) {
+  mzgpu_ctx* ctx = r->ctx;
+  if (r->failed != MZGPU_OK) {
+    ctx->last_error = r->failed_msg;
+    return r->failed;
+  }
+  MZ_TRY(mzgpu_spine_set_physical_compaction(r->input, r->input->upper));
+  const int c = r->mono_class;
+  if (n_ub) {
+    const u32 iw = r->lanes.in_words;
+    DevMem masked, cons;
+    Lazy4 clen;
+    if (r->must_consolidate) {
+      // consolidate_named_if: rows that agree on (key, lane values, time) fold, a +1 / -1 pair vanishes
+      u64 ccap = 0;
+      MZ_TRY(masked.alloc(ctx, n_ub * iw * 8));
+      MZ_TRY(mz_monotonic_mask(ctx, d_rows, n, n_ub, iw, r->mono_mask[0], r->mono_mask[1], masked.as<u64>()));
+      MZ_TRY(consolidate_dev(ctx, (int)iw * 8, masked.p, n, n_ub, &cons, &ccap, &clen));
+      d_rows = cons.as<u64>();
+      n = dlen_of(clen, 0);
+      if (clen.known) n_ub = clen.v[0];
+    }
+    Seg s;
+    DevMem erows, econs;
+    Lazy4 elen;
+    u64 ecap = 0;
+    MZ_TRY(s.rows.alloc(ctx, n_ub * mz_mono_arr_bytes(c)));
+    MZ_TRY(erows.alloc(ctx, n_ub * 16));
+    MZ_TRY(s.len.make_pending(ctx));
+    MZ_TRY(mz_monotonic_explode(ctx, c, d_rows, n, n_ub, r->lanes, r->mono, s.rows.as<u64>(), erows.as<u64>(),
+                                s.len.dptr()));
+    s.len.mark_written();
+    s.ub = n_ub;
+    // the rejected rows' error collection: (time, number of rejected rows)
+    MZ_TRY(consolidate_dev(ctx, 16, erows.p, dlen_of(s.len, 1), n_ub, &econs, &ecap, &elen));
+    MZ_TRY(buf_append_dev(errs, econs.p, dlen_of(elen, 0), elen.known ? elen.v[0] : n_ub));
+    MZ_TRY(batcher_push_seg(r->batcher, std::move(s)));
+  }
+  mzgpu_batch* batch = nullptr;
+  MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
+  std::vector<mzgpu_batch*> prior;
+  r->input->all_batches(prior);
+  TraceView tv;
+  int32_t st = trace_view(ctx, prior, &tv);
+  const u64 b_ub = batch->len_ub;
+  const u64 out_rb = (u64)mz_mono_out_bytes(c);
+  if (st == MZGPU_OK && b_ub > 0) {
+    if ((b_ub + 255) / 256 <= MZ_LB_TILES && 2 * b_ub <= MZ_BOUND_MAX_ROWS) {
+      DevMem corr;
+      Lazy4 clen;
+      st = corr.alloc(ctx, 2 * b_ub * out_rb);
+      if (st == MZGPU_OK) st = clen.make_pending(ctx);
+      if (st == MZGPU_OK) {
+        st = mz_monotonic_corrections_async(ctx, c, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv, r->mono,
+                                            corr.as<u64>(), 2 * b_ub, clen.dptr());
+        clen.mark_written();
+      }
+      // consolidated by construction: keys ascending, each key's rows sorted by its thread
+      if (st == MZGPU_OK) st = buf_append_dev(out, corr.p, dlen_of(clen, 0), 2 * b_ub);
+    } else {
+      DevMem corr;
+      u64 n_corr = 0;
+      st = batch_resolve(batch);
+      if (st == MZGPU_OK)
+        st = mz_monotonic_corrections(ctx, c, batch->rows.as<u64>(), batch->st.v[0], tv, r->mono, &corr, &n_corr);
+      if (st == MZGPU_OK && n_corr) st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
+    }
+  }
+  // as in reduce_main: the sealed batch joins the trace whatever happened, and a failure after the seal
+  // kills the operator
+  int32_t ins = MZGPU_OK;
+  if (batch->desc.lower != batch->desc.upper) ins = mzgpu_spine_insert(r->input, batch);
+  mzgpu_batch_release(batch);
+  if (st == MZGPU_OK) st = ins;
+  if (st != MZGPU_OK && !ctx->sticky) {
+    r->failed = st;
+    r->failed_msg = ctx->last_error;
+  }
+  return st;
+}
+
+static bool monotonic_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
+  return r->mono_class != 0 && in_rb == r->lanes.in_words * 8 && out->rb == (uint32_t)mz_mono_out_bytes(r->mono_class) &&
+         errs->rb == 16 && out != errs;
+}
+extern "C" int32_t mzgpu_reduce_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                          mzgpu_buf* out, mzgpu_buf* errs) {
+  if (r == nullptr || out == nullptr || errs == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = r->ctx;
+  MZ_CHECK_CTX(ctx);
+  const uint32_t in_rb = r->lanes.in_words * 8;
+  if (!monotonic_io_ok(r, in_rb, out, errs)) {
+    MZ_SET_ERR(ctx, "reduce_monotonic: output buffer of %u-byte rows / error buffer of %u-byte rows", out->rb,
+               errs->rb);
+    return MZGPU_E_INVALID;
+  }
+  ctx->stats.rows_in += n;
+  DevMem in;
+  const u64* d_rows = (const u64*)rows;
+  if (mem == MZGPU_MEM_HOST && n) {
+    MZ_TRY(in.alloc(ctx, n * in_rb));
+    MZ_TRY(copy_in(ctx, in.p, rows, n * in_rb, mem));
+    d_rows = in.as<u64>();
+  }
+  return monotonic_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
+}
+extern "C" int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                              mzgpu_buf* errs) {
+  if (r == nullptr || rows == nullptr || out == nullptr || errs == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(r->ctx);
+  if (!monotonic_io_ok(r, rows->rb, out, errs)) {
+    MZ_SET_ERR(r->ctx, "reduce_monotonic: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes",
+               rows->rb, out->rb, errs->rb);
+    return MZGPU_E_INVALID;
+  }
+  r->ctx->stats.rows_in += rows->ub;
+  return monotonic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
 }
 
 // ============================================================ Row keys as words (f1, first step)

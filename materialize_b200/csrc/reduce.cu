@@ -494,9 +494,10 @@ __device__ __forceinline__ void prior_sum(const TraceView& tv, u64 key, u64* S) 
 // the time word), and keys are written in ascending order by construction, so with this the
 // kernel's whole output is already what consolidate() would return: the separate sort launch
 // (40 us for a few hundred rows) is gone.
-template <int C>
-__device__ __forceinline__ void sort_key_corrections(u64* __restrict__ out, u64 pos, u32 c) {
-  constexpr int OW = LaneRows<C>::OUT_NW, TWO = LaneRows<C>::OUT_TW;
+// Rows out[pos .. pos + c) of OW words sorted by their words 1 .. TWO (insertion sort: a key has a
+// handful of corrections).
+template <int OW, int TWO>
+__device__ __forceinline__ void sort_run_rows(u64* __restrict__ out, u64 pos, u32 c) {
   for (u32 x = 1; x < c; ++x) {
     u64 r[OW];
     load_row<OW>(out, pos + x, r);
@@ -518,6 +519,10 @@ __device__ __forceinline__ void sort_key_corrections(u64* __restrict__ out, u64 
     }
     if (y != x) store_row<OW>(out, pos + y, r);
   }
+}
+template <int C>
+__device__ __forceinline__ void sort_key_corrections(u64* __restrict__ out, u64 pos, u32 c) {
+  sort_run_rows<LaneRows<C>::OUT_NW, LaneRows<C>::OUT_TW>(out, pos, c);
 }
 
 // output row (key, finalized aggregates, time, diff, zero padding)
@@ -1438,6 +1443,230 @@ __global__ void __launch_bounds__(RT) k_distinct_presence(const __grid_constant_
   }
 }
 
+// ------------------------------------------------------------ monotonic MIN / MAX
+// build_monotonic (reduce.rs:1138-1253) for append-only inputs: ensure_monotonic keeps a row iff its diff is
+// positive (src/timely-util/src/operator.rs:425-456), the kept row's values move into the diff as one
+// Min / Max monoid per aggregate, and the arrangement accumulates them (RowT<48> / RowT<112>, MZ_SG_MAX).
+// Lane word = value ^ xm[l] (MonoXor): a max of the lane words is the lane's MIN or MAX, and the same xor
+// decodes it.
+
+// Input rows -> one arrangement row per row with diff > 0 (at arr[cnt[0]++]) and one R16 (time, +1) row per
+// other row (at errs[cnt[1]++]); warp-aggregated slots, so the order within each output is arbitrary (the
+// seal sorts the one, the error consolidation the other).
+template <int C>
+__global__ void __launch_bounds__(RT) k_monotonic_explode(const u64* __restrict__ rows, const DLen dn,
+                                                          const __grid_constant__ LaneSet ls, const MonoXor mx,
+                                                          u64* __restrict__ arr, u64* __restrict__ errs,
+                                                          unsigned long long* __restrict__ cnt) {
+  constexpr int NW = MonoRows<C>::ARR_NW;
+  const u64 n = dlen_get(dn);
+  const u32 iw = ls.in_words, lane = lane_id();
+  for (u64 base = (u64)blockIdx.x * RT; base < n; base += (u64)gridDim.x * RT) {
+    const u64 i = base + threadIdx.x;
+    const bool valid = i < n;
+    const u64* r = rows + (valid ? i : 0) * iw;
+    const i64 diff = valid ? (i64)r[iw - 1] : 0;
+    const bool ok = valid && diff > 0, bad = valid && diff <= 0;
+    const u32 mok = __ballot_sync(0xffffffffu, ok), mbad = __ballot_sync(0xffffffffu, bad);
+    unsigned long long bok = 0, bbad = 0;
+    if (lane == 0) {
+      if (mok) bok = atomicAdd(&cnt[0], (unsigned long long)__popc(mok));
+      if (mbad) bbad = atomicAdd(&cnt[1], (unsigned long long)__popc(mbad));
+    }
+    bok = __shfl_sync(0xffffffffu, bok, 0);
+    bbad = __shfl_sync(0xffffffffu, bbad, 0);
+    const u32 lt = (1u << lane) - 1;
+    if (ok) {
+      const u64 key = r[0], v1 = r[1], v2 = iw == 5 ? r[2] : 0;
+      u64 o[NW];
+      o[0] = key;
+      o[1] = r[iw - 2];
+#pragma unroll
+      for (int l = 0; l < C; ++l)
+        o[2 + l] = (u32)l < ls.n ? lane_value(ls.lane[l], key, v1, v2) ^ mx.xm[l] : 0;
+#pragma unroll
+      for (int w = 2 + C; w < NW; ++w) o[w] = 0;
+      store_row<NW>(arr, bok + __popc(mok & lt), o);
+    }
+    if (bad) {
+      const u64 e[2] = {r[iw - 2], 1};
+      store_row<2>(errs, bbad + __popc(mbad & lt), e);
+    }
+  }
+}
+
+// consolidate_named_if's data: the input rows with every value bit no lane reads cleared
+__global__ void __launch_bounds__(RT) k_monotonic_mask(const u64* __restrict__ rows, const DLen dn, u32 iw, u64 m1,
+                                                       u64 m2, u64* __restrict__ out) {
+  const u64 n = dlen_get(dn);
+  for (u64 i = (u64)blockIdx.x * RT + threadIdx.x; i < n; i += (u64)gridDim.x * RT) {
+    const u64* r = rows + i * iw;
+    u64* o = out + i * iw;
+    for (u32 w = 0; w < iw; ++w) o[w] = r[w];
+    o[1] &= m1;
+    if (iw == 5) o[2] &= m2;
+  }
+}
+
+// The key's accumulated lane words over the prior batches (max over its runs, one hash probe per batch);
+// false if no batch holds the key.
+template <int C>
+__device__ __forceinline__ bool mono_prior(const TraceView& tv, u64 key, u64* S) {
+  constexpr int NW = MonoRows<C>::ARR_NW, ND = NW - 2;
+  const u64 h0 = mix64(key);
+  bool found = false;
+  for (u32 b = 0; b < tv.n_batches; ++b) {
+    const BatchView& bv = tv.b[b];
+    const u64 mask = bv_mask(bv);
+    u64 h = h0 & mask;
+    while (true) {
+      const ulonglong2 sl = *reinterpret_cast<const ulonglong2*>(&bv.table[h]);
+      if (sl.y == 0) break;
+      if (sl.x == key) {
+        const u64 first = (sl.y & MZ_SLOT_ROW_MASK) - 1;
+        const u32 len = (u32)(sl.y >> 44);
+        const u64 bn = len != 0 ? first + len : bv_n(bv);
+        for (u64 r = first; r < bn; ++r) {
+          const u64* row = bv.rows + r * NW;
+          if (len == 0 && row[0] != key) break;
+          diff_add<ND, MZ_SG_MAX>(S, row + 2);
+          found = true;
+        }
+        break;
+      }
+      h = (h + 1) & mask;
+    }
+  }
+  return found;
+}
+
+// output row (key, C decoded values, time, diff)
+template <int C>
+__device__ __forceinline__ void put_mono_row(u64* __restrict__ out, u64 at, u64 key, const u64* S, const MonoXor& mx,
+                                             u64 t, u64 diff) {
+  u64 r[MonoRows<C>::OUT_NW];
+  r[0] = key;
+#pragma unroll
+  for (int l = 0; l < C; ++l) r[1 + l] = (u32)l < mx.n ? S[l] ^ mx.xm[l] : 0;
+  r[1 + C] = t;
+  r[2 + C] = diff;
+  store_row<MonoRows<C>::OUT_NW>(out, at, r);
+}
+
+// The key's rows [i, ...) of the new batch in time order on top of its prior accumulation S0 (had: the key
+// was in the arrangement): (-old, +new) whenever the accumulated lane words change, +new alone for the
+// key's first row.  Returns the count; writes at out[pos ...], sorted, if do_write.
+template <int C>
+__device__ __forceinline__ u32 mono_walk(const u64* __restrict__ rows, u64 n, u64 i, u64 key, const u64* S0, bool had,
+                                         const MonoXor& mx, bool do_write, u64* __restrict__ out, u64 pos) {
+  constexpr int NW = MonoRows<C>::ARR_NW, ND = NW - 2;
+  u64 S[ND];
+#pragma unroll
+  for (int w = 0; w < ND; ++w) S[w] = S0[w];
+  u32 c = 0;
+  for (u64 j = i; j < n; ++j) {
+    const u64* row = rows + j * NW;
+    if (row[0] != key) break;
+    u64 T[ND];
+#pragma unroll
+    for (int w = 0; w < ND; ++w) T[w] = S[w];
+    diff_add<ND, MZ_SG_MAX>(T, row + 2);
+    bool same = had;
+#pragma unroll
+    for (int w = 0; w < ND; ++w) same = same && T[w] == S[w];
+    if (!same) {
+      if (had) {
+        if (do_write) put_mono_row<C>(out, pos + c, key, S, mx, row[1], ~0ull);
+        ++c;
+      }
+      if (do_write) put_mono_row<C>(out, pos + c, key, T, mx, row[1], 1);
+      ++c;
+    }
+    had = true;
+#pragma unroll
+    for (int w = 0; w < ND; ++w) S[w] = T[w];
+  }
+  if (do_write && c > 1) sort_run_rows<MonoRows<C>::OUT_NW, C + 1>(out, pos, c);
+  return c;
+}
+
+// the two-pass form (count, read back, write) for a batch past the single-pass bound
+template <int C, bool WRITE>
+__global__ void __launch_bounds__(RT) k_monotonic_corrections(const u64* __restrict__ rows, u64 n,
+                                                              const __grid_constant__ TraceView prior, const MonoXor mx,
+                                                              u32* __restrict__ tile_counts,
+                                                              const u32* __restrict__ tile_base,
+                                                              u64* __restrict__ out) {
+  constexpr int NW = MonoRows<C>::ARR_NW, ND = NW - 2;
+  __shared__ u32 sm[34];
+  const u64 i = (u64)blockIdx.x * RT + threadIdx.x;
+  u32 cnt = 0;
+  const bool head = i < n && (i == 0 || rows[(i - 1) * NW] != rows[i * NW]);
+  u64 key = 0;
+  u64 S0[ND];
+#pragma unroll
+  for (int w = 0; w < ND; ++w) S0[w] = 0;
+  bool had = false;
+  if (head) {
+    key = rows[i * NW];
+    had = mono_prior<C>(prior, key, S0);
+    cnt = mono_walk<C>(rows, n, i, key, S0, had, mx, false, nullptr, 0);
+  }
+  u32 total;
+  const u32 ex = block_exclusive_scan(cnt, sm, &total);
+  if (!WRITE) {
+    if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
+  } else if (head && cnt > 0) {
+    mono_walk<C>(rows, n, i, key, S0, had, mx, true, out, (u64)tile_base[blockIdx.x] + ex);
+  }
+}
+
+// single-pass form (sizes on the device, chained tiles), as k_corrections_lb
+template <int C>
+__global__ void __launch_bounds__(RT) k_monotonic_corrections_lb(const u64* __restrict__ rows, const DLen dn,
+                                                                 const __grid_constant__ TraceView prior,
+                                                                 const MonoXor mx, const LookBack lb,
+                                                                 u64* __restrict__ out, u64 out_cap,
+                                                                 u64* __restrict__ out_len, u64* __restrict__ status) {
+  constexpr int NW = MonoRows<C>::ARR_NW, ND = NW - 2;
+  __shared__ u32 sm[34];
+  __shared__ u32 s_tile;
+  __shared__ u64 s_b;
+  const u64 n = dlen_get(dn);
+  const u64 n_tiles = (n + RT - 1) / RT;
+  while (true) {
+    const u32 tile = lb_next_tile(lb, &s_tile);
+    if ((u64)tile >= n_tiles) {
+      if (n_tiles == 0 && tile == 0 && threadIdx.x == 0) *out_len = 0;
+      break;
+    }
+    const u64 i = (u64)tile * RT + threadIdx.x;
+    u32 cnt = 0;
+    const bool head = i < n && (i == 0 || rows[(i - 1) * NW] != rows[i * NW]);
+    u64 key = 0;
+    u64 S0[ND];
+#pragma unroll
+    for (int w = 0; w < ND; ++w) S0[w] = 0;
+    bool had = false;
+    if (head) {
+      key = rows[i * NW];
+      had = mono_prior<C>(prior, key, S0);
+      cnt = mono_walk<C>(rows, n, i, key, S0, had, mx, false, nullptr, 0);
+    }
+    u32 total;
+    const u32 ex = block_exclusive_scan(cnt, sm, &total);
+    const u64 excl = lb_exclusive_prefix(lb, tile, (u64)total, &s_b);
+    if (head && cnt > 0) {
+      const u64 pos = excl + ex;
+      if (pos + cnt > out_cap)
+        atomicMax((unsigned long long*)status, (unsigned long long)(pos + cnt));
+      else
+        mono_walk<C>(rows, n, i, key, S0, had, mx, true, out, pos);
+    }
+    if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *out_len = excl + total;
+  }
+}
+
 }  // namespace
 
 int32_t mz_distinct_pairs(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
@@ -1595,6 +1824,75 @@ int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_ro
     else
       MZ_LAUNCH(ctx, k_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, lb, d_out,
                 out_cap, d_out_len, ctx->d_status);
+    return MZGPU_OK;
+  });
+}
+
+int32_t mz_monotonic_explode(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
+                             const MonoXor& mx, u64* d_arr, u64* d_errs, u64* d_cnt) {
+  MZ_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 16, ctx->stream));
+  if (n_ub == 0) return MZGPU_OK;
+  u64 grid = (n_ub + RT - 1) / RT;
+  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (ls.in_words * 8 + mz_mono_arr_bytes(c)) : 0);
+  return mz_dispatch<MonoClasses>(ctx, c, "monotonic explode", [&](auto C) {
+    MZ_LAUNCH(ctx, k_monotonic_explode<C>, (unsigned)grid, RT, 0, d_rows, n, ls, mx, d_arr, d_errs,
+              (unsigned long long*)d_cnt);
+    return MZGPU_OK;
+  });
+}
+
+int32_t mz_monotonic_mask(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, u32 in_words, u64 m1, u64 m2,
+                          u64* d_out) {
+  if (n_ub == 0) return MZGPU_OK;
+  u64 grid = (n_ub + RT - 1) / RT;
+  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * in_words * 16 : 0);
+  MZ_LAUNCH(ctx, k_monotonic_mask, (unsigned)grid, RT, 0, d_rows, n, in_words, m1, m2, d_out);
+  return MZGPU_OK;
+}
+
+// at most two output rows per new (key, time) row: capacity 2 * n_ub suffices
+int32_t mz_monotonic_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, DLen n, u64 n_ub,
+                                       const TraceView& prior, const MonoXor& mx, u64* d_out, u64 out_cap,
+                                       u64* d_out_len) {
+  LookBack lb;
+  MZ_TRY(mz_lookback_begin(ctx, (n_ub + RT - 1) / RT, &lb));
+  u64 grid = (n_ub + RT - 1) / RT;
+  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  if (grid == 0) grid = 1;
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (2 * mz_mono_arr_bytes(c) + 16 + 2 * mz_mono_out_bytes(c)) : 0);
+  return mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
+    MZ_LAUNCH(ctx, k_monotonic_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, mx, lb, d_out,
+              out_cap, d_out_len, ctx->d_status);
+    return MZGPU_OK;
+  });
+}
+
+int32_t mz_monotonic_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
+                                 const MonoXor& mx, DevMem* out, u64* n_out) {
+  *n_out = 0;
+  if (n == 0) return out->alloc(ctx, 16);
+  const u64 n_tiles = (n + RT - 1) / RT;
+  DevMem tiles;
+  MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
+  u64* d_total = ctx->d_scratch + 30;
+  MZ_TRY(mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
+    MZ_LAUNCH(ctx, (k_monotonic_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, mx,
+              tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
+    return MZGPU_OK;
+  }));
+  MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
+  MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 30, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  MZ_SYNC(ctx);
+  ctx->stats.d2h_bytes += 8;
+  const u64 total = ctx->h_scratch[30];
+  MZ_TRY(out->alloc(ctx, total * mz_mono_out_bytes(c)));
+  *n_out = total;
+  if (total == 0) return MZGPU_OK;
+  return mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
+    MZ_LAUNCH(ctx, (k_monotonic_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, mx,
+              (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
     return MZGPU_OK;
   });
 }

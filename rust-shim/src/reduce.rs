@@ -103,6 +103,37 @@ impl Drop for GpuReduceLanes {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
 }
 
+/// `build_monotonic` (`HierarchicalPlan::Monotonic`, reduce.rs:160-250 of src/compute-types/src/plan; the
+/// planner's choice for append-only inputs): several MIN / MAX aggregates per key, the best value of each
+/// kept in the arrangement's diff (`sys::mzgpu_reduce_monotonic_new` documents the row layouts and the lane
+/// encoding).  Lanes are `sys::AccumLane`s of kind `AGG_MIN` / `AGG_MAX`; `sign_extend != 0` is signed
+/// order.  `must_consolidate` is the plan's flag.  A float64 lane (`sys::MONO_F64`) comes back as
+/// `MZGPU_E_UNSUPPORTED`, and so does nothing else: the caller keeps the Rust operator for such plans and
+/// for an `mfp_after` with a filter.
+pub struct GpuReduceMonotonic { h: *mut sys::Reduce, pub arr_row_bytes: u32, pub out_row_bytes: u32 }
+
+impl GpuReduceMonotonic {
+    pub fn new(in_row_bytes: u32, lanes: &[sys::AccumLane], must_consolidate: bool) -> Result<Self, (i32, String)> {
+        let (mut arr, mut out) = (0u32, 0u32);
+        let mut h = std::ptr::null_mut();
+        unsafe {
+            sys::check(worker_ctx(), sys::mzgpu_reduce_monotonic_row_bytes(lanes.len() as u32, &mut arr, &mut out))?;
+            sys::check(worker_ctx(), sys::mzgpu_reduce_monotonic_new(worker_ctx(), in_row_bytes, lanes.as_ptr(),
+                                                                    lanes.len() as u32, must_consolidate as i32, &mut h))?;
+        }
+        Ok(GpuReduceMonotonic { h, arr_row_bytes: arr, out_row_bytes: out })
+    }
+    /// One activation over a device buffer of input rows: corrections (`out_row_bytes` wide) are appended to
+    /// `out`, the `ensure_monotonic` errors (R16: time, count) to `errs`.
+    pub fn step(&mut self, rows: *mut sys::Buf, upper: u64, out: *mut sys::Buf, errs: *mut sys::Buf) -> Result<(), (i32, String)> {
+        unsafe { sys::check(worker_ctx(), sys::mzgpu_reduce_monotonic_buf(self.h, rows, upper, out, errs)) }
+    }
+    pub fn input_trace(&self) -> *mut sys::Spine { unsafe { sys::mzgpu_reduce_input_trace(self.h) } }
+}
+impl Drop for GpuReduceMonotonic {
+    fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
+}
+
 impl Drop for GpuReduce {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
 }

@@ -50,6 +50,8 @@ pub const AGG_TOPK: i32 = 6;
 pub const MAX_ACCUM_LANES: usize = 8;
 /// OR'd into `AccumLane::kind`: the lane is COUNT(DISTINCT col) / SUM(DISTINCT col) (int64 lanes only).
 pub const ACCUM_DISTINCT: i32 = 0x100;
+/// OR'd into a monotonic MIN / MAX lane's kind: a float64 column (always `E_UNSUPPORTED`).
+pub const MONO_F64: i32 = 0x200;
 /// A column pick (mzgpu_field): bits [shift, shift + bits) of word `src`.
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)]
 pub struct Field { pub src: u8, pub shift: u8, pub bits: u8, pub dst_shift: u8 }
@@ -198,6 +200,10 @@ extern "C" {
     pub fn mzgpu_reduce_lanes_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf) -> i32;
     pub fn mzgpu_reduce_lanes_distinct_trace(r: *mut Reduce, lane: u32) -> *mut Spine;
     pub fn mzgpu_reduce_lanes_new_having(ctx: *mut Ctx, in_row_bytes: u32, lanes: *const AccumLane, n_lanes: u32, having: *const Having, out: *mut *mut Reduce) -> i32;
+    pub fn mzgpu_reduce_monotonic_row_bytes(n_lanes: u32, arr_row_bytes: *mut u32, out_row_bytes: *mut u32) -> i32;
+    pub fn mzgpu_reduce_monotonic_new(ctx: *mut Ctx, in_row_bytes: u32, lanes: *const AccumLane, n_lanes: u32, must_consolidate: i32, out: *mut *mut Reduce) -> i32;
+    pub fn mzgpu_reduce_monotonic(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_reduce_monotonic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_rowkey_pack(row_bytes: *const u8, len: u64, key_out: *mut u64) -> i32;
     pub fn mzgpu_rowkeys_pack(data: *const u8, offsets: *const u64, n: u64, keys_out: *mut u64, n_done: *mut u64) -> i32;
     pub fn mzgpu_rowkey_unpack(key: u64, row_bytes_out: *mut u8, len_out: *mut u64) -> i32;
