@@ -396,6 +396,103 @@ def main():
                                         40).step_dev(d, 1),
     )
     del host
+
+    # Monotonic TopK: the same insert-only regime, Top1 (ORDER BY val1 DESC: the latest row per key) and
+    # limit 3, against the TopK operator on the R32 (key, val1) projection over the first `nb_cmp` batches
+    # (that operator refuses a group of more than 32 distinct values late, and reports it).
+    for limit in (1, 3):
+        name = f"cfg4 incremental insert-only monotonic TopK limit={limit} val1 desc vs TopK operator, {nb}x{per} R40"
+        if args.only and args.only not in name:
+            continue
+        nb_cmp = min(nb, 3)
+        c = mz.Context(0)
+        ins = [r40_cfg4(c, 11, per, first=b * per, t=b, diff=1) for b in range(nb)]
+
+        def run_topk_mono(k, limit=limit, ins=ins):
+            cm = mz.Context(0)
+            bufs = [mz.DeviceRows(cm, 40).upload(ins[b]) for b in range(k)]
+            op = mz.TopKMonotonic(cm, [mz.order_lane(1, descending=True)], limit, 40)
+            out, errs = mz.DeviceRows(cm, 40), mz.DeviceRows(cm, 16)
+            cm.sync()
+            t0 = time.perf_counter()
+            for b, d in enumerate(bufs):
+                op.step_dev(d, b + 1, out, errs)
+                op.input_trace().set_logical_compaction(b + 1)
+            cm.sync()
+            dt = time.perf_counter() - t0
+            r = (dt, out.download(), len(errs), len(op.input_trace().export()), cm.stats()["device_bytes_peak"])
+            del op, out, errs, bufs
+            cm.close()
+            return r
+
+        def run_topk_old(k, limit=limit, ins=ins):
+            from materialize_b200 import _ffi as F
+
+            cf = mz.Context(0)
+            bufs = []
+            for b in range(k):
+                p = np.zeros(per, dtype=mz.R32)
+                p["key"], p["val"], p["time"], p["diff"] = ins[b]["key"], ins[b]["val1"], ins[b]["time"], 1
+                bufs.append(mz.DeviceRows(cf, 32).upload(p))
+            op = mz.TopK(cf, limit, 0, True)
+            out = mz.DeviceRows(cf, 64)
+            cf.sync()
+            t0 = time.perf_counter()
+            status = "ok"
+            try:
+                for b in range(k):
+                    op.step_dev(bufs[b], b + 1, out)
+                cf.sync()
+            except mz.MzGpuError as e:
+                status = f"error {e.status}"
+            dt = time.perf_counter() - t0
+            arr = len(mz.Spine(cf, 32, _borrowed=F.lib.mzgpu_reduce_input_trace(op.h)).export()) if status == "ok" else None
+            r = (dt, out.download() if status == "ok" else None, arr, cf.stats()["device_bytes_peak"], status)
+            del op, out, bufs
+            cf.close()
+            return r
+
+        dm = df = None
+        for rnd in range(3):  # round 0 warms up
+            t_m, mout, n_err, marr, peak_m = run_topk_mono(nb_cmp)
+            t_f, fout, farr, peak_f, fstatus = run_topk_old(nb_cmp)
+            if rnd > 0:
+                dm = t_m if dm is None else min(dm, t_m)
+                df = t_f if df is None else min(df, t_f)
+        agree = None
+        if fout is not None:
+            cm_, cf_ = {}, {}
+            for k_, v_, d_ in zip(mout["key"].tolist(), mout["val1"].tolist(), mout["diff"].tolist()):
+                cm_[(k_, v_)] = cm_.get((k_, v_), 0) + d_
+            for k_, v_, d_ in zip(fout["key"].tolist(), fout["sum_lo"].tolist(), fout["diff"].tolist()):
+                cf_[(k_, v_)] = cf_.get((k_, v_), 0) + d_
+            agree = n_err == 0 and {k: d for k, d in cm_.items() if d} == {k: d for k, d in cf_.items() if d}
+        dm_all, _, _, marr_all, peak_all = run_topk_mono(nb)
+        res["cases"].append(
+            {"case": name, "rows": nb_cmp * per, "batches_compared": nb_cmp,
+             "seconds_monotonic_topk": dm, "seconds_topk_operator": df, "topk_operator_status": fstatus,
+             "outputs_agree": agree, "arrangement_rows_monotonic_topk": marr,
+             "arrangement_bytes_monotonic_topk": 72 * marr, "arrangement_rows_topk_operator": farr,
+             "arrangement_bytes_topk_operator": None if farr is None else 32 * farr,
+             "device_bytes_peak_monotonic_topk": peak_m, "device_bytes_peak_topk_operator": peak_f,
+             "monotonic_topk_all_batches": {"batches": nb, "seconds": dm_all, "arrangement_rows": marr_all,
+                                            "device_bytes_peak": peak_all}}
+        )
+        print(name, f"{dm:.4f} s / {df:.4f} s ({fstatus}), agree={agree}, all {nb}: {dm_all:.4f} s",
+              file=sys.stderr, flush=True)
+        del ins
+        c.close()
+
+    for limit in (1, 3):
+        name = f"bulk monotonic TopK limit={limit} val1 desc n={n4} zipf0.9 keys={nk} R40"
+        host = r40_cfg4(ctx, 5, n4) if not args.only or args.only in name else None
+        lanes_case(
+            name,
+            n4,
+            lambda c, host=host: mz.DeviceRows(c, 40).upload(host),
+            lambda c, d, limit=limit: mz.TopKMonotonic(c, [mz.order_lane(1, descending=True)], limit, 40).step_dev(d, 1),
+        )
+        del host
     txt = json.dumps(res, indent=1)
     if args.out:
         open(args.out, "w").write(txt)

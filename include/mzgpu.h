@@ -778,8 +778,7 @@ int32_t mzgpu_reduce_lanes_new_having(mzgpu_ctx* ctx, uint32_t in_row_bytes, con
  * spines, and accumulate there by the per-word max.
  *
  * Not supported: float64 MIN / MAX (OrderedFloat ties -0.0 with +0.0, and NaNs with different payloads,
- * so which bits survive would depend on arrival order), MonotonicTop1Plan / MonotonicTopKPlan, HAVING on
- * this operator, and COUNT / SUM in the same operator (a MonotonicPlan holds MIN / MAX-type functions
+ * so which bits survive would depend on arrival order), HAVING on this operator, and COUNT / SUM in the same operator (a MonotonicPlan holds MIN / MAX-type functions
  * only). */
 /* OR'd into a MIN / MAX lane's kind: the column is float64.  Always MZGPU_E_UNSUPPORTED (see above), so
  * that a caller describing such a plan keeps its own path. */
@@ -806,6 +805,66 @@ int32_t mzgpu_reduce_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, in
                                mzgpu_buf* out, mzgpu_buf* errs);
 int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
                                    mzgpu_buf* errs);
+
+/* ---- monotonic TopK: Top-1 and Top-K over append-only input, with only the window arranged
+ * (TopKPlan::MonotonicTop1 / MonotonicTopK, src/compute/src/render/top_k.rs:102-214; the planner picks them
+ * for every offset-0 TopK over an append-only input, src/compute-types/src/plan/top_k.rs:47-92).  One operator
+ * covers both: Top1 is limit = 1, the same collection and the same one-row-per-key state.
+ *
+ * Input: R32 or R40 rows; `key` is the group key and the row is (key, val1[, val2]).
+ * Order: rows of a key compare by the order lanes in sequence (the plan's order_key; n_order = 0 is no ORDER
+ * BY).  A lane's field is sign-extended and compared signed when sign_extend != 0, unsigned otherwise, and
+ * reversed when descending.  Rows equal on every lane are ordered by val1, then val2, as unsigned words:
+ * the fixed-width stand-in for compare_columns(order_key, l, r, || l.cmp(r)) (Top1Monoid,
+ * top_k.rs:866-932), which breaks ties by the whole row's Datum order.  The two agree when every column the
+ * plan can tie on is listed as a lane, or when signed columns are encoded with the sign bit flipped (then
+ * the unsigned word order is the Datum order).
+ *
+ * One activation, as build_monotonic's steps:
+ *   1. must_consolidate != 0: the rows are consolidated by the whole row, then time (consolidate_named_if,
+ *      top_k.rs:446-511).
+ *   2. ensure_monotonic (src/timely-util/src/operator.rs:425-456): a row is kept iff its diff > 0.  Every
+ *      other row is one error at its time: `errs` receives R16 rows (key = time, diff = rows rejected at that
+ *      time), consolidated, as mzgpu_reduce_monotonic does.
+ *   3. A kept row's multiplicity counts toward the limit (TopKBatch, top_k.rs:765-850): a limit can cut
+ *      inside one row's copies, and Top1 always yields diff 1 (top_k.rs:564).
+ *   4. Output: rows of the INPUT width appended to `out`, consolidated and sorted: (key, val1[, val2], time,
+ *      diff), diff the change of that row's multiplicity inside the window.  At every time the window is the
+ *      first `limit` units per key of the accumulated kept input, in the order above (the TopK the
+ *      reference's thinning, topk stage and delayed retraction feedback, top_k.rs:116-214, compute).
+ *      They are ordinary R32 / R40 rows.
+ * State: mzgpu_reduce_input_trace(r) returns the window arrangement, MZGPU_ROW_RTOPK rows
+ *     (key, o0, o1, o2, val1, val2, time | diff, pad), o_j the encoded lane j: the field (sign-extended
+ * when signed) ^ 2^63 if signed, complemented if descending; unused words and val2 of R32 input are 0.  The
+ * caller compacts it like any other trace; after logical compaction and merges it holds exactly the live
+ * window, at most `limit` units per key.  Work per touched key is bounded by its live window plus its
+ * not-yet-compacted rows, not by its history.
+ * limit: >= 0; MZGPU_TOPK_NO_LIMIT is LIMIT NULL / None (Diff::MAX, top_k.rs:564, :721): every kept row enters
+ * and no state is read.
+ * Checked on the host before any launch; a failure leaves no operator behind and the context usable:
+ *   MZGPU_E_INVALID: in_row_bytes not 32 / 40, VAL2 on R32 input, a zero-width or out-of-range field, unknown
+ *       flag bits, n_order > MZGPU_MAX_ORDER_LANES, or a NULL `order` with n_order > 0;
+ *   MZGPU_E_UNSUPPORTED: a float64 order lane (MZGPU_ORDER_F64: OrderedFloat ties -0.0 with +0.0 and NaN
+ *       payloads), or a negative limit (the reference's NegLimit error path, top_k.rs:67-98).
+ * Not supported: offset > 0 (never planned as monotonic), limit expressions (INTEGRATION.md), NULLs. */
+typedef struct mzgpu_order_lane { /* one ColumnOrder of the plan's order_key */
+  uint32_t sign_extend;           /* != 0: signed order of the sign-extended field */
+  uint32_t descending;            /* ColumnOrder::desc */
+  uint32_t flags;                 /* 0, or MZGPU_ORDER_F64 */
+  mzgpu_field field;              /* src MZGPU_SRC_VAL1, or MZGPU_SRC_VAL2 of R40 input; shift; bits */
+} mzgpu_order_lane;
+#define MZGPU_ORDER_F64 0x1 /* the column is float64: always MZGPU_E_UNSUPPORTED */
+#define MZGPU_MAX_ORDER_LANES 3
+#define MZGPU_TOPK_NO_LIMIT INT64_MAX
+#define MZGPU_ROW_RTOPK 72
+int32_t mzgpu_topk_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_order_lane* order,
+                                 uint32_t n_order, int64_t limit, int32_t must_consolidate, mzgpu_reduce** out);
+/* One activation, with the protocol of mzgpu_reduce_monotonic[_buf]: `rows` are n input rows with times in
+ * [previous upper, upper); the window changes (input-width rows) are appended to `out`, the errors (R16) to
+ * `errs` (required).  After a failed activation the operator reports that status from then on. */
+int32_t mzgpu_topk_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                             mzgpu_buf* out, mzgpu_buf* errs);
+int32_t mzgpu_topk_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs);
 
 /* ------------------------------ f1 (first step): Row keys as fixed-width words */
 /* A `Row` orders by byte length first, then by its bytes (RowRef::cmp,

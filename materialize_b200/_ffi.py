@@ -110,6 +110,11 @@ DTYPES.update({LANE_ROW_BYTES[c][0]: RACC_LANES[c] for c in LANE_CLASSES[1:]})
 DTYPES.update({LANE_ROW_BYTES[c][1]: ROUT_LANES[c] for c in LANE_CLASSES[1:]})
 DTYPES.update({MONO_ROW_BYTES[c][0]: RMONO[c] for c in MONO_CLASSES})
 DTYPES.update({MONO_ROW_BYTES[c][1]: MONO_OUT[c] for c in MONO_CLASSES})
+# The monotonic TopK's window rows (mzgpu_topk_monotonic_new): o0..o2 the encoded order lanes (field ^ 2^63
+# for a signed lane, complemented for a descending one), so word order within a key is the plan's order.
+RTOPK = np.dtype([("key", "<u8"), ("order", "<u8", (3,)), ("val1", "<u8"), ("val2", "<u8"), ("time", "<u8"),
+                  ("diff", "<i8"), ("_pad", "<u8")])
+DTYPES[72] = RTOPK
 
 MEM_HOST, MEM_DEVICE = 0, 1
 FRONTIER_EMPTY = 2**64 - 1
@@ -119,6 +124,9 @@ AGG_COUNT_SUM_I64, AGG_COUNT_SUM_F64, AGG_DISTINCT, AGG_THRESHOLD, AGG_MIN, AGG_
 MAX_ACCUM_LANES = 8
 ACCUM_DISTINCT = 0x100  # OR'd into a lane's kind: COUNT(DISTINCT col) / SUM(DISTINCT col)
 MONO_F64 = 0x200  # OR'd into a monotonic MIN / MAX lane's kind: a float64 column (always E_UNSUPPORTED)
+MAX_ORDER_LANES = 3
+ORDER_F64 = 0x1  # an order lane's flags: a float64 column (always E_UNSUPPORTED)
+TOPK_NO_LIMIT = 2**63 - 1  # LIMIT NULL
 COMM_ID_BYTES = 128
 P2P_HANDLE_BYTES = 64
 
@@ -129,6 +137,10 @@ class Field(C.Structure):
 
 class AccumLane(C.Structure):
     _fields_ = [("kind", C.c_int32), ("sign_extend", C.c_uint32), ("field", Field)]
+
+
+class OrderLane(C.Structure):
+    _fields_ = [("sign_extend", C.c_uint32), ("descending", C.c_uint32), ("flags", C.c_uint32), ("field", Field)]
 
 
 # HAVING programs of the lanes operator (mzgpu_having, include/mzgpu.h)
@@ -299,6 +311,9 @@ SIGNATURES = {
     "mzgpu_reduce_monotonic_new": (i32, [vp, u32, vp, u32, i32, PV]),
     "mzgpu_reduce_monotonic": (i32, [vp, vp, u64, i32, u64, vp, vp]),
     "mzgpu_reduce_monotonic_buf": (i32, [vp, vp, u64, vp, vp]),
+    "mzgpu_topk_monotonic_new": (i32, [vp, u32, vp, u32, C.c_int64, i32, PV]),
+    "mzgpu_topk_monotonic": (i32, [vp, vp, u64, i32, u64, vp, vp]),
+    "mzgpu_topk_monotonic_buf": (i32, [vp, vp, u64, vp, vp]),
     "mzgpu_comm_unique_id": (i32, [C.POINTER(C.c_uint8)]),
     "mzgpu_comm_init": (i32, [vp, C.POINTER(C.c_uint8)]),
     "mzgpu_exchange": (i32, [vp, vp, vp]),

@@ -24,6 +24,9 @@ from ._ffi import (  # noqa: F401  (re-exported)
     MONO_F64,
     MONO_OUT,
     RMONO,
+    ORDER_F64,
+    RTOPK,
+    TOPK_NO_LIMIT,
     AGG_COUNT_SUM_F64,
     AGG_DISTINCT,
     AGG_THRESHOLD,
@@ -620,6 +623,13 @@ def accum_lane(kind, src=SRC_VAL1, shift=0, bits=64, sign_extend=False):
     return (int(kind), int(src), int(shift), int(bits), bool(sign_extend))
 
 
+
+def order_lane(src=SRC_VAL1, shift=0, bits=64, sign_extend=False, descending=False, f64=False):
+    """One ColumnOrder of TopKMonotonic's order key: the bit-field `bits` wide at `shift` of value word `src`
+    (1 = val / val1, 2 = val2), compared signed (sign-extended) when `sign_extend`, reversed when
+    `descending`.  `f64` marks a float64 column, which the operator refuses (E_UNSUPPORTED)."""
+    return (int(src), int(shift), int(bits), bool(sign_extend), bool(descending), bool(f64))
+
 # HAVING ops (mzgpu_having_op): one constructor per opcode.  An op is (code, arg, shift, bits,
 # sign_extend, constant value or None); having() builds the descriptor and its constant pool.
 def h_key(shift=0, bits=64, sign_extend=False):
@@ -760,6 +770,50 @@ class ReduceLanes:
         """The (key, value) pair arrangement (R32 rows) of distinct lane `lane`; None for any other lane."""
         h = F.lib.mzgpu_reduce_lanes_distinct_trace(self.h, lane)
         return Spine(self.ctx, 32, _borrowed=h) if h else None
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_reduce_free(self.h)
+            self.h = None
+
+
+class TopKMonotonic:
+    """MonotonicTop1 / MonotonicTopK over append-only input (mzgpu_topk_monotonic_new): the first `limit`
+    rows per key in the order of `order` (order_lane() tuples, at most 3; ties by val1, then val2), with only
+    that window arranged.  Top1 is limit=1; LIMIT NULL is TOPK_NO_LIMIT.  Input rows are R32
+    (in_row_bytes=32) or R40 (40).  step() returns (changes, errors): the window's changes as rows of the
+    input width, and R16 error rows (key = time, diff = rows with diff <= 0 at that time)."""
+
+    def __init__(self, ctx, order, limit, in_row_bytes=32, must_consolidate=False):
+        self.ctx = ctx
+        self.in_row_bytes = in_row_bytes
+        arr = (F.OrderLane * max(1, len(order)))()
+        for i, (src, shift, bits, sx, desc, f64) in enumerate(order):
+            arr[i].sign_extend = 1 if sx else 0
+            arr[i].descending = 1 if desc else 0
+            arr[i].flags = F.ORDER_F64 if f64 else 0
+            arr[i].field = F.Field(src, shift, bits, 0)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_topk_monotonic_new(ctx.h, in_row_bytes, arr, len(order), int(limit),
+                                                 1 if must_consolidate else 0, C.byref(h)))
+        self.h = h
+
+    def step(self, rows, upper):
+        rows = np.ascontiguousarray(rows)
+        out, errs = DeviceRows(self.ctx, self.in_row_bytes), DeviceRows(self.ctx, 16)
+        self.ctx.check(F.lib.mzgpu_topk_monotonic(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
+        return out.download(), errs.download()
+
+    def step_dev(self, dev_rows, upper, out=None, errs=None):
+        """One activation over device-resident rows; changes and errors are appended on the device."""
+        out = out if out is not None else DeviceRows(self.ctx, self.in_row_bytes)
+        errs = errs if errs is not None else DeviceRows(self.ctx, 16)
+        self.ctx.check(F.lib.mzgpu_topk_monotonic_buf(self.h, dev_rows.h, upper, out.h, errs.h))
+        return out, errs
+
+    def input_trace(self):
+        """The window arrangement (RTOPK rows)."""
+        return Spine(self.ctx, 72, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
 
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:

@@ -34,7 +34,7 @@ struct mzgpu_ctx {
   u64* h_scratch = nullptr;  // 64 words
   u64* d_scratch = nullptr;  // 64 words
   u64* h_big = nullptr;      // pinned, 512 words (exchange counts)
-  u64 last_minmax[12] = {0};  // min/max of every key word seen by the last bulk sort (mz_sort_perm)
+  u64 last_minmax[14] = {0};  // min/max of every key word seen by the last bulk sort (mz_sort_perm)
   bool last_minmax_valid = false;
   // pinned bounce buffers for host<->device row copies
   void* h_bounce = nullptr;
@@ -550,6 +550,13 @@ template <>
 struct RowT<112> {  // 5-8 lanes, 4 pad words
   static constexpr int NW = 14, NK = 2, ND = 12, TW = 1, DK = 1, SG = MZ_SG_MAX;
 };
+// Monotonic TopK window rows (mzgpu_topk_monotonic_new): key, o0, o1, o2, val1, val2, time | diff, pad.
+// o0..o2 are the encoded order lanes (TopKOrder below), so unsigned word order within a key is the
+// plan's order, ties broken by (val1, val2).  The only row with more than 6 key words.
+template <>
+struct RowT<72> {
+  static constexpr int NW = 9, NK = 7, ND = 2, TW = 6, DK = 6, SG = MZ_SG_SUM;
+};
 // DK = number of leading "data" words (key words before the time word): two
 // rows with equal DK words are the same (key, val).
 //
@@ -567,8 +574,8 @@ struct IntSet {
   static constexpr const char* kind = "row width";
   static constexpr bool has(int v) { return ((v == V) || ...); }
 };
-using RowWidths = IntSet<16, 32, 40, 64, 80, 128, 224, 416, 48, 112>;  // every RowT: sort, consolidate, fused
-using BatchWidths = IntSet<32, 64, 80, 128, 224, 416, 48, 112>;         // sorted batches: merge, extract, index
+using RowWidths = IntSet<16, 32, 40, 64, 80, 128, 224, 416, 48, 112, 72>;  // every RowT: sort, consolidate, fused
+using BatchWidths = IntSet<32, 64, 80, 128, 224, 416, 48, 112, 72>;         // sorted batches: merge, extract, index
 using ExchangeWidths = IntSet<32, 80>;
 struct LaneClasses : IntSet<1, 2, 4, 8> {  // accumulable reduce with 1, 2, 4 or 8 lanes (LaneRows below)
   static constexpr const char* kind = "lane class";
@@ -1133,6 +1140,26 @@ int32_t mz_monotonic_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch
                                        u64* d_out_len);
 int32_t mz_monotonic_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
                                  const MonoXor& mx, DevMem* out, u64* n_out);
+// the monotonic TopK (mzgpu_topk_monotonic_new): order word j of a row = field_get(lane j) (sign-extended when
+// signed) ^ xm[j] (2^63 for a signed lane, then all ones for a descending one); lanes n..2 stay zero
+struct TopKOrder {
+  mzgpu_field f[3];
+  u32 sign_extend[3];
+  u64 xm[3];
+  u32 n;
+  u32 in_words;  // 4 (R32) or 5 (R40)
+  i64 limit;     // >= 0; INT64_MAX is LIMIT NULL
+};
+// rows with diff > 0 -> 72-byte window rows at d_arr, every other row -> an R16 (time, +1) row at d_errs;
+// their counts are left in d_cnt[0] and d_cnt[1] (two words of a counter block, zeroed here)
+int32_t mz_topk_explode(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TopKOrder& to, u64* d_arr,
+                        u64* d_errs, u64* d_cnt);
+// The window changes of the new 72-byte rows (sorted, consolidated) against the window arrangement `prior`:
+// 72-byte rows at d_win and the same rows at the input width at d_out (each key's sorted), out_cap rows each.
+int32_t mz_topk_window_async(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TraceView& prior,
+                             const TopKOrder& to, u64* d_win, u64* d_out, u64 out_cap, u64* d_out_len);
+int32_t mz_topk_window(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView& prior, const TopKOrder& to,
+                       DevMem* win, DevMem* out, u64* n_out);
 
 // correction.cu (time-major rows: (time, key, val | diff))
 // column.cu (columnar wire format, f4)

@@ -48,17 +48,27 @@ constexpr u64 MSD_FAST_MAX_ROWS = 1ull << 20;
 constexpr u64 MSD_EXACT_MAX_ROWS = 1ull << 18;
 constexpr u32 MSD_LOCAL_MAX = 1024;  // largest bucket the in-CTA sort takes
 
-struct FusedCtl {
+// KW = key words the block has room for: 6, or 7 for the TopK window rows (RowT<72>), whose seventh key
+// word may need a seventh radix round.  Only the header's size depends on it (FusedKW below).
+template <int KW>
+struct FusedCtlT {
   u32 barrier;
   u32 overflow;  // fast MSD path: a bucket outgrew its fixed-capacity region (the exact path runs instead)
   u32 pad[2];
-  u64 minmax[12];  // [2k] = max of ~word (so zero is the identity), [2k+1] = max of word
+  u64 minmax[2 * KW];  // [2k] = max of ~word (so zero is the identity), [2k+1] = max of word
   u64 n_seg;
   u64 n_out;
-  u32 hist[MAX_ROUNDS * 8 * 256];
+  u32 hist[KW * 8 * 256];
   u32 bcnt[MSD_FAST_MAX_BUCKETS];  // MSD paths: rows per bucket
 };
+using FusedCtl = FusedCtlT<MAX_ROUNDS>;
 constexpr size_t CTL_HEADER = offsetof(FusedCtl, hist);
+template <int NK>
+constexpr int FusedKW = NK > MAX_ROUNDS ? NK : MAX_ROUNDS;
+// the control block of a row width: every launch zeroes the next launch's header at its own KW, so a
+// header past CTL_HEADER is cleared by the host before the launch that uses it (fused_prepare)
+template <int RB>
+using FusedCtlOf = FusedCtlT<FusedKW<RowT<RB>::NK>>;
 
 struct FusedArgs {
   const u64* a;
@@ -171,7 +181,7 @@ __device__ __forceinline__ void load_in_row(const FusedArgs& a, u64 na, u64 sinc
 // emitted at offsets from a look-back over chunks of eight buckets (one chunk per
 // CTA iteration).  No shared-memory sort, no block-wide scans: ~5 us per chunk.
 template <int RB, int R>
-__device__ __forceinline__ void msd_warp_buckets(const FusedArgs& a, FusedCtl* ctl, const u32* base, u32 NB, u32 c,
+__device__ __forceinline__ void msd_warp_buckets(const FusedArgs& a, FusedCtlOf<RB>* ctl, const u32* base, u32 NB, u32 c,
                                                  u32 G, u64 na, u64 since, u64* s_cnt /* 8 + 1 words */,
                                                  u64* s_lb) {
   constexpr int NW = RowT<RB>::NW, NK = RowT<RB>::NK, ND = RowT<RB>::ND, TW = RowT<RB>::TW;
@@ -373,7 +383,7 @@ __device__ __forceinline__ void msd_warp_buckets(const FusedArgs& a, FusedCtl* c
 //    (`inline_index`): the warp knows the final position of every row it ships once the
 //    look-back has given the chunk's base, so no table pass (and no grid barrier) follows.
 template <int RB, int R, int KW>
-__device__ __forceinline__ void msd_warp_buckets2(const FusedArgs& a, FusedCtl* ctl, u32 NB, u32 c, u32 G, u64 na,
+__device__ __forceinline__ void msd_warp_buckets2(const FusedArgs& a, FusedCtlOf<RB>* ctl, u32 NB, u32 c, u32 G, u64 na,
                                                   u64 since, u64 mask, bool inline_index, u64* s_cnt, u64* s_lb,
                                                   u64* s_keys /* [FT/32][32*R] */, u32* s_stat /* [2] */) {
   constexpr int NW = RowT<RB>::NW, NK = RowT<RB>::NK, ND = RowT<RB>::ND, TW = RowT<RB>::TW;
@@ -642,13 +652,13 @@ union FusedSmem {
 template <int RB>
 __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, const u32 gdim) {
   constexpr int NW = RowT<RB>::NW, NK = RowT<RB>::NK, ND = RowT<RB>::ND, TW = RowT<RB>::TW;
-  constexpr int SG = RowT<RB>::SG;
+  constexpr int SG = RowT<RB>::SG, KW = FusedKW<NK>;  // KW: key words (and radix rounds) planned at most
   __shared__ FusedSmem sm;
   __shared__ u32 sm_scan[34];
-  __shared__ int s_nwords, s_nrounds, s_word[6], s_shift[6], s_round[6], s_rbits[MAX_ROUNDS];
-  __shared__ int s_shift128[6], s_w128, s_keybits;
+  __shared__ int s_nwords, s_nrounds, s_word[KW], s_shift[KW], s_round[KW], s_rbits[KW];
+  __shared__ int s_shift128[KW], s_w128, s_keybits;
   __shared__ u32 s_max_bucket, s_max_unit;
-  __shared__ u64 s_minv[6];
+  __shared__ u64 s_minv[KW];
   const u32 tid = threadIdx.x;
   const u64 na = dlen_get(a.na), nb = dlen_get(a.nb);
   const u64 n = na + nb;
@@ -680,7 +690,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
   }
   if (c >= G) return;
   const u64 gtid = (u64)c * FT + tid, gstride = (u64)G * FT;
-  FusedCtl* ctl = a.ctl;
+  FusedCtlOf<RB>* ctl = reinterpret_cast<FusedCtlOf<RB>*>(a.ctl);
   u32 epoch = 0;
   const u64 since = a.since;
 
@@ -710,7 +720,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
   // ---- phase 0: zero scratch, results, next launch's header; min/max of every key word
   {
     if (c == 0) {
-      for (u32 i = tid; i < CTL_HEADER / 4; i += FT) ((u32*)a.ctl_next)[i] = 0;
+      for (u32 i = tid; i < offsetof(FusedCtlOf<RB>, hist) / 4; i += FT) ((u32*)a.ctl_next)[i] = 0;
       if (tid == 0) {
         a.res[0] = 0;
         a.res[1] = mask;
@@ -722,7 +732,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
         a.kres[3] = 0;
       }
     }
-    for (u64 i = gtid; i < (u64)MAX_ROUNDS * 8 * 256; i += gstride) ctl->hist[i] = 0;
+    for (u64 i = gtid; i < (u64)KW * 8 * 256; i += gstride) ctl->hist[i] = 0;
     for (u64 i = gtid; i < (u64)NB; i += gstride) ctl->bcnt[i] = 0;
     for (u64 i = gtid; i < (u64)(NB + 7) / 8; i += gstride) {  // look-back state: one word per chunk of eight buckets
       a.lb_ship[i] = 0;
@@ -774,7 +784,7 @@ __device__ __forceinline__ void fused_body(const FusedArgs& a, const u32 c, cons
   // ---- plan (every CTA computes the same plan from the global min/max)
   if (tid == 0) {
     int used = 0, nwords = 0, round = 0;
-    for (int r = 0; r < MAX_ROUNDS; ++r) s_rbits[r] = 0;
+    for (int r = 0; r < KW; ++r) s_rbits[r] = 0;
     for (int k = NK - 1; k >= 0; --k) {
       u64 lo = ~*(volatile u64*)&ctl->minmax[2 * k], hi = *(volatile u64*)&ctl->minmax[2 * k + 1];
       int bits = n > 0 ? bit_width_dev(hi - lo) : 0;
@@ -1633,6 +1643,9 @@ int32_t fused_prepare(mzgpu_ctx* ctx, const FusedJob& job, FusedOut* res, int sl
     a.ctl_next = (FusedCtl*)ctx->d_fused_ctl_many[2 * slot + (ctx->fused_flip_many[slot] ^ 1)];
     ctx->fused_flip_many[slot] ^= 1;
   }
+  // the launch before may have zeroed only CTL_HEADER bytes of this header
+  if (offsetof(FusedCtlOf<RB>, hist) > CTL_HEADER)
+    MZ_CUDA(ctx, cudaMemsetAsync(a.ctl, 0, offsetof(FusedCtlOf<RB>, hist), ctx->stream));
   a.k0 = (u64*)(sp + o_k0);
   a.k1 = (u64*)(sp + o_k1);
   a.v0 = (u32*)(sp + o_v0);
@@ -1818,7 +1831,7 @@ int32_t fused_defer_t(mzgpu_ctx* ctx, FusedDeferred* d, const FusedJob& job, Fus
 
 }  // namespace
 
-size_t mz_fused_ctl_bytes() { return sizeof(FusedCtl); }
+size_t mz_fused_ctl_bytes() { return sizeof(FusedCtlT<FusedKW<RowT<72>::NK>>); }
 
 int32_t mz_fused_flush(mzgpu_ctx* ctx) {
   FusedDeferred* d = (FusedDeferred*)ctx->fused_deferred;

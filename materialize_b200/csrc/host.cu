@@ -1353,7 +1353,7 @@ static int32_t seal_run_unfused(SealPlan* p, mzgpu_batch** batch_out) {
   b->frontier_known = true;
   // the bulk sort has seen the range of the time word: if every buffered time precedes
   // `upper` everything ships and the extract pass (two more copies of the rows) is skipped
-  const int tw = b->rb == 32 ? 2 : 1;
+  const int tw = b->rb == 32 ? 2 : (b->rb == 72 ? RowT<72>::TW : 1);
   const bool all_ship = ctx->last_minmax_valid && ctx->last_minmax[2 * tw + 1] < upper;
   if (upper == MZGPU_FRONTIER_EMPTY || n_cons == 0 || all_ship) {
     MZ_TRY(make_batch(ctx, b->rb, std::move(cons), n_cons, d, batch_out));
@@ -2526,6 +2526,9 @@ struct mzgpu_reduce {
   MonoXor mono = {};
   bool must_consolidate = false;
   u64 mono_mask[2] = {0, 0};
+  // mzgpu_topk_monotonic_new: the order lanes and limit (must_consolidate above is its flag too)
+  bool topk_mono = false;
+  TopKOrder tko = {};
   int32_t failed = MZGPU_OK;  // set when an activation failed after its seal (reduce_dev)
   std::string failed_msg;
   ~mzgpu_reduce() {
@@ -2784,7 +2787,8 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
 
 extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_t n,
                                             int32_t mem, uint64_t upper, mzgpu_buf* out) {
-  if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->lane_class || r->mono_class)
+  if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->lane_class || r->mono_class ||
+      r->topk_mono)
     return MZGPU_E_INVALID;
   mzgpu_ctx* ctx = r->ctx;
   MZ_CHECK_CTX(ctx);
@@ -2801,7 +2805,7 @@ extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* ro
 extern "C" int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
                                                 mzgpu_buf* out) {
   if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64 || r->lane_class ||
-      r->mono_class)
+      r->mono_class || r->topk_mono)
     return MZGPU_E_INVALID;
   MZ_CHECK_CTX(r->ctx);
   r->ctx->stats.rows_in += rows->ub;
@@ -3224,6 +3228,194 @@ extern "C" int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, 
   }
   r->ctx->stats.rows_in += rows->ub;
   return monotonic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
+}
+
+// ------------------------------------------------------- monotonic TopK
+extern "C" int32_t mzgpu_topk_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_order_lane* order,
+                                            uint32_t n_order, int64_t limit, int32_t must_consolidate,
+                                            mzgpu_reduce** out) {
+  MZ_CHECK_CTX(ctx);
+  if (out == nullptr || (order == nullptr && n_order) || (in_row_bytes != 32 && in_row_bytes != 40)) {
+    MZ_SET_ERR(ctx, "topk_monotonic: bad arguments (input rows of %u bytes)", in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  if (n_order > MZGPU_MAX_ORDER_LANES) {
+    MZ_SET_ERR(ctx, "topk_monotonic: %u order lanes (0..%d)", n_order, MZGPU_MAX_ORDER_LANES);
+    return MZGPU_E_INVALID;
+  }
+  TopKOrder to = {};
+  int unsupported = -1;  // the first float64 lane, reported once every lane is known to be well-formed
+  for (uint32_t j = 0; j < n_order; ++j) {
+    const mzgpu_order_lane& L = order[j];
+    const mzgpu_field& f = L.field;
+    const char* bad = nullptr;
+    if ((L.flags & ~(uint32_t)MZGPU_ORDER_F64) != 0)
+      bad = "unknown flag bits";
+    else if (f.src != MZGPU_SRC_VAL1 && !(f.src == MZGPU_SRC_VAL2 && in_row_bytes == 40))
+      bad = "source word is not a value word of the input row";
+    else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
+      bad = "field is empty or out of range";
+    if (bad != nullptr) {
+      MZ_SET_ERR(ctx, "topk_monotonic: order lane %u: %s", j, bad);
+      return MZGPU_E_INVALID;
+    }
+    if ((L.flags & MZGPU_ORDER_F64) != 0 && unsupported < 0) unsupported = (int)j;
+    to.f[j] = f;
+    to.sign_extend[j] = L.sign_extend != 0;
+    to.xm[j] = (L.sign_extend ? 1ull << 63 : 0) ^ (L.descending ? ~0ull : 0);
+  }
+  if (unsupported >= 0) {
+    MZ_SET_ERR(ctx, "topk_monotonic: order lane %d: float64 order columns are not supported (OrderedFloat ties "
+                    "-0.0 with +0.0 and NaN payloads)", unsupported);
+    return MZGPU_E_UNSUPPORTED;
+  }
+  if (limit < 0) {
+    MZ_SET_ERR(ctx, "topk_monotonic: negative limit %lld", (long long)limit);
+    return MZGPU_E_UNSUPPORTED;
+  }
+  to.n = n_order;
+  to.in_words = in_row_bytes / 8;
+  to.limit = limit;
+  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
+  r->ctx = ctx;
+  r->agg_kind = -1;
+  r->topk_mono = true;
+  r->tko = to;
+  r->must_consolidate = must_consolidate != 0;
+  MZ_TRY(mzgpu_batcher_new(ctx, MZGPU_ROW_RTOPK, &r->batcher));
+  MZ_TRY(mzgpu_spine_new(ctx, MZGPU_ROW_RTOPK, 1, &r->input));
+  *out = r.release();
+  return MZGPU_OK;
+}
+
+// One activation: [consolidate ->] ensure_monotonic + explode -> sort -> window changes -> seal the changes.
+static int32_t topk_monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                                  mzgpu_buf* errs) {
+  mzgpu_ctx* ctx = r->ctx;
+  if (r->failed != MZGPU_OK) {
+    ctx->last_error = r->failed_msg;
+    return r->failed;
+  }
+  MZ_TRY(mzgpu_spine_set_physical_compaction(r->input, r->input->upper));
+  const TopKOrder& to = r->tko;
+  const u32 iw = to.in_words;
+  const u64 RB = MZGPU_ROW_RTOPK;
+  int32_t st = MZGPU_OK;
+  if (n_ub) {
+    DevMem cons;
+    Lazy4 clen;
+    if (r->must_consolidate) {  // consolidate_named_if on (group_key, row): whole rows, then time
+      u64 ccap = 0;
+      MZ_TRY(consolidate_dev(ctx, (int)iw * 8, d_rows, n, n_ub, &cons, &ccap, &clen));
+      d_rows = cons.as<u64>();
+      n = dlen_of(clen, 0);
+      if (clen.known) n_ub = clen.v[0];
+    }
+    DevMem arr, erows, econs, sorted;
+    Lazy4 alen, elen, slen;
+    u64 ecap = 0, scap = 0;
+    MZ_TRY(arr.alloc(ctx, n_ub * RB));
+    MZ_TRY(erows.alloc(ctx, n_ub * 16));
+    MZ_TRY(alen.make_pending(ctx));
+    MZ_TRY(mz_topk_explode(ctx, d_rows, n, n_ub, to, arr.as<u64>(), erows.as<u64>(), alen.dptr()));
+    alen.mark_written();
+    // the rejected rows' error collection: (time, number of rejected rows)
+    MZ_TRY(consolidate_dev(ctx, 16, erows.p, dlen_of(alen, 1), n_ub, &econs, &ecap, &elen));
+    MZ_TRY(buf_append_dev(errs, econs.p, dlen_of(elen, 0), elen.known ? elen.v[0] : n_ub));
+    // the kept rows sorted and consolidated by (key, order, row, time); never arranged themselves
+    MZ_TRY(consolidate_dev(ctx, (int)RB, arr.p, dlen_of(alen, 0), n_ub, &sorted, &scap, &slen));
+    arr.release();
+    const u64 s_ub = slen.known ? slen.v[0] : n_ub;
+    std::vector<mzgpu_batch*> prior;
+    r->input->all_batches(prior);
+    TraceView tv;
+    MZ_TRY(trace_view(ctx, prior, &tv));
+    // Output bound of one new row of multiplicity m: it enters at most once, and the units it adds evict or
+    // cut at most min(m, limit) rows, so 1 + limit rows per new row (exactly one without a limit).
+    const i64 L = to.limit;
+    const u64 per_row = L == INT64_MAX ? 1 : (u64)L + 1;
+    Seg w;
+    w.ub = 0;
+    if (L != 0 && s_ub > 0) {
+      if ((s_ub + 255) / 256 <= MZ_LB_TILES && (u64)L < MZ_BOUND_MAX_ROWS && per_row * s_ub <= MZ_BOUND_MAX_ROWS) {
+        const u64 cap = per_row * s_ub;
+        DevMem proj;
+        st = w.rows.alloc(ctx, cap * RB);
+        if (st == MZGPU_OK) st = proj.alloc(ctx, cap * iw * 8);
+        if (st == MZGPU_OK) st = w.len.make_pending(ctx);
+        if (st == MZGPU_OK) {
+          st = mz_topk_window_async(ctx, sorted.as<u64>(), dlen_of(slen, 0), s_ub, tv, to, w.rows.as<u64>(),
+                                    proj.as<u64>(), cap, w.len.dptr());
+          w.len.mark_written();
+          w.ub = cap;
+        }
+        // consolidated by construction: keys ascending, each key's rows sorted by its thread
+        if (st == MZGPU_OK) st = buf_append_dev(out, proj.p, dlen_of(w.len, 0), cap);
+      } else {
+        DevMem proj;
+        u64 n_win = 0;
+        if (st == MZGPU_OK) st = slen.resolve();
+        if (st == MZGPU_OK)
+          st = mz_topk_window(ctx, sorted.as<u64>(), slen.v[0], tv, to, &w.rows, &proj, &n_win);
+        if (st == MZGPU_OK && n_win) {
+          w.len.set(ctx, n_win);
+          w.ub = n_win;
+          st = buf_append_dev(out, proj.p, dlen_imm(n_win), n_win);
+        }
+      }
+    }
+    if (st != MZGPU_OK) return st;  // nothing sealed yet: the operator stays usable
+    if (w.ub) MZ_TRY(batcher_push_seg(r->batcher, std::move(w)));
+  }
+  mzgpu_batch* batch = nullptr;
+  MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
+  // as in monotonic_dev: a failure after the seal kills the operator
+  int32_t ins = MZGPU_OK;
+  if (batch->desc.lower != batch->desc.upper) ins = mzgpu_spine_insert(r->input, batch);
+  mzgpu_batch_release(batch);
+  st = ins;
+  if (st != MZGPU_OK && !ctx->sticky) {
+    r->failed = st;
+    r->failed_msg = ctx->last_error;
+  }
+  return st;
+}
+
+static bool topk_monotonic_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
+  return r->topk_mono && in_rb == r->tko.in_words * 8 && out->rb == in_rb && errs->rb == 16 && out != errs;
+}
+extern "C" int32_t mzgpu_topk_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                        mzgpu_buf* out, mzgpu_buf* errs) {
+  if (r == nullptr || out == nullptr || errs == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = r->ctx;
+  MZ_CHECK_CTX(ctx);
+  const uint32_t in_rb = r->tko.in_words * 8;
+  if (!topk_monotonic_io_ok(r, in_rb, out, errs)) {
+    MZ_SET_ERR(ctx, "topk_monotonic: output buffer of %u-byte rows / error buffer of %u-byte rows", out->rb,
+               errs->rb);
+    return MZGPU_E_INVALID;
+  }
+  ctx->stats.rows_in += n;
+  DevMem in;
+  const u64* d_rows = (const u64*)rows;
+  if (mem == MZGPU_MEM_HOST && n) {
+    MZ_TRY(in.alloc(ctx, n * in_rb));
+    MZ_TRY(copy_in(ctx, in.p, rows, n * in_rb, mem));
+    d_rows = in.as<u64>();
+  }
+  return topk_monotonic_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
+}
+extern "C" int32_t mzgpu_topk_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                            mzgpu_buf* errs) {
+  if (r == nullptr || rows == nullptr || out == nullptr || errs == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(r->ctx);
+  if (!topk_monotonic_io_ok(r, rows->rb, out, errs)) {
+    MZ_SET_ERR(r->ctx, "topk_monotonic: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes",
+               rows->rb, out->rb, errs->rb);
+    return MZGPU_E_INVALID;
+  }
+  r->ctx->stats.rows_in += rows->ub;
+  return topk_monotonic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
 }
 
 // ============================================================ Row keys as words (f1, first step)

@@ -1667,6 +1667,277 @@ __global__ void __launch_bounds__(RT) k_monotonic_corrections_lb(const u64* __re
   }
 }
 
+// ------------------------------------------------------------ monotonic TopK
+// MonotonicTop1 / MonotonicTopK (src/compute/src/render/top_k.rs:102-214) for append-only inputs:
+// ensure_monotonic keeps a row iff its diff is positive, and the arrangement holds only the window, the
+// first `limit` units per key in order.  Window rows are RowT<72>: key, o0, o1, o2, val1, val2, time | diff.
+constexpr int TK_NW = 9;
+
+// Input rows -> one window row per row with diff > 0 (at arr[cnt[0]++]) and one R16 (time, +1) row per
+// other row (at errs[cnt[1]++]); warp-aggregated slots, as k_monotonic_explode.
+__global__ void __launch_bounds__(RT) k_topk_explode(const u64* __restrict__ rows, const DLen dn,
+                                                     const __grid_constant__ TopKOrder to, u64* __restrict__ arr,
+                                                     u64* __restrict__ errs, unsigned long long* __restrict__ cnt) {
+  const u64 n = dlen_get(dn);
+  const u32 iw = to.in_words, lane = lane_id();
+  for (u64 base = (u64)blockIdx.x * RT; base < n; base += (u64)gridDim.x * RT) {
+    const u64 i = base + threadIdx.x;
+    const bool valid = i < n;
+    const u64* r = rows + (valid ? i : 0) * iw;
+    const i64 diff = valid ? (i64)r[iw - 1] : 0;
+    const bool ok = valid && diff > 0, bad = valid && diff <= 0;
+    const u32 mok = __ballot_sync(0xffffffffu, ok), mbad = __ballot_sync(0xffffffffu, bad);
+    unsigned long long bok = 0, bbad = 0;
+    if (lane == 0) {
+      if (mok) bok = atomicAdd(&cnt[0], (unsigned long long)__popc(mok));
+      if (mbad) bbad = atomicAdd(&cnt[1], (unsigned long long)__popc(mbad));
+    }
+    bok = __shfl_sync(0xffffffffu, bok, 0);
+    bbad = __shfl_sync(0xffffffffu, bbad, 0);
+    const u32 lt = (1u << lane) - 1;
+    if (ok) {
+      const u64 key = r[0], v1 = r[1], v2 = iw == 5 ? r[2] : 0;
+      u64 o[TK_NW];
+      o[0] = key;
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        u64 v = 0;
+        if ((u32)j < to.n) {
+          v = field_get(to.f[j], key, v1, v2);
+          const u32 bits = to.f[j].bits;
+          if (to.sign_extend[j] && bits < 64 && ((v >> (bits - 1)) & 1)) v |= ~0ull << bits;
+          v ^= to.xm[j];
+        }
+        o[1 + j] = v;
+      }
+      o[4] = v1;
+      o[5] = v2;
+      o[6] = r[iw - 2];
+      o[7] = (u64)diff;
+      o[8] = 0;
+      store_row<TK_NW>(arr, bok + __popc(mok & lt), o);
+    }
+    if (bad) {
+      const u64 e[2] = {r[iw - 2], 1};
+      store_row<2>(errs, bbad + __popc(mbad & lt), e);
+    }
+  }
+}
+
+// the key's run in every batch of the window arrangement (one hash probe per batch); returns the count
+__device__ __forceinline__ int tk_runs(const TraceView& tv, u64 key, u64* lo, u64* hi, uint8_t* bsel) {
+  int nc = 0;
+  const u64 h0 = mix64(key);
+  for (u32 b = 0; b < tv.n_batches; ++b) {
+    const BatchView& bv = tv.b[b];
+    const u64 mask = bv_mask(bv);
+    u64 h = h0 & mask;
+    while (true) {
+      const ulonglong2 sl = *reinterpret_cast<const ulonglong2*>(&bv.table[h]);
+      if (sl.y == 0) break;
+      if (sl.x == key) {
+        const u64 first = (sl.y & MZ_SLOT_ROW_MASK) - 1;
+        const u32 len = (u32)(sl.y >> 44);
+        u64 end = first + len;
+        if (len == 0) {  // run length not recorded: upper bound search (rows are sorted by key)
+          u64 l = first + 1, r = bv_n(bv);
+          while (l < r) {
+            const u64 mid = (l + r) >> 1;
+            if (bv.rows[mid * TK_NW] == key)
+              l = mid + 1;
+            else
+              r = mid;
+          }
+          end = l;
+        }
+        lo[nc] = first;
+        hi[nc] = end;
+        bsel[nc] = (uint8_t)b;
+        ++nc;
+        break;
+      }
+      h = (h + 1) & mask;
+    }
+  }
+  return nc;
+}
+
+// a < b on the row words 1..5 (o0, o1, o2, val1, val2): the order within a key
+__device__ __forceinline__ bool tk_less(const u64* a, const u64* b) {
+#pragma unroll
+  for (int w = 1; w <= 5; ++w)
+    if (a[w] != b[w]) return a[w] < b[w];
+  return false;
+}
+__device__ __forceinline__ bool tk_same(const u64* a, const u64* b) {
+  return a[1] == b[1] && a[2] == b[2] && a[3] == b[3] && a[4] == b[4] && a[5] == b[5];
+}
+
+// The window changes of one key whose new rows are nrows[i, nhi) (sorted by (row, time), consolidated,
+// every diff positive).  The key's live window is the merge of its runs in the window arrangement, diffs
+// summed.  The new rows are replayed one distinct time t at a time: the window at t is the first `limit`
+// units of (window ∪ new rows with time <= t), so a row r holds min(units of r, limit - units before r),
+// clamped at 0, and every row whose share changes from the previous time emits (r, t, change).  A pass
+// stops where the units before reach the limit at the previous time: no row past that point is in either
+// window, now or at any later time, so the next time is the least later time among the rows it visited.
+// Returns the count; writes the window rows at win[pos ...] and the same rows at the input width (IW words)
+// at out[pos ...], the latter sorted, if WRITE.
+template <int IW, bool WRITE>
+__device__ __noinline__ u32 tk_key(const TraceView& tv, const u64* __restrict__ nrows, u64 i, u64 nhi, u64 key,
+                                   i64 limit, u64* __restrict__ win, u64* __restrict__ out, u64 pos) {
+  if (limit == 0) return 0;
+  u64 lo0[MM_MAX_RUNS], hi[MM_MAX_RUNS], lo[MM_MAX_RUNS];
+  uint8_t bsel[MM_MAX_RUNS];
+  // LIMIT NULL: every kept row enters, nothing is read
+  const int nc = limit == INT64_MAX ? 0 : tk_runs(tv, key, lo0, hi, bsel);
+  bool have_prev = false, have_cur = false;
+  u64 tprev = 0, tcur = 0;
+  u32 c = 0;
+  while (true) {
+    for (int k = 0; k < nc; ++k) lo[k] = lo0[k];
+    u64 nlo = i;
+    i64 cp = 0, cc = 0;  // units before the current row at the previous / current time
+    bool have_next = false;
+    u64 tnext = ~0ull;
+    while (cp < limit) {
+      const u64* best = nullptr;
+      for (int k = 0; k < nc; ++k) {
+        if (lo[k] >= hi[k]) continue;
+        const u64* r = tv.b[bsel[k]].rows + lo[k] * TK_NW;
+        if (best == nullptr || tk_less(r, best)) best = r;
+      }
+      if (nlo < nhi) {
+        const u64* r = nrows + nlo * TK_NW;
+        if (best == nullptr || tk_less(r, best)) best = r;
+      }
+      if (best == nullptr) break;
+      u64 g[TK_NW];
+      load_row<TK_NW>(best, 0, g);
+      i64 o = 0, np = 0, ncur = 0;
+      for (int k = 0; k < nc; ++k) {
+        const u64* rows = tv.b[bsel[k]].rows;
+        while (lo[k] < hi[k] && tk_same(rows + lo[k] * TK_NW, g)) {
+          o += (i64)rows[lo[k] * TK_NW + 7];
+          ++lo[k];
+        }
+      }
+      while (nlo < nhi && tk_same(nrows + nlo * TK_NW, g)) {
+        const u64 t = nrows[nlo * TK_NW + 6];
+        const i64 d = (i64)nrows[nlo * TK_NW + 7];
+        if (have_prev && t <= tprev) np += d;
+        if (have_cur && t <= tcur) ncur += d;
+        if ((!have_cur || t > tcur) && t < tnext) {
+          tnext = t;
+          have_next = true;
+        }
+        ++nlo;
+      }
+      const i64 mp = o + np, mc = o + ncur;
+      const i64 wp = limit - cp <= 0 ? 0 : (mp < limit - cp ? mp : limit - cp);
+      const i64 wc = limit - cc <= 0 ? 0 : (mc < limit - cc ? mc : limit - cc);
+      if (have_cur && wc != wp) {
+        if (WRITE) {
+          g[0] = key;
+          g[6] = tcur;
+          g[7] = (u64)(wc - wp);
+          g[8] = 0;
+          store_row<TK_NW>(win, pos + c, g);
+          u64 p[IW];
+          p[0] = key;
+          p[1] = g[4];
+          if (IW == 5) p[2] = g[5];
+          p[IW - 2] = tcur;
+          p[IW - 1] = (u64)(wc - wp);
+          store_row<IW>(out, pos + c, p);
+        }
+        ++c;
+      }
+      cp += mp;
+      cc += mc;
+    }
+    if (!have_next) break;
+    tprev = tcur;
+    have_prev = have_cur;
+    tcur = tnext;
+    have_cur = true;
+  }
+  if (WRITE && c > 1) sort_run_rows<IW, IW - 2>(out, pos, c);
+  return c;
+}
+
+// the key's new rows [i, end): end of its run in the new batch
+__device__ __forceinline__ u64 tk_run_end(const u64* __restrict__ rows, u64 n, u64 i, u64 key) {
+  u64 j = i + 1;
+  while (j < n && rows[j * TK_NW] == key) ++j;
+  return j;
+}
+
+// single-pass form (sizes on the device, chained tiles), as k_monotonic_corrections_lb: one thread per key
+// run of the new rows
+template <int IW>
+__global__ void __launch_bounds__(RT) k_topk_window_lb(const u64* __restrict__ rows, const DLen dn,
+                                                       const __grid_constant__ TraceView prior, const i64 limit,
+                                                       const LookBack lb, u64* __restrict__ win, u64* __restrict__ out,
+                                                       u64 out_cap, u64* __restrict__ out_len, u64* __restrict__ status) {
+  __shared__ u32 sm[34];
+  __shared__ u32 s_tile;
+  __shared__ u64 s_b;
+  const u64 n = dlen_get(dn);
+  const u64 n_tiles = (n + RT - 1) / RT;
+  while (true) {
+    const u32 tile = lb_next_tile(lb, &s_tile);
+    if ((u64)tile >= n_tiles) {
+      if (n_tiles == 0 && tile == 0 && threadIdx.x == 0) *out_len = 0;
+      break;
+    }
+    const u64 i = (u64)tile * RT + threadIdx.x;
+    u32 cnt = 0;
+    const bool head = i < n && (i == 0 || rows[(i - 1) * TK_NW] != rows[i * TK_NW]);
+    u64 key = 0, end = 0;
+    if (head) {
+      key = rows[i * TK_NW];
+      end = tk_run_end(rows, n, i, key);
+      cnt = tk_key<IW, false>(prior, rows, i, end, key, limit, nullptr, nullptr, 0);
+    }
+    u32 total;
+    const u32 ex = block_exclusive_scan(cnt, sm, &total);
+    const u64 excl = lb_exclusive_prefix(lb, tile, (u64)total, &s_b);
+    if (head && cnt > 0) {
+      const u64 pos = excl + ex;
+      if (pos + cnt > out_cap)
+        atomicMax((unsigned long long*)status, (unsigned long long)(pos + cnt));
+      else
+        tk_key<IW, true>(prior, rows, i, end, key, limit, win, out, pos);
+    }
+    if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *out_len = excl + total;
+  }
+}
+
+// the two-pass form (count, read back, write) for a batch past the single-pass bound
+template <int IW, bool WRITE>
+__global__ void __launch_bounds__(RT) k_topk_window(const u64* __restrict__ rows, u64 n,
+                                                    const __grid_constant__ TraceView prior, const i64 limit,
+                                                    u32* __restrict__ tile_counts, const u32* __restrict__ tile_base,
+                                                    u64* __restrict__ win, u64* __restrict__ out) {
+  __shared__ u32 sm[34];
+  const u64 i = (u64)blockIdx.x * RT + threadIdx.x;
+  u32 cnt = 0;
+  const bool head = i < n && (i == 0 || rows[(i - 1) * TK_NW] != rows[i * TK_NW]);
+  u64 key = 0, end = 0;
+  if (head) {
+    key = rows[i * TK_NW];
+    end = tk_run_end(rows, n, i, key);
+    cnt = tk_key<IW, false>(prior, rows, i, end, key, limit, nullptr, nullptr, 0);
+  }
+  u32 total;
+  const u32 ex = block_exclusive_scan(cnt, sm, &total);
+  if (!WRITE) {
+    if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
+  } else if (head && cnt > 0) {
+    tk_key<IW, true>(prior, rows, i, end, key, limit, win, out, (u64)tile_base[blockIdx.x] + ex);
+  }
+}
+
 }  // namespace
 
 int32_t mz_distinct_pairs(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
@@ -1893,6 +2164,65 @@ int32_t mz_monotonic_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows,
   return mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
     MZ_LAUNCH(ctx, (k_monotonic_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, mx,
               (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
+    return MZGPU_OK;
+  });
+}
+
+int32_t mz_topk_explode(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TopKOrder& to, u64* d_arr,
+                        u64* d_errs, u64* d_cnt) {
+  MZ_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 16, ctx->stream));
+  if (n_ub == 0) return MZGPU_OK;
+  u64 grid = (n_ub + RT - 1) / RT;
+  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (to.in_words * 8 + TK_NW * 8) : 0);
+  MZ_LAUNCH(ctx, k_topk_explode, (unsigned)grid, RT, 0, d_rows, n, to, d_arr, d_errs, (unsigned long long*)d_cnt);
+  return MZGPU_OK;
+}
+
+struct TopKInWords : IntSet<4, 5> {  // R32 / R40 input
+  static constexpr const char* kind = "input row words";
+};
+
+int32_t mz_topk_window_async(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TraceView& prior,
+                             const TopKOrder& to, u64* d_win, u64* d_out, u64 out_cap, u64* d_out_len) {
+  LookBack lb;
+  MZ_TRY(mz_lookback_begin(ctx, (n_ub + RT - 1) / RT, &lb));
+  u64 grid = (n_ub + RT - 1) / RT;
+  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  if (grid == 0) grid = 1;
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * 2 * TK_NW * 8 : 0);
+  return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
+    MZ_LAUNCH(ctx, k_topk_window_lb<IW>, (unsigned)grid, RT, 0, d_rows, n, prior, to.limit, lb, d_win, d_out,
+              out_cap, d_out_len, ctx->d_status);
+    return MZGPU_OK;
+  });
+}
+
+int32_t mz_topk_window(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView& prior, const TopKOrder& to,
+                       DevMem* win, DevMem* out, u64* n_out) {
+  *n_out = 0;
+  if (n == 0) return MZGPU_OK;
+  const u64 n_tiles = (n + RT - 1) / RT;
+  DevMem tiles;
+  MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
+  u64* d_total = ctx->d_scratch + 30;
+  MZ_TRY(mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
+    MZ_LAUNCH(ctx, (k_topk_window<IW, false>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, to.limit,
+              tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr, (u64*)nullptr);
+    return MZGPU_OK;
+  }));
+  MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
+  MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 30, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  MZ_SYNC(ctx);
+  ctx->stats.d2h_bytes += 8;
+  const u64 total = ctx->h_scratch[30];
+  *n_out = total;
+  if (total == 0) return MZGPU_OK;
+  MZ_TRY(win->alloc(ctx, total * TK_NW * 8));
+  MZ_TRY(out->alloc(ctx, total * to.in_words * 8));
+  return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
+    MZ_LAUNCH(ctx, (k_topk_window<IW, true>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, to.limit,
+              (u32*)nullptr, tiles.as<u32>(), win->as<u64>(), out->as<u64>());
     return MZGPU_OK;
   });
 }

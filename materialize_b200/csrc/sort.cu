@@ -256,7 +256,8 @@ int32_t sort_perm_t(mzgpu_ctx* ctx, const u64* d_rows, u64 n, DevMem* perm_out) 
     int used = 0;
     for (int k = NK - 1; k >= 0; --k) {
       if (wbits[k] == 0) continue;
-      if (used + wbits[k] > 64) {
+      // (a chunk holds at most 6 words: only the 7-word TopK window rows can reach that)
+      if (used + wbits[k] > 64 || cur.nwords == 6) {
         chunks.push_back(cur);
         cur.nwords = 0;
         used = 0;

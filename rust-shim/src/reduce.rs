@@ -134,6 +134,35 @@ impl Drop for GpuReduceMonotonic {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
 }
 
+/// `TopKPlan::MonotonicTop1` / `MonotonicTopK` (top_k.rs:102-214 of src/compute/src/render): the first
+/// `limit` rows per key of an append-only input, with only that window arranged
+/// (`sys::mzgpu_topk_monotonic_new` documents the order and the window rows).  Top1 is `limit = 1`;
+/// `LIMIT NULL` is `sys::TOPK_NO_LIMIT`.  A negative literal limit or a float64 order column
+/// (`sys::ORDER_F64`) comes back as `MZGPU_E_UNSUPPORTED`: the caller keeps the Rust operator for those,
+/// and for a limit given as an expression.
+pub struct GpuTopKMonotonic { h: *mut sys::Reduce }
+
+impl GpuTopKMonotonic {
+    pub fn new(in_row_bytes: u32, order: &[sys::OrderLane], limit: i64, must_consolidate: bool) -> Result<Self, (i32, String)> {
+        let mut h = std::ptr::null_mut();
+        unsafe {
+            sys::check(worker_ctx(), sys::mzgpu_topk_monotonic_new(worker_ctx(), in_row_bytes, order.as_ptr(),
+                                                                  order.len() as u32, limit, must_consolidate as i32, &mut h))?;
+        }
+        Ok(GpuTopKMonotonic { h })
+    }
+    /// One activation over a device buffer of input rows: the window changes (input-width rows) are appended
+    /// to `out`, the `ensure_monotonic` errors (R16: time, count) to `errs`.
+    pub fn step(&mut self, rows: *mut sys::Buf, upper: u64, out: *mut sys::Buf, errs: *mut sys::Buf) -> Result<(), (i32, String)> {
+        unsafe { sys::check(worker_ctx(), sys::mzgpu_topk_monotonic_buf(self.h, rows, upper, out, errs)) }
+    }
+    /// The window arrangement (72-byte rows), compacted by the caller like any other trace.
+    pub fn window_trace(&self) -> *mut sys::Spine { unsafe { sys::mzgpu_reduce_input_trace(self.h) } }
+}
+impl Drop for GpuTopKMonotonic {
+    fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
+}
+
 impl Drop for GpuReduce {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
 }

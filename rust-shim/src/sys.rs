@@ -58,6 +58,13 @@ pub struct Field { pub src: u8, pub shift: u8, pub bits: u8, pub dst_shift: u8 }
 /// One aggregate lane of the multi-column accumulable reduce (mzgpu_accum_lane).
 #[repr(C)] #[derive(Clone, Copy, Debug, Default)]
 pub struct AccumLane { pub kind: i32, pub sign_extend: u32, pub field: Field }
+/// One `ColumnOrder` of a monotonic TopK's order key (`mzgpu_order_lane`).
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct OrderLane { pub sign_extend: u32, pub descending: u32, pub flags: u32, pub field: Field }
+/// `OrderLane::flags`: the column is float64 (always `E_UNSUPPORTED`).
+pub const ORDER_F64: u32 = 0x1;
+/// `LIMIT NULL` of a monotonic TopK.
+pub const TOPK_NO_LIMIT: i64 = i64::MAX;
 /// HAVING: the filter half of a reduce's mfp_after (mzgpu_having; include/mzgpu.h has the semantics).
 pub const HAVING_MAX_PREDICATES: usize = 4;
 pub const HAVING_MAX_OPS: usize = 16;
@@ -204,6 +211,9 @@ extern "C" {
     pub fn mzgpu_reduce_monotonic_new(ctx: *mut Ctx, in_row_bytes: u32, lanes: *const AccumLane, n_lanes: u32, must_consolidate: i32, out: *mut *mut Reduce) -> i32;
     pub fn mzgpu_reduce_monotonic(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_reduce_monotonic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_topk_monotonic_new(ctx: *mut Ctx, in_row_bytes: u32, order: *const OrderLane, n_order: u32, limit: i64, must_consolidate: i32, out: *mut *mut Reduce) -> i32;
+    pub fn mzgpu_topk_monotonic(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_topk_monotonic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_rowkey_pack(row_bytes: *const u8, len: u64, key_out: *mut u64) -> i32;
     pub fn mzgpu_rowkeys_pack(data: *const u8, offsets: *const u64, n: u64, keys_out: *mut u64, n_done: *mut u64) -> i32;
     pub fn mzgpu_rowkey_unpack(key: u64, row_bytes_out: *mut u8, len_out: *mut u64) -> i32;
