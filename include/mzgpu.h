@@ -220,8 +220,12 @@ typedef struct mzgpu_closure {
  * count yields the error row ("Non-positive accumulation in MinsMaxesHierarchical", flags bit1),
  * otherwise func(values).  Values compare as unsigned 64-bit integers.  ROUT rows: sum_lo = the
  * aggregate, count = sum_hi = 0.  The reference buckets large groups into a reduction tree; this
- * operator evaluates a key's values directly and reports MZGPU_E_UNSUPPORTED (at the next
- * read-back) for a key with more than 32 distinct live values. */
+ * operator evaluates a key's values directly, for any number of distinct live values (a key with more
+ * than 32 is walked in value order over its runs).  An activation is evaluated in one pass: a sealed
+ * batch of more than 24 Mi rows (MIN / MAX) is refused with MZGPU_E_UNSUPPORTED and the operator
+ * reports that status from then on.  The limit applies to the batch's actual row count: a sealed batch
+ * whose length bound is past it (such as one sealed from a device-resident input whose buffer bound is
+ * loose) has its length read back first, and runs if the rows fit. */
 #define MZGPU_AGG_MIN 4
 #define MZGPU_AGG_MAX 5
 /* TopK per key (BasicTopKPlan, src/compute/src/render/top_k.rs:215-248 and the reduction logic of
@@ -231,8 +235,12 @@ typedef struct mzgpu_closure {
  * The operator emits the changes of that window directly (the reference emits its negated complement
  * and concatenates it with the input: the same collection).  ROUT rows: sum_lo = the value,
  * diff = the change of the value's multiplicity inside the window, count = sum_hi = 0.  The staged
- * bucket tree (build_topk, :251-380) bounds per-key work for huge groups; as for MIN/MAX a key with more
- * than 32 distinct live values is reported MZGPU_E_UNSUPPORTED.  Created by mzgpu_topk_new. */
+ * bucket tree (build_topk, :251-380) bounds per-key work for huge groups; here, as for MIN/MAX, groups
+ * of any width are evaluated, and only a WINDOW of more than 32 distinct values (LIMIT above 32, or
+ * none, on a key that wide) is reported MZGPU_E_UNSUPPORTED (at the next read-back; the report poisons
+ * the context).  The single-pass bound is 48 Mi / (2 * min(limit, 32) + 2) rows of the sealed batch
+ * (LIMIT NULL counts as 32: 762,600 rows; LIMIT 1: 12 Mi), refused as for MIN / MAX.  Created by
+ * mzgpu_topk_new. */
 #define MZGPU_AGG_TOPK 6
 
 /* ---------------------------------------------------------------- handles */

@@ -593,8 +593,17 @@ def map_rows(ctx, rows, closure):
 
 
 class ReduceAccumulable:
+    """One-column reduce (mzgpu_reduce_new).  The operator is freed with this object, and a Spine from
+    input_trace() borrows the operator's arrangement: it must not outlive the operator."""
+
+    # the input arrangement's rows: exploded accumulators (mzgpu_racc), or the (key, value) rows
+    # themselves for MIN / MAX / TopK
+    row_bytes = 80
+
     def __init__(self, ctx, agg_kind=F.AGG_COUNT_SUM_I64):
         self.ctx = ctx
+        if agg_kind in (F.AGG_MIN, F.AGG_MAX):
+            self.row_bytes = 32
         h = C.c_void_p()
         ctx.check(F.lib.mzgpu_reduce_new(ctx.h, agg_kind, C.byref(h)))
         self.h = h
@@ -612,7 +621,12 @@ class ReduceAccumulable:
         return out
 
     def input_trace(self):
-        return Spine(self.ctx, 80, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+        return Spine(self.ctx, self.row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_reduce_free(self.h)
+            self.h = None
 
 
 def accum_lane(kind, src=SRC_VAL1, shift=0, bits=64, sign_extend=False):
@@ -870,17 +884,14 @@ class TopK(ReduceAccumulable):
     """TopK per key over (key, value) rows (BasicTopKPlan, src/compute/src/render/top_k.rs:215-248,
     521-673): `limit` < 0 or None = no limit; stepped like every other reduce kind."""
 
+    row_bytes = 32
+
     def __init__(self, ctx, limit, offset=0, descending=False):
         self.ctx = ctx
         h = C.c_void_p()
         lim = -1 if limit is None else int(limit)
         ctx.check(F.lib.mzgpu_topk_new(ctx.h, lim, int(offset), 1 if descending else 0, C.byref(h)))
         self.h = h
-
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            F.lib.mzgpu_reduce_free(self.h)
-            self.h = None
 
 
 def route(key, peers):

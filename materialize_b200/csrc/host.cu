@@ -2720,40 +2720,48 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
   const u64 out_rb = (u64)mz_lane_out_bytes(lc);
   const LaneSet* ls = r->lane_class ? &r->lanes : nullptr;
   const mzgpu_having* hv = r->has_having ? &r->having : nullptr;
-  if (st == MZGPU_OK && b_ub > 0) {
-    if ((b_ub + 255) / 256 <= MZ_LB_TILES && per_row * b_ub <= MZ_BOUND_MAX_ROWS) {
+  // The single-pass form needs per_row output rows per row of the batch within MZ_BOUND_MAX_ROWS.  The
+  // bound is checked against the batch's length bound; when that is loose (a device-resident input
+  // buffer's capacity), the length is read back and checked again before the two-pass form is used.
+  auto single_pass_fits = [&](u64 n) { return (n + 255) / 256 <= MZ_LB_TILES && per_row * n <= MZ_BOUND_MAX_ROWS; };
+  u64 s_ub = b_ub;
+  if (st == MZGPU_OK && b_ub > 0 && !single_pass_fits(b_ub)) {
+    st = batch_resolve(batch);
+    if (st == MZGPU_OK) s_ub = batch->st.v[0];
+  }
+  if (st == MZGPU_OK && s_ub > 0) {
+    if (single_pass_fits(s_ub)) {
       DevMem corr, cons;
       Lazy4 clen, flen;
       u64 ccap = 0;
-      st = corr.alloc(ctx, per_row * b_ub * out_rb);
+      st = corr.alloc(ctx, per_row * s_ub * out_rb);
       if (st == MZGPU_OK) st = clen.make_pending(ctx);
       if (st == MZGPU_OK) {
         if (minmax)
-          st = mz_reduce_minmax_async(ctx, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv, r->agg_kind,
-                                      r->topk, corr.as<u64>(), per_row * b_ub, clen.dptr());
+          st = mz_reduce_minmax_async(ctx, batch->rows.as<u64>(), batch_dlen(batch), s_ub, tv, r->agg_kind,
+                                      r->topk, corr.as<u64>(), per_row * s_ub, clen.dptr());
         else
-          st = mz_reduce_corrections_async(ctx, lc, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv,
-                                           r->agg_kind, ls, corr.as<u64>(), per_row * b_ub, clen.dptr(), hv);
+          st = mz_reduce_corrections_async(ctx, lc, batch->rows.as<u64>(), batch_dlen(batch), s_ub, tv,
+                                           r->agg_kind, ls, corr.as<u64>(), per_row * s_ub, clen.dptr(), hv);
         clen.mark_written();
       }
       if (st == MZGPU_OK && !minmax) {
         // the accumulable kinds' corrections leave the kernel consolidated (reduce.cu:
         // sort_key_corrections): keys ascending, each key's few rows sorted by its thread
-        st = buf_append_dev(out, corr.p, dlen_of(clen, 0), per_row * b_ub);
+        st = buf_append_dev(out, corr.p, dlen_of(clen, 0), per_row * s_ub);
       } else {
         if (st == MZGPU_OK)
-          st = consolidate_dev(ctx, 64, corr.p, dlen_of(clen, 0), per_row * b_ub, &cons, &ccap, &flen);
+          st = consolidate_dev(ctx, 64, corr.p, dlen_of(clen, 0), per_row * s_ub, &cons, &ccap, &flen);
         if (st == MZGPU_OK)
-          st = buf_append_dev(out, cons.p, dlen_of(flen, 0), flen.known ? flen.v[0] : per_row * b_ub);
+          st = buf_append_dev(out, cons.p, dlen_of(flen, 0), flen.known ? flen.v[0] : per_row * s_ub);
       }
     } else {
       DevMem corr, cons;
       u64 n_corr = 0, ccap = 0;
       Lazy4 flen;
-      st = batch_resolve(batch);
-      if (st == MZGPU_OK && minmax) {
+      if (minmax) {
         MZ_SET_ERR(ctx, "MIN/MAX/TopK reduce: batch of %llu rows exceeds the single-pass bound",
-                   (unsigned long long)b_ub);
+                   (unsigned long long)s_ub);
         st = MZGPU_E_UNSUPPORTED;
       }
       if (st == MZGPU_OK)
