@@ -6,6 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import lanes_paths_ref as R
 from having_oracle import ERR_SHIFT, ReduceLanesHaving, cmp, count, div, int_, key, num, sum_
 from test_oracle_distinct_lanes import D, distinct_activations
 from test_oracle_having import (
@@ -25,6 +26,7 @@ from test_oracle_having import (
     run_having_sum,
     run_steps,
 )
+from test_gpu_reduce_paths import _key_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -100,16 +102,19 @@ def test_evaluator_cases_on_one_key_gpu_operators(mz, ctx, oracle):
             assert (int(g[0]["flags"]) >> ERR_SHIFT) & 7 == want[1], (preds, want)
 
 
-@pytest.mark.parametrize("n_lanes", [1, 2, 4])
+@pytest.mark.parametrize("n_lanes", [1, 2, 4, 8])
 def test_two_pass_path_past_the_single_pass_bound(mz, n_lanes):
     """Batches of 26 M distinct keys: at two output rows per new (key, time) that is past the single-pass bound
-    (48 Mi output rows), so the corrections run in the two-pass form, k_corrections_having<C, false / true>;
-    the profile report shows which kernels ran.  One time per key and activation, so the filtered corrections
-    are exactly the unfiltered operator's corrections that the filter lets through, with the error bits added:
-    the predicates are COUNT / (key & 255) >= 0 (a division by zero on every 256th key) and SUM(lane 0) < 0.
-    The second activation retracts half of the keys and adds a row to the other half (the prior batch is
-    read back through the hash index)."""
-    lanes = [(I64, VAL1, 0, 32, True), (I64, VAL2, 0, 64, False), (I64, VAL1, 32, 32, True), (F64, VAL2, 0, 64, False)][:n_lanes]
+    (48 Mi output rows), so the corrections run in the two-pass form, k_corrections<C, false / true> without a
+    filter and k_corrections_having<C, false / true> with one; the profile report shows which kernels ran.
+    The unfiltered output is compared row for row with the NumPy expectation of tests/lanes_paths_ref.py (in
+    key-rank slices, to bound host memory), and its arrangement on 2000 sampled keys.  One time per key and
+    activation, so the filtered corrections are exactly the unfiltered operator's corrections that the filter
+    lets through, with the error bits added: the predicates are COUNT / (key & 255) >= 0 (a division by zero
+    on every 256th key) and SUM(lane 0) < 0.  The second activation retracts half of the keys and adds a row
+    to the other half (the prior batch is read back through the hash index).  val2 holds float64 bits
+    (NaN, +-inf, -0.0 among them) for the float64 lane."""
+    lanes = R.LANES8[:n_lanes]  # bit-fields of val1 and val2 and, from 4 lanes on, the float64 lane of val2
     preds = [[count(0), key(0, 8), div(64), int_(0), cmp("ge")], [sum_(0), num(0), cmp("lt")]]
     rng = np.random.default_rng(50 + n_lanes)
     n = 26_000_000
@@ -117,14 +122,16 @@ def test_two_pass_path_past_the_single_pass_bound(mz, n_lanes):
     first = np.zeros(n, dtype=mz.R40)
     first["key"] = keys
     first["val1"] = rng.integers(0, 2**64, size=n, dtype=np.uint64)
-    first["val2"] = rng.integers(-(2**40), 2**40, size=n, dtype=np.int64).view(np.uint64)
+    first["val2"] = R.f64_words(rng, n)
     first["diff"] = 1
     second = first.copy()
     second["time"] = 1
     back = rng.random(n) < 0.5
     second["diff"] = np.where(back, -1, 1)
     second["val1"] = np.where(back, first["val1"], rng.integers(0, 2**64, size=n, dtype=np.uint64))
+    second["val2"] = np.where(back, first["val2"], R.f64_words(rng, n))
     batches = [(first, 1), (second, 2)]
+    w1, w2 = (np.ascontiguousarray(b).view(np.uint64).reshape(n, 5) for b in (first, second))
 
     def run(having):
         c = mz.Context(0)
@@ -133,16 +140,33 @@ def test_two_pass_path_past_the_single_pass_bound(mz, n_lanes):
         c.profile_report()
         outs = [op.step(b, upper) for b, upper in batches]
         kernels = set(c.profile_report())
+        if having is None:
+            pick = np.sort(rng.choice(n, size=2000, replace=False))
+            got = _key_rows(mz, c, op, w1[pick, 0])
+            assert got.tobytes() == R.two_pass_arrangement("lanes", lanes, w1, w2, pick).tobytes()
+        print(f"having two-pass, {n_lanes} lanes{'' if having is None else ', filtered'}: device_bytes_peak",
+              c.stats()["device_bytes_peak"])
         del op
         c.close()
         return outs, kernels
 
     plain, plain_kernels = run(None)
+    # the unfiltered output, row for row, in key-rank slices of the expectation
+    keys = np.sort(first["key"])
+    width = 1 << 22
+    for lo in range(0, n, width):
+        hi = min(n, lo + width)
+        want = R.two_pass_expect("lanes", lanes, w1, w2, lo, hi)[:2]
+        for got, w in zip(plain, want):
+            a, b = np.searchsorted(got["key"], keys[lo]), np.searchsorted(got["key"], keys[hi - 1], side="right")
+            g = np.ascontiguousarray(got[a:b]).view(np.uint64).reshape(b - a, -1)
+            assert g.shape == w.shape and g.tobytes() == w.tobytes(), (lo, g.shape, w.shape)
     filtered, kernels = run(mz.having(*preds))
     def ran(names, kernel):  # the profile report writes the launch's kernel expression with "_" for " "
         return any(kernel.replace(" ", "_") in k for k in names)
 
-    assert ran(plain_kernels, "(k_corrections<C, true>)"), plain_kernels
+    assert ran(plain_kernels, "(k_corrections<C, false>)") and ran(plain_kernels, "(k_corrections<C, true>)"), plain_kernels
+    assert not ran(plain_kernels, "k_corrections_lb"), plain_kernels
     assert ran(kernels, "(k_corrections_having<C, false>)"), kernels
     assert ran(kernels, "(k_corrections_having<C, true>)"), kernels
     assert not ran(kernels, "k_corrections_lb"), kernels

@@ -63,7 +63,7 @@ def ctx(mz):
 
 
 class Trace:
-    """Profiling over a block: the names of every kernel launched in it."""
+    """Profiling over a block: the names of every kernel launched in it, and each one's launch count."""
 
     def __init__(self, ctx):
         self.ctx = ctx
@@ -76,7 +76,8 @@ class Trace:
     def __exit__(self, *exc):
         try:
             if exc[0] is None:
-                self.kernels = {k.strip("()") for k in self.ctx.profile_report()}
+                self.launches = {k.strip("()"): v["launches"] for k, v in self.ctx.profile_report().items()}
+                self.kernels = set(self.launches)
         finally:
             self.ctx.profile(False)
 
@@ -104,7 +105,7 @@ MM = dict(never=("k_explode", "k_corrections"))
 
 # ------------------------------------------------------------------ helpers
 def words(a):
-    return aref.words(a, a.dtype.itemsize)
+    return np.ascontiguousarray(a).view(np.uint64).reshape(len(a), a.dtype.itemsize // 8)
 
 
 def r32(mz, w):
@@ -145,16 +146,17 @@ def same_arrangement(g, r):
     same(tr.export(), r.export(tr.get_logical_compaction()))
 
 
-def trace_batches(mz, ctx, g):
-    """The input trace's batches, oldest first (each retained, so they outlive later merges)."""
-    sp = g.input_trace()
+def trace_batches(mz, ctx, g, sp=None):
+    """The batches of g's input trace (or of the spine sp), oldest first (each retained, so they outlive
+    later merges)."""
+    sp = sp if sp is not None else g.input_trace()
     arr = (C.c_void_p * 128)()
     n = C.c_uint32(0)
     ctx.check(mz._ffi.lib.mzgpu_spine_batches_through(sp.h, sp.read_upper(), arr, 128, C.byref(n)))
     out = []
     for i in range(n.value):
         mz._ffi.lib.mzgpu_batch_retain(arr[i])
-        out.append(mz.Batch(ctx, C.c_void_p(arr[i]), g.row_bytes))
+        out.append(mz.Batch(ctx, C.c_void_p(arr[i]), sp.row_bytes))
     return out
 
 
@@ -166,9 +168,10 @@ def slot_len(b, key):
     return None if len(hit) == 0 else int(s[hit[0], 1]) >> 44
 
 
-def zero_slot_batch(mz, ctx, g, key):
-    """A batch of the input trace holding `key` with run length 0 in its slot, and that batch's keys."""
-    for b in trace_batches(mz, ctx, g):
+def zero_slot_batch(mz, ctx, g, key, sp=None):
+    """A batch of the input trace (or of the spine sp) holding `key` with run length 0 in its slot, and
+    that batch's keys."""
+    for b in trace_batches(mz, ctx, g, sp):
         if slot_len(b, key) == 0:
             return b, np.unique(words(b.rows())[:, 0])
     raise AssertionError(f"no batch stores key {key} with slot length 0")
@@ -369,16 +372,17 @@ def _two_pass_expect(kind, keys, v1, v2, back):
     return first, second
 
 
-def _key_rows(mz, ctx, g, keys):
-    """The input trace's rows of `keys`, found through each batch's cursor (seek_keys), consolidated."""
+def _key_rows(mz, ctx, g, keys, merge=aref.consolidate):
+    """The input trace's rows of `keys`, found through each batch's cursor (seek_keys), merged by `merge`
+    (which takes (n, words) u64 rows; the default sums a one-word diff)."""
     keys = np.unique(np.asarray(keys, dtype=np.uint64))
     parts = []
     for b in trace_batches(mz, ctx, g):
         for run in b.seek_keys(keys):
             if run["len"] > 0 and run["key"] in keys:
                 parts.append(words(b.rows_range(int(run["first"]), int(run["len"]))))
-    nw = g.row_bytes // 8
-    return aref.consolidate(np.concatenate(parts) if parts else np.zeros((0, nw), dtype=np.uint64))
+    nw = g.input_trace().row_bytes // 8
+    return merge(np.concatenate(parts) if parts else np.zeros((0, nw), dtype=np.uint64))
 
 
 def _two_pass_arrangement(kind, keys, v1, v2, back):
