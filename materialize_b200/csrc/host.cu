@@ -2626,17 +2626,54 @@ static int32_t distinct_step(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_u
   return batcher_push_seg(r->batcher, std::move(s));
 }
 
+// The start of every reduce activation.  An earlier activation that lost its corrections left the operator
+// dead (not the worker): it reports that status.  Batches sealed by earlier activations are merge-eligible
+// now; their lengths have reached the host with whatever the caller read since (no extra wait).
+static int32_t reduce_begin(mzgpu_reduce* r) {
+  if (r->failed != MZGPU_OK) {
+    r->ctx->last_error = r->failed_msg;
+    return r->failed;
+  }
+  return mzgpu_spine_set_physical_compaction(r->input, r->input->upper);
+}
+
+// A failure once an activation has sealed a batch means its corrections are missing from the output, which
+// no later activation can repair: the operator reports the first such status from now on (a sticky context
+// reports its own).
+static int32_t reduce_kill_on_failure(mzgpu_reduce* r, int32_t st) {
+  if (st != MZGPU_OK && !r->ctx->sticky && r->failed == MZGPU_OK) {
+    r->failed = st;
+    r->failed_msg = r->ctx->last_error;
+  }
+  return st;
+}
+
+// A sealed batch joins its trace whatever happened since the seal (the seal consumed the batcher's rows and
+// advanced its frontier, and the arrangement stays consistent with that frontier); returns the insert's status.
+static int32_t trace_join(mzgpu_spine* trace, mzgpu_batch* batch) {
+  int32_t ins = MZGPU_OK;
+  if (batch->desc.lower != batch->desc.upper) ins = mzgpu_spine_insert(trace, batch);
+  mzgpu_batch_release(batch);
+  return ins;
+}
+
+// The end of an activation after its seal: the batch joins the input trace, then the kill rule on the first
+// failure of the two.
+static int32_t reduce_seal_tail(mzgpu_reduce* r, mzgpu_batch* batch, int32_t st) {
+  const int32_t ins = trace_join(r->input, batch);
+  return reduce_kill_on_failure(r, st != MZGPU_OK ? st : ins);
+}
+
+// The single-pass (look-back) form of the correction kernels covers a batch of n rows with at most per_row
+// output rows each when its tiles fit the look-back state and its output fits MZ_BOUND_MAX_ROWS.
+static bool single_pass_fits(u64 n, u64 per_row) {
+  return (n + 255) / 256 <= MZ_LB_TILES && per_row * n <= MZ_BOUND_MAX_ROWS;
+}
+
 static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
                            bool minmax, u64 per_row);
 static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out) {
-  mzgpu_ctx* ctx = r->ctx;
-  if (r->failed != MZGPU_OK) {  // an earlier activation lost its corrections: the operator is dead, not the worker
-    ctx->last_error = r->failed_msg;
-    return r->failed;
-  }
-  // batches sealed by earlier activations are merge-eligible now; their lengths
-  // have reached the host with whatever the caller read since (no extra wait)
-  MZ_TRY(mzgpu_spine_set_physical_compaction(r->input, r->input->upper));
+  MZ_TRY(reduce_begin(r));
   for (int j = 0; j < r->n_distinct; ++j)
     MZ_TRY(mzgpu_spine_set_physical_compaction(r->pairs[j], r->pairs[j]->upper));
   // explode_one: values move into the diff; the exploded rows become a stash segment
@@ -2657,17 +2694,11 @@ static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, 
   auto finish_pairs = [&](int32_t st) -> int32_t {
     for (int j = 0; j < r->n_distinct; ++j) {
       if (pair_new[j] == nullptr) continue;
-      int32_t ins = MZGPU_OK;
-      if (pair_new[j]->desc.lower != pair_new[j]->desc.upper) ins = mzgpu_spine_insert(r->pairs[j], pair_new[j]);
-      mzgpu_batch_release(pair_new[j]);
+      const int32_t ins = trace_join(r->pairs[j], pair_new[j]);
       pair_new[j] = nullptr;
       if (st == MZGPU_OK) st = ins;
     }
-    if (st != MZGPU_OK && pairs_sealed && !ctx->sticky && r->failed == MZGPU_OK) {
-      r->failed = st;
-      r->failed_msg = ctx->last_error;
-    }
-    return st;
+    return pairs_sealed ? reduce_kill_on_failure(r, st) : st;
   };
   if (r->n_distinct) {
     const int32_t ds = distinct_step(r, d_rows, n, n_ub, upper, pair_new, &pairs_sealed);
@@ -2720,17 +2751,16 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
   const u64 out_rb = (u64)mz_lane_out_bytes(lc);
   const LaneSet* ls = r->lane_class ? &r->lanes : nullptr;
   const mzgpu_having* hv = r->has_having ? &r->having : nullptr;
-  // The single-pass form needs per_row output rows per row of the batch within MZ_BOUND_MAX_ROWS.  The
-  // bound is checked against the batch's length bound; when that is loose (a device-resident input
-  // buffer's capacity), the length is read back and checked again before the two-pass form is used.
-  auto single_pass_fits = [&](u64 n) { return (n + 255) / 256 <= MZ_LB_TILES && per_row * n <= MZ_BOUND_MAX_ROWS; };
+  // The single-pass bound is checked against the batch's length bound; when that is loose (a
+  // device-resident input buffer's capacity), the length is read back and checked again before the
+  // two-pass form is used.
   u64 s_ub = b_ub;
-  if (st == MZGPU_OK && b_ub > 0 && !single_pass_fits(b_ub)) {
+  if (st == MZGPU_OK && b_ub > 0 && !single_pass_fits(b_ub, per_row)) {
     st = batch_resolve(batch);
     if (st == MZGPU_OK) s_ub = batch->st.v[0];
   }
   if (st == MZGPU_OK && s_ub > 0) {
-    if (single_pass_fits(s_ub)) {
+    if (single_pass_fits(s_ub, per_row)) {
       DevMem corr, cons;
       Lazy4 clen, flen;
       u64 ccap = 0;
@@ -2778,19 +2808,21 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
       }
     }
   }
-  // The seal above consumed the batcher's rows and advanced its frontier, so the batch joins the
-  // input trace whatever happened since (the arrangement stays consistent with the frontier); a
-  // failure after the seal means this activation's corrections are missing from `out`, which no
-  // later activation can repair: the operator reports that status from now on.
-  int32_t ins = MZGPU_OK;
-  if (batch->desc.lower != batch->desc.upper) ins = mzgpu_spine_insert(r->input, batch);
-  mzgpu_batch_release(batch);
-  if (st == MZGPU_OK) st = ins;
-  if (st != MZGPU_OK && !ctx->sticky) {
-    r->failed = st;
-    r->failed_msg = ctx->last_error;
+  return reduce_seal_tail(r, batch, st);
+}
+
+// The rows of a host-form reduce entry point (n rows of in_rb bytes) counted into rows_in and, when they are in
+// host memory, uploaded into `in`; *d_rows is where the activation reads them.
+static int32_t reduce_rows_in(mzgpu_ctx* ctx, const void* rows, uint64_t n, int32_t mem, uint32_t in_rb, DevMem* in,
+                              const u64** d_rows) {
+  ctx->stats.rows_in += n;
+  *d_rows = (const u64*)rows;
+  if (mem == MZGPU_MEM_HOST && n) {
+    MZ_TRY(in->alloc(ctx, n * in_rb));
+    MZ_TRY(copy_in(ctx, in->p, rows, n * in_rb, mem));
+    *d_rows = in->as<u64>();
   }
-  return st;
+  return MZGPU_OK;
 }
 
 extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_t n,
@@ -2800,14 +2832,9 @@ extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* ro
     return MZGPU_E_INVALID;
   mzgpu_ctx* ctx = r->ctx;
   MZ_CHECK_CTX(ctx);
-  ctx->stats.rows_in += n;
   DevMem in;
-  const u64* d_rows = (const u64*)rows;
-  if (mem == MZGPU_MEM_HOST && n) {
-    MZ_TRY(in.alloc(ctx, n * 32));
-    MZ_TRY(copy_in(ctx, in.p, rows, n * 32, mem));
-    d_rows = in.as<u64>();
-  }
+  const u64* d_rows;
+  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, 32, &in, &d_rows));
   return reduce_dev(r, d_rows, dlen_imm(n), n, upper, out);
 }
 extern "C" int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
@@ -3027,14 +3054,9 @@ extern "C" int32_t mzgpu_reduce_lanes(mzgpu_reduce* r, const void* rows, uint64_
     MZ_SET_ERR(ctx, "reduce_lanes: output buffer of %u-byte rows", out->rb);
     return MZGPU_E_INVALID;
   }
-  ctx->stats.rows_in += n;
   DevMem in;
-  const u64* d_rows = (const u64*)rows;
-  if (mem == MZGPU_MEM_HOST && n) {
-    MZ_TRY(in.alloc(ctx, n * in_rb));
-    MZ_TRY(copy_in(ctx, in.p, rows, n * in_rb, mem));
-    d_rows = in.as<u64>();
-  }
+  const u64* d_rows;
+  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
   return reduce_dev(r, d_rows, dlen_imm(n), n, upper, out);
 }
 extern "C" int32_t mzgpu_reduce_lanes_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out) {
@@ -3121,11 +3143,7 @@ extern "C" int32_t mzgpu_reduce_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_by
 static int32_t monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
                              mzgpu_buf* errs) {
   mzgpu_ctx* ctx = r->ctx;
-  if (r->failed != MZGPU_OK) {
-    ctx->last_error = r->failed_msg;
-    return r->failed;
-  }
-  MZ_TRY(mzgpu_spine_set_physical_compaction(r->input, r->input->upper));
+  MZ_TRY(reduce_begin(r));
   const int c = r->mono_class;
   if (n_ub) {
     const u32 iw = r->lanes.in_words;
@@ -3166,7 +3184,7 @@ static int32_t monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_u
   const u64 b_ub = batch->len_ub;
   const u64 out_rb = (u64)mz_mono_out_bytes(c);
   if (st == MZGPU_OK && b_ub > 0) {
-    if ((b_ub + 255) / 256 <= MZ_LB_TILES && 2 * b_ub <= MZ_BOUND_MAX_ROWS) {
+    if (single_pass_fits(b_ub, 2)) {  // (the bound alone: a loose one takes the two-pass form)
       DevMem corr;
       Lazy4 clen;
       st = corr.alloc(ctx, 2 * b_ub * out_rb);
@@ -3187,17 +3205,7 @@ static int32_t monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_u
       if (st == MZGPU_OK && n_corr) st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
     }
   }
-  // as in reduce_main: the sealed batch joins the trace whatever happened, and a failure after the seal
-  // kills the operator
-  int32_t ins = MZGPU_OK;
-  if (batch->desc.lower != batch->desc.upper) ins = mzgpu_spine_insert(r->input, batch);
-  mzgpu_batch_release(batch);
-  if (st == MZGPU_OK) st = ins;
-  if (st != MZGPU_OK && !ctx->sticky) {
-    r->failed = st;
-    r->failed_msg = ctx->last_error;
-  }
-  return st;
+  return reduce_seal_tail(r, batch, st);
 }
 
 static bool monotonic_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
@@ -3215,14 +3223,9 @@ extern "C" int32_t mzgpu_reduce_monotonic(mzgpu_reduce* r, const void* rows, uin
                errs->rb);
     return MZGPU_E_INVALID;
   }
-  ctx->stats.rows_in += n;
   DevMem in;
-  const u64* d_rows = (const u64*)rows;
-  if (mem == MZGPU_MEM_HOST && n) {
-    MZ_TRY(in.alloc(ctx, n * in_rb));
-    MZ_TRY(copy_in(ctx, in.p, rows, n * in_rb, mem));
-    d_rows = in.as<u64>();
-  }
+  const u64* d_rows;
+  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
   return monotonic_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
 }
 extern "C" int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
@@ -3300,11 +3303,7 @@ extern "C" int32_t mzgpu_topk_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_byte
 static int32_t topk_monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
                                   mzgpu_buf* errs) {
   mzgpu_ctx* ctx = r->ctx;
-  if (r->failed != MZGPU_OK) {
-    ctx->last_error = r->failed_msg;
-    return r->failed;
-  }
-  MZ_TRY(mzgpu_spine_set_physical_compaction(r->input, r->input->upper));
+  MZ_TRY(reduce_begin(r));
   const TopKOrder& to = r->tko;
   const u32 iw = to.in_words;
   const u64 RB = MZGPU_ROW_RTOPK;
@@ -3345,7 +3344,7 @@ static int32_t topk_monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u6
     Seg w;
     w.ub = 0;
     if (L != 0 && s_ub > 0) {
-      if ((s_ub + 255) / 256 <= MZ_LB_TILES && (u64)L < MZ_BOUND_MAX_ROWS && per_row * s_ub <= MZ_BOUND_MAX_ROWS) {
+      if ((u64)L < MZ_BOUND_MAX_ROWS && single_pass_fits(s_ub, per_row)) {
         const u64 cap = per_row * s_ub;
         DevMem proj;
         st = w.rows.alloc(ctx, cap * RB);
@@ -3377,16 +3376,7 @@ static int32_t topk_monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u6
   }
   mzgpu_batch* batch = nullptr;
   MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
-  // as in monotonic_dev: a failure after the seal kills the operator
-  int32_t ins = MZGPU_OK;
-  if (batch->desc.lower != batch->desc.upper) ins = mzgpu_spine_insert(r->input, batch);
-  mzgpu_batch_release(batch);
-  st = ins;
-  if (st != MZGPU_OK && !ctx->sticky) {
-    r->failed = st;
-    r->failed_msg = ctx->last_error;
-  }
-  return st;
+  return reduce_seal_tail(r, batch, MZGPU_OK);
 }
 
 static bool topk_monotonic_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
@@ -3403,14 +3393,9 @@ extern "C" int32_t mzgpu_topk_monotonic(mzgpu_reduce* r, const void* rows, uint6
                errs->rb);
     return MZGPU_E_INVALID;
   }
-  ctx->stats.rows_in += n;
   DevMem in;
-  const u64* d_rows = (const u64*)rows;
-  if (mem == MZGPU_MEM_HOST && n) {
-    MZ_TRY(in.alloc(ctx, n * in_rb));
-    MZ_TRY(copy_in(ctx, in.p, rows, n * in_rb, mem));
-    d_rows = in.as<u64>();
-  }
+  const u64* d_rows;
+  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
   return topk_monotonic_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
 }
 extern "C" int32_t mzgpu_topk_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,

@@ -1940,6 +1940,40 @@ __global__ void __launch_bounds__(RT) k_topk_window(const u64* __restrict__ rows
 
 }  // namespace
 
+// the grid of a launch over `tiles` tiles of RT rows: at most 8 blocks per SM (grid-stride or look-back loops)
+static unsigned grid_of(mzgpu_ctx* ctx, u64 tiles) { return (unsigned)std::min<u64>(tiles, (u64)ctx->num_sms * 8); }
+
+// Single-pass (look-back) correction kernels: the look-back state, the grid (at most 8 blocks per SM; at least
+// one, which writes the length of no rows) and the bytes moved when the length is known on the host.
+static int32_t lb_launch_setup(mzgpu_ctx* ctx, DLen n, u64 n_ub, u64 bytes_per_row, LookBack* lb, unsigned* grid) {
+  const u64 tiles = (n_ub + RT - 1) / RT;
+  MZ_TRY(mz_lookback_begin(ctx, tiles, lb));
+  *grid = std::max(grid_of(ctx, tiles), 1u);
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * bytes_per_row : 0);
+  return MZGPU_OK;
+}
+
+// Two-pass correction kernels over n > 0 rows: count(tile_counts, n_tiles) launches the count pass, one
+// read-back of the scanned counts gives the total, alloc(total) makes the outputs, write(tile_base, n_tiles)
+// launches the write pass if there are rows.
+template <class Count, class Alloc, class Write>
+static int32_t two_pass(mzgpu_ctx* ctx, u64 n, u64* n_out, Count count, Alloc alloc, Write write) {
+  const u64 n_tiles = (n + RT - 1) / RT;
+  DevMem tiles;
+  MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
+  u64* d_total = ctx->d_scratch + 30;
+  MZ_TRY(count(tiles.as<u32>(), n_tiles));
+  MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
+  MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 30, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  MZ_SYNC(ctx);
+  ctx->stats.d2h_bytes += 8;
+  const u64 total = ctx->h_scratch[30];
+  MZ_TRY(alloc(total));
+  *n_out = total;
+  if (total == 0) return MZGPU_OK;
+  return write((const u32*)tiles.as<u32>(), n_tiles);
+}
+
 int32_t mz_distinct_pairs(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
                           u64* const* d_pairs, u64* const* d_lens) {
   PairMap pm;
@@ -1951,11 +1985,9 @@ int32_t mz_distinct_pairs(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, c
     pm.lane[pm.k] = l;
     pm.k++;
   }
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
-  if (grid == 0) grid = 1;  // (the lengths are written even for no rows)
+  const unsigned grid = std::max(grid_of(ctx, (n_ub + RT - 1) / RT), 1u);  // (the lengths are written for no rows)
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * (ls.in_words * 8 + 32 * pm.k) : 0);
-  MZ_LAUNCH(ctx, k_distinct_pairs, (unsigned)grid, RT, 0, d_rows, n, ls, pm);
+  MZ_LAUNCH(ctx, k_distinct_pairs, grid, RT, 0, d_rows, n, ls, pm);
   return MZGPU_OK;
 }
 
@@ -1985,13 +2017,12 @@ int32_t mz_distinct_presence(mzgpu_ctx* ctx, int c, int k, const DistinctJobHost
     const u64 t0 = x * MZ_LB_TILES, lt = std::min<u64>(tiles - std::min(tiles, t0), MZ_LB_TILES);
     LookBack lb;
     MZ_TRY(mz_lookback_begin(ctx, lt, &lb));
-    u64 grid = std::min<u64>(lt, (u64)ctx->num_sms * 8);
-    if (grid == 0) grid = 1;
+    const unsigned grid = std::max(grid_of(ctx, lt), 1u);
     const DLen base = x == 0 ? dlen_imm(0) : DLen{len->dptr() + ((x - 1) & 1), 0};
     u64* out_len = len->dptr() + (x & 1);
     MZ_BYTES(ctx, x == 0 ? bytes : 0);
     MZ_TRY(mz_dispatch<LaneClasses>(ctx, c, "distinct presence", [&](auto C) {
-      MZ_LAUNCH(ctx, k_distinct_presence<C>, (unsigned)grid, RT, 0, m, t0, lb, base, d_out, out_cap, out_len,
+      MZ_LAUNCH(ctx, k_distinct_presence<C>, grid, RT, 0, m, t0, lb, base, d_out, out_cap, out_len,
                 ctx->d_status);
       return MZGPU_OK;
     }));
@@ -2008,33 +2039,28 @@ int32_t mz_reduce_minmax_async(mzgpu_ctx* ctx, const u64* d_batch_rows, DLen n, 
                                const TraceView& prior, int agg_kind, const TopKParams& tp, u64* d_out,
                                u64 out_cap, u64* d_out_len) {
   LookBack lb;
-  MZ_TRY(mz_lookback_begin(ctx, (n_ub + RT - 1) / RT, &lb));
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
-  if (grid == 0) grid = 1;
-  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (32 + 16 + 32 + 128) : 0);
-  MZ_LAUNCH(ctx, k_minmax_lb, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, tp, lb, d_out, out_cap,
+  unsigned grid;
+  MZ_TRY(lb_launch_setup(ctx, n, n_ub, 32 + 16 + 32 + 128, &lb, &grid));
+  MZ_LAUNCH(ctx, k_minmax_lb, grid, RT, 0, d_batch_rows, n, prior, agg_kind, tp, lb, d_out, out_cap,
             d_out_len, ctx->d_status);
   return MZGPU_OK;
 }
 
 int32_t mz_explode(mzgpu_ctx* ctx, const u64* d_r32, DLen n, u64 n_ub, int agg_kind, u64* d_racc) {
   if (n_ub == 0) return MZGPU_OK;
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  const unsigned grid = grid_of(ctx, (n_ub + RT - 1) / RT);
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * 112 : 0);
-  MZ_LAUNCH(ctx, k_explode, (unsigned)grid, RT, 0, d_r32, n, agg_kind, d_racc);
+  MZ_LAUNCH(ctx, k_explode, grid, RT, 0, d_r32, n, agg_kind, d_racc);
   return MZGPU_OK;
 }
 
 int32_t mz_explode_lanes(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u64 n_ub, const LaneSet& ls,
                          u64* d_arr) {
   if (n_ub == 0) return MZGPU_OK;
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  const unsigned grid = grid_of(ctx, (n_ub + RT - 1) / RT);
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * (ls.in_words * 8 + mz_lane_arr_bytes(c)) : 0);
   return mz_dispatch<LaneClasses>(ctx, c, "explode", [&](auto C) {
-    MZ_LAUNCH(ctx, k_explode_lanes<C>, (unsigned)grid, RT, 0, d_rows, n, ls, d_arr);
+    MZ_LAUNCH(ctx, k_explode_lanes<C>, grid, RT, 0, d_rows, n, ls, d_arr);
     return MZGPU_OK;
   });
 }
@@ -2044,36 +2070,30 @@ int32_t mz_reduce_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u6
   *n_out = 0;
   if (n == 0) return out->alloc(ctx, 16);
   const u32 fm = ls != nullptr ? ls->f64_mask : 0, nl = ls != nullptr ? ls->n : 1;
-  const u64 n_tiles = (n + RT - 1) / RT;
-  DevMem tiles;
-  MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
-  u64* d_total = ctx->d_scratch + 30;
-  MZ_TRY(mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
-    if (hv != nullptr)
-      MZ_LAUNCH(ctx, (k_corrections_having<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, fm, nl, *hv,
-                tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
-    else
-      MZ_LAUNCH(ctx, (k_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
-                tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
-    return MZGPU_OK;
-  }));
-  MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
-  MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 30, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  MZ_SYNC(ctx);
-  ctx->stats.d2h_bytes += 8;
-  const u64 total = ctx->h_scratch[30];
-  MZ_TRY(out->alloc(ctx, total * mz_lane_out_bytes(c)));
-  *n_out = total;
-  if (total == 0) return MZGPU_OK;
-  return mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
-    if (hv != nullptr)
-      MZ_LAUNCH(ctx, (k_corrections_having<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, fm, nl, *hv,
-                (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
-    else
-      MZ_LAUNCH(ctx, (k_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
-                (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
-    return MZGPU_OK;
-  });
+  auto count = [&](u32* tile_counts, u64 n_tiles) {
+    return mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
+      if (hv != nullptr)
+        MZ_LAUNCH(ctx, (k_corrections_having<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, fm, nl,
+                  *hv, tile_counts, (const u32*)nullptr, (u64*)nullptr);
+      else
+        MZ_LAUNCH(ctx, (k_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
+                  tile_counts, (const u32*)nullptr, (u64*)nullptr);
+      return MZGPU_OK;
+    });
+  };
+  auto alloc = [&](u64 total) { return out->alloc(ctx, total * mz_lane_out_bytes(c)); };
+  auto write = [&](const u32* tile_base, u64 n_tiles) {
+    return mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
+      if (hv != nullptr)
+        MZ_LAUNCH(ctx, (k_corrections_having<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, fm, nl,
+                  *hv, (u32*)nullptr, tile_base, out->as<u64>());
+      else
+        MZ_LAUNCH(ctx, (k_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl,
+                  (u32*)nullptr, tile_base, out->as<u64>());
+      return MZGPU_OK;
+    });
+  };
+  return two_pass(ctx, n, n_out, count, alloc, write);
 }
 
 // Single-pass form: batch length read on the device; at most two output rows per
@@ -2083,17 +2103,14 @@ int32_t mz_reduce_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_ro
                                     u64 out_cap, u64* d_out_len, const mzgpu_having* hv) {
   const u32 fm = ls != nullptr ? ls->f64_mask : 0, nl = ls != nullptr ? ls->n : 1;
   LookBack lb;
-  MZ_TRY(mz_lookback_begin(ctx, (n_ub + RT - 1) / RT, &lb));
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
-  if (grid == 0) grid = 1;
-  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (2 * mz_lane_arr_bytes(c) + 16 + 2 * mz_lane_out_bytes(c)) : 0);
+  unsigned grid;
+  MZ_TRY(lb_launch_setup(ctx, n, n_ub, 2 * mz_lane_arr_bytes(c) + 16 + 2 * mz_lane_out_bytes(c), &lb, &grid));
   return mz_dispatch<LaneClasses>(ctx, c, "reduce", [&](auto C) {
     if (hv != nullptr)
-      MZ_LAUNCH(ctx, k_corrections_lb_having<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, fm, nl, *hv, lb,
-                d_out, out_cap, d_out_len, ctx->d_status);
+      MZ_LAUNCH(ctx, k_corrections_lb_having<C>, grid, RT, 0, d_batch_rows, n, prior, fm, nl, *hv, lb, d_out,
+                out_cap, d_out_len, ctx->d_status);
     else
-      MZ_LAUNCH(ctx, k_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, lb, d_out,
+      MZ_LAUNCH(ctx, k_corrections_lb<C>, grid, RT, 0, d_batch_rows, n, prior, agg_kind, fm, nl, lb, d_out,
                 out_cap, d_out_len, ctx->d_status);
     return MZGPU_OK;
   });
@@ -2103,11 +2120,10 @@ int32_t mz_monotonic_explode(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u
                              const MonoXor& mx, u64* d_arr, u64* d_errs, u64* d_cnt) {
   MZ_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 16, ctx->stream));
   if (n_ub == 0) return MZGPU_OK;
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  const unsigned grid = grid_of(ctx, (n_ub + RT - 1) / RT);
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * (ls.in_words * 8 + mz_mono_arr_bytes(c)) : 0);
   return mz_dispatch<MonoClasses>(ctx, c, "monotonic explode", [&](auto C) {
-    MZ_LAUNCH(ctx, k_monotonic_explode<C>, (unsigned)grid, RT, 0, d_rows, n, ls, mx, d_arr, d_errs,
+    MZ_LAUNCH(ctx, k_monotonic_explode<C>, grid, RT, 0, d_rows, n, ls, mx, d_arr, d_errs,
               (unsigned long long*)d_cnt);
     return MZGPU_OK;
   });
@@ -2116,10 +2132,9 @@ int32_t mz_monotonic_explode(mzgpu_ctx* ctx, int c, const u64* d_rows, DLen n, u
 int32_t mz_monotonic_mask(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, u32 in_words, u64 m1, u64 m2,
                           u64* d_out) {
   if (n_ub == 0) return MZGPU_OK;
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  const unsigned grid = grid_of(ctx, (n_ub + RT - 1) / RT);
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * in_words * 16 : 0);
-  MZ_LAUNCH(ctx, k_monotonic_mask, (unsigned)grid, RT, 0, d_rows, n, in_words, m1, m2, d_out);
+  MZ_LAUNCH(ctx, k_monotonic_mask, grid, RT, 0, d_rows, n, in_words, m1, m2, d_out);
   return MZGPU_OK;
 }
 
@@ -2128,13 +2143,10 @@ int32_t mz_monotonic_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch
                                        const TraceView& prior, const MonoXor& mx, u64* d_out, u64 out_cap,
                                        u64* d_out_len) {
   LookBack lb;
-  MZ_TRY(mz_lookback_begin(ctx, (n_ub + RT - 1) / RT, &lb));
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
-  if (grid == 0) grid = 1;
-  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (2 * mz_mono_arr_bytes(c) + 16 + 2 * mz_mono_out_bytes(c)) : 0);
+  unsigned grid;
+  MZ_TRY(lb_launch_setup(ctx, n, n_ub, 2 * mz_mono_arr_bytes(c) + 16 + 2 * mz_mono_out_bytes(c), &lb, &grid));
   return mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
-    MZ_LAUNCH(ctx, k_monotonic_corrections_lb<C>, (unsigned)grid, RT, 0, d_batch_rows, n, prior, mx, lb, d_out,
+    MZ_LAUNCH(ctx, k_monotonic_corrections_lb<C>, grid, RT, 0, d_batch_rows, n, prior, mx, lb, d_out,
               out_cap, d_out_len, ctx->d_status);
     return MZGPU_OK;
   });
@@ -2144,38 +2156,31 @@ int32_t mz_monotonic_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows,
                                  const MonoXor& mx, DevMem* out, u64* n_out) {
   *n_out = 0;
   if (n == 0) return out->alloc(ctx, 16);
-  const u64 n_tiles = (n + RT - 1) / RT;
-  DevMem tiles;
-  MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
-  u64* d_total = ctx->d_scratch + 30;
-  MZ_TRY(mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
-    MZ_LAUNCH(ctx, (k_monotonic_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, mx,
-              tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr);
-    return MZGPU_OK;
-  }));
-  MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
-  MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 30, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  MZ_SYNC(ctx);
-  ctx->stats.d2h_bytes += 8;
-  const u64 total = ctx->h_scratch[30];
-  MZ_TRY(out->alloc(ctx, total * mz_mono_out_bytes(c)));
-  *n_out = total;
-  if (total == 0) return MZGPU_OK;
-  return mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
-    MZ_LAUNCH(ctx, (k_monotonic_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, mx,
-              (u32*)nullptr, tiles.as<u32>(), out->as<u64>());
-    return MZGPU_OK;
-  });
+  auto count = [&](u32* tile_counts, u64 n_tiles) {
+    return mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
+      MZ_LAUNCH(ctx, (k_monotonic_corrections<C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, mx,
+                tile_counts, (const u32*)nullptr, (u64*)nullptr);
+      return MZGPU_OK;
+    });
+  };
+  auto alloc = [&](u64 total) { return out->alloc(ctx, total * mz_mono_out_bytes(c)); };
+  auto write = [&](const u32* tile_base, u64 n_tiles) {
+    return mz_dispatch<MonoClasses>(ctx, c, "monotonic reduce", [&](auto C) {
+      MZ_LAUNCH(ctx, (k_monotonic_corrections<C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, mx,
+                (u32*)nullptr, tile_base, out->as<u64>());
+      return MZGPU_OK;
+    });
+  };
+  return two_pass(ctx, n, n_out, count, alloc, write);
 }
 
 int32_t mz_topk_explode(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TopKOrder& to, u64* d_arr,
                         u64* d_errs, u64* d_cnt) {
   MZ_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 16, ctx->stream));
   if (n_ub == 0) return MZGPU_OK;
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
+  const unsigned grid = grid_of(ctx, (n_ub + RT - 1) / RT);
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * (to.in_words * 8 + TK_NW * 8) : 0);
-  MZ_LAUNCH(ctx, k_topk_explode, (unsigned)grid, RT, 0, d_rows, n, to, d_arr, d_errs, (unsigned long long*)d_cnt);
+  MZ_LAUNCH(ctx, k_topk_explode, grid, RT, 0, d_rows, n, to, d_arr, d_errs, (unsigned long long*)d_cnt);
   return MZGPU_OK;
 }
 
@@ -2186,13 +2191,10 @@ struct TopKInWords : IntSet<4, 5> {  // R32 / R40 input
 int32_t mz_topk_window_async(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TraceView& prior,
                              const TopKOrder& to, u64* d_win, u64* d_out, u64 out_cap, u64* d_out_len) {
   LookBack lb;
-  MZ_TRY(mz_lookback_begin(ctx, (n_ub + RT - 1) / RT, &lb));
-  u64 grid = (n_ub + RT - 1) / RT;
-  if (grid > (u64)ctx->num_sms * 8) grid = (u64)ctx->num_sms * 8;
-  if (grid == 0) grid = 1;
-  MZ_BYTES(ctx, n.p == nullptr ? n.imm * 2 * TK_NW * 8 : 0);
+  unsigned grid;
+  MZ_TRY(lb_launch_setup(ctx, n, n_ub, 2 * TK_NW * 8, &lb, &grid));
   return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
-    MZ_LAUNCH(ctx, k_topk_window_lb<IW>, (unsigned)grid, RT, 0, d_rows, n, prior, to.limit, lb, d_win, d_out,
+    MZ_LAUNCH(ctx, k_topk_window_lb<IW>, grid, RT, 0, d_rows, n, prior, to.limit, lb, d_win, d_out,
               out_cap, d_out_len, ctx->d_status);
     return MZGPU_OK;
   });
@@ -2202,27 +2204,24 @@ int32_t mz_topk_window(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView
                        DevMem* win, DevMem* out, u64* n_out) {
   *n_out = 0;
   if (n == 0) return MZGPU_OK;
-  const u64 n_tiles = (n + RT - 1) / RT;
-  DevMem tiles;
-  MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
-  u64* d_total = ctx->d_scratch + 30;
-  MZ_TRY(mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
-    MZ_LAUNCH(ctx, (k_topk_window<IW, false>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, to.limit,
-              tiles.as<u32>(), (const u32*)nullptr, (u64*)nullptr, (u64*)nullptr);
-    return MZGPU_OK;
-  }));
-  MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
-  MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 30, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  MZ_SYNC(ctx);
-  ctx->stats.d2h_bytes += 8;
-  const u64 total = ctx->h_scratch[30];
-  *n_out = total;
-  if (total == 0) return MZGPU_OK;
-  MZ_TRY(win->alloc(ctx, total * TK_NW * 8));
-  MZ_TRY(out->alloc(ctx, total * to.in_words * 8));
-  return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
-    MZ_LAUNCH(ctx, (k_topk_window<IW, true>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, to.limit,
-              (u32*)nullptr, tiles.as<u32>(), win->as<u64>(), out->as<u64>());
-    return MZGPU_OK;
-  });
+  auto count = [&](u32* tile_counts, u64 n_tiles) {
+    return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
+      MZ_LAUNCH(ctx, (k_topk_window<IW, false>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, to.limit, tile_counts,
+                (const u32*)nullptr, (u64*)nullptr, (u64*)nullptr);
+      return MZGPU_OK;
+    });
+  };
+  auto alloc = [&](u64 total) {
+    if (total == 0) return MZGPU_OK;  // (no window change: the outputs stay unallocated)
+    MZ_TRY(win->alloc(ctx, total * TK_NW * 8));
+    return out->alloc(ctx, total * to.in_words * 8);
+  };
+  auto write = [&](const u32* tile_base, u64 n_tiles) {
+    return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
+      MZ_LAUNCH(ctx, (k_topk_window<IW, true>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, to.limit,
+                (u32*)nullptr, tile_base, win->as<u64>(), out->as<u64>());
+      return MZGPU_OK;
+    });
+  };
+  return two_pass(ctx, n, n_out, count, alloc, write);
 }
