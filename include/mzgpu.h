@@ -338,7 +338,9 @@ int32_t mzgpu_buf_consolidate(mzgpu_buf* buf);
 
 /* ------------------------------------------ a2-a5: batcher and batches */
 /* Batcher::new (src/timely-util/src/operator.rs:572-575).  row_bytes selects
- * R32 (KeyValBatcher) or RACC (the accumulable arrangement's batcher). */
+ * R32 (KeyValBatcher) or RACC (the accumulable arrangement's batcher).  R40 rows
+ * (the hierarchical MIN / MAX reduce's arrangement) are accepted as well, by
+ * batchers, builders and spines alike. */
 int32_t mzgpu_batcher_new(mzgpu_ctx* ctx, uint32_t row_bytes, mzgpu_batcher** out);
 void mzgpu_batcher_free(mzgpu_batcher* b);
 /* Batcher::push_container: sort + consolidate the container into a chain and
@@ -813,6 +815,53 @@ int32_t mzgpu_reduce_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, in
                                mzgpu_buf* out, mzgpu_buf* errs);
 int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
                                    mzgpu_buf* errs);
+
+/* ---- hierarchical MIN / MAX reduce: several MIN / MAX columns per key over input with retractions, one output
+ * row per key (HierarchicalPlan::Bucketed with several aggr_funcs, BucketedPlan in
+ * src/compute-types/src/plan/reduce.rs:232-250, which the planner picks for MIN / MAX over any collection that can
+ * retract; rendered by build_bucketed / build_bucketed_negated_output, src/compute/src/render/reduce.rs:796-1135).
+ *
+ * Lanes reuse mzgpu_accum_lane exactly as mzgpu_reduce_monotonic_new does: kind = MZGPU_AGG_MIN or MZGPU_AGG_MAX,
+ * sign_extend chooses signed or unsigned order, field picks the bit-field (src MZGPU_SRC_VAL1, or MZGPU_SRC_VAL2 of
+ * R40 input).  MZGPU_MONO_F64 is MZGPU_E_UNSUPPORTED for the same OrderedFloat reason.  Input is R32 or R40 rows.
+ *
+ * Per key, at every time t, the key's live multiset is its input rows with times <= t, each masked to the value
+ * bits some lane reads and consolidated by (key, masked val1, masked val2) -- the reference arranges (key, row of
+ * the aggregates' inputs), so two rows that differ only in bits no lane reads are one value row and a +1 / -1 pair
+ * of them cancels.  Then:
+ *   every live count positive: the key's output row holds, per lane, the MIN / MAX of its field over the live
+ *       rows (the natural values, as the monotonic operator emits them);
+ *   some live count negative ("non-positive accumulation"): no output row while the key is in that state, and one
+ *       error for it;
+ *   no live row: no output row.
+ * Output (`out`): rows of the monotonic output widths, MZGPU_ROW_MONO_OUT4 (56 B, 1-4 lanes) or
+ *     MZGPU_ROW_MONO_OUT8 (88 B, 5-8 lanes): key, the C values (unused lanes zero), time, diff.  A change in any lane
+ *     emits (-old, +new) at the time of the change.  The rows leave the operator consolidated and sorted per key.
+ * Errors (`errs`, R32 rows (key, 0, time, diff), consolidated): +1 when a key enters the non-positive state at
+ *     time t, -1 when it leaves it.  This is a fixed-width stand-in for the reference's per-key error "saw
+ *     non-positive accumulation for key ... in hierarchical mins-maxes aggregate"; the reference's ok output for such
+ *     a key depends on how its buckets hash, and is deliberately not reproduced.
+ * State: mzgpu_reduce_input_trace(r) returns the operator's arrangement: the masked input rows at the input width
+ *     (R32 or R40) with ordinary SUM diffs.  The caller compacts it like any other trace.  Work per touched key is
+ *     its distinct live value rows while they fit a 32-entry table, and one ordered pass over its runs per new time
+ *     beyond that.
+ * Checked on the host before any launch, in the order of mzgpu_reduce_monotonic_new: MZGPU_E_INVALID for a
+ * malformed descriptor (in_row_bytes not 32 / 40, a kind other than MIN / MAX, any flag bit but MZGPU_MONO_F64, VAL2
+ * on R32 input, a zero-width or out-of-range field, n_lanes of 0 or above 8), then MZGPU_E_UNSUPPORTED for a float64
+ * lane.  A failure leaves no operator behind (*out is not written) and the context usable.  The handle is freed with
+ * mzgpu_reduce_free.
+ * Not supported: COUNT / SUM lanes in the same operator (ReducePlan::Collation: a caller zips this operator's output
+ * with mzgpu_reduce_lanes_new's by key), HAVING on MIN / MAX, float64 lanes, NULLs, and the bucket tree itself. */
+int32_t mzgpu_reduce_hierarchical_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                                      uint32_t n_lanes, mzgpu_reduce** out);
+/* One activation, with the protocol of mzgpu_reduce_monotonic[_buf]: `rows` are n input rows of in_row_bytes with
+ * times in [previous upper, upper); the corrections (rows of the class's output width) are appended to `out` and
+ * the errors (R32) to `errs` (required).  After a failed activation the operator reports that status from then
+ * on. */
+int32_t mzgpu_reduce_hierarchical(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                  mzgpu_buf* out, mzgpu_buf* errs);
+int32_t mzgpu_reduce_hierarchical_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                      mzgpu_buf* errs);
 
 /* ---- monotonic TopK: Top-1 and Top-K over append-only input, with only the window arranged
  * (TopKPlan::MonotonicTop1 / MonotonicTopK, src/compute/src/render/top_k.rs:102-214; the planner picks them

@@ -311,6 +311,9 @@ SIGNATURES = {
     "mzgpu_reduce_monotonic_new": (i32, [vp, u32, vp, u32, i32, PV]),
     "mzgpu_reduce_monotonic": (i32, [vp, vp, u64, i32, u64, vp, vp]),
     "mzgpu_reduce_monotonic_buf": (i32, [vp, vp, u64, vp, vp]),
+    "mzgpu_reduce_hierarchical_new": (i32, [vp, u32, vp, u32, PV]),
+    "mzgpu_reduce_hierarchical": (i32, [vp, vp, u64, i32, u64, vp, vp]),
+    "mzgpu_reduce_hierarchical_buf": (i32, [vp, vp, u64, vp, vp]),
     "mzgpu_topk_monotonic_new": (i32, [vp, u32, vp, u32, C.c_int64, i32, PV]),
     "mzgpu_topk_monotonic": (i32, [vp, vp, u64, i32, u64, vp, vp]),
     "mzgpu_topk_monotonic_buf": (i32, [vp, vp, u64, vp, vp]),

@@ -880,6 +880,50 @@ class ReduceMonotonic:
             self.h = None
 
 
+class ReduceHierarchical:
+    """MIN / MAX of several value columns per key over input with retractions (mzgpu_reduce_hierarchical_new,
+    build_bucketed).  `lanes` are accum_lane(AGG_MIN | AGG_MAX, ...) tuples, as for ReduceMonotonic.  Input rows
+    are R32 (in_row_bytes=32) or R40 (40).  step() returns (corrections, errors): corrections of dtype
+    MONO_OUT[class] (lane l in ["vals"][:, l]), errors R32 rows (key, 0, time, +1 entering / -1 leaving the
+    non-positive-accumulation state).  The arrangement (input_trace) holds the masked input rows."""
+
+    def __init__(self, ctx, lanes, in_row_bytes=32):
+        self.ctx = ctx
+        self.n_lanes = len(lanes)
+        self.in_row_bytes = in_row_bytes
+        arr = (F.AccumLane * max(1, len(lanes)))()
+        for i, (kind, src, shift, bits, sx) in enumerate(lanes):
+            arr[i].kind = kind
+            arr[i].sign_extend = 1 if sx else 0
+            arr[i].field = F.Field(src, shift, bits, 0)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_reduce_hierarchical_new(ctx.h, in_row_bytes, arr, len(lanes), C.byref(h)))
+        self.h = h
+        self.lane_class = F.mono_class(self.n_lanes)
+        self.out_row_bytes = F.MONO_ROW_BYTES[self.lane_class][1]
+
+    def step(self, rows, upper):
+        rows = np.ascontiguousarray(rows)
+        out, errs = DeviceRows(self.ctx, self.out_row_bytes), DeviceRows(self.ctx, 32)
+        self.ctx.check(F.lib.mzgpu_reduce_hierarchical(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
+        return out.download(), errs.download()
+
+    def step_dev(self, dev_rows, upper, out=None, errs=None):
+        """One activation over device-resident rows; corrections and errors are appended on the device."""
+        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
+        errs = errs if errs is not None else DeviceRows(self.ctx, 32)
+        self.ctx.check(F.lib.mzgpu_reduce_hierarchical_buf(self.h, dev_rows.h, upper, out.h, errs.h))
+        return out, errs
+
+    def input_trace(self):
+        return Spine(self.ctx, self.in_row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_reduce_free(self.h)
+            self.h = None
+
+
 class TopK(ReduceAccumulable):
     """TopK per key over (key, value) rows (BasicTopKPlan, src/compute/src/render/top_k.rs:215-248,
     521-673): `limit` < 0 or None = no limit; stepped like every other reduce kind."""

@@ -575,7 +575,8 @@ struct IntSet {
   static constexpr bool has(int v) { return ((v == V) || ...); }
 };
 using RowWidths = IntSet<16, 32, 40, 64, 80, 128, 224, 416, 48, 112, 72>;  // every RowT: sort, consolidate, fused
-using BatchWidths = IntSet<32, 64, 80, 128, 224, 416, 48, 112, 72>;         // sorted batches: merge, extract, index
+// sorted batches: merge, extract, index (40: the hierarchical MIN / MAX reduce arranges its R40 input)
+using BatchWidths = IntSet<32, 64, 80, 128, 224, 416, 48, 112, 72, 40>;
 using ExchangeWidths = IntSet<32, 80>;
 struct LaneClasses : IntSet<1, 2, 4, 8> {  // accumulable reduce with 1, 2, 4 or 8 lanes (LaneRows below)
   static constexpr const char* kind = "lane class";
@@ -1140,6 +1141,17 @@ int32_t mz_monotonic_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch
                                        u64* d_out_len);
 int32_t mz_monotonic_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
                                  const MonoXor& mx, DevMem* out, u64* n_out);
+// the hierarchical MIN / MAX reduce (mzgpu_reduce_hierarchical_new): corrections of a sealed batch of masked
+// input rows (ls.in_words words) against the prior arrangement, rows of the monotonic output width of class c
+// (consolidated), and R32 error rows (key, 0, time, +-1; unordered) at d_errs[*d_err_len++] (the counter is
+// zeroed here).  Single pass: out_cap = 2 * n_ub and err_cap = n_ub always suffice.
+int32_t mz_hier_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, DLen n, u64 n_ub,
+                                  const TraceView& prior, const LaneSet& ls, const MonoXor& mx, u64* d_out,
+                                  u64 out_cap, u64* d_out_len, u64* d_errs, u64 err_cap, u64* d_err_len);
+// the two-pass form (count, read back, write) for a batch past the single-pass bound; err_cap = n suffices
+int32_t mz_hier_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
+                            const LaneSet& ls, const MonoXor& mx, DevMem* out, u64* n_out, u64* d_errs, u64 err_cap,
+                            u64* d_err_len);
 // the monotonic TopK (mzgpu_topk_monotonic_new): order word j of a row = field_get(lane j) (sign-extended when
 // signed) ^ xm[j] (2^63 for a signed lane, then all ones for a descending one); lanes n..2 stay zero
 struct TopKOrder {

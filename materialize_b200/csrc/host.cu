@@ -1353,7 +1353,7 @@ static int32_t seal_run_unfused(SealPlan* p, mzgpu_batch** batch_out) {
   b->frontier_known = true;
   // the bulk sort has seen the range of the time word: if every buffered time precedes
   // `upper` everything ships and the extract pass (two more copies of the rows) is skipped
-  const int tw = b->rb == 32 ? 2 : (b->rb == 72 ? RowT<72>::TW : 1);
+  const int tw = b->rb == 32 ? 2 : (b->rb == 72 ? RowT<72>::TW : (b->rb == 40 ? RowT<40>::TW : 1));
   const bool all_ship = ctx->last_minmax_valid && ctx->last_minmax[2 * tw + 1] < upper;
   if (upper == MZGPU_FRONTIER_EMPTY || n_cons == 0 || all_ship) {
     MZ_TRY(make_batch(ctx, b->rb, std::move(cons), n_cons, d, batch_out));
@@ -2526,6 +2526,9 @@ struct mzgpu_reduce {
   MonoXor mono = {};
   bool must_consolidate = false;
   u64 mono_mask[2] = {0, 0};
+  // mzgpu_reduce_hierarchical_new: lane class (4, 8; 0 for every other operator); lanes, mono and mono_mask
+  // above hold its lanes, their encodings and the value bits they read
+  int hier_class = 0;
   // mzgpu_topk_monotonic_new: the order lanes and limit (must_consolidate above is its flag too)
   bool topk_mono = false;
   TopKOrder tko = {};
@@ -2828,7 +2831,7 @@ static int32_t reduce_rows_in(mzgpu_ctx* ctx, const void* rows, uint64_t n, int3
 extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_t n,
                                             int32_t mem, uint64_t upper, mzgpu_buf* out) {
   if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->lane_class || r->mono_class ||
-      r->topk_mono)
+      r->topk_mono || r->hier_class)
     return MZGPU_E_INVALID;
   mzgpu_ctx* ctx = r->ctx;
   MZ_CHECK_CTX(ctx);
@@ -2840,7 +2843,7 @@ extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* ro
 extern "C" int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
                                                 mzgpu_buf* out) {
   if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64 || r->lane_class ||
-      r->mono_class || r->topk_mono)
+      r->mono_class || r->topk_mono || r->hier_class)
     return MZGPU_E_INVALID;
   MZ_CHECK_CTX(r->ctx);
   r->ctx->stats.rows_in += rows->ub;
@@ -3080,20 +3083,22 @@ extern "C" int32_t mzgpu_reduce_monotonic_row_bytes(uint32_t n_lanes, uint32_t* 
   return MZGPU_OK;
 }
 
-extern "C" int32_t mzgpu_reduce_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
-                                              uint32_t n_lanes, int32_t must_consolidate, mzgpu_reduce** out) {
-  MZ_CHECK_CTX(ctx);
-  if (out == nullptr || (lanes == nullptr && n_lanes) || (in_row_bytes != 32 && in_row_bytes != 40)) {
-    MZ_SET_ERR(ctx, "reduce_monotonic: bad arguments (input rows of %u bytes)", in_row_bytes);
+// The MIN / MAX lanes of the monotonic and hierarchical reduces, checked on the host (`what` names the operator
+// in the messages): MZGPU_E_INVALID for a malformed descriptor, then MZGPU_E_UNSUPPORTED for a float64 lane.
+// Fills the lanes, their encodings (value ^ xm: every lane an unsigned max) and the value bits they read.
+static int32_t minmax_lanes(mzgpu_ctx* ctx, const char* what, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                            uint32_t n_lanes, LaneSet* ls_out, MonoXor* mx_out, u64* mask) {
+  if (in_row_bytes != 32 && in_row_bytes != 40) {
+    MZ_SET_ERR(ctx, "%s: bad arguments (input rows of %u bytes)", what, in_row_bytes);
     return MZGPU_E_INVALID;
   }
   if (n_lanes == 0 || n_lanes > MZGPU_MAX_ACCUM_LANES) {
-    MZ_SET_ERR(ctx, "reduce_monotonic: %u lanes (1..%d)", n_lanes, MZGPU_MAX_ACCUM_LANES);
+    MZ_SET_ERR(ctx, "%s: %u lanes (1..%d)", what, n_lanes, MZGPU_MAX_ACCUM_LANES);
     return MZGPU_E_INVALID;
   }
   LaneSet ls = {};
   MonoXor mx = {};
-  u64 mask[2] = {0, 0};
+  mask[0] = mask[1] = 0;
   int unsupported = -1;  // the first float64 lane, reported once every lane is known to be well-formed
   for (uint32_t l = 0; l < n_lanes; ++l) {
     const mzgpu_accum_lane& L = lanes[l];
@@ -3107,7 +3112,7 @@ extern "C" int32_t mzgpu_reduce_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_by
     else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
       bad = "field is empty or out of range";
     if (bad != nullptr) {
-      MZ_SET_ERR(ctx, "reduce_monotonic: lane %u: %s", l, bad);
+      MZ_SET_ERR(ctx, "%s: lane %u: %s", what, l, bad);
       return MZGPU_E_INVALID;
     }
     if ((L.kind & MZGPU_MONO_F64) != 0 && unsupported < 0) unsupported = (int)l;
@@ -3116,13 +3121,29 @@ extern "C" int32_t mzgpu_reduce_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_by
     mask[f.src == MZGPU_SRC_VAL2 ? 1 : 0] |= (f.bits == 64 ? ~0ull : ((1ull << f.bits) - 1)) << f.shift;
   }
   if (unsupported >= 0) {
-    MZ_SET_ERR(ctx, "reduce_monotonic: lane %d: float64 MIN / MAX is not supported (OrderedFloat ties -0.0 with "
-                    "+0.0 and NaN payloads, so the surviving bits would depend on arrival order)", unsupported);
+    MZ_SET_ERR(ctx, "%s: lane %d: float64 MIN / MAX is not supported (OrderedFloat ties -0.0 with "
+                    "+0.0 and NaN payloads, so the surviving bits would depend on arrival order)", what, unsupported);
     return MZGPU_E_UNSUPPORTED;
   }
   ls.n = n_lanes;
   ls.in_words = in_row_bytes / 8;
   mx.n = n_lanes;
+  *ls_out = ls;
+  *mx_out = mx;
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_reduce_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                                              uint32_t n_lanes, int32_t must_consolidate, mzgpu_reduce** out) {
+  MZ_CHECK_CTX(ctx);
+  if (out == nullptr || (lanes == nullptr && n_lanes)) {
+    MZ_SET_ERR(ctx, "reduce_monotonic: bad arguments (input rows of %u bytes)", in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  LaneSet ls;
+  MonoXor mx;
+  u64 mask[2];
+  MZ_TRY(minmax_lanes(ctx, "reduce_monotonic", in_row_bytes, lanes, n_lanes, &ls, &mx, mask));
   std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
   r->ctx = ctx;
   r->agg_kind = -1;
@@ -3239,6 +3260,136 @@ extern "C" int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, 
   }
   r->ctx->stats.rows_in += rows->ub;
   return monotonic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
+}
+
+// ------------------------------------------------------- hierarchical MIN / MAX reduce
+extern "C" int32_t mzgpu_reduce_hierarchical_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
+                                                 uint32_t n_lanes, mzgpu_reduce** out) {
+  MZ_CHECK_CTX(ctx);
+  if (out == nullptr || (lanes == nullptr && n_lanes)) {
+    MZ_SET_ERR(ctx, "reduce_hierarchical: bad arguments (input rows of %u bytes)", in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  LaneSet ls;
+  MonoXor mx;
+  u64 mask[2];
+  MZ_TRY(minmax_lanes(ctx, "reduce_hierarchical", in_row_bytes, lanes, n_lanes, &ls, &mx, mask));
+  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
+  r->ctx = ctx;
+  r->agg_kind = -1;
+  r->hier_class = mz_mono_class(n_lanes);
+  r->lanes = ls;
+  r->mono = mx;
+  r->mono_mask[0] = mask[0];
+  r->mono_mask[1] = mask[1];
+  // the arrangement holds the masked input rows themselves, with ordinary SUM diffs
+  MZ_TRY(mzgpu_batcher_new(ctx, in_row_bytes, &r->batcher));
+  MZ_TRY(mzgpu_spine_new(ctx, in_row_bytes, 1, &r->input));
+  *out = r.release();
+  return MZGPU_OK;
+}
+
+// One activation of build_bucketed: mask -> arrange -> per-key MIN / MAX of the live rows, and the keys'
+// non-positive-accumulation errors.
+static int32_t hierarchical_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                                mzgpu_buf* errs) {
+  mzgpu_ctx* ctx = r->ctx;
+  MZ_TRY(reduce_begin(r));
+  const int c = r->hier_class;
+  const u32 iw = r->lanes.in_words;
+  if (n_ub) {
+    // (key, the bits the lanes read, time, diff): rows that differ only in unread bits are one value row
+    Seg s;
+    MZ_TRY(s.rows.alloc(ctx, n_ub * iw * 8));
+    MZ_TRY(mz_monotonic_mask(ctx, d_rows, n, n_ub, iw, r->mono_mask[0], r->mono_mask[1], s.rows.as<u64>()));
+    if (n.p == nullptr) {
+      s.len.set(ctx, n.imm);
+      s.ub = n.imm;
+    } else {
+      MZ_TRY(s.len.make_pending(ctx));
+      MZ_CUDA(ctx, cudaMemcpyAsync(s.len.dptr(), n.p, 8, cudaMemcpyDeviceToDevice, ctx->stream));
+      s.len.mark_written();
+      s.ub = n_ub;
+    }
+    MZ_TRY(batcher_push_seg(r->batcher, std::move(s)));
+  }
+  mzgpu_batch* batch = nullptr;
+  MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
+  std::vector<mzgpu_batch*> prior;
+  r->input->all_batches(prior);
+  TraceView tv;
+  int32_t st = trace_view(ctx, prior, &tv);
+  const u64 b_ub = batch->len_ub;
+  if (st == MZGPU_OK && b_ub > 0) {
+    DevMem corr, erows, econs;
+    Lazy4 elen, eflen;
+    u64 ecap = 0, e_ub = b_ub;
+    st = elen.make_pending(ctx);
+    if (single_pass_fits(b_ub, 2)) {  // (the bound alone: a loose one takes the two-pass form)
+      Lazy4 clen;
+      if (st == MZGPU_OK) st = corr.alloc(ctx, 2 * b_ub * mz_mono_out_bytes(c));
+      if (st == MZGPU_OK) st = erows.alloc(ctx, b_ub * 32);
+      if (st == MZGPU_OK) st = clen.make_pending(ctx);
+      if (st == MZGPU_OK) {
+        st = mz_hier_corrections_async(ctx, c, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv, r->lanes, r->mono,
+                                       corr.as<u64>(), 2 * b_ub, clen.dptr(), erows.as<u64>(), b_ub, elen.dptr());
+        clen.mark_written();
+        elen.mark_written();
+      }
+      // consolidated by construction: keys ascending, each key's rows sorted by its thread
+      if (st == MZGPU_OK) st = buf_append_dev(out, corr.p, dlen_of(clen, 0), 2 * b_ub);
+    } else {
+      u64 n_corr = 0;
+      if (st == MZGPU_OK) st = batch_resolve(batch);
+      if (st == MZGPU_OK) e_ub = batch->st.v[0];
+      if (st == MZGPU_OK) st = erows.alloc(ctx, std::max<u64>(e_ub, 1) * 32);
+      if (st == MZGPU_OK) {
+        st = mz_hier_corrections(ctx, c, batch->rows.as<u64>(), e_ub, tv, r->lanes, r->mono, &corr, &n_corr,
+                                 erows.as<u64>(), e_ub, elen.dptr());
+        elen.mark_written();
+      }
+      if (st == MZGPU_OK && n_corr) st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
+    }
+    // the error rows leave the kernel unordered: (key, 0, time, +-1), at most one per key and time
+    if (st == MZGPU_OK && e_ub > 0) st = consolidate_dev(ctx, 32, erows.p, dlen_of(elen, 0), e_ub, &econs, &ecap, &eflen);
+    if (st == MZGPU_OK && e_ub > 0)
+      st = buf_append_dev(errs, econs.p, dlen_of(eflen, 0), eflen.known ? eflen.v[0] : e_ub);
+  }
+  return reduce_seal_tail(r, batch, st);
+}
+
+static bool hierarchical_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
+  return r->hier_class != 0 && in_rb == r->lanes.in_words * 8 && out->rb == (uint32_t)mz_mono_out_bytes(r->hier_class) &&
+         errs->rb == 32 && out != errs;
+}
+extern "C" int32_t mzgpu_reduce_hierarchical(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem,
+                                             uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs) {
+  if (r == nullptr || out == nullptr || errs == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = r->ctx;
+  MZ_CHECK_CTX(ctx);
+  const uint32_t in_rb = r->lanes.in_words * 8;
+  if (!hierarchical_io_ok(r, in_rb, out, errs)) {
+    MZ_SET_ERR(ctx, "reduce_hierarchical: output buffer of %u-byte rows / error buffer of %u-byte rows", out->rb,
+               errs->rb);
+    return MZGPU_E_INVALID;
+  }
+  DevMem in;
+  const u64* d_rows;
+  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
+  return hierarchical_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
+}
+extern "C" int32_t mzgpu_reduce_hierarchical_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                                 mzgpu_buf* errs) {
+  if (r == nullptr || rows == nullptr || out == nullptr || errs == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(r->ctx);
+  if (!hierarchical_io_ok(r, rows->rb, out, errs)) {
+    MZ_SET_ERR(r->ctx,
+               "reduce_hierarchical: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes",
+               rows->rb, out->rb, errs->rb);
+    return MZGPU_E_INVALID;
+  }
+  r->ctx->stats.rows_in += rows->ub;
+  return hierarchical_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
 }
 
 // ------------------------------------------------------- monotonic TopK

@@ -873,6 +873,44 @@ struct RunCur {
   u64 lo, hi;  // rows [lo, hi) of the key, sorted by (val, time)
 };
 constexpr int MM_MAX_RUNS = MZ_MAX_TRACE_BATCHES + 1;
+// The key's run in every batch of `tv` (rows of NW words, sorted by key): one hash probe per batch.
+template <int NW>
+__device__ __forceinline__ int key_runs(const TraceView& tv, u64 key, RunCur* cur) {
+  int nc = 0;
+  const u64 h0 = mix64(key);
+  for (u32 b = 0; b < tv.n_batches; ++b) {
+    const BatchView& bv = tv.b[b];
+    const u64 mask = bv_mask(bv);
+    u64 h = h0 & mask;
+    while (true) {
+      const ulonglong2 sl = *reinterpret_cast<const ulonglong2*>(&bv.table[h]);
+      if (sl.y == 0) break;
+      if (sl.x == key) {
+        const u64 first = (sl.y & MZ_SLOT_ROW_MASK) - 1;
+        const u32 len = (u32)(sl.y >> 44);
+        u64 end = first + len;
+        if (len == 0) {  // run length not recorded: upper bound search (rows are sorted by key)
+          u64 lo = first + 1, hi = bv_n(bv);
+          while (lo < hi) {
+            const u64 mid = (lo + hi) >> 1;
+            if (bv.rows[mid * NW] == key)
+              lo = mid + 1;
+            else
+              hi = mid;
+          }
+          end = lo;
+        }
+        cur[nc].rows = bv.rows;
+        cur[nc].lo = first;
+        cur[nc].hi = end;
+        ++nc;
+        break;
+      }
+      h = (h + 1) & mask;
+    }
+  }
+  return nc;
+}
 __device__ __noinline__ int mm_runs(const TraceView& tv, u64 key, RunCur* cur) {
   int nc = 0;
   const u64 h0 = mix64(key);
@@ -953,6 +991,72 @@ __device__ __forceinline__ void mm_stream(const RunCur* cur, int nc, const u64* 
       }
     }
     if (!f(v, cnt)) break;
+  }
+}
+// The value words (1 .. NV) of a row of R32 (NV = 1) or R40 (NV = 2) input, compared as one unsigned tuple.
+template <int NV>
+__device__ __forceinline__ bool vals_less(const u64* a, const u64* b) {
+  if (NV == 1) return a[0] < b[0];
+  return a[0] != b[0] ? a[0] < b[0] : a[1] < b[1];
+}
+template <int NV>
+__device__ __forceinline__ bool vals_eq(const u64* a, const u64* b) {
+  return NV == 1 ? a[0] == b[0] : (a[0] == b[0] && a[1] == b[1]);
+}
+// mm_stream over rows of NW words (key, NW - 3 value words, time, diff), the distinct values compared as
+// unsigned tuples: f(value, count) gets the word itself for R32 rows, a pointer to the value words otherwise.
+// (mm_stream and mm_runs stay as they are: written through these templates, k_minmax_lb and walk_topk
+// compile to different code.)
+template <int NW, class F>
+__device__ __forceinline__ void mm_stream_rows(const RunCur* cur, int nc, const u64* nrows, u64 nlo, u64 nhi, bool use_new,
+                                          u64 t_limit, bool desc, F f) {
+  constexpr int NV = NW - 3;
+  u64 lo[MM_MAX_RUNS], hi[MM_MAX_RUNS];
+  for (int c = 0; c < nc; ++c) {
+    lo[c] = cur[c].lo;
+    hi[c] = cur[c].hi;
+  }
+  const int nn = use_new ? nc + 1 : nc;
+  if (use_new) {
+    lo[nc] = nlo;
+    hi[nc] = nhi;
+  }
+  while (true) {
+    bool have = false;
+    u64 v[NV];
+#pragma unroll
+    for (int w = 0; w < NV; ++w) v[w] = 0;
+    for (int c = 0; c < nn; ++c) {
+      if (lo[c] >= hi[c]) continue;
+      const u64* rows = c < nc ? cur[c].rows : nrows;
+      u64 hv[NV];
+#pragma unroll
+      for (int w = 0; w < NV; ++w) hv[w] = rows[(desc ? hi[c] - 1 : lo[c]) * NW + 1 + w];
+      if (!have || (desc ? vals_less<NV>(v, hv) : vals_less<NV>(hv, v))) {
+#pragma unroll
+        for (int w = 0; w < NV; ++w) v[w] = hv[w];
+        have = true;
+      }
+    }
+    if (!have) break;
+    i64 cnt = 0;
+    for (int c = 0; c < nn; ++c) {
+      const u64* rows = c < nc ? cur[c].rows : nrows;
+      while (lo[c] < hi[c]) {
+        const u64 r = desc ? hi[c] - 1 : lo[c];
+        if (!vals_eq<NV>(rows + r * NW + 1, v)) break;
+        if (c < nc || rows[r * NW + NW - 2] <= t_limit) cnt += (i64)rows[r * NW + NW - 1];
+        if (desc)
+          --hi[c];
+        else
+          ++lo[c];
+      }
+    }
+    if constexpr (NV == 1) {
+      if (!f(v[0], cnt)) break;
+    } else {
+      if (!f((const u64*)v, cnt)) break;
+    }
   }
 }
 // MIN / MAX of a wide group: one ascending pass (every value is looked at: the error row needs
@@ -1667,6 +1771,255 @@ __global__ void __launch_bounds__(RT) k_monotonic_corrections_lb(const u64* __re
   }
 }
 
+// ------------------------------------------------------------ hierarchical MIN / MAX
+// build_bucketed / build_bucketed_negated_output (reduce.rs:796-1135) over input that retracts: the
+// arrangement holds the input rows masked to the bits the lanes read (key, val1[, val2], time | diff, an
+// ordinary SUM diff).  Per key and time the output is every lane's MIN / MAX over the live rows while every
+// live count is positive; a negative count puts the key in the error state instead (no row, one error).
+// One thread per key run of the new batch keeps the key's distinct value rows in a local table; a key with
+// more than MM_CAP of them takes the ordered merge of its runs (mm_stream), one pass per new time.
+template <int NV>
+struct HierAcc {
+  u64 v[MM_CAP][NV];
+  i64 c[MM_CAP];
+  int m;
+  bool overflow;
+};
+template <int NV>
+__device__ __forceinline__ void hier_add(HierAcc<NV>& a, const u64* v, i64 d) {
+  for (int j = 0; j < a.m; ++j)
+    if (vals_eq<NV>(a.v[j], v)) {
+      a.c[j] += d;
+      return;
+    }
+  int at = -1;
+  for (int j = 0; j < a.m && at < 0; ++j)  // reuse a dead entry before growing
+    if (a.c[j] == 0) at = j;
+  if (at < 0) {
+    if (a.m == MM_CAP) {
+      a.overflow = true;
+      return;
+    }
+    at = a.m++;
+  }
+#pragma unroll
+  for (int w = 0; w < NV; ++w) a.v[at][w] = v[w];
+  a.c[at] = d;
+}
+// the key's rows in the prior batches (one hash probe per batch) into the table
+template <int IW>
+__device__ __forceinline__ void hier_prior(const TraceView& tv, u64 key, HierAcc<IW - 3>& a) {
+  const u64 h0 = mix64(key);
+  for (u32 b = 0; b < tv.n_batches && !a.overflow; ++b) {
+    const BatchView& bv = tv.b[b];
+    const u64 mask = bv_mask(bv);
+    u64 h = h0 & mask;
+    while (true) {
+      const ulonglong2 sl = *reinterpret_cast<const ulonglong2*>(&bv.table[h]);
+      if (sl.y == 0) break;
+      if (sl.x == key) {
+        const u64 first = (sl.y & MZ_SLOT_ROW_MASK) - 1;
+        const u32 len = (u32)(sl.y >> 44);
+        const u64 bn = len != 0 ? first + len : bv_n(bv);
+        for (u64 r = first; r < bn; ++r) {
+          const u64* row = bv.rows + r * IW;
+          if (len == 0 && row[0] != key) break;
+          hier_add<IW - 3>(a, row + 1, (i64)row[IW - 1]);
+        }
+        break;
+      }
+      h = (h + 1) & mask;
+    }
+  }
+}
+// one live value row folded into the lane words S (value ^ xm: a max of the words is the lane's MIN / MAX)
+template <int C, int NV>
+__device__ __forceinline__ void hier_fold(const LaneSet& ls, const MonoXor& mx, u64 key, const u64* v, u64* S) {
+#pragma unroll
+  for (int l = 0; l < C; ++l) {
+    if ((u32)l >= ls.n) continue;
+    const u64 w = lane_value(ls.lane[l], key, v[0], NV == 2 ? v[1] : 0) ^ mx.xm[l];
+    S[l] = w > S[l] ? w : S[l];
+  }
+}
+__device__ __forceinline__ const u64* hier_vals(const u64& v) { return &v; }
+__device__ __forceinline__ const u64* hier_vals(const u64* v) { return v; }
+constexpr u32 HIER_ROW = 1, HIER_ERR = 2;  // the key's state: it has an output row / it is in the error state
+
+// The key's rows [i, ...) of the new batch (sorted by (values, time)) replayed in time order on top of its
+// prior rows: (-old, +new) output rows whenever the lanes' values or the row's presence change, and an R32
+// error row (key, 0, t, +1 entering / -1 leaving the error state) whenever that state changes.  Returns the
+// output row count and the error row count (*n_err).  With do_write the output rows go to out[pos ...],
+// sorted, and the error rows to errs[*err_len++] (a key's at most one error row per new time).
+template <int IW, int C>
+__device__ __noinline__ u32 hier_walk(const u64* __restrict__ rows, u64 n, u64 i, u64 key, const TraceView& prior,
+                                      const LaneSet& ls, const MonoXor& mx, bool do_write, u64* __restrict__ out,
+                                      u64 pos, u64* __restrict__ errs, u64 err_cap,
+                                      unsigned long long* __restrict__ err_len, u64* __restrict__ status, u32* n_err) {
+  constexpr int NV = IW - 3, TW = IW - 2, DW = IW - 1;
+  HierAcc<NV> a;
+  a.m = 0;
+  a.overflow = false;
+  hier_prior<IW>(prior, key, a);
+  u64 i_end = i;
+  while (i_end < n && rows[i_end * IW] == key) ++i_end;
+  RunCur runs[MM_MAX_RUNS];
+  int n_runs = -1;
+  auto eval_at = [&](bool use_new, u64 t_limit, u64* S) -> u32 {
+#pragma unroll
+    for (int l = 0; l < C; ++l) S[l] = 0;
+    bool any = false, bad = false;
+    auto visit = [&](const u64* v, i64 c) {
+      if (c == 0) return;
+      any = true;
+      if (c < 0)
+        bad = true;
+      else
+        hier_fold<C, NV>(ls, mx, key, v, S);
+    };
+    if (!a.overflow) {
+      for (int j = 0; j < a.m; ++j) visit(a.v[j], a.c[j]);
+    } else {
+      if (n_runs < 0) n_runs = key_runs<IW>(prior, key, runs);
+      mm_stream_rows<IW>(runs, n_runs, rows, i, i_end, use_new, t_limit, false, [&](auto v, i64 c) -> bool {
+        visit(hier_vals(v), c);
+        return true;
+      });
+    }
+    return bad ? HIER_ERR : (any ? HIER_ROW : 0);
+  };
+  u64 oldS[C];
+  u32 olds = eval_at(false, 0, oldS);
+  u32 c = 0, e = 0;
+  bool first = true;
+  u64 t_prev = 0;
+  while (true) {
+    // next distinct time of this key
+    bool found = false;
+    u64 t_cur = 0;
+    for (u64 j = i; j < i_end; ++j) {
+      const u64 t = rows[j * IW + TW];
+      if ((first || t > t_prev) && (!found || t < t_cur)) {
+        t_cur = t;
+        found = true;
+      }
+    }
+    if (!found) break;
+    for (u64 j = i; j < i_end; ++j)
+      if (rows[j * IW + TW] == t_cur) hier_add<NV>(a, rows + j * IW + 1, (i64)rows[j * IW + DW]);
+    u64 newS[C];
+    const u32 news = eval_at(true, t_cur, newS);
+    const bool had = (olds & HIER_ROW) != 0, has = (news & HIER_ROW) != 0;
+    bool same = had == has;
+#pragma unroll
+    for (int l = 0; l < C; ++l) same = same && (!has || oldS[l] == newS[l]);
+    if (!same) {
+      if (had) {
+        if (do_write) put_mono_row<C>(out, pos + c, key, oldS, mx, t_cur, ~0ull);
+        ++c;
+      }
+      if (has) {
+        if (do_write) put_mono_row<C>(out, pos + c, key, newS, mx, t_cur, 1);
+        ++c;
+      }
+    }
+    if ((olds ^ news) & HIER_ERR) {
+      if (do_write) {
+        const u64 slot = atomicAdd(err_len, 1ull);
+        const u64 r[4] = {key, 0, t_cur, (news & HIER_ERR) ? 1ull : ~0ull};
+        if (slot < err_cap)
+          store_row<4>(errs, slot, r);
+        else
+          atomicMax((unsigned long long*)status, (unsigned long long)(slot + 1));
+      }
+      ++e;
+    }
+    olds = news;
+#pragma unroll
+    for (int l = 0; l < C; ++l) oldS[l] = newS[l];
+    first = false;
+    t_prev = t_cur;
+  }
+  if (do_write && c > 1) sort_run_rows<MonoRows<C>::OUT_NW, C + 1>(out, pos, c);
+  *n_err = e;
+  return c;
+}
+
+// single-pass form (sizes on the device, chained tiles), as k_minmax_lb: one thread per key run of the new
+// batch.  Output rows leave consolidated (keys ascending, each key's rows sorted by its thread); error rows
+// leave in arbitrary order.
+template <int IW, int C>
+__global__ void __launch_bounds__(RT) k_hier_corrections_lb(const u64* __restrict__ rows, const DLen dn,
+                                                            const __grid_constant__ TraceView prior,
+                                                            const __grid_constant__ LaneSet ls, const MonoXor mx,
+                                                            const LookBack lb, u64* __restrict__ out, u64 out_cap,
+                                                            u64* __restrict__ out_len, u64* __restrict__ errs,
+                                                            u64 err_cap, unsigned long long* __restrict__ err_len,
+                                                            u64* __restrict__ status) {
+  __shared__ u32 sm[34];
+  __shared__ u32 s_tile;
+  __shared__ u64 s_b;
+  const u64 n = dlen_get(dn);
+  const u64 n_tiles = (n + RT - 1) / RT;
+  while (true) {
+    const u32 tile = lb_next_tile(lb, &s_tile);
+    if ((u64)tile >= n_tiles) {
+      if (n_tiles == 0 && tile == 0 && threadIdx.x == 0) *out_len = 0;
+      break;
+    }
+    const u64 i = (u64)tile * RT + threadIdx.x;
+    u32 cnt = 0, ecnt = 0;
+    const bool head = i < n && (i == 0 || rows[(i - 1) * IW] != rows[i * IW]);
+    u64 key = 0;
+    if (head) {
+      key = rows[i * IW];
+      cnt = hier_walk<IW, C>(rows, n, i, key, prior, ls, mx, false, nullptr, 0, nullptr, 0, nullptr, nullptr, &ecnt);
+    }
+    u32 total;
+    const u32 ex = block_exclusive_scan(cnt, sm, &total);
+    const u64 excl = lb_exclusive_prefix(lb, tile, (u64)total, &s_b);
+    if (head && (cnt > 0 || ecnt > 0)) {
+      const u64 pos = excl + ex;
+      if (pos + cnt > out_cap)
+        atomicMax((unsigned long long*)status, (unsigned long long)(pos + cnt));
+      else
+        hier_walk<IW, C>(rows, n, i, key, prior, ls, mx, true, out, pos, errs, err_cap, err_len, status, &ecnt);
+    }
+    if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *out_len = excl + total;
+  }
+}
+
+// the two-pass form (count, read back, write) for a batch past the single-pass bound; the error rows are
+// written by the write pass
+template <int IW, int C, bool WRITE>
+__global__ void __launch_bounds__(RT) k_hier_corrections(const u64* __restrict__ rows, u64 n,
+                                                         const __grid_constant__ TraceView prior,
+                                                         const __grid_constant__ LaneSet ls, const MonoXor mx,
+                                                         u32* __restrict__ tile_counts,
+                                                         const u32* __restrict__ tile_base, u64* __restrict__ out,
+                                                         u64* __restrict__ errs, u64 err_cap,
+                                                         unsigned long long* __restrict__ err_len,
+                                                         u64* __restrict__ status) {
+  __shared__ u32 sm[34];
+  const u64 i = (u64)blockIdx.x * RT + threadIdx.x;
+  u32 cnt = 0, ecnt = 0;
+  const bool head = i < n && (i == 0 || rows[(i - 1) * IW] != rows[i * IW]);
+  u64 key = 0;
+  if (head) {
+    key = rows[i * IW];
+    cnt = hier_walk<IW, C>(rows, n, i, key, prior, ls, mx, false, nullptr, 0, nullptr, 0, nullptr, nullptr, &ecnt);
+  }
+  u32 total;
+  const u32 ex = block_exclusive_scan(cnt, sm, &total);
+  if (!WRITE) {
+    if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
+  } else if (head && (cnt > 0 || ecnt > 0)) {
+    // (a pass with no output rows at all has no tile_base: it only writes error rows)
+    const u64 pos = cnt > 0 ? (u64)tile_base[blockIdx.x] + ex : 0;
+    hier_walk<IW, C>(rows, n, i, key, prior, ls, mx, true, out, pos, errs, err_cap, err_len, status, &ecnt);
+  }
+}
+
 // ------------------------------------------------------------ monotonic TopK
 // MonotonicTop1 / MonotonicTopK (src/compute/src/render/top_k.rs:102-214) for append-only inputs:
 // ensure_monotonic keeps a row iff its diff is positive, and the arrangement holds only the window, the
@@ -2174,6 +2527,63 @@ int32_t mz_monotonic_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows,
   return two_pass(ctx, n, n_out, count, alloc, write);
 }
 
+struct InRowWords : IntSet<4, 5> {  // R32 / R40 input
+  static constexpr const char* kind = "input row words";
+};
+
+// the hierarchical reduce's kernels for the input width (ls.in_words) and lane class c
+template <class F>
+static int32_t hier_dispatch(mzgpu_ctx* ctx, int c, const LaneSet& ls, F&& f) {
+  return mz_dispatch<InRowWords>(ctx, (int)ls.in_words, "hierarchical reduce", [&](auto IW) {
+    return mz_dispatch<MonoClasses>(ctx, c, "hierarchical reduce", [&](auto C) { return f(IW, C); });
+  });
+}
+
+// at most two output rows and one error row per new (key, time) row: capacities 2 * n_ub and n_ub suffice
+int32_t mz_hier_corrections_async(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, DLen n, u64 n_ub,
+                                  const TraceView& prior, const LaneSet& ls, const MonoXor& mx, u64* d_out,
+                                  u64 out_cap, u64* d_out_len, u64* d_errs, u64 err_cap, u64* d_err_len) {
+  MZ_CUDA(ctx, cudaMemsetAsync(d_err_len, 0, 8, ctx->stream));
+  LookBack lb;
+  unsigned grid;
+  MZ_TRY(lb_launch_setup(ctx, n, n_ub, 2 * ls.in_words * 8 + 2 * mz_mono_out_bytes(c), &lb, &grid));
+  return hier_dispatch(ctx, c, ls, [&](auto IW, auto C) {
+    MZ_LAUNCH(ctx, (k_hier_corrections_lb<IW, C>), grid, RT, 0, d_batch_rows, n, prior, ls, mx, lb, d_out, out_cap,
+              d_out_len, d_errs, err_cap, (unsigned long long*)d_err_len, ctx->d_status);
+    return MZGPU_OK;
+  });
+}
+
+int32_t mz_hier_corrections(mzgpu_ctx* ctx, int c, const u64* d_batch_rows, u64 n, const TraceView& prior,
+                            const LaneSet& ls, const MonoXor& mx, DevMem* out, u64* n_out, u64* d_errs, u64 err_cap,
+                            u64* d_err_len) {
+  *n_out = 0;
+  MZ_CUDA(ctx, cudaMemsetAsync(d_err_len, 0, 8, ctx->stream));
+  if (n == 0) return out->alloc(ctx, 16);
+  auto count = [&](u32* tile_counts, u64 n_tiles) {
+    return hier_dispatch(ctx, c, ls, [&](auto IW, auto C) {
+      MZ_LAUNCH(ctx, (k_hier_corrections<IW, C, false>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, ls, mx,
+                tile_counts, (const u32*)nullptr, (u64*)nullptr, (u64*)nullptr, (u64)0, (unsigned long long*)nullptr,
+                ctx->d_status);
+      return MZGPU_OK;
+    });
+  };
+  auto alloc = [&](u64 total) { return out->alloc(ctx, std::max<u64>(total, 1) * mz_mono_out_bytes(c)); };
+  auto write = [&](const u32* tile_base, u64 n_tiles) {
+    return hier_dispatch(ctx, c, ls, [&](auto IW, auto C) {
+      MZ_LAUNCH(ctx, (k_hier_corrections<IW, C, true>), (unsigned)n_tiles, RT, 0, d_batch_rows, n, prior, ls, mx,
+                (u32*)nullptr, tile_base, out->as<u64>(), d_errs, err_cap, (unsigned long long*)d_err_len,
+                ctx->d_status);
+      return MZGPU_OK;
+    });
+  };
+  const u64 n_tiles = (n + RT - 1) / RT;
+  MZ_TRY(two_pass(ctx, n, n_out, count, alloc, write));
+  // a batch whose keys change no output row can still move keys into or out of the error state
+  if (*n_out == 0) return write(nullptr, n_tiles);
+  return MZGPU_OK;
+}
+
 int32_t mz_topk_explode(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TopKOrder& to, u64* d_arr,
                         u64* d_errs, u64* d_cnt) {
   MZ_CUDA(ctx, cudaMemsetAsync(d_cnt, 0, 16, ctx->stream));
@@ -2184,16 +2594,12 @@ int32_t mz_topk_explode(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, con
   return MZGPU_OK;
 }
 
-struct TopKInWords : IntSet<4, 5> {  // R32 / R40 input
-  static constexpr const char* kind = "input row words";
-};
-
 int32_t mz_topk_window_async(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TraceView& prior,
                              const TopKOrder& to, u64* d_win, u64* d_out, u64 out_cap, u64* d_out_len) {
   LookBack lb;
   unsigned grid;
   MZ_TRY(lb_launch_setup(ctx, n, n_ub, 2 * TK_NW * 8, &lb, &grid));
-  return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
+  return mz_dispatch<InRowWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
     MZ_LAUNCH(ctx, k_topk_window_lb<IW>, grid, RT, 0, d_rows, n, prior, to.limit, lb, d_win, d_out,
               out_cap, d_out_len, ctx->d_status);
     return MZGPU_OK;
@@ -2205,7 +2611,7 @@ int32_t mz_topk_window(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView
   *n_out = 0;
   if (n == 0) return MZGPU_OK;
   auto count = [&](u32* tile_counts, u64 n_tiles) {
-    return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
+    return mz_dispatch<InRowWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
       MZ_LAUNCH(ctx, (k_topk_window<IW, false>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, to.limit, tile_counts,
                 (const u32*)nullptr, (u64*)nullptr, (u64*)nullptr);
       return MZGPU_OK;
@@ -2217,7 +2623,7 @@ int32_t mz_topk_window(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView
     return out->alloc(ctx, total * to.in_words * 8);
   };
   auto write = [&](const u32* tile_base, u64 n_tiles) {
-    return mz_dispatch<TopKInWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
+    return mz_dispatch<InRowWords>(ctx, (int)to.in_words, "topk window", [&](auto IW) {
       MZ_LAUNCH(ctx, (k_topk_window<IW, true>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, to.limit,
                 (u32*)nullptr, tile_base, win->as<u64>(), out->as<u64>());
       return MZGPU_OK;

@@ -134,6 +134,36 @@ impl Drop for GpuReduceMonotonic {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
 }
 
+/// `build_bucketed` (`HierarchicalPlan::Bucketed`, reduce.rs:232-250 of src/compute-types/src/plan; the
+/// planner's choice for MIN / MAX over a collection that can retract): several MIN / MAX aggregates per key,
+/// one output row per key (`sys::mzgpu_reduce_hierarchical_new` documents the semantics and the rows).  Lanes
+/// are `sys::AccumLane`s of kind `AGG_MIN` / `AGG_MAX`; `sign_extend != 0` is signed order.  A float64 lane
+/// (`sys::MONO_F64`) comes back as `MZGPU_E_UNSUPPORTED`: the caller keeps the Rust operator for such plans.
+pub struct GpuReduceHierarchical { h: *mut sys::Reduce, pub out_row_bytes: u32 }
+
+impl GpuReduceHierarchical {
+    pub fn new(in_row_bytes: u32, lanes: &[sys::AccumLane]) -> Result<Self, (i32, String)> {
+        let mut out = 0u32;
+        let mut h = std::ptr::null_mut();
+        unsafe {
+            sys::check(worker_ctx(), sys::mzgpu_reduce_monotonic_row_bytes(lanes.len() as u32, std::ptr::null_mut(), &mut out))?;
+            sys::check(worker_ctx(), sys::mzgpu_reduce_hierarchical_new(worker_ctx(), in_row_bytes, lanes.as_ptr(),
+                                                                       lanes.len() as u32, &mut h))?;
+        }
+        Ok(GpuReduceHierarchical { h, out_row_bytes: out })
+    }
+    /// One activation over a device buffer of input rows: corrections (`out_row_bytes` wide) are appended to
+    /// `out`, the non-positive-accumulation errors (R32: key, 0, time, +1 / -1) to `errs`.
+    pub fn step(&mut self, rows: *mut sys::Buf, upper: u64, out: *mut sys::Buf, errs: *mut sys::Buf) -> Result<(), (i32, String)> {
+        unsafe { sys::check(worker_ctx(), sys::mzgpu_reduce_hierarchical_buf(self.h, rows, upper, out, errs)) }
+    }
+    /// The arrangement of the masked input rows (R32 / R40, the input width).
+    pub fn input_trace(&self) -> *mut sys::Spine { unsafe { sys::mzgpu_reduce_input_trace(self.h) } }
+}
+impl Drop for GpuReduceHierarchical {
+    fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
+}
+
 /// `TopKPlan::MonotonicTop1` / `MonotonicTopK` (top_k.rs:102-214 of src/compute/src/render): the first
 /// `limit` rows per key of an append-only input, with only that window arranged
 /// (`sys::mzgpu_topk_monotonic_new` documents the order and the window rows).  Top1 is `limit = 1`;

@@ -211,6 +211,9 @@ extern "C" {
     pub fn mzgpu_reduce_monotonic_new(ctx: *mut Ctx, in_row_bytes: u32, lanes: *const AccumLane, n_lanes: u32, must_consolidate: i32, out: *mut *mut Reduce) -> i32;
     pub fn mzgpu_reduce_monotonic(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_reduce_monotonic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_reduce_hierarchical_new(ctx: *mut Ctx, in_row_bytes: u32, lanes: *const AccumLane, n_lanes: u32, out: *mut *mut Reduce) -> i32;
+    pub fn mzgpu_reduce_hierarchical(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_reduce_hierarchical_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_topk_monotonic_new(ctx: *mut Ctx, in_row_bytes: u32, order: *const OrderLane, n_order: u32, limit: i64, must_consolidate: i32, out: *mut *mut Reduce) -> i32;
     pub fn mzgpu_topk_monotonic(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_topk_monotonic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
