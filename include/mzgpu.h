@@ -923,6 +923,61 @@ int32_t mzgpu_topk_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int3
                              mzgpu_buf* out, mzgpu_buf* errs);
 int32_t mzgpu_topk_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs);
 
+/* ---- basic TopK: whole rows over input with retractions, up to three order columns, OFFSET
+ * (TopKPlan::Basic, which the planner picks for every TopK that is not monotonic: input that retracts, such as
+ * a join's output, and every TopK with an OFFSET, src/compute-types/src/plan/top_k.rs:47-92; rendered by
+ * build_topk / build_topk_stage / build_topk_negated_stage, src/compute/src/render/top_k.rs:215-444, 521-673).
+ *
+ * Input: R32 or R40 rows with any diffs; `key` is the group key and the row is (key, val1[, val2]).
+ * Order: as for mzgpu_topk_monotonic_new (the same mzgpu_order_lane, 0 to 3 lanes, each signed or unsigned
+ * and possibly descending).  Rows equal on every lane are ordered by val1, then val2, as unsigned words: the
+ * fixed-width stand-in for compare_columns(order_key, l, r, || l.cmp(r)), which breaks ties by the whole row's
+ * Datum order.  The two agree when every column the plan can tie on is listed as a lane, or when signed columns
+ * are encoded with the sign bit flipped (then the unsigned word order is the Datum order).
+ *
+ * Per key, at every time t, the key's live rows are its input rows with times <= t consolidated by
+ * (key, val1, val2).  Then:
+ *   every live count positive: the window is the units in positions [offset, offset + limit) of the ordered
+ *       multiset, counting multiplicities, so a limit or an offset can cut inside one row's copies (as
+ *       build_topk_negated_stage does, top_k.rs:605-669);
+ *   some live count negative (the reference's "Negative multiplicities in TopK"): the key is in the error state
+ *       and has no window;
+ *   no live row: no window.
+ * Output (`out`): rows of the INPUT width, (key, val1[, val2], time, diff), diff the change of that row's
+ *     multiplicity inside the window, consolidated and sorted per key: the collection the reference builds as
+ *     input.concat(negated_output).
+ * Errors (`errs`, R32 rows (key, 0, time, diff), consolidated): +1 when a key enters the error state at time t,
+ *     -1 when it leaves it.  This is the fixed-width stand-in that mzgpu_reduce_hierarchical_new uses; the
+ *     reference's ok output for such a key depends on how its buckets hash, and is deliberately not reproduced.
+ * State:
+ *   mzgpu_reduce_input_trace(r) returns the whole live input, one MZGPU_ROW_RTOPK row per input row (encoded
+ *       as for mzgpu_topk_monotonic_new) with ordinary SUM diffs.  The caller compacts it like any other trace.
+ *   mzgpu_topk_basic_negatives_trace(r) returns the negatives arrangement (borrowed, for inspection and size
+ *       logging): R32 rows (key, 0, time, delta) whose deltas, summed over a key, count that key's rows with a
+ *       negative accumulated count.  The operator advances its logical and physical compaction to `upper` after
+ *       each activation, so after merges it holds about one row per key in the error state.
+ * Work per touched key and new time: its window prefix (its rows up to unit offset + limit, plus cancelled rows
+ *     not yet compacted), plus its new rows, plus one binary search per prior batch per touched row.  It does not
+ *     depend on the group's size, with one exception: a key entering or leaving the error state under LIMIT NULL
+ *     emits its whole window.
+ * limit: >= 0; MZGPU_TOPK_NO_LIMIT is LIMIT NULL / None.  offset: OFFSET, any value.
+ * Checked on the host before any launch; a failure leaves no operator behind and the context usable:
+ *   MZGPU_E_INVALID: everything mzgpu_topk_monotonic_new refuses as invalid;
+ *   MZGPU_E_UNSUPPORTED: a float64 order lane, a negative limit (the reference's NegLimit path), or
+ *       offset + limit past INT64_MAX with a finite limit (the reference then makes the limit an expression,
+ *       top_k.rs:284-303).
+ * Not supported: limit expressions, NULLs, float64 order columns, and the bucket tree itself (the negatives
+ * arrangement is what bounds the work instead). */
+int32_t mzgpu_topk_basic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_order_lane* order, uint32_t n_order,
+                             int64_t limit, uint64_t offset, mzgpu_reduce** out);
+/* One activation, with the protocol of mzgpu_reduce_hierarchical[_buf]: `rows` are n input rows with times in
+ * [previous upper, upper); the window changes (input-width rows) are appended to `out`, the errors (R32) to
+ * `errs` (required; not `out`).  After a failed activation the operator reports that status from then on. */
+int32_t mzgpu_topk_basic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper, mzgpu_buf* out,
+                         mzgpu_buf* errs);
+int32_t mzgpu_topk_basic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs);
+mzgpu_spine* mzgpu_topk_basic_negatives_trace(mzgpu_reduce* r); /* borrowed, for inspection and size logging */
+
 /* ------------------------------ f1 (first step): Row keys as fixed-width words */
 /* A `Row` orders by byte length first, then by its bytes (RowRef::cmp,
  * src/repr/src/row.rs:704-722; the arrangement key order of RowRowSpine,

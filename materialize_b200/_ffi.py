@@ -317,6 +317,10 @@ SIGNATURES = {
     "mzgpu_topk_monotonic_new": (i32, [vp, u32, vp, u32, C.c_int64, i32, PV]),
     "mzgpu_topk_monotonic": (i32, [vp, vp, u64, i32, u64, vp, vp]),
     "mzgpu_topk_monotonic_buf": (i32, [vp, vp, u64, vp, vp]),
+    "mzgpu_topk_basic_new": (i32, [vp, u32, vp, u32, C.c_int64, u64, PV]),
+    "mzgpu_topk_basic": (i32, [vp, vp, u64, i32, u64, vp, vp]),
+    "mzgpu_topk_basic_buf": (i32, [vp, vp, u64, vp, vp]),
+    "mzgpu_topk_basic_negatives_trace": (vp, [vp]),
     "mzgpu_comm_unique_id": (i32, [C.POINTER(C.c_uint8)]),
     "mzgpu_comm_init": (i32, [vp, C.POINTER(C.c_uint8)]),
     "mzgpu_exchange": (i32, [vp, vp, vp]),

@@ -835,6 +835,54 @@ class TopKMonotonic:
             self.h = None
 
 
+class TopKBasic:
+    """BasicTopKPlan over input with retractions (mzgpu_topk_basic_new): per key the units in positions
+    [offset, offset + limit) of its live rows in the order of `order` (order_lane() tuples, at most 3; ties by
+    val1, then val2).  LIMIT NULL is TOPK_NO_LIMIT.  Input rows are R32 (in_row_bytes=32) or R40 (40), with any
+    diffs.  step() returns (changes, errors): the window's changes as rows of the input width, and R32 error rows
+    (key, 0, time, +1 entering / -1 leaving the negative-count state)."""
+
+    def __init__(self, ctx, order, limit, offset=0, in_row_bytes=32):
+        self.ctx = ctx
+        self.in_row_bytes = in_row_bytes
+        arr = (F.OrderLane * max(1, len(order)))()
+        for i, (src, shift, bits, sx, desc, f64) in enumerate(order):
+            arr[i].sign_extend = 1 if sx else 0
+            arr[i].descending = 1 if desc else 0
+            arr[i].flags = F.ORDER_F64 if f64 else 0
+            arr[i].field = F.Field(src, shift, bits, 0)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_topk_basic_new(ctx.h, in_row_bytes, arr, len(order), int(limit), int(offset),
+                                             C.byref(h)))
+        self.h = h
+
+    def step(self, rows, upper):
+        rows = np.ascontiguousarray(rows)
+        out, errs = DeviceRows(self.ctx, self.in_row_bytes), DeviceRows(self.ctx, 32)
+        self.ctx.check(F.lib.mzgpu_topk_basic(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
+        return out.download(), errs.download()
+
+    def step_dev(self, dev_rows, upper, out=None, errs=None):
+        """One activation over device-resident rows; changes and errors are appended on the device."""
+        out = out if out is not None else DeviceRows(self.ctx, self.in_row_bytes)
+        errs = errs if errs is not None else DeviceRows(self.ctx, 32)
+        self.ctx.check(F.lib.mzgpu_topk_basic_buf(self.h, dev_rows.h, upper, out.h, errs.h))
+        return out, errs
+
+    def input_trace(self):
+        """The whole live input (RTOPK rows)."""
+        return Spine(self.ctx, 72, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+
+    def negatives_trace(self):
+        """The negatives arrangement: R32 rows (key, 0, time, delta), summed per key its negative-count rows."""
+        return Spine(self.ctx, 32, _borrowed=F.lib.mzgpu_topk_basic_negatives_trace(self.h))
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_reduce_free(self.h)
+            self.h = None
+
+
 class ReduceMonotonic:
     """MIN / MAX of several value columns per key over append-only input (mzgpu_reduce_monotonic_new,
     build_monotonic).  `lanes` are accum_lane(AGG_MIN | AGG_MAX, ...) tuples; sign_extend=True makes a lane

@@ -1172,6 +1172,20 @@ int32_t mz_topk_window_async(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub
                              const TopKOrder& to, u64* d_win, u64* d_out, u64 out_cap, u64* d_out_len);
 int32_t mz_topk_window(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView& prior, const TopKOrder& to,
                        DevMem* win, DevMem* out, u64* n_out);
+// the basic TopK (mzgpu_topk_basic_new): every input row -> one 72-byte row (row i at d_arr[i])
+int32_t mz_topk_basic_explode(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TopKOrder& to, u64* d_arr);
+// The changes of the new 72-byte rows (sorted, consolidated, any diff) against the input arrangement `prior` and
+// the negatives arrangement `negs_tv` (R32): window changes at the input width at d_out (consolidated), R32 error
+// rows (key, 0, time, +-1) at d_errs[d_side_len[0]++] and R32 negatives deltas (key, 0, time, delta) at
+// d_negs[d_side_len[1]++], both unordered (the two counters are zeroed here).  side_cap = the new row count
+// suffices (at most one of each per key and new time).  Single pass: out_cap = 2 * limit per new row suffices.
+int32_t mz_topk_basic_async(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TraceView& prior,
+                            const TraceView& negs_tv, const TopKOrder& to, i64 offset, u64* d_out, u64 out_cap,
+                            u64* d_out_len, u64* d_errs, u64* d_negs, u64 side_cap, u64* d_side_len);
+// the two-pass form (count, read back, write): past the single-pass bound, and for LIMIT NULL
+int32_t mz_topk_basic(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView& prior, const TraceView& negs_tv,
+                      const TopKOrder& to, i64 offset, DevMem* out, u64* n_out, u64* d_errs, u64* d_negs,
+                      u64 side_cap, u64* d_side_len);
 
 // correction.cu (time-major rows: (time, key, val | diff))
 // column.cu (columnar wire format, f4)

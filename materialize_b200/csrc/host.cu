@@ -2532,11 +2532,19 @@ struct mzgpu_reduce {
   // mzgpu_topk_monotonic_new: the order lanes and limit (must_consolidate above is its flag too)
   bool topk_mono = false;
   TopKOrder tko = {};
+  // mzgpu_topk_basic_new (tko above holds its order lanes and limit): the offset (clamped to INT64_MAX), and the
+  // batcher and R32 arrangement of the negatives, (key, 0, time, change in the key's negative-count rows)
+  bool topk_basic = false;
+  i64 topk_offset = 0;
+  mzgpu_batcher* neg_batcher = nullptr;
+  mzgpu_spine* negs = nullptr;
   int32_t failed = MZGPU_OK;  // set when an activation failed after its seal (reduce_dev)
   std::string failed_msg;
   ~mzgpu_reduce() {
     delete batcher;
     delete input;
+    delete neg_batcher;
+    delete negs;
     for (int j = 0; j < n_distinct; ++j) {
       delete pair_batcher[j];
       delete pairs[j];
@@ -2831,7 +2839,7 @@ static int32_t reduce_rows_in(mzgpu_ctx* ctx, const void* rows, uint64_t n, int3
 extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_t n,
                                             int32_t mem, uint64_t upper, mzgpu_buf* out) {
   if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->lane_class || r->mono_class ||
-      r->topk_mono || r->hier_class)
+      r->topk_mono || r->hier_class || r->topk_basic)
     return MZGPU_E_INVALID;
   mzgpu_ctx* ctx = r->ctx;
   MZ_CHECK_CTX(ctx);
@@ -2843,7 +2851,7 @@ extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* ro
 extern "C" int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
                                                 mzgpu_buf* out) {
   if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64 || r->lane_class ||
-      r->mono_class || r->topk_mono || r->hier_class)
+      r->mono_class || r->topk_mono || r->hier_class || r->topk_basic)
     return MZGPU_E_INVALID;
   MZ_CHECK_CTX(r->ctx);
   r->ctx->stats.rows_in += rows->ub;
@@ -3393,16 +3401,16 @@ extern "C" int32_t mzgpu_reduce_hierarchical_buf(mzgpu_reduce* r, mzgpu_buf* row
 }
 
 // ------------------------------------------------------- monotonic TopK
-extern "C" int32_t mzgpu_topk_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_order_lane* order,
-                                            uint32_t n_order, int64_t limit, int32_t must_consolidate,
-                                            mzgpu_reduce** out) {
-  MZ_CHECK_CTX(ctx);
+// The order lanes of a TopK operator, checked as the header states (MZGPU_E_INVALID for a malformed
+// descriptor, then MZGPU_E_UNSUPPORTED for a float64 lane or a negative limit) into *to.
+static int32_t topk_order(mzgpu_ctx* ctx, const char* name, uint32_t in_row_bytes, const mzgpu_order_lane* order,
+                          uint32_t n_order, int64_t limit, mzgpu_reduce** out, TopKOrder* to_out) {
   if (out == nullptr || (order == nullptr && n_order) || (in_row_bytes != 32 && in_row_bytes != 40)) {
-    MZ_SET_ERR(ctx, "topk_monotonic: bad arguments (input rows of %u bytes)", in_row_bytes);
+    MZ_SET_ERR(ctx, "%s: bad arguments (input rows of %u bytes)", name, in_row_bytes);
     return MZGPU_E_INVALID;
   }
   if (n_order > MZGPU_MAX_ORDER_LANES) {
-    MZ_SET_ERR(ctx, "topk_monotonic: %u order lanes (0..%d)", n_order, MZGPU_MAX_ORDER_LANES);
+    MZ_SET_ERR(ctx, "%s: %u order lanes (0..%d)", name, n_order, MZGPU_MAX_ORDER_LANES);
     return MZGPU_E_INVALID;
   }
   TopKOrder to = {};
@@ -3418,7 +3426,7 @@ extern "C" int32_t mzgpu_topk_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_byte
     else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
       bad = "field is empty or out of range";
     if (bad != nullptr) {
-      MZ_SET_ERR(ctx, "topk_monotonic: order lane %u: %s", j, bad);
+      MZ_SET_ERR(ctx, "%s: order lane %u: %s", name, j, bad);
       return MZGPU_E_INVALID;
     }
     if ((L.flags & MZGPU_ORDER_F64) != 0 && unsupported < 0) unsupported = (int)j;
@@ -3427,17 +3435,27 @@ extern "C" int32_t mzgpu_topk_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_byte
     to.xm[j] = (L.sign_extend ? 1ull << 63 : 0) ^ (L.descending ? ~0ull : 0);
   }
   if (unsupported >= 0) {
-    MZ_SET_ERR(ctx, "topk_monotonic: order lane %d: float64 order columns are not supported (OrderedFloat ties "
-                    "-0.0 with +0.0 and NaN payloads)", unsupported);
+    MZ_SET_ERR(ctx, "%s: order lane %d: float64 order columns are not supported (OrderedFloat ties "
+                    "-0.0 with +0.0 and NaN payloads)", name, unsupported);
     return MZGPU_E_UNSUPPORTED;
   }
   if (limit < 0) {
-    MZ_SET_ERR(ctx, "topk_monotonic: negative limit %lld", (long long)limit);
+    MZ_SET_ERR(ctx, "%s: negative limit %lld", name, (long long)limit);
     return MZGPU_E_UNSUPPORTED;
   }
   to.n = n_order;
   to.in_words = in_row_bytes / 8;
   to.limit = limit;
+  *to_out = to;
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_topk_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_order_lane* order,
+                                            uint32_t n_order, int64_t limit, int32_t must_consolidate,
+                                            mzgpu_reduce** out) {
+  MZ_CHECK_CTX(ctx);
+  TopKOrder to;
+  MZ_TRY(topk_order(ctx, "topk_monotonic", in_row_bytes, order, n_order, limit, out, &to));
   std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
   r->ctx = ctx;
   r->agg_kind = -1;
@@ -3560,6 +3578,161 @@ extern "C" int32_t mzgpu_topk_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, ui
   }
   r->ctx->stats.rows_in += rows->ub;
   return topk_monotonic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
+}
+
+// ------------------------------------------------------- basic TopK
+extern "C" int32_t mzgpu_topk_basic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_order_lane* order,
+                                        uint32_t n_order, int64_t limit, uint64_t offset, mzgpu_reduce** out) {
+  MZ_CHECK_CTX(ctx);
+  TopKOrder to;
+  MZ_TRY(topk_order(ctx, "topk_basic", in_row_bytes, order, n_order, limit, out, &to));
+  if (limit != MZGPU_TOPK_NO_LIMIT && offset > (u64)(INT64_MAX - limit)) {
+    MZ_SET_ERR(ctx, "topk_basic: offset %llu + limit %lld overflows a 64-bit count (a limit expression)",
+               (unsigned long long)offset, (long long)limit);
+    return MZGPU_E_UNSUPPORTED;
+  }
+  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
+  r->ctx = ctx;
+  r->agg_kind = -1;
+  r->topk_basic = true;
+  r->tko = to;
+  // (no count reaches 2^63: an offset past it leaves every window empty, as INT64_MAX does)
+  r->topk_offset = (i64)std::min<u64>(offset, (u64)INT64_MAX);
+  MZ_TRY(mzgpu_batcher_new(ctx, MZGPU_ROW_RTOPK, &r->batcher));
+  MZ_TRY(mzgpu_spine_new(ctx, MZGPU_ROW_RTOPK, 1, &r->input));
+  MZ_TRY(mzgpu_batcher_new(ctx, 32, &r->neg_batcher));
+  MZ_TRY(mzgpu_spine_new(ctx, 32, 1, &r->negs));
+  *out = r.release();
+  return MZGPU_OK;
+}
+extern "C" mzgpu_spine* mzgpu_topk_basic_negatives_trace(mzgpu_reduce* r) { return r ? r->negs : nullptr; }
+
+// One activation of build_topk_negated_stage: explode -> arrange (sort, consolidate, seal) -> per key the
+// negative counts, error states and window changes of the new times -> seal the negatives.
+static int32_t topk_basic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                              mzgpu_buf* errs) {
+  mzgpu_ctx* ctx = r->ctx;
+  MZ_TRY(reduce_begin(r));
+  const TopKOrder& to = r->tko;
+  const u32 iw = to.in_words;
+  if (n_ub) {
+    Seg s;
+    MZ_TRY(s.rows.alloc(ctx, n_ub * MZGPU_ROW_RTOPK));
+    MZ_TRY(mz_topk_basic_explode(ctx, d_rows, n, n_ub, to, s.rows.as<u64>()));
+    if (n.p == nullptr) {
+      s.len.set(ctx, n.imm);
+      s.ub = n.imm;
+    } else {
+      MZ_TRY(s.len.make_pending(ctx));
+      MZ_CUDA(ctx, cudaMemcpyAsync(s.len.dptr(), n.p, 8, cudaMemcpyDeviceToDevice, ctx->stream));
+      s.len.mark_written();
+      s.ub = n_ub;
+    }
+    MZ_TRY(batcher_push_seg(r->batcher, std::move(s)));
+  }
+  mzgpu_batch* batch = nullptr;
+  MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
+  std::vector<mzgpu_batch*> prior, nprior;
+  r->input->all_batches(prior);
+  r->negs->all_batches(nprior);
+  TraceView tv, nv;
+  int32_t st = trace_view(ctx, prior, &tv);
+  if (st == MZGPU_OK) st = trace_view(ctx, nprior, &nv);
+  const u64 b_ub = batch->len_ub;
+  Seg ns;  // the negatives deltas: the negatives batcher's new rows
+  if (st == MZGPU_OK && b_ub > 0) {
+    DevMem corr, erows, econs;
+    Lazy4 slen, eflen;  // slen: [0] error rows, [1] negatives rows
+    u64 ecap = 0, s_ub = b_ub;
+    st = slen.make_pending(ctx);
+    // Output rows per new row, finite limit: a change at one new time of a key is a row whose share of the
+    // window differs between the previous and the current time, so it holds a unit of the old window or of the
+    // new one; each window is at most `limit` units, hence at most 2 * limit rows per new time, and a key has
+    // no more new times than new rows.
+    const i64 L = to.limit;
+    if (L != MZGPU_TOPK_NO_LIMIT && (u64)L < MZ_BOUND_MAX_ROWS && single_pass_fits(b_ub, 2 * (u64)L)) {
+      const u64 cap = 2 * (u64)L * b_ub;
+      Lazy4 clen;
+      if (st == MZGPU_OK) st = corr.alloc(ctx, std::max<u64>(cap, 1) * iw * 8);
+      if (st == MZGPU_OK) st = erows.alloc(ctx, b_ub * 32);
+      if (st == MZGPU_OK) st = ns.rows.alloc(ctx, b_ub * 32);
+      if (st == MZGPU_OK) st = clen.make_pending(ctx);
+      if (st == MZGPU_OK) {
+        st = mz_topk_basic_async(ctx, batch->rows.as<u64>(), batch_dlen(batch), b_ub, tv, nv, to, r->topk_offset,
+                                 corr.as<u64>(), cap, clen.dptr(), erows.as<u64>(), ns.rows.as<u64>(), b_ub,
+                                 slen.dptr());
+        clen.mark_written();
+        slen.mark_written();
+      }
+      // consolidated by construction: keys ascending, each key's rows sorted by its thread
+      if (st == MZGPU_OK) st = buf_append_dev(out, corr.p, dlen_of(clen, 0), cap);
+    } else {
+      u64 n_corr = 0;
+      if (st == MZGPU_OK) st = batch_resolve(batch);
+      if (st == MZGPU_OK) s_ub = batch->st.v[0];
+      if (st == MZGPU_OK) st = erows.alloc(ctx, std::max<u64>(s_ub, 1) * 32);
+      if (st == MZGPU_OK) st = ns.rows.alloc(ctx, std::max<u64>(s_ub, 1) * 32);
+      if (st == MZGPU_OK) {
+        st = mz_topk_basic(ctx, batch->rows.as<u64>(), s_ub, tv, nv, to, r->topk_offset, &corr, &n_corr,
+                           erows.as<u64>(), ns.rows.as<u64>(), s_ub, slen.dptr());
+        slen.mark_written();
+      }
+      if (st == MZGPU_OK && n_corr) st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
+    }
+    // the error rows leave the kernel unordered: (key, 0, time, +-1), at most one per key and time
+    if (st == MZGPU_OK && s_ub > 0)
+      st = consolidate_dev(ctx, 32, erows.p, dlen_of(slen, 0), s_ub, &econs, &ecap, &eflen);
+    if (st == MZGPU_OK && s_ub > 0)
+      st = buf_append_dev(errs, econs.p, dlen_of(eflen, 0), eflen.known ? eflen.v[0] : s_ub);
+    // the negatives deltas, unordered too: the seal below sorts and consolidates them
+    if (st == MZGPU_OK && s_ub > 0) {
+      ns.len = std::move(slen);
+      ns.word = 1;
+      ns.ub = s_ub;
+    }
+  }
+  int32_t nst = st;
+  if (nst == MZGPU_OK && ns.ub) nst = batcher_push_seg(r->neg_batcher, std::move(ns));
+  mzgpu_batch* nb = nullptr;
+  if (nst == MZGPU_OK) nst = batcher_seal(r->neg_batcher, upper, &nb, nullptr);
+  if (nb != nullptr) {
+    const int32_t ins = trace_join(r->negs, nb);
+    if (nst == MZGPU_OK) nst = ins;
+  }
+  if (nst == MZGPU_OK) nst = mzgpu_spine_set_logical_compaction(r->negs, upper);
+  if (nst == MZGPU_OK) nst = mzgpu_spine_set_physical_compaction(r->negs, upper);
+  return reduce_seal_tail(r, batch, nst);
+}
+
+static bool topk_basic_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
+  return r->topk_basic && in_rb == r->tko.in_words * 8 && out->rb == in_rb && errs->rb == 32 && out != errs;
+}
+extern "C" int32_t mzgpu_topk_basic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                    mzgpu_buf* out, mzgpu_buf* errs) {
+  if (r == nullptr || out == nullptr || errs == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = r->ctx;
+  MZ_CHECK_CTX(ctx);
+  const uint32_t in_rb = r->tko.in_words * 8;
+  if (!topk_basic_io_ok(r, in_rb, out, errs)) {
+    MZ_SET_ERR(ctx, "topk_basic: output buffer of %u-byte rows / error buffer of %u-byte rows", out->rb, errs->rb);
+    return MZGPU_E_INVALID;
+  }
+  DevMem in;
+  const u64* d_rows;
+  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
+  return topk_basic_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
+}
+extern "C" int32_t mzgpu_topk_basic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                        mzgpu_buf* errs) {
+  if (r == nullptr || rows == nullptr || out == nullptr || errs == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(r->ctx);
+  if (!topk_basic_io_ok(r, rows->rb, out, errs)) {
+    MZ_SET_ERR(r->ctx, "topk_basic: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes",
+               rows->rb, out->rb, errs->rb);
+    return MZGPU_E_INVALID;
+  }
+  r->ctx->stats.rows_in += rows->ub;
+  return topk_basic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
 }
 
 // ============================================================ Row keys as words (f1, first step)

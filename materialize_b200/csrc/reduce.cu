@@ -2026,6 +2026,30 @@ __global__ void __launch_bounds__(RT) k_hier_corrections(const u64* __restrict__
 // first `limit` units per key in order.  Window rows are RowT<72>: key, o0, o1, o2, val1, val2, time | diff.
 constexpr int TK_NW = 9;
 
+// the 72-byte row of input row r (to.in_words words) with diff `diff`, as k_topk_explode writes it (which keeps
+// its own copy: calling this changed its generated code)
+__device__ __forceinline__ void tk_encode(const TopKOrder& to, const u64* r, i64 diff, u64* o) {
+  const u32 iw = to.in_words;
+  const u64 key = r[0], v1 = r[1], v2 = iw == 5 ? r[2] : 0;
+  o[0] = key;
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    u64 v = 0;
+    if ((u32)j < to.n) {
+      v = field_get(to.f[j], key, v1, v2);
+      const u32 bits = to.f[j].bits;
+      if (to.sign_extend[j] && bits < 64 && ((v >> (bits - 1)) & 1)) v |= ~0ull << bits;
+      v ^= to.xm[j];
+    }
+    o[1 + j] = v;
+  }
+  o[4] = v1;
+  o[5] = v2;
+  o[6] = r[iw - 2];
+  o[7] = (u64)diff;
+  o[8] = 0;
+}
+
 // Input rows -> one window row per row with diff > 0 (at arr[cnt[0]++]) and one R16 (time, +1) row per
 // other row (at errs[cnt[1]++]); warp-aggregated slots, as k_monotonic_explode.
 __global__ void __launch_bounds__(RT) k_topk_explode(const u64* __restrict__ rows, const DLen dn,
@@ -2288,6 +2312,289 @@ __global__ void __launch_bounds__(RT) k_topk_window(const u64* __restrict__ rows
     if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
   } else if (head && cnt > 0) {
     tk_key<IW, true>(prior, rows, i, end, key, limit, win, out, (u64)tile_base[blockIdx.x] + ex);
+  }
+}
+
+// ------------------------------------------------------------ basic TopK
+// BasicTopKPlan (build_topk_negated_stage, top_k.rs:521-673) over input that retracts: the input arrangement
+// holds every input row as a 72-byte row with an ordinary SUM diff, and a negatives arrangement holds R32 rows
+// (key, 0, time, delta) whose sum per key is the number of the key's rows with a negative accumulated count.
+
+// Input rows -> one 72-byte row each, whatever its diff (row i at arr[i])
+__global__ void __launch_bounds__(RT) k_topk_basic_explode(const u64* __restrict__ rows, const DLen dn,
+                                                           const __grid_constant__ TopKOrder to, u64* __restrict__ arr) {
+  const u64 n = dlen_get(dn);
+  for (u64 i = (u64)blockIdx.x * RT + threadIdx.x; i < n; i += (u64)gridDim.x * RT) {
+    const u64* r = rows + i * to.in_words;
+    u64 o[TK_NW];
+    tk_encode(to, r, (i64)r[to.in_words - 1], o);
+    store_row<TK_NW>(arr, i, o);
+  }
+}
+
+// the accumulated count of row g (words 1..5) in the key's prior runs [lo, hi): one lower-bound search per run
+// (a run is sorted by (o0, o1, o2, val1, val2, time); before compaction a row may hold several times)
+__device__ __forceinline__ i64 tkb_prior_count(const TraceView& tv, const u64* lo, const u64* hi,
+                                               const uint8_t* bsel, int nc, const u64* g) {
+  i64 s = 0;
+  for (int k = 0; k < nc; ++k) {
+    const u64* rows = tv.b[bsel[k]].rows;
+    u64 l = lo[k], r = hi[k];
+    while (l < r) {
+      const u64 mid = (l + r) >> 1;
+      if (tk_less(rows + mid * TK_NW, g))
+        l = mid + 1;
+      else
+        r = mid;
+    }
+    for (; l < hi[k] && tk_same(rows + l * TK_NW, g); ++l) s += (i64)rows[l * TK_NW + 7];
+  }
+  return s;
+}
+
+// the key's negative-count rows before the new batch: the sum of its deltas in the negatives arrangement (R32
+// rows; one hash probe per batch)
+__device__ __forceinline__ i64 tkb_neg_prior(const TraceView& nv, u64 key) {
+  i64 s = 0;
+  const u64 h0 = mix64(key);
+  for (u32 b = 0; b < nv.n_batches; ++b) {
+    const BatchView& bv = nv.b[b];
+    const u64 mask = bv_mask(bv);
+    u64 h = h0 & mask;
+    while (true) {
+      const ulonglong2 sl = *reinterpret_cast<const ulonglong2*>(&bv.table[h]);
+      if (sl.y == 0) break;
+      if (sl.x == key) {
+        const u64 first = (sl.y & MZ_SLOT_ROW_MASK) - 1;
+        const u32 len = (u32)(sl.y >> 44);
+        const u64 bn = len != 0 ? first + len : bv_n(bv);
+        for (u64 r = first; r < bn && bv.rows[r * 4] == key; ++r) s += (i64)bv.rows[r * 4 + 3];
+        break;
+      }
+      h = (h + 1) & mask;
+    }
+  }
+  return s;
+}
+
+// the units of a row of m units with c units before it inside the window [off, end)
+__device__ __forceinline__ i64 tkb_share(i64 c, i64 m, i64 off, i64 end) {
+  const i64 a = c > off ? c : off;
+  const i64 b = m > end - c ? end : c + m;
+  return b > a ? b - a : 0;
+}
+
+// The changes of one key whose new rows are nrows[i, nhi) (sorted by (row, time), consolidated, any diff),
+// replayed one distinct new time t at a time against its prior runs in the input arrangement:
+//   (a) the key's negative-count rows at t: the negatives arrangement's count before the batch, plus, for each
+//       touched row, whether its count (prior count by search, plus its new diffs <= t) is negative now and was
+//       before.  A change emits (key, 0, t, delta) to `negs`; entering / leaving the error state (count > 0)
+//       emits (key, 0, t, +1 / -1) to `errs`.  Both go to atomic slots (side_len[0] / [1], capacity side_cap;
+//       an overflow is recorded in *status).
+//   (b) the window changes from the previous time: an ordered merge of the prior runs with the new rows <= t,
+//       a row's share the overlap of [before, before + count) with [offset, offset + limit), empty for a side
+//       in the error state.  The walk stops once the units before the current row reach the window's end at
+//       both times (counts can shrink, so one time's position bounds nothing).  Without a limit it stops at
+//       the offset instead: past it every row is whole in both windows and only the new rows at t change,
+//       unless the key enters or leaves the error state, which walks the whole window.
+// Returns the output row count and the side row count (*n_side).  With WRITE the output rows (input width) go
+// to out[pos ...], sorted.
+template <int IW, bool WRITE>
+__device__ __noinline__ u32 tkb_key(const TraceView& tv, const TraceView& nv, const u64* __restrict__ nrows, u64 i,
+                                    u64 nhi, u64 key, i64 limit, i64 off, u64* __restrict__ out, u64 pos,
+                                    u64* __restrict__ errs, u64* __restrict__ negs, u64 side_cap,
+                                    unsigned long long* __restrict__ side_len, u64* __restrict__ status,
+                                    u32* n_side) {
+  u64 lo0[MM_MAX_RUNS], hi[MM_MAX_RUNS], lo[MM_MAX_RUNS];
+  uint8_t bsel[MM_MAX_RUNS];
+  const int nc = tk_runs(tv, key, lo0, hi, bsel);
+  const bool no_limit = limit == INT64_MAX;
+  const i64 end = no_limit ? INT64_MAX : off + limit;  // (the host refuses an overflowing offset + limit)
+  const i64 n0 = tkb_neg_prior(nv, key);
+  i64 nprev = n0;
+  bool have_prev = false;
+  u64 tprev = 0;
+  u32 c = 0, e = 0;
+  auto side = [&](u64* dst, int which, u64 t, i64 d) {
+    if (WRITE) {
+      const u64 slot = atomicAdd(&side_len[which], 1ull);
+      const u64 r[4] = {key, 0, t, (u64)d};
+      if (slot < side_cap)
+        store_row<4>(dst, slot, r);
+      else
+        atomicMax((unsigned long long*)status, (unsigned long long)(slot + 1));
+    }
+    ++e;
+  };
+  auto emit = [&](const u64* g, u64 t, i64 d) {
+    if (WRITE) {
+      u64 p[IW];
+      p[0] = key;
+      p[1] = g[4];
+      if (IW == 5) p[2] = g[5];
+      p[IW - 2] = t;
+      p[IW - 1] = (u64)d;
+      store_row<IW>(out, pos + c, p);
+    }
+    ++c;
+  };
+  while (true) {
+    bool found = false;
+    u64 tcur = 0;
+    for (u64 j = i; j < nhi; ++j) {
+      const u64 t = nrows[j * TK_NW + 6];
+      if ((!have_prev || t > tprev) && (!found || t < tcur)) {
+        tcur = t;
+        found = true;
+      }
+    }
+    if (!found) break;
+    // (a)
+    i64 ncur = n0;
+    for (u64 j = i; j < nhi;) {
+      const u64* g = nrows + j * TK_NW;
+      const i64 p = tkb_prior_count(tv, lo0, hi, bsel, nc, g);
+      i64 s = p;
+      for (; j < nhi && tk_same(nrows + j * TK_NW, g); ++j)
+        if (nrows[j * TK_NW + 6] <= tcur) s += (i64)nrows[j * TK_NW + 7];
+      ncur += (i64)(s < 0) - (i64)(p < 0);
+    }
+    const bool errp = nprev > 0, errc = ncur > 0;
+    if (ncur != nprev) side(negs, 1, tcur, ncur - nprev);
+    if (errp != errc) side(errs, 0, tcur, errc ? 1 : -1);
+    // (b)
+    if (limit > 0 && !(errp && errc)) {
+      const bool tail = no_limit && !errp && !errc;
+      const i64 stop = tail ? off : end;
+      for (int k = 0; k < nc; ++k) lo[k] = lo0[k];
+      u64 nlo = i;
+      i64 cp = 0, cc = 0;  // units before the current row at the previous / current time
+      while ((!errp && cp < stop) || (!errc && cc < stop)) {
+        const u64* best = nullptr;
+        for (int k = 0; k < nc; ++k) {
+          if (lo[k] >= hi[k]) continue;
+          const u64* r = tv.b[bsel[k]].rows + lo[k] * TK_NW;
+          if (best == nullptr || tk_less(r, best)) best = r;
+        }
+        if (nlo < nhi) {
+          const u64* r = nrows + nlo * TK_NW;
+          if (best == nullptr || tk_less(r, best)) best = r;
+        }
+        if (best == nullptr) break;
+        u64 g[TK_NW];
+        load_row<TK_NW>(best, 0, g);
+        i64 o = 0, np = 0, ncu = 0;
+        for (int k = 0; k < nc; ++k) {
+          const u64* rows = tv.b[bsel[k]].rows;
+          while (lo[k] < hi[k] && tk_same(rows + lo[k] * TK_NW, g)) {
+            o += (i64)rows[lo[k] * TK_NW + 7];
+            ++lo[k];
+          }
+        }
+        while (nlo < nhi && tk_same(nrows + nlo * TK_NW, g)) {
+          const u64 t = nrows[nlo * TK_NW + 6];
+          const i64 d = (i64)nrows[nlo * TK_NW + 7];
+          if (have_prev && t <= tprev) np += d;
+          if (t <= tcur) ncu += d;
+          ++nlo;
+        }
+        const i64 mp = o + np, mc = o + ncu;
+        const i64 wp = errp ? 0 : tkb_share(cp, mp, off, end), wc = errc ? 0 : tkb_share(cc, mc, off, end);
+        if (wc != wp) emit(g, tcur, wc - wp);
+        cp += mp;
+        cc += mc;
+      }
+      if (tail)
+        for (; nlo < nhi; ++nlo)
+          if (nrows[nlo * TK_NW + 6] == tcur) emit(nrows + nlo * TK_NW, tcur, (i64)nrows[nlo * TK_NW + 7]);
+    }
+    nprev = ncur;
+    tprev = tcur;
+    have_prev = true;
+  }
+  if (WRITE && c > 1) sort_run_rows<IW, IW - 2>(out, pos, c);
+  *n_side = e;
+  return c;
+}
+
+// single-pass form (sizes on the device, chained tiles), as k_hier_corrections_lb: one thread per key run of
+// the new rows.  Output rows leave consolidated; error and negatives rows leave in arbitrary order.
+template <int IW>
+__global__ void __launch_bounds__(RT) k_topk_basic_lb(const u64* __restrict__ rows, const DLen dn,
+                                                      const __grid_constant__ TraceView prior,
+                                                      const __grid_constant__ TraceView negv, const i64 limit,
+                                                      const i64 off, const LookBack lb, u64* __restrict__ out,
+                                                      u64 out_cap, u64* __restrict__ out_len, u64* __restrict__ errs,
+                                                      u64* __restrict__ negs, u64 side_cap,
+                                                      unsigned long long* __restrict__ side_len,
+                                                      u64* __restrict__ status) {
+  __shared__ u32 sm[34];
+  __shared__ u32 s_tile;
+  __shared__ u64 s_b;
+  const u64 n = dlen_get(dn);
+  const u64 n_tiles = (n + RT - 1) / RT;
+  while (true) {
+    const u32 tile = lb_next_tile(lb, &s_tile);
+    if ((u64)tile >= n_tiles) {
+      if (n_tiles == 0 && tile == 0 && threadIdx.x == 0) *out_len = 0;
+      break;
+    }
+    const u64 i = (u64)tile * RT + threadIdx.x;
+    u32 cnt = 0, ecnt = 0;
+    const bool head = i < n && (i == 0 || rows[(i - 1) * TK_NW] != rows[i * TK_NW]);
+    u64 key = 0, end = 0;
+    if (head) {
+      key = rows[i * TK_NW];
+      end = tk_run_end(rows, n, i, key);
+      cnt = tkb_key<IW, false>(prior, negv, rows, i, end, key, limit, off, nullptr, 0, nullptr, nullptr, 0, nullptr,
+                               nullptr, &ecnt);
+    }
+    u32 total;
+    const u32 ex = block_exclusive_scan(cnt, sm, &total);
+    const u64 excl = lb_exclusive_prefix(lb, tile, (u64)total, &s_b);
+    if (head && (cnt > 0 || ecnt > 0)) {
+      const u64 pos = excl + ex;
+      if (pos + cnt > out_cap)
+        atomicMax((unsigned long long*)status, (unsigned long long)(pos + cnt));
+      else
+        tkb_key<IW, true>(prior, negv, rows, i, end, key, limit, off, out, pos, errs, negs, side_cap, side_len,
+                          status, &ecnt);
+    }
+    if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *out_len = excl + total;
+  }
+}
+
+// the two-pass form (count, read back, write) for a batch past the single-pass bound and for LIMIT NULL; the
+// error and negatives rows are written by the write pass
+template <int IW, bool WRITE>
+__global__ void __launch_bounds__(RT) k_topk_basic(const u64* __restrict__ rows, u64 n,
+                                                   const __grid_constant__ TraceView prior,
+                                                   const __grid_constant__ TraceView negv, const i64 limit,
+                                                   const i64 off, u32* __restrict__ tile_counts,
+                                                   const u32* __restrict__ tile_base, u64* __restrict__ out,
+                                                   u64* __restrict__ errs, u64* __restrict__ negs, u64 side_cap,
+                                                   unsigned long long* __restrict__ side_len,
+                                                   u64* __restrict__ status) {
+  __shared__ u32 sm[34];
+  const u64 i = (u64)blockIdx.x * RT + threadIdx.x;
+  u32 cnt = 0, ecnt = 0;
+  const bool head = i < n && (i == 0 || rows[(i - 1) * TK_NW] != rows[i * TK_NW]);
+  u64 key = 0, end = 0;
+  if (head) {
+    key = rows[i * TK_NW];
+    end = tk_run_end(rows, n, i, key);
+    cnt = tkb_key<IW, false>(prior, negv, rows, i, end, key, limit, off, nullptr, 0, nullptr, nullptr, 0, nullptr,
+                             nullptr, &ecnt);
+  }
+  u32 total;
+  const u32 ex = block_exclusive_scan(cnt, sm, &total);
+  if (!WRITE) {
+    if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
+  } else if (head && (cnt > 0 || ecnt > 0)) {
+    // (a pass with no output rows at all has no tile_base: it only writes error and negatives rows)
+    const u64 pos = cnt > 0 ? (u64)tile_base[blockIdx.x] + ex : 0;
+    tkb_key<IW, true>(prior, negv, rows, i, end, key, limit, off, out, pos, errs, negs, side_cap, side_len, status,
+                      &ecnt);
   }
 }
 
@@ -2630,4 +2937,56 @@ int32_t mz_topk_window(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView
     });
   };
   return two_pass(ctx, n, n_out, count, alloc, write);
+}
+
+int32_t mz_topk_basic_explode(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TopKOrder& to, u64* d_arr) {
+  if (n_ub == 0) return MZGPU_OK;
+  const unsigned grid = grid_of(ctx, (n_ub + RT - 1) / RT);
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (to.in_words * 8 + TK_NW * 8) : 0);
+  MZ_LAUNCH(ctx, k_topk_basic_explode, grid, RT, 0, d_rows, n, to, d_arr);
+  return MZGPU_OK;
+}
+
+int32_t mz_topk_basic_async(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const TraceView& prior,
+                            const TraceView& negs_tv, const TopKOrder& to, i64 offset, u64* d_out, u64 out_cap,
+                            u64* d_out_len, u64* d_errs, u64* d_negs, u64 side_cap, u64* d_side_len) {
+  MZ_CUDA(ctx, cudaMemsetAsync(d_side_len, 0, 16, ctx->stream));
+  LookBack lb;
+  unsigned grid;
+  MZ_TRY(lb_launch_setup(ctx, n, n_ub, 2 * TK_NW * 8 + 2 * to.in_words * 8, &lb, &grid));
+  return mz_dispatch<InRowWords>(ctx, (int)to.in_words, "topk basic", [&](auto IW) {
+    MZ_LAUNCH(ctx, k_topk_basic_lb<IW>, grid, RT, 0, d_rows, n, prior, negs_tv, to.limit, offset, lb, d_out, out_cap,
+              d_out_len, d_errs, d_negs, side_cap, (unsigned long long*)d_side_len, ctx->d_status);
+    return MZGPU_OK;
+  });
+}
+
+int32_t mz_topk_basic(mzgpu_ctx* ctx, const u64* d_rows, u64 n, const TraceView& prior, const TraceView& negs_tv,
+                      const TopKOrder& to, i64 offset, DevMem* out, u64* n_out, u64* d_errs, u64* d_negs,
+                      u64 side_cap, u64* d_side_len) {
+  *n_out = 0;
+  MZ_CUDA(ctx, cudaMemsetAsync(d_side_len, 0, 16, ctx->stream));
+  if (n == 0) return MZGPU_OK;
+  auto count = [&](u32* tile_counts, u64 n_tiles) {
+    return mz_dispatch<InRowWords>(ctx, (int)to.in_words, "topk basic", [&](auto IW) {
+      MZ_LAUNCH(ctx, (k_topk_basic<IW, false>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, negs_tv, to.limit, offset,
+                tile_counts, (const u32*)nullptr, (u64*)nullptr, (u64*)nullptr, (u64*)nullptr, (u64)0,
+                (unsigned long long*)nullptr, ctx->d_status);
+      return MZGPU_OK;
+    });
+  };
+  auto alloc = [&](u64 total) { return out->alloc(ctx, std::max<u64>(total, 1) * to.in_words * 8); };
+  auto write = [&](const u32* tile_base, u64 n_tiles) {
+    return mz_dispatch<InRowWords>(ctx, (int)to.in_words, "topk basic", [&](auto IW) {
+      MZ_LAUNCH(ctx, (k_topk_basic<IW, true>), (unsigned)n_tiles, RT, 0, d_rows, n, prior, negs_tv, to.limit, offset,
+                (u32*)nullptr, tile_base, out->as<u64>(), d_errs, d_negs, side_cap, (unsigned long long*)d_side_len,
+                ctx->d_status);
+      return MZGPU_OK;
+    });
+  };
+  const u64 n_tiles = (n + RT - 1) / RT;
+  MZ_TRY(two_pass(ctx, n, n_out, count, alloc, write));
+  // a batch whose keys change no window can still change their negative counts and error states
+  if (*n_out == 0) return write(nullptr, n_tiles);
+  return MZGPU_OK;
 }

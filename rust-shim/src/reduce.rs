@@ -193,6 +193,37 @@ impl Drop for GpuTopKMonotonic {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
 }
 
+/// `BasicTopKPlan` (`build_topk` / `build_topk_negated_stage`): whole rows over input that retracts, with an
+/// OFFSET (`sys::mzgpu_topk_basic_new` documents the order, the window and the error rows).  Each `ColumnOrder`
+/// is one order lane; `LIMIT NULL` is `sys::TOPK_NO_LIMIT`.  A negative literal limit, a float64 order column,
+/// or `offset + limit` past `i64::MAX` comes back as `MZGPU_E_UNSUPPORTED`: the caller keeps the Rust operator
+/// for those, and for a limit given as an expression.
+pub struct GpuTopKBasic { h: *mut sys::Reduce }
+
+impl GpuTopKBasic {
+    pub fn new(in_row_bytes: u32, order: &[sys::OrderLane], limit: i64, offset: u64) -> Result<Self, (i32, String)> {
+        let mut h = std::ptr::null_mut();
+        unsafe {
+            sys::check(worker_ctx(), sys::mzgpu_topk_basic_new(worker_ctx(), in_row_bytes, order.as_ptr(),
+                                                              order.len() as u32, limit, offset, &mut h))?;
+        }
+        Ok(GpuTopKBasic { h })
+    }
+    /// One activation over a device buffer of input rows: the window changes (input-width rows) are appended
+    /// to `out`, the error-state changes (R32: key, 0, time, +1 / -1) to `errs`, the error collection.
+    pub fn step(&mut self, rows: *mut sys::Buf, upper: u64, out: *mut sys::Buf, errs: *mut sys::Buf) -> Result<(), (i32, String)> {
+        unsafe { sys::check(worker_ctx(), sys::mzgpu_topk_basic_buf(self.h, rows, upper, out, errs)) }
+    }
+    /// The input arrangement (72-byte rows), compacted by the caller like any other trace.
+    pub fn input_trace(&self) -> *mut sys::Spine { unsafe { sys::mzgpu_reduce_input_trace(self.h) } }
+    /// The negatives arrangement (R32), compacted by the operator itself; for inspection and size logging.
+    pub fn negatives_trace(&self) -> *mut sys::Spine { unsafe { sys::mzgpu_topk_basic_negatives_trace(self.h) } }
+}
+
+impl Drop for GpuTopKBasic {
+    fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
+}
+
 impl Drop for GpuReduce {
     fn drop(&mut self) { unsafe { sys::mzgpu_reduce_free(self.h) } }
 }

@@ -217,6 +217,10 @@ extern "C" {
     pub fn mzgpu_topk_monotonic_new(ctx: *mut Ctx, in_row_bytes: u32, order: *const OrderLane, n_order: u32, limit: i64, must_consolidate: i32, out: *mut *mut Reduce) -> i32;
     pub fn mzgpu_topk_monotonic(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_topk_monotonic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_topk_basic_new(ctx: *mut Ctx, in_row_bytes: u32, order: *const OrderLane, n_order: u32, limit: i64, offset: u64, out: *mut *mut Reduce) -> i32;
+    pub fn mzgpu_topk_basic(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_topk_basic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_topk_basic_negatives_trace(r: *mut Reduce) -> *mut Spine;
     pub fn mzgpu_rowkey_pack(row_bytes: *const u8, len: u64, key_out: *mut u64) -> i32;
     pub fn mzgpu_rowkeys_pack(data: *const u8, offsets: *const u64, n: u64, keys_out: *mut u64, n_done: *mut u64) -> i32;
     pub fn mzgpu_rowkey_unpack(key: u64, row_bytes_out: *mut u8, len_out: *mut u64) -> i32;
