@@ -978,6 +978,129 @@ int32_t mzgpu_topk_basic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t 
 int32_t mzgpu_topk_basic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs);
 mzgpu_spine* mzgpu_topk_basic_negatives_trace(mzgpu_reduce* r); /* borrowed, for inspection and size logging */
 
+/* ---- temporal filters: the device MfpPlan (src/expr/src/linear.rs:1730-1990), with the updates it produces at
+ * future times held in a bucket chain until the frontier reaches them (the temporal delay operator,
+ * src/compute/src/extensions/temporal_bucket.rs, over BucketChain, src/timely-util/src/temporal.rs:59-211).
+ *
+ * Input: R32 or R40 rows with any diffs.  Output: R32 or R40 rows whose words (key, val1 and, for R40, val2)
+ * are each an OR of up to MZGPU_MAX_FIELDS input bit-fields (mzgpu_field, src MZGPU_SRC_KEY / VAL1 / VAL2, where
+ * VAL2 is the R40 input's second value word).  Map expressions are not projected: as with HAVING, the map part
+ * stays with the caller, and an expression a predicate reads is written inline in it.
+ *
+ * Non-temporal predicates (0..MZGPU_MFP_MAX_PREDICATES) are programs of the HAVING interpreter
+ * (mzgpu_having_op; same types, width rules, errors and three-valued AND / OR / NOT) evaluated in order as
+ * SafeMfpPlan::evaluate_inner does: the first one that is not TRUE drops the row; an error stops evaluation
+ * and becomes an error update at the row's (time, diff).  The one difference: MZGPU_HOP_COL (the HAVING
+ * opcode MZGPU_HOP_KEY) pushes a bit-field of source word `arg` (MZGPU_SRC_*) instead of the key.
+ * MZGPU_HOP_COUNT / SUM / NUM / FLOAT are MZGPU_E_INVALID here.  No value is NULL: nullable columns are
+ * outside the fixed-width subset.
+ *
+ * Temporal predicates (0..MZGPU_MFP_MAX_TEMPORAL) read `mz_now() CMP expr` with CMP one of MZGPU_CMP_EQ / LT /
+ * LE / GT / GE; expr is a program that leaves one MZTS (u64 mz_timestamp).  The bound lists are derived as
+ * MfpPlan::create_from does (linear.rs:1772-1804), in predicate order: EQ adds expr to the lower bounds and
+ * step_mz_timestamp(expr) to the upper bounds, LT adds expr to the upper bounds, LE adds step(expr) to them,
+ * GT adds step(expr) to the lower bounds and GE adds expr to them.  step_mz_timestamp(u64::MAX) is
+ * MzTimestampStepOverflow.  Beyond the integer ops a temporal program has:
+ *   MZGPU_HOP_COL_MZTS     push MZTS: the unsigned bit-field of word `arg` (uint8_to_mz_timestamp, an
+ *                          mz_timestamp column); cannot fail
+ *   MZGPU_HOP_INT_TO_MZTS  INT -> MZTS (bigint / integer_to_mz_timestamp); a negative value is
+ *                          MzTimestampOutOfRange with the value as payload
+ *   MZGPU_HOP_COL_TS       push TS: a `timestamp` column, the (sign-extended) field as i64 microseconds
+ *                          since 1970-01-01 00:00:00
+ *   MZGPU_HOP_COL_DATE     push DATE: a `date` column, the (sign-extended) field as i32 days since 1970-01-01
+ *   MZGPU_HOP_TS_ADD_IV    TS + the constant interval consts[konst] (lo = microseconds as i64, hi = days in
+ *                          bits 0-31 and months in bits 32-63, both i32); a result outside
+ *                          [LOW_DATE, HIGH_DATE] = [-4713-12-31, 262142-12-31] is TimestampOutOfRange
+ *                          (add_timestamplike_interval, src/expr/src/scalar/func.rs:200-213)
+ *   MZGPU_HOP_TS_TO_MZTS   TS -> MZTS: milliseconds, rounded toward -inf (timestamp_millis); a negative
+ *                          result is MzTimestampOutOfRange with the microseconds as payload
+ *   MZGPU_HOP_DATE_TO_MZTS DATE -> MZTS: days * 86,400,000; a negative result is MzTimestampOutOfRange with
+ *                          the days as payload
+ * MZTS, TS and DATE values are MZGPU_E_UNSUPPORTED in a non-temporal predicate: it keeps payload-carrying
+ * errors out of AND / OR, whose order would compare error strings.
+ *
+ * Per input row (time, diff), exactly MfpPlan::evaluate (linear.rs:1865-1971), with valid(t) = t < until
+ * (until = MZGPU_FRONTIER_EMPTY: every time is valid):
+ *   the predicates; then lower = max(time, every lower bound), evaluated in order, the first error wins; a
+ *   row whose lower is not valid is dropped before any upper bound is evaluated; upper = the minimum of the
+ *   upper bounds, clamped to at least lower, and evaluation stops once upper == lower (later upper-bound
+ *   errors are never raised); an invalid upper becomes "none"; if lower != upper the output gets
+ *   (row, lower, +diff) and, if there is an upper, (row, upper, -diff).
+ * Errors are R32 rows (code, payload, time, diff) in `errs`, consolidated.  The codes are numbered in the
+ * order of the EvalError variants (src/expr/src/scalar.rs:1724-1750): the four HAVING codes, then
+ * MZGPU_MFP_ERR_MZ_TIMESTAMP_OUT_OF_RANGE (payload: the operand, as the reference's message embeds it),
+ * MZGPU_MFP_ERR_MZ_TIMESTAMP_STEP_OVERFLOW and MZGPU_MFP_ERR_TIMESTAMP_OUT_OF_RANGE (payload 0).
+ *
+ * mzgpu_mfp_step(op, rows, upper, out, errs): evaluates the new rows and appends to `out` every resulting
+ * update with time < upper together with every held update that has become due, consolidated (the
+ * project's consolidated row order), and appends the errors to `errs`.  Everything else is held.  `upper`
+ * must not decrease (MZGPU_E_FRONTIER).  upper == MZGPU_FRONTIER_EMPTY ("no more times") releases everything,
+ * time u64::MAX included.  The _buf form reads rows and their count from the device and returns nothing to
+ * the host (beyond what consolidating a release whose bound exceeds the fused kernel's limit reads back).
+ *
+ * Row counts stay on the device: a step's buffers are sized by host bounds (2 updates per new row; a held
+ * slice by its segment's bound until the segment's header has been read back, which happens asynchronously and
+ * never blocks a step).  Held updates live in a bucket chain: buckets [start, start + 2^bits) covering [upper, 2^64), each owning
+ * device row segments.  A step inserts its held rows with one partition pass over at most 64 bucket bounds
+ * (a histogram and a scatter, no sort; a step's held rows are inserted at the start of the next step, or by
+ * mzgpu_mfp_frontier / mzgpu_mfp_stats, once their count is known), peels the buckets below `upper` and splits the
+ * one that straddles it
+ * (a two-way time partition), then restores the chain (adjacent buckets within two bits of each other)
+ * with fuel counted in rows, MZGPU_MFP_RESTORE_FUEL per step (temporal_bucket.rs:159-165).
+ *
+ * mzgpu_mfp_frontier(op, &t): t = the least held time, or MZGPU_FRONTIER_EMPTY when nothing is held: where the
+ * caller holds its capability, as the delay operator does.  On any other status t is not written (a failed
+ * read must not look like "nothing held").  mzgpu_mfp_stats(op, out): out[0] = held rows, out[1] = buckets,
+ * out[2] = rows the store read and wrote in the last step (insert, peel, splits and restore; the new rows'
+ * evaluation and the release's consolidation are not store work).  Both wait for the device.
+ *
+ * Refused on the host before any launch (no operator is created and the context stays usable):
+ * MZGPU_E_INVALID for a malformed plan (row widths, projection fields, predicate / temporal / op / constant
+ * counts, unknown opcodes or compare ops, stack underflow or overflow, operand types, a program that does
+ * not leave one BOOL / one MZTS); MZGPU_E_UNSUPPORTED for a well-formed plan outside the subset (an interval
+ * with months, or whose days and microseconds leave i64 microseconds; MZTS / TS / DATE in a non-temporal
+ * predicate; a float64 column, MZGPU_HOP_COL_F64), so that the caller keeps the Rust operator at render time. */
+#define MZGPU_MFP_MAX_PREDICATES 4
+#define MZGPU_MFP_MAX_TEMPORAL 4
+#define MZGPU_MFP_MAX_OPS 16 /* per program */
+#define MZGPU_MFP_MAX_CONSTS 8
+#define MZGPU_MFP_RESTORE_FUEL 1000000
+#define MZGPU_HOP_COL MZGPU_HOP_KEY /* push INT: bits [shift, shift + bits) of source word arg */
+#define MZGPU_HOP_COL_MZTS 15
+#define MZGPU_HOP_INT_TO_MZTS 16
+#define MZGPU_HOP_COL_TS 17
+#define MZGPU_HOP_COL_DATE 18
+#define MZGPU_HOP_TS_ADD_IV 19
+#define MZGPU_HOP_TS_TO_MZTS 20
+#define MZGPU_HOP_DATE_TO_MZTS 21
+#define MZGPU_HOP_COL_F64 22 /* a float64 column (word arg): always MZGPU_E_UNSUPPORTED */
+#define MZGPU_MFP_ERR_MZ_TIMESTAMP_OUT_OF_RANGE 5
+#define MZGPU_MFP_ERR_MZ_TIMESTAMP_STEP_OVERFLOW 6
+#define MZGPU_MFP_ERR_TIMESTAMP_OUT_OF_RANGE 7
+typedef struct mzgpu_mfp {
+  uint32_t in_row_bytes;  /* 32 or 40 */
+  uint32_t out_row_bytes; /* 32 or 40 */
+  uint32_t n_fields[3];   /* fields of the output key, val1, val2 (val2: R40 output only) */
+  mzgpu_field fields[3][MZGPU_MAX_FIELDS];
+  uint32_t n_predicates;
+  uint32_t n_temporal;
+  uint32_t n_consts;
+  uint32_t temporal_cmp[MZGPU_MFP_MAX_TEMPORAL]; /* MZGPU_CMP_EQ / LT / LE / GT / GE */
+  uint32_t n_ops[MZGPU_MFP_MAX_PREDICATES];
+  uint32_t n_temporal_ops[MZGPU_MFP_MAX_TEMPORAL];
+  mzgpu_having_op ops[MZGPU_MFP_MAX_PREDICATES][MZGPU_MFP_MAX_OPS];
+  mzgpu_having_op temporal_ops[MZGPU_MFP_MAX_TEMPORAL][MZGPU_MFP_MAX_OPS];
+  mzgpu_having_const consts[MZGPU_MFP_MAX_CONSTS];
+} mzgpu_mfp;
+typedef struct mzgpu_mfp_op mzgpu_mfp_op;
+int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t until, mzgpu_mfp_op** out);
+void mzgpu_mfp_free(mzgpu_mfp_op* op);
+int32_t mzgpu_mfp_step(mzgpu_mfp_op* op, const void* rows, uint64_t n, int32_t mem, uint64_t upper, mzgpu_buf* out,
+                       mzgpu_buf* errs);
+int32_t mzgpu_mfp_step_buf(mzgpu_mfp_op* op, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs);
+int32_t mzgpu_mfp_frontier(mzgpu_mfp_op* op, uint64_t* out);
+int32_t mzgpu_mfp_stats(mzgpu_mfp_op* op, uint64_t out[3]);
+
 /* ------------------------------ f1 (first step): Row keys as fixed-width words */
 /* A `Row` orders by byte length first, then by its bytes (RowRef::cmp,
  * src/repr/src/row.rs:704-722; the arrangement key order of RowRowSpine,

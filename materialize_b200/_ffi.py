@@ -173,6 +173,33 @@ class Having(C.Structure):
     ]
 
 
+# temporal filters (mzgpu_mfp, include/mzgpu.h)
+MFP_MAX_PREDICATES, MFP_MAX_TEMPORAL, MFP_MAX_OPS, MFP_MAX_CONSTS = 4, 4, 16, 8
+MFP_RESTORE_FUEL = 1000000
+HOP_COL = HOP_KEY
+HOP_COL_MZTS, HOP_INT_TO_MZTS, HOP_COL_TS, HOP_COL_DATE = 15, 16, 17, 18
+HOP_TS_ADD_IV, HOP_TS_TO_MZTS, HOP_DATE_TO_MZTS, HOP_COL_F64 = 19, 20, 21, 22
+MFP_ERR_MZ_TIMESTAMP_OUT_OF_RANGE, MFP_ERR_MZ_TIMESTAMP_STEP_OVERFLOW, MFP_ERR_TIMESTAMP_OUT_OF_RANGE = 5, 6, 7
+
+
+class Mfp(C.Structure):
+    _fields_ = [
+        ("in_row_bytes", C.c_uint32),
+        ("out_row_bytes", C.c_uint32),
+        ("n_fields", C.c_uint32 * 3),
+        ("fields", (Field * 6) * 3),
+        ("n_predicates", C.c_uint32),
+        ("n_temporal", C.c_uint32),
+        ("n_consts", C.c_uint32),
+        ("temporal_cmp", C.c_uint32 * MFP_MAX_TEMPORAL),
+        ("n_ops", C.c_uint32 * MFP_MAX_PREDICATES),
+        ("n_temporal_ops", C.c_uint32 * MFP_MAX_TEMPORAL),
+        ("ops", (HavingOp * MFP_MAX_OPS) * MFP_MAX_PREDICATES),
+        ("temporal_ops", (HavingOp * MFP_MAX_OPS) * MFP_MAX_TEMPORAL),
+        ("consts", HavingConst * MFP_MAX_CONSTS),
+    ]
+
+
 class Filter(C.Structure):
     _fields_ = [("field", Field), ("op", C.c_uint32), ("rhs", C.c_uint64)]
 
@@ -321,6 +348,12 @@ SIGNATURES = {
     "mzgpu_topk_basic": (i32, [vp, vp, u64, i32, u64, vp, vp]),
     "mzgpu_topk_basic_buf": (i32, [vp, vp, u64, vp, vp]),
     "mzgpu_topk_basic_negatives_trace": (vp, [vp]),
+    "mzgpu_mfp_new": (i32, [vp, C.POINTER(Mfp), u64, PV]),
+    "mzgpu_mfp_free": (None, [vp]),
+    "mzgpu_mfp_step": (i32, [vp, vp, u64, i32, u64, vp, vp]),
+    "mzgpu_mfp_step_buf": (i32, [vp, vp, u64, vp, vp]),
+    "mzgpu_mfp_frontier": (i32, [vp, C.POINTER(u64)]),
+    "mzgpu_mfp_stats": (i32, [vp, C.POINTER(u64)]),
     "mzgpu_comm_unique_id": (i32, [C.POINTER(C.c_uint8)]),
     "mzgpu_comm_init": (i32, [vp, C.POINTER(C.c_uint8)]),
     "mzgpu_exchange": (i32, [vp, vp, vp]),

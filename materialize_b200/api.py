@@ -883,6 +883,88 @@ class TopKBasic:
             self.h = None
 
 
+def hop(code, arg=0, shift=0, bits=0, sign_extend=0, konst=0):
+    """One op of a HAVING / MFP program (mzgpu_having_op) as a tuple."""
+    return (code, arg, shift, bits, sign_extend, konst)
+
+
+def col(src, shift=0, bits=64, signed=False, code=F.HOP_COL):
+    """Push a bit-field of source word `src` (SRC_KEY / SRC_VAL1 / SRC_VAL2): INT, or with `code` an
+    MZTS (HOP_COL_MZTS), TS (HOP_COL_TS) or DATE (HOP_COL_DATE) column."""
+    return hop(code, src, shift, bits, 1 if signed else 0)
+
+
+def interval_const(micros=0, days=0, months=0):
+    """An interval constant for HOP_TS_ADD_IV: (lo, hi) with lo = microseconds, hi = days | months << 32."""
+    return (micros & (2**64 - 1), (days & 0xFFFFFFFF) | ((months & 0xFFFFFFFF) << 32))
+
+
+class Mfp:
+    """A temporal filter (mzgpu_mfp_new): the MfpPlan of a `WHERE mz_now() ...` query.  `fields` gives the
+    output words (key, val1, val2) as lists of (src, shift, bits, dst_shift); `predicates` are op lists (hop());
+    `temporal` is a list of (cmp, ops) for `mz_now() cmp expr`; `consts` are (lo, hi) pairs.  step() returns
+    (updates, errors): the updates of time < upper, consolidated, and R32 error rows (code, payload, time, diff);
+    future updates are held until an upper passes them."""
+
+    def __init__(self, ctx, fields, predicates=(), temporal=(), consts=(), in_row_bytes=32, out_row_bytes=32,
+                 until=F.FRONTIER_EMPTY):
+        self.ctx, self.in_row_bytes, self.out_row_bytes = ctx, in_row_bytes, out_row_bytes
+        m = F.Mfp()
+        m.in_row_bytes, m.out_row_bytes = in_row_bytes, out_row_bytes
+        for w, fl in enumerate(fields):
+            m.n_fields[w] = len(fl)
+            for i, f in enumerate(fl[:6]):
+                m.fields[w][i] = F.Field(*f)
+        m.n_predicates, m.n_temporal, m.n_consts = len(predicates), len(temporal), len(consts)
+
+        def put(dst, ops):
+            for i, o in enumerate(ops[:F.MFP_MAX_OPS]):
+                dst[i].code, dst[i].arg, dst[i].shift, dst[i].bits, dst[i].sign_extend, dst[i].konst = o
+
+        for p, ops in enumerate(predicates[:F.MFP_MAX_PREDICATES]):
+            m.n_ops[p] = len(ops)
+            put(m.ops[p], ops)
+        for p, (cmp, ops) in enumerate(temporal[:F.MFP_MAX_TEMPORAL]):
+            m.temporal_cmp[p] = cmp
+            m.n_temporal_ops[p] = len(ops)
+            put(m.temporal_ops[p], ops)
+        for k, (lo, hi) in enumerate(consts[:F.MFP_MAX_CONSTS]):
+            m.consts[k].lo, m.consts[k].hi = lo & (2**64 - 1), hi & (2**64 - 1)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_mfp_new(ctx.h, C.byref(m), until, C.byref(h)))
+        self.h = h
+
+    def step(self, rows, upper):
+        rows = np.ascontiguousarray(rows)
+        out, errs = DeviceRows(self.ctx, self.out_row_bytes), DeviceRows(self.ctx, 32)
+        self.ctx.check(F.lib.mzgpu_mfp_step(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
+        return out.download(), errs.download()
+
+    def step_dev(self, dev_rows, upper, out=None, errs=None):
+        """One step over device-resident rows; updates and errors are appended on the device."""
+        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
+        errs = errs if errs is not None else DeviceRows(self.ctx, 32)
+        self.ctx.check(F.lib.mzgpu_mfp_step_buf(self.h, dev_rows.h, upper, out.h, errs.h))
+        return out, errs
+
+    def frontier(self):
+        """The least held time, or FRONTIER_EMPTY."""
+        t = C.c_uint64(0)
+        self.ctx.check(F.lib.mzgpu_mfp_frontier(self.h, C.byref(t)))
+        return t.value
+
+    def stats(self):
+        """(held rows, buckets, rows the store read and wrote in the last step)."""
+        a = (C.c_uint64 * 3)()
+        self.ctx.check(F.lib.mzgpu_mfp_stats(self.h, a))
+        return tuple(int(x) for x in a)
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_mfp_free(self.h)
+            self.h = None
+
+
 class ReduceMonotonic:
     """MIN / MAX of several value columns per key over append-only input (mzgpu_reduce_monotonic_new,
     build_monotonic).  `lanes` are accum_lane(AGG_MIN | AGG_MAX, ...) tuples; sign_extend=True makes a lane

@@ -1221,3 +1221,33 @@ int32_t mz_partition_many(mzgpu_ctx* ctx, u32 k, const int* row_bytes, const voi
                           u64* d_send_by_peer /* [peer][k] */);
 int32_t mz_partition(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, DLen n, u64 n_ub, u32 peers, void* d_out,
                      u64* d_counts /* 64 words */, u64* d_cursors /* 64 words */);
+
+// mfp.cu: the temporal filter (mzgpu_mfp_new).  A plan as the kernels read it: the caller's descriptor plus
+// the derived bound lists (program index in bits 0-2, bit 3: wrapped in step_mz_timestamp), in the order of
+// MfpPlan::create_from.
+struct MfpDevPlan {
+  mzgpu_mfp plan;
+  u32 n_lower, n_upper;
+  u32 lower[MZGPU_MFP_MAX_TEMPORAL], upper[MZGPU_MFP_MAX_TEMPORAL];
+  i64 iv_us[MZGPU_MFP_MAX_CONSTS];  // interval constants folded to microseconds (MZGPU_HOP_TS_ADD_IV)
+};
+// a segment: MZ_MFP_HDR header words (slice j's rows are [hdr[j], hdr[j + 1])), then the rows
+#define MZ_MFP_HDR 72
+#define MZ_MFP_MAX_SLOTS 65  // 64 bucket bounds and the overflow slot of an insert round
+#define MZ_MFP_SLICES 32     // source slices per partition launch
+struct MfpSlices {
+  const u64* base[MZ_MFP_SLICES];
+  u32 idx[MZ_MFP_SLICES];
+  u32 n;
+};
+struct MfpBounds {
+  u64 v[MZ_MFP_MAX_SLOTS];  // ascending; a row at time t goes to slot (# v <= t) - 1
+  u32 nb;
+};
+int32_t mz_mfp_eval(mzgpu_ctx* ctx, const MfpDevPlan& pl, const u64* d_rows, DLen n, u64 n_ub, u64 upper, u64 until,
+                    u64* ready, u64* held, u64* errs, u64* err_len);
+// partition the rows of `chunks` into the nb slots of segment `dst`; `hist` and `cursor` are
+// MZ_MFP_MAX_SLOTS words each, adjacent (cursor == hist + MZ_MFP_MAX_SLOTS); *total (if set) gets the row count
+int32_t mz_mfp_partition(mzgpu_ctx* ctx, int rb, const MfpSlices* chunks, u32 n_chunks, u64 rows_ub,
+                         const MfpBounds& b, u64* hist, u64* cursor, u64* dst, u64* total, u64* touched);
+int32_t mz_mfp_min_time(mzgpu_ctx* ctx, int rb, const MfpSlices* chunks, u32 n_chunks, u64 rows_ub, u64* d_min);

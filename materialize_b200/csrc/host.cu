@@ -8,6 +8,7 @@
 #include <algorithm>
 #include <cstring>
 #include <deque>
+#include <map>
 #include <memory>
 #include <new>
 
@@ -4620,4 +4621,617 @@ extern "C" int32_t mzgpu_partition_many(mzgpu_ctx* ctx, uint32_t k, mzgpu_buf** 
 }
 extern "C" int32_t mzgpu_exchange(mzgpu_ctx* ctx, mzgpu_buf* in, mzgpu_buf* out) {
   return mzgpu_exchange_many(ctx, 1, &in, &out);
+}
+
+// ========================================================== temporal filter
+// mzgpu_mfp_new (include/mzgpu.h): the device MfpPlan, and a BucketChain (src/timely-util/src/temporal.rs:59-211)
+// of the updates it produced for future times.  A bucket [start, start + 2^bits) owns slices of device segments
+// (mfp.cu); the host knows a bound on each slice's rows, and its exact size once the segment's header has been
+// copied back.  Those copies are asynchronous into pinned memory and are read once the step that issued them has
+// completed: the host never waits for them, except in mzgpu_mfp_frontier / mzgpu_mfp_stats.
+struct MfpSeg {
+  DevMem mem;  // MZ_MFP_HDR header words, then the rows
+  u64 ub = 0;
+  bool known = false;  // off[] holds the header
+  u64 off[MZ_MFP_MAX_SLOTS + 1];
+  int slot = -1;  // pinned mirror slot of the header copy in flight
+  u64 seq = 0;    // the step that issued it
+  u64* base() { return (u64*)mem.p; }
+};
+struct MfpSlice {
+  std::shared_ptr<MfpSeg> seg;
+  u32 idx;
+};
+static u64 mfp_slice_ub(const MfpSlice& s) {
+  return s.seg->known ? s.seg->off[s.idx + 1] - s.seg->off[s.idx] : s.seg->ub;
+}
+// A bound on the rows of several slices: the slices of one segment whose header is not known yet together
+// hold at most the segment's bound, however many of them there are.
+static u64 mfp_slices_ub(const std::vector<MfpSlice>& v) {
+  u64 known = 0;
+  std::vector<std::pair<const MfpSeg*, u64>> unknown;
+  for (const MfpSlice& s : v) {
+    if (s.seg->known) {
+      known += mfp_slice_ub(s);
+      continue;
+    }
+    bool seen = false;
+    for (auto& u : unknown) seen = seen || u.first == s.seg.get();
+    if (!seen) unknown.emplace_back(s.seg.get(), s.seg->ub);
+  }
+  for (auto& u : unknown) known += u.second;
+  return known;
+}
+struct MfpBucket {
+  u32 bits;
+  std::vector<MfpSlice> slices;
+};
+#define MZ_MFP_MIRROR 4096  // header copies in flight per operator
+struct mzgpu_mfp_op {
+  mzgpu_ctx* ctx;
+  MfpDevPlan pl;
+  int ow;
+  u64 until;
+  u64 upper = 0;
+  std::map<u64, MfpBucket> chain;
+  DevMem scratch;  // hist[65], cursor[65], touched, min time
+  u64* h_mirror = nullptr;
+  std::vector<int> free_slots;
+  std::vector<std::shared_ptr<MfpSeg>> inflight;
+  // held rows of earlier steps not in the chain yet: inserted at the next step (or read), once their header
+  // copy has arrived, so that the insert is sized by the exact count rather than the step's bound
+  std::vector<std::shared_ptr<MfpSeg>> pending;
+  std::deque<std::pair<u64, cudaEvent_t>> events;
+  u64 step_seq = 0, done_seq = 0;
+  u64* hist() { return (u64*)scratch.p; }
+  u64* touched() { return (u64*)scratch.p + 2 * MZ_MFP_MAX_SLOTS; }
+  u64* dmin() { return (u64*)scratch.p + 2 * MZ_MFP_MAX_SLOTS + 1; }
+  ~mzgpu_mfp_op() {
+    inflight.clear();
+    chain.clear();
+    for (auto& e : events) cudaEventDestroy(e.second);
+    if (h_mirror) cudaFreeHost(h_mirror);
+  }
+};
+
+// bucket end (start + 2^bits), false when it is past u64::MAX (advance_by_power_of_two's None)
+static bool mfp_bucket_end(u64 start, u32 bits, u64* end) {
+  if (bits >= 64) return false;
+  const u64 e = start + (1ull << bits);
+  if (e < start || e == 0) return false;
+  *end = e;
+  return true;
+}
+
+// Read every header copy whose step has completed (wait = true: after waiting for the device, every one,
+// and the headers never copied are read directly); drop empty slices.
+static int32_t mfp_poll(mzgpu_mfp_op* op, bool wait) {
+  mzgpu_ctx* ctx = op->ctx;
+  if (wait) MZ_SYNC(ctx);
+  while (!op->events.empty()) {
+    const cudaError_t e = wait ? cudaSuccess : cudaEventQuery(op->events.front().second);
+    if (e == cudaErrorNotReady) break;
+    MZ_CUDA(ctx, e);
+    op->done_seq = op->events.front().first;
+    cudaEventDestroy(op->events.front().second);
+    op->events.pop_front();
+  }
+  std::vector<std::shared_ptr<MfpSeg>> still;
+  for (auto& s : op->inflight) {
+    if (s->seq <= op->done_seq) {
+      memcpy(s->off, op->h_mirror + (size_t)s->slot * MZ_MFP_HDR, sizeof(s->off));
+      s->known = true;
+      op->free_slots.push_back(s->slot);
+      s->slot = -1;
+    } else {
+      still.push_back(std::move(s));
+    }
+  }
+  op->inflight.swap(still);
+  for (auto& kv : op->chain) {
+    auto& v = kv.second.slices;
+    if (wait)
+      for (auto& sl : v)
+        if (!sl.seg->known && sl.seg->slot < 0) {
+          MZ_TRY(copy_out(ctx, sl.seg->off, sl.seg->base(), sizeof(sl.seg->off), MZGPU_MEM_HOST));
+          sl.seg->known = true;
+        }
+    v.erase(std::remove_if(v.begin(), v.end(), [](const MfpSlice& s) { return s.seg->known && mfp_slice_ub(s) == 0; }),
+            v.end());
+  }
+  return MZGPU_OK;
+}
+
+// Copy a segment's header back asynchronously (read by mfp_poll once the step has completed); with the pinned
+// mirror full, the header stays unknown until a waiting call reads it.
+static int32_t mfp_mirror(mzgpu_mfp_op* op, const std::shared_ptr<MfpSeg>& seg) {
+  if (op->free_slots.empty()) return MZGPU_OK;
+  mzgpu_ctx* ctx = op->ctx;
+  seg->slot = op->free_slots.back();
+  op->free_slots.pop_back();
+  seg->seq = op->step_seq;
+  MZ_CUDA(ctx, cudaMemcpyAsync(op->h_mirror + (size_t)seg->slot * MZ_MFP_HDR, seg->base(), sizeof(seg->off),
+                               cudaMemcpyDeviceToHost, ctx->stream));
+  op->inflight.push_back(seg);
+  return MZGPU_OK;
+}
+
+// Partition the rows of `src` into the nb slots of a new segment (a row at time t goes to slot
+// (# bounds <= t) - 1); *total, if set, gets its row count on the device.
+static int32_t mfp_partition(mzgpu_mfp_op* op, const std::vector<MfpSlice>& src, const u64* bounds, u32 nb,
+                             std::shared_ptr<MfpSeg>* out, u64* total, bool mirror) {
+  mzgpu_ctx* ctx = op->ctx;
+  const int nw = op->ow / 8;
+  auto seg = std::make_shared<MfpSeg>();
+  seg->ub = mfp_slices_ub(src);
+  std::vector<MfpSlices> chunks;
+  for (const MfpSlice& s : src) {
+    if (mfp_slice_ub(s) == 0) continue;
+    if (chunks.empty() || chunks.back().n == MZ_MFP_SLICES) {
+      chunks.emplace_back();
+      chunks.back().n = 0;
+    }
+    MfpSlices& c = chunks.back();
+    c.base[c.n] = s.seg->base();
+    c.idx[c.n] = s.idx;
+    c.n++;
+  }
+  MZ_TRY(seg->mem.alloc(ctx, (MZ_MFP_HDR + seg->ub * (u64)nw) * 8));
+  if (seg->ub == 0) {
+    MZ_CUDA(ctx, cudaMemsetAsync(seg->mem.p, 0, MZ_MFP_HDR * 8, ctx->stream));
+    if (total) MZ_CUDA(ctx, cudaMemsetAsync(total, 0, 8, ctx->stream));
+    memset(seg->off, 0, sizeof(seg->off));
+    seg->known = true;
+  } else {
+    MfpBounds b;
+    memset(&b, 0, sizeof(b));
+    b.nb = nb;
+    for (u32 j = 0; j < nb; ++j) b.v[j] = bounds[j];
+    MZ_TRY(mz_mfp_partition(ctx, op->ow, chunks.data(), (u32)chunks.size(), seg->ub, b, op->hist(),
+                            op->hist() + MZ_MFP_MAX_SLOTS, seg->base(), total, op->touched()));
+    if (mirror) MZ_TRY(mfp_mirror(op, seg));
+  }
+  *out = std::move(seg);
+  return MZGPU_OK;
+}
+
+// BucketChain::split_and_insert: halve the bucket with a two-way time partition (no launch for an empty one)
+static int32_t mfp_split(mzgpu_mfp_op* op, u64 start, MfpBucket&& bk, int64_t* fuel) {
+  const u32 bits = bk.bits - 1;
+  const u64 mid = start + (1ull << bits);
+  MfpBucket lo{bits, {}}, hi{bits, {}};
+  const u64 ub = mfp_slices_ub(bk.slices);
+  if (ub > 0) {
+    const u64 bnd[2] = {start, mid};
+    std::shared_ptr<MfpSeg> seg;
+    MZ_TRY(mfp_partition(op, bk.slices, bnd, 2, &seg, nullptr, true));
+    lo.slices.push_back({seg, 0});
+    hi.slices.push_back({seg, 1});
+    *fuel -= (int64_t)ub;
+  }
+  op->chain[start] = std::move(lo);
+  op->chain[mid] = std::move(hi);
+  return MZGPU_OK;
+}
+
+// BucketChain::peel: the slices of every bucket below `upper`, splitting the one that straddles it
+static int32_t mfp_peel(mzgpu_mfp_op* op, u64 upper, std::vector<MfpSlice>* peeled) {
+  int64_t no_fuel = 0;
+  while (!op->chain.empty()) {
+    auto it = op->chain.begin();
+    const u64 start = it->first;
+    if (upper != MZGPU_FRONTIER_EMPTY && upper <= start) break;
+    MfpBucket bk = std::move(it->second);
+    op->chain.erase(it);
+    u64 end = 0;
+    const bool has_end = mfp_bucket_end(start, bk.bits, &end);
+    if (upper != MZGPU_FRONTIER_EMPTY && (!has_end || upper < end)) {
+      MZ_TRY(mfp_split(op, start, std::move(bk), &no_fuel));
+    } else {
+      for (auto& s : bk.slices) peeled->push_back(std::move(s));
+    }
+  }
+  return MZGPU_OK;
+}
+
+// BucketChain::restore with fuel counted in rows (a split costs its bucket's row bound)
+static int32_t mfp_restore(mzgpu_mfp_op* op) {
+  int64_t fuel = MZGPU_MFP_RESTORE_FUEL;
+  std::map<u64, MfpBucket> fresh;
+  int64_t last = -2;
+  while (fuel > 0 && !op->chain.empty()) {
+    auto it = op->chain.begin();
+    const u64 t = it->first;
+    MfpBucket bk = std::move(it->second);
+    op->chain.erase(it);
+    if ((int64_t)bk.bits <= last + 2) {
+      last = bk.bits;
+      fresh.emplace(t, std::move(bk));
+    } else {
+      MZ_TRY(mfp_split(op, t, std::move(bk), &fuel));
+    }
+  }
+  for (auto& kv : op->chain) fresh.emplace(kv.first, std::move(kv.second));
+  op->chain.swap(fresh);
+  return MZGPU_OK;
+}
+
+// the held rows of a step into the chain: rounds of up to 64 buckets, the rows past a round's last bucket in
+// an overflow slot that the next round partitions again
+static int32_t mfp_insert(mzgpu_mfp_op* op, MfpSlice held) {
+  if (mfp_slice_ub(held) == 0) return MZGPU_OK;
+  std::vector<MfpSlice> src{std::move(held)};
+  auto it = op->chain.begin();
+  while (it != op->chain.end()) {
+    std::vector<MfpBucket*> bs;
+    u64 bnd[MZ_MFP_MAX_SLOTS];
+    u32 nb = 0;
+    for (; it != op->chain.end() && nb < MZ_MFP_MAX_SLOTS - 1; ++it) {
+      bnd[nb++] = it->first;
+      bs.push_back(&it->second);
+    }
+    const u32 k = nb;
+    if (it != op->chain.end()) bnd[nb++] = it->first;
+    std::shared_ptr<MfpSeg> seg;
+    MZ_TRY(mfp_partition(op, src, bnd, nb, &seg, nullptr, true));
+    for (u32 j = 0; j < k; ++j) bs[j]->slices.push_back({seg, j});
+    if (it == op->chain.end()) break;
+    src.assign(1, MfpSlice{seg, k});
+  }
+  return MZGPU_OK;
+}
+
+// insert the held rows of earlier steps (their times are at least the upper they were evaluated at, which the
+// chain still covers)
+static int32_t mfp_flush_pending(mzgpu_mfp_op* op) {
+  std::vector<std::shared_ptr<MfpSeg>> p;
+  p.swap(op->pending);
+  for (auto& seg : p) MZ_TRY(mfp_insert(op, {seg, 0}));
+  return MZGPU_OK;
+}
+
+// append `n` device rows (count on the device, bound ub) to `dst`, consolidated
+static int32_t mfp_emit(mzgpu_ctx* ctx, int rb, const u64* d_rows, DLen n, u64 ub, mzgpu_buf* dst) {
+  if (ub == 0) return MZGPU_OK;
+  DevMem cons;
+  u64 cap = 0;
+  Lazy4 len;
+  MZ_TRY(consolidate_dev(ctx, rb, d_rows, n, ub, &cons, &cap, &len));
+  return buf_append_dev(dst, cons.p, dlen_of(len, 0), std::min(cap, ub));
+}
+
+static int32_t mfp_step_dev(mzgpu_mfp_op* op, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                            mzgpu_buf* errs) {
+  mzgpu_ctx* ctx = op->ctx;
+  if (out == nullptr || errs == nullptr || out == errs || (int)out->rb != op->ow || errs->rb != 32) {
+    MZ_SET_ERR(ctx, "mfp_step: out must hold %d-byte rows and errs 32-byte rows (distinct buffers)", op->ow);
+    return MZGPU_E_INVALID;
+  }
+  if (upper < op->upper) {
+    MZ_SET_ERR(ctx, "mfp_step: upper %llu is below the previous upper %llu", (unsigned long long)upper,
+               (unsigned long long)op->upper);
+    return MZGPU_E_FRONTIER;
+  }
+  MZ_TRY(mfp_poll(op, false));
+  op->step_seq++;
+  MZ_CUDA(ctx, cudaMemsetAsync(op->touched(), 0, 8, ctx->stream));
+  MZ_TRY(mfp_flush_pending(op));
+  const int onw = op->ow / 8;
+  // 1. evaluate the new rows: ready, held and error rows
+  auto ready = std::make_shared<MfpSeg>(), held = std::make_shared<MfpSeg>();
+  ready->ub = held->ub = 2 * n_ub;
+  DevMem err_rows;
+  Lazy4 err_len;
+  if (n_ub > 0) {
+    MZ_TRY(ready->mem.alloc(ctx, (MZ_MFP_HDR + 2 * n_ub * (u64)onw) * 8));
+    MZ_TRY(held->mem.alloc(ctx, (MZ_MFP_HDR + 2 * n_ub * (u64)onw) * 8));
+    MZ_TRY(err_rows.alloc(ctx, n_ub * 32));
+    MZ_TRY(err_len.make_pending(ctx));
+    MZ_CUDA(ctx, cudaMemsetAsync(ready->mem.p, 0, 16, ctx->stream));
+    MZ_CUDA(ctx, cudaMemsetAsync(held->mem.p, 0, 16, ctx->stream));
+    MZ_CUDA(ctx, cudaMemsetAsync(err_len.dptr(), 0, 8, ctx->stream));
+    MZ_TRY(mz_mfp_eval(ctx, op->pl, d_rows, n, n_ub, upper, op->until, ready->base(), held->base(),
+                       (u64*)err_rows.p, err_len.dptr()));
+    err_len.mark_written();
+  } else {
+    ready->known = held->known = true;
+    memset(ready->off, 0, sizeof(ready->off));
+    memset(held->off, 0, sizeof(held->off));
+  }
+  // 2. peel the due buckets; 3. release them with the ready rows, consolidated
+  std::vector<MfpSlice> rel;
+  MZ_TRY(mfp_peel(op, upper, &rel));
+  rel.push_back({ready, 0});
+  if (mfp_slices_ub(rel) > 0) {
+    Lazy4 tot;
+    MZ_TRY(tot.make_pending(ctx));
+    std::shared_ptr<MfpSeg> all;
+    const u64 zero = 0;
+    MZ_TRY(mfp_partition(op, rel, &zero, 1, &all, tot.dptr(), false));
+    tot.mark_written();
+    MZ_TRY(mfp_emit(ctx, op->ow, all->base() + MZ_MFP_HDR, dlen_of(tot, 0), all->ub, out));
+  }
+  rel.clear();
+  // 4. restore the chain; 5. hold the rest (inserted by the next step or read)
+  MZ_TRY(mfp_restore(op));
+  if (n_ub > 0) {
+    MZ_TRY(mfp_mirror(op, held));
+    op->pending.push_back(held);
+  }
+  // 6. errors
+  if (n_ub > 0) MZ_TRY(mfp_emit(ctx, 32, (const u64*)err_rows.p, dlen_of(err_len, 0), n_ub, errs));
+  cudaEvent_t ev;
+  MZ_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  MZ_CUDA(ctx, cudaEventRecord(ev, ctx->stream));
+  op->events.emplace_back(op->step_seq, ev);
+  op->upper = upper;
+  return MZGPU_OK;
+}
+
+// The checks of one program (include/mzgpu.h): a type per stack slot, simulated op by op.  MZGPU_E_INVALID is
+// returned at once; a well-formed construct outside the subset is noted in *unsupported (the first one).
+static int32_t validate_mfp_program(mzgpu_ctx* ctx, const mzgpu_mfp& m, const mzgpu_having_op* ops, uint32_t n_ops,
+                                    bool temporal, uint32_t p, i64* iv_us, const char** unsupported) {
+  enum Ty { INT32, INT64, BOOL, MZTS, TS, DATE };
+  const char* what = temporal ? "temporal predicate" : "predicate";
+  auto bad = [&](uint32_t i, const char* why) {
+    MZ_SET_ERR(ctx, "mfp: %s %u, op %u: %s", what, p, i, why);
+    return MZGPU_E_INVALID;
+  };
+  auto outside = [&](uint32_t i, const char* why) {
+    if (*unsupported == nullptr) {
+      MZ_SET_ERR(ctx, "mfp: %s %u, op %u: %s", what, p, i, why);
+      *unsupported = why;
+    }
+  };
+  const uint32_t max_src = m.in_row_bytes == 40 ? MZGPU_SRC_VAL2 : MZGPU_SRC_VAL1;
+  if (n_ops == 0 || n_ops > MZGPU_MFP_MAX_OPS) return bad(0, "op count (1..16)");
+  Ty ty[MZGPU_HAVING_MAX_STACK];
+  int sp = 0;
+  for (uint32_t i = 0; i < n_ops; ++i) {
+    const mzgpu_having_op& o = ops[i];
+    const uint32_t code = o.code;
+    const bool col = code == MZGPU_HOP_COL || code == MZGPU_HOP_COL_MZTS || code == MZGPU_HOP_COL_TS ||
+                     code == MZGPU_HOP_COL_DATE || code == MZGPU_HOP_COL_F64;
+    if (col || code == MZGPU_HOP_INT) {
+      if (sp == MZGPU_HAVING_MAX_STACK) return bad(i, "stack overflow (depth 8)");
+      Ty t = INT64;
+      if (col) {
+        if (o.arg > max_src) return bad(i, "column word out of range");
+        if (o.bits == 0 || o.bits > 64 || (uint32_t)o.shift + o.bits > 64 || o.sign_extend > 1)
+          return bad(i, "column field is empty or out of range");
+        if (code == MZGPU_HOP_COL) t = (o.bits < 32 || (o.bits == 32 && o.sign_extend)) ? INT32 : INT64;
+        if (code == MZGPU_HOP_COL_MZTS) {
+          if (o.sign_extend) return bad(i, "an mz_timestamp column is unsigned");
+          t = MZTS;
+        }
+        if (code == MZGPU_HOP_COL_TS) t = TS;
+        if (code == MZGPU_HOP_COL_DATE) {
+          if (o.bits > 32 || (o.bits == 32 && !o.sign_extend)) return bad(i, "a date column is at most an i32");
+          t = DATE;
+        }
+        if (code == MZGPU_HOP_COL_F64) {
+          if (o.bits != 64) return bad(i, "a float64 column is a whole word");
+          outside(i, "float64 columns");
+        }
+      } else {
+        if (o.konst >= m.n_consts) return bad(i, "constant index out of range");
+        const mzgpu_having_const& k = m.consts[o.konst];
+        if (k.hi != ((int64_t)k.lo < 0 ? ~0ull : 0ull)) return bad(i, "INT constant outside i64");
+        t = (int64_t)k.lo >= INT32_MIN && (int64_t)k.lo <= INT32_MAX ? INT32 : INT64;
+      }
+      if (!temporal && (t == MZTS || t == TS || t == DATE)) outside(i, "mz_timestamp values in a non-temporal predicate");
+      ty[sp++] = t;
+      continue;
+    }
+    if (code >= MZGPU_HOP_INT_TO_MZTS && code <= MZGPU_HOP_DATE_TO_MZTS) {  // unary (COL_TS / COL_DATE above)
+      if (sp < 1) return bad(i, "stack underflow");
+      Ty& a = ty[sp - 1];
+      if (code == MZGPU_HOP_INT_TO_MZTS) {
+        if (a != INT32 && a != INT64) return bad(i, "cast to mz_timestamp of a non-integer");
+        a = MZTS;
+      } else if (code == MZGPU_HOP_TS_TO_MZTS) {
+        if (a != TS) return bad(i, "timestamp cast of a non-timestamp");
+        a = MZTS;
+      } else if (code == MZGPU_HOP_DATE_TO_MZTS) {
+        if (a != DATE) return bad(i, "date cast of a non-date");
+        a = MZTS;
+      } else {  // MZGPU_HOP_TS_ADD_IV
+        if (a != TS) return bad(i, "interval added to a non-timestamp");
+        if (o.konst >= m.n_consts) return bad(i, "constant index out of range");
+        const mzgpu_having_const& k = m.consts[o.konst];
+        const int32_t days = (int32_t)(uint32_t)k.hi, months = (int32_t)(uint32_t)(k.hi >> 32);
+        const __int128 us = (__int128)days * 86400000000ll + (__int128)(int64_t)k.lo;
+        if (months != 0) outside(i, "intervals with months");
+        else if (us < (__int128)INT64_MIN || us > (__int128)INT64_MAX) outside(i, "interval beyond i64 microseconds");
+        else iv_us[o.konst] = (i64)us;
+      }
+      if (!temporal) outside(i, "mz_timestamp values in a non-temporal predicate");
+      continue;
+    }
+    if (code == MZGPU_HOP_NOT) {
+      if (sp < 1) return bad(i, "stack underflow");
+      if (ty[sp - 1] != BOOL) return bad(i, "NOT of a non-BOOL");
+      continue;
+    }
+    if (code < MZGPU_HOP_ADD || code > MZGPU_HOP_OR) return bad(i, "unknown opcode");
+    if (sp < 2) return bad(i, "stack underflow");
+    const Ty a = ty[sp - 2], b = ty[sp - 1];
+    --sp;
+    const bool ia = a == INT32 || a == INT64, ib = b == INT32 || b == INT64;
+    if (code == MZGPU_HOP_AND || code == MZGPU_HOP_OR) {
+      if (a != BOOL || b != BOOL) return bad(i, "AND / OR of a non-BOOL");
+    } else if (code == MZGPU_HOP_CMP) {
+      if (o.arg > MZGPU_CMP_GE) return bad(i, "unknown compare op");
+      if ((a == BOOL) != (b == BOOL)) return bad(i, "BOOL compared with a value");
+      if (a == BOOL) outside(i, "BOOL comparisons");
+      else if (!ia || !ib) outside(i, "comparisons of mz_timestamp, timestamp or date values");
+      ty[sp - 1] = BOOL;
+    } else {
+      if (o.arg != 32 && o.arg != 64) return bad(i, "width is not 32 or 64");
+      if (!ia || !ib) return bad(i, "arithmetic on a non-integer");
+      if (o.arg == 32 && (a != INT32 || b != INT32)) return bad(i, "32-bit operation on an operand that is not int32");
+      ty[sp - 1] = o.arg == 32 ? INT32 : INT64;
+    }
+  }
+  if (sp != 1 || ty[0] != (temporal ? MZTS : BOOL))
+    return bad(n_ops, temporal ? "the program does not leave one mz_timestamp" : "the predicate does not leave one BOOL");
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t until, mzgpu_mfp_op** out) {
+  MZ_CHECK_CTX(ctx);
+  if (plan == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  const mzgpu_mfp& m = *plan;
+  if ((m.in_row_bytes != 32 && m.in_row_bytes != 40) || (m.out_row_bytes != 32 && m.out_row_bytes != 40)) {
+    MZ_SET_ERR(ctx, "mfp: rows are 32 or 40 bytes (in %u, out %u)", m.in_row_bytes, m.out_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  if (m.n_predicates > MZGPU_MFP_MAX_PREDICATES || m.n_temporal > MZGPU_MFP_MAX_TEMPORAL ||
+      m.n_consts > MZGPU_MFP_MAX_CONSTS) {
+    MZ_SET_ERR(ctx, "mfp: %u predicates (0..4), %u temporal predicates (0..4), %u constants (0..8)", m.n_predicates,
+               m.n_temporal, m.n_consts);
+    return MZGPU_E_INVALID;
+  }
+  const uint32_t max_src = m.in_row_bytes == 40 ? MZGPU_SRC_VAL2 : MZGPU_SRC_VAL1;
+  for (int k = 0; k < 3; ++k) {
+    if (m.n_fields[k] > MZGPU_MAX_FIELDS || (k == 2 && m.out_row_bytes == 32 && m.n_fields[2] != 0)) {
+      MZ_SET_ERR(ctx, "mfp: %u fields for output word %d", m.n_fields[k], k);
+      return MZGPU_E_INVALID;
+    }
+    for (uint32_t f = 0; f < m.n_fields[k]; ++f) {
+      MZ_TRY(validate_field(ctx, m.fields[k][f], true));
+      if (m.fields[k][f].src > max_src || (uint32_t)m.fields[k][f].shift + m.fields[k][f].bits > 64) {
+        MZ_SET_ERR(ctx, "mfp: output word %d, field %u reads past the input row", k, f);
+        return MZGPU_E_INVALID;
+      }
+    }
+  }
+  MfpDevPlan pl;
+  memset(&pl, 0, sizeof(pl));
+  pl.plan = m;
+  const char* unsupported = nullptr;
+  std::string unsupported_msg;
+  for (uint32_t p = 0; p < m.n_predicates; ++p) {
+    MZ_TRY(validate_mfp_program(ctx, m, m.ops[p], m.n_ops[p], false, p, pl.iv_us, &unsupported));
+    if (unsupported && unsupported_msg.empty()) unsupported_msg = ctx->last_error;
+  }
+  for (uint32_t p = 0; p < m.n_temporal; ++p) {
+    const uint32_t c = m.temporal_cmp[p];
+    if (c > MZGPU_CMP_GE) {
+      MZ_SET_ERR(ctx, "mfp: temporal predicate %u: unknown compare op %u", p, c);
+      return MZGPU_E_INVALID;
+    }
+    if (c == MZGPU_CMP_NE && unsupported == nullptr) {
+      MZ_SET_ERR(ctx, "mfp: temporal predicate %u: mz_now() <> expr is not a temporal filter", p);
+      unsupported = "<>";
+    }
+    MZ_TRY(validate_mfp_program(ctx, m, m.temporal_ops[p], m.n_temporal_ops[p], true, p, pl.iv_us, &unsupported));
+    if (unsupported && unsupported_msg.empty()) unsupported_msg = ctx->last_error;
+    // MfpPlan::create_from (src/expr/src/linear.rs:1772-1804)
+    if (c == MZGPU_CMP_EQ) {
+      pl.lower[pl.n_lower++] = p;
+      pl.upper[pl.n_upper++] = p | 8;
+    } else if (c == MZGPU_CMP_LT) {
+      pl.upper[pl.n_upper++] = p;
+    } else if (c == MZGPU_CMP_LE) {
+      pl.upper[pl.n_upper++] = p | 8;
+    } else if (c == MZGPU_CMP_GT) {
+      pl.lower[pl.n_lower++] = p | 8;
+    } else if (c == MZGPU_CMP_GE) {
+      pl.lower[pl.n_lower++] = p;
+    }
+  }
+  if (unsupported) {
+    ctx->last_error = unsupported_msg;
+    return MZGPU_E_UNSUPPORTED;
+  }
+  auto op = std::unique_ptr<mzgpu_mfp_op>(new mzgpu_mfp_op());
+  op->ctx = ctx;
+  op->pl = pl;
+  op->ow = (int)m.out_row_bytes;
+  op->until = until;
+  MZ_TRY(op->scratch.alloc(ctx, (2 * MZ_MFP_MAX_SLOTS + 2) * 8));
+  MZ_CUDA(ctx, cudaMemsetAsync(op->scratch.p, 0, (2 * MZ_MFP_MAX_SLOTS + 2) * 8, ctx->stream));
+  MZ_CUDA(ctx, cudaMallocHost((void**)&op->h_mirror, (size_t)MZ_MFP_MIRROR * MZ_MFP_HDR * 8));
+  for (int s = MZ_MFP_MIRROR - 1; s >= 0; --s) op->free_slots.push_back(s);
+  op->chain.emplace(0, MfpBucket{64, {}});  // BucketChain::new: one bucket over the whole domain
+  *out = op.release();
+  return MZGPU_OK;
+}
+
+extern "C" void mzgpu_mfp_free(mzgpu_mfp_op* op) { delete op; }
+
+extern "C" int32_t mzgpu_mfp_step(mzgpu_mfp_op* op, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                  mzgpu_buf* out, mzgpu_buf* errs) {
+  if (op == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = op->ctx;
+  MZ_CHECK_CTX(ctx);
+  const uint32_t irb = op->pl.plan.in_row_bytes;
+  ctx->stats.rows_in += n;
+  DevMem in;
+  const void* d = rows;
+  if (mem == MZGPU_MEM_HOST && n) {
+    MZ_TRY(in.alloc(ctx, n * irb));
+    MZ_TRY(copy_in(ctx, in.p, rows, n * irb, mem));
+    d = in.p;
+  }
+  return mfp_step_dev(op, (const u64*)d, dlen_imm(n), n, upper, out, errs);
+}
+
+extern "C" int32_t mzgpu_mfp_step_buf(mzgpu_mfp_op* op, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                      mzgpu_buf* errs) {
+  if (op == nullptr || rows == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(op->ctx);
+  if (rows->rb != op->pl.plan.in_row_bytes || rows == out || rows == errs) {
+    MZ_SET_ERR(op->ctx, "mfp_step_buf: input rows must be %u bytes wide and not an output buffer",
+               op->pl.plan.in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  return mfp_step_dev(op, (const u64*)rows->mem.p, buf_dlen(rows), rows->ub, upper, out, errs);
+}
+
+extern "C" int32_t mzgpu_mfp_frontier(mzgpu_mfp_op* op, uint64_t* out) {
+  if (op == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = op->ctx;
+  MZ_CHECK_CTX(ctx);
+  MZ_TRY(mfp_poll(op, true));
+  MZ_TRY(mfp_flush_pending(op));
+  MZ_TRY(mfp_poll(op, true));
+  *out = MZGPU_FRONTIER_EMPTY;
+  for (auto& kv : op->chain) {
+    if (kv.second.slices.empty()) continue;  // (after the poll, every slice left holds rows)
+    std::vector<MfpSlices> chunks;
+    MfpSlices c;
+    c.n = 0;
+    for (const MfpSlice& s : kv.second.slices) {
+      if (c.n == MZ_MFP_SLICES) {
+        chunks.push_back(c);
+        c.n = 0;
+      }
+      c.base[c.n] = s.seg->base();
+      c.idx[c.n++] = s.idx;
+    }
+    chunks.push_back(c);
+    MZ_TRY(mz_mfp_min_time(ctx, op->ow, chunks.data(), (u32)chunks.size(), mfp_slices_ub(kv.second.slices),
+                           op->dmin()));
+    MZ_TRY(copy_out(ctx, out, op->dmin(), 8, MZGPU_MEM_HOST));
+    return MZGPU_OK;
+  }
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_mfp_stats(mzgpu_mfp_op* op, uint64_t out[3]) {
+  if (op == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(op->ctx);
+  MZ_TRY(mfp_poll(op, true));
+  MZ_TRY(mfp_flush_pending(op));
+  MZ_TRY(mfp_poll(op, true));
+  u64 held = 0;
+  for (auto& kv : op->chain)
+    for (const MfpSlice& s : kv.second.slices) held += mfp_slice_ub(s);
+  out[0] = held;
+  out[1] = op->chain.size();
+  MZ_TRY(copy_out(op->ctx, &out[2], op->touched(), 8, MZGPU_MEM_HOST));
+  return MZGPU_OK;
 }

@@ -1,0 +1,455 @@
+// mfp.cu — temporal filters: the device MfpPlan (include/mzgpu.h, mzgpu_mfp_new) and the partition
+// kernels of the bucket chain that holds its future updates (host.cu: mzgpu_mfp_op).
+//
+// Every row store of the operator is a segment: MZ_MFP_HDR header words (off[0..nb], the row range of
+// each of its nb slices, written on the device) followed by the rows.  Row counts never come back to
+// the host to launch the next kernel: grids are sized by host bounds and kernels read the lengths.
+#include "common.cuh"
+
+namespace {
+
+constexpr int ET = 256;  // threads per block of every kernel here
+
+// ------------------------------------------------------------------ the interpreter
+// A stack value: v (an INT as i64, a BOOL as 0 / 1, an MZTS as u64 bits, a TS as i64 microseconds,
+// a DATE as i64 days), err (0 or an MZGPU_*_ERR_* code, ordered as the EvalError variants) and the
+// error payload.  No value is NULL (no nullable column is in the subset).  Types are host-checked
+// (host.cu: validate_mfp_program), so the device only follows the opcodes.
+struct MVal {
+  u64 v;
+  u32 err;
+  u64 pay;
+};
+
+__device__ __forceinline__ u32 mfp_arith(u32 code, int w, i64 a, i64 b, i64* r) {
+  i64 x;
+  bool ovf = false;
+  if (code == MZGPU_HOP_ADD) {
+    x = (i64)((u64)a + (u64)b);
+    ovf = ((a ^ x) & (b ^ x)) < 0;
+  } else if (code == MZGPU_HOP_SUB) {
+    x = (i64)((u64)a - (u64)b);
+    ovf = ((a ^ b) & (a ^ x)) < 0;
+  } else if (code == MZGPU_HOP_MUL) {
+    x = (i64)((u64)a * (u64)b);
+    ovf = __mul64hi((long long)a, (long long)b) != (x >> 63);
+  } else {
+    if (b == 0) return MZGPU_HAVING_ERR_DIVISION_BY_ZERO;
+    if (b == -1 && a == (w == 32 ? (i64)(-2147483647 - 1) : (i64)0x8000000000000000ull))
+      return w == 32 ? MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE : MZGPU_HAVING_ERR_INT64_OUT_OF_RANGE;
+    x = a / b;
+  }
+  if (w == 32 && x != (i64)(int)x) ovf = true;
+  if (ovf) return MZGPU_HAVING_ERR_NUMERIC_FIELD_OVERFLOW;
+  *r = x;
+  return 0;
+}
+
+// [LOW_DATE, HIGH_DATE + 1 day) in microseconds since 1970-01-01 (src/repr/src/adt/timestamp.rs:577-592)
+constexpr i64 TS_LOW_US = -210863692800000000ll;
+constexpr i64 TS_HIGH_US = 8210266876799999999ll;
+
+__device__ __forceinline__ u64 mfp_field(const u64* w, const mzgpu_having_op& o) {
+  u64 a = w[o.arg] >> o.shift;
+  if (o.bits < 64) {
+    a &= (1ull << o.bits) - 1;
+    if (o.sign_extend && ((a >> (o.bits - 1)) & 1)) a |= ~0ull << o.bits;
+  }
+  return a;
+}
+
+// Runs one program; returns the value left on the stack.
+__device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, const MfpDevPlan& pl, const u64* w) {
+  constexpr int D = MZGPU_HAVING_MAX_STACK;
+  u64 v[D], pay[D];
+  u32 err[D];
+  int sp = 0;
+  for (u32 i = 0; i < n_ops; ++i) {
+    const mzgpu_having_op o = ops[i];
+    const u32 code = o.code;
+    if (code == MZGPU_HOP_COL || code == MZGPU_HOP_COL_MZTS || code == MZGPU_HOP_COL_TS ||
+        code == MZGPU_HOP_COL_DATE || code == MZGPU_HOP_INT) {
+      v[sp] = code == MZGPU_HOP_INT ? pl.plan.consts[o.konst].lo : mfp_field(w, o);
+      err[sp] = 0;
+      pay[sp] = 0;
+      ++sp;
+      continue;
+    }
+    const int y = sp - 1;
+    if (code == MZGPU_HOP_NOT) {
+      if (err[y] == 0) v[y] ^= 1;
+      continue;
+    }
+    if (code >= MZGPU_HOP_INT_TO_MZTS) {  // the unary casts and TS + interval
+      if (err[y] != 0) continue;
+      const i64 a = (i64)v[y];
+      if (code == MZGPU_HOP_INT_TO_MZTS || code == MZGPU_HOP_TS_TO_MZTS || code == MZGPU_HOP_DATE_TO_MZTS) {
+        i64 r = a;
+        if (code == MZGPU_HOP_TS_TO_MZTS) r = a >= 0 ? a / 1000 : -((-(a + 1)) / 1000) - 1;  // toward -inf
+        if (code == MZGPU_HOP_DATE_TO_MZTS) r = a * 86400000ll;                             // i32 days: no overflow
+        if (r < 0) {
+          err[y] = MZGPU_MFP_ERR_MZ_TIMESTAMP_OUT_OF_RANGE;
+          pay[y] = (u64)a;
+        } else {
+          v[y] = (u64)r;
+        }
+      } else if (code == MZGPU_HOP_TS_ADD_IV) {  // the interval is folded to i64 microseconds on the host
+        const i64 b = pl.iv_us[o.konst];
+        const i64 r = (i64)((u64)a + (u64)b);
+        if ((((a ^ r) & (b ^ r)) < 0) || r < TS_LOW_US || r > TS_HIGH_US) {
+          err[y] = MZGPU_MFP_ERR_TIMESTAMP_OUT_OF_RANGE;
+          pay[y] = 0;
+        } else {
+          v[y] = (u64)r;
+        }
+      }
+      continue;
+    }
+    --sp;
+    const int x = sp - 1;
+    const u32 ex = err[x], ey = err[y];
+    if (code == MZGPU_HOP_AND || code == MZGPU_HOP_OR) {
+      // variadic And / Or: the dominant value wins over an error, else the larger error
+      const u64 dom = code == MZGPU_HOP_AND ? 0 : 1;
+      if ((ex == 0 && v[x] == dom) || (ey == 0 && v[y] == dom)) {
+        v[x] = dom;
+        err[x] = 0;
+      } else if (ey > ex) {
+        err[x] = ey;
+        pay[x] = pay[y];
+      }
+      continue;
+    }
+    if (ex != 0 || ey != 0) {  // the first operand's error, else the second's
+      if (ex == 0) {
+        err[x] = ey;
+        pay[x] = pay[y];
+      }
+      continue;
+    }
+    if (code == MZGPU_HOP_CMP) {
+      const i64 a = (i64)v[x], b = (i64)v[y];
+      bool r;
+      switch (o.arg) {
+        case MZGPU_CMP_EQ: r = a == b; break;
+        case MZGPU_CMP_NE: r = a != b; break;
+        case MZGPU_CMP_LT: r = a < b; break;
+        case MZGPU_CMP_LE: r = a <= b; break;
+        case MZGPU_CMP_GT: r = a > b; break;
+        default: r = a >= b; break;
+      }
+      v[x] = r ? 1 : 0;
+      continue;
+    }
+    i64 r = 0;
+    const u32 e = mfp_arith(code, o.arg, (i64)v[x], (i64)v[y], &r);
+    if (e != 0) {
+      err[x] = e;
+      pay[x] = 0;
+    } else {
+      v[x] = (u64)r;
+    }
+  }
+  MVal out;
+  out.v = v[0];
+  out.err = err[0];
+  out.pay = pay[0];
+  return out;
+}
+
+// inclusive warp scan of small counts; returns the exclusive prefix, *total = the warp's sum
+__device__ __forceinline__ u32 warp_excl(u32 c, u32* total) {
+  const int lane = threadIdx.x & 31;
+  u32 s = c;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const u32 t = __shfl_up_sync(0xffffffffu, s, d);
+    if (lane >= d) s += t;
+  }
+  *total = __shfl_sync(0xffffffffu, s, 31);
+  return s - c;
+}
+
+// one warp-aggregated reservation of `c` rows at *cursor
+__device__ __forceinline__ u64 warp_reserve(u32 c, unsigned long long* cursor) {
+  u32 total;
+  const u32 ex = warp_excl(c, &total);
+  u64 base = 0;
+  if ((threadIdx.x & 31) == 31 && total) base = atomicAdd(cursor, (unsigned long long)total);
+  base = __shfl_sync(0xffffffffu, base, 31);
+  return base + ex;
+}
+
+// k_mfp_eval<IW, OW>: every input row through MfpPlan::evaluate (include/mzgpu.h).  An output update at a
+// time < upper (any time, if upper is MZGPU_FRONTIER_EMPTY) goes to the `ready` segment, any other to
+// `held`; errors to `errs` (R32).  Each segment's count is header word 1, the error count *err_len.
+template <int IW, int OW>
+__global__ void __launch_bounds__(ET) k_mfp_eval(const u64* __restrict__ in, const DLen dn,
+                                                  const __grid_constant__ MfpDevPlan pl, u64 upper, u64 until,
+                                                  u64* __restrict__ ready, u64* __restrict__ held,
+                                                  u64* __restrict__ errs, u64* __restrict__ err_len) {
+  constexpr int INW = IW / 8, ONW = OW / 8;
+  const u64 n = dlen_get(dn);
+  const u64 stride = (u64)gridDim.x * ET;
+  for (u64 base = (u64)blockIdx.x * ET; base < n; base += stride) {  // warp-uniform trip count
+    const u64 i = base + threadIdx.x;
+    u64 w[3] = {0, 0, 0};
+    u64 time = 0, diff = 0;
+    // outputs: up to two updates (time, diff) and one error (code, payload)
+    u32 n_upd = 0, e_code = 0;
+    u64 t0 = 0, t1 = 0, e_pay = 0;
+    if (i < n) {
+      const u64* r = in + i * INW;
+      w[0] = r[0];
+      w[1] = r[1];
+      if (INW == 5) w[2] = r[2];
+      time = r[INW - 2];
+      diff = r[INW - 1];
+      bool keep = true;
+      for (u32 p = 0; p < pl.plan.n_predicates && keep; ++p) {
+        const MVal m = mfp_run(pl.plan.ops[p], pl.plan.n_ops[p], pl, w);
+        if (m.err) {
+          e_code = m.err;
+          keep = false;
+        } else if (m.v == 0) {
+          keep = false;
+        }
+      }
+      u64 lower = time;
+      for (u32 b = 0; b < pl.n_lower && keep; ++b) {
+        const int q = pl.lower[b] & 7;
+        MVal m = mfp_run(pl.plan.temporal_ops[q], pl.plan.n_temporal_ops[q], pl, w);
+        if (!m.err && (pl.lower[b] & 8)) {  // step_mz_timestamp
+          if (m.v == ~0ull) m.err = MZGPU_MFP_ERR_MZ_TIMESTAMP_STEP_OVERFLOW;
+          else m.v += 1;
+        }
+        if (m.err) {
+          e_code = m.err;
+          e_pay = m.pay;
+          keep = false;
+        } else if (m.v > lower) {
+          lower = m.v;
+        }
+      }
+      // valid(t) = t < until; until = MZGPU_FRONTIER_EMPTY (no until) makes every time valid
+      if (keep && until != MZGPU_FRONTIER_EMPTY && lower >= until) keep = false;  // dropped before any upper bound
+      bool has_up = false;
+      u64 up = 0;
+      for (u32 b = 0; b < pl.n_upper && keep; ++b) {
+        if (has_up && up == lower) break;  // cannot be produced: later bounds are not evaluated
+        const int q = pl.upper[b] & 7;
+        MVal m = mfp_run(pl.plan.temporal_ops[q], pl.plan.n_temporal_ops[q], pl, w);
+        if (!m.err && (pl.upper[b] & 8)) {
+          if (m.v == ~0ull) m.err = MZGPU_MFP_ERR_MZ_TIMESTAMP_STEP_OVERFLOW;
+          else m.v += 1;
+        }
+        if (m.err) {
+          e_code = m.err;
+          e_pay = m.pay;
+          keep = false;
+        } else {
+          up = has_up && up < m.v ? up : m.v;
+          has_up = true;
+          if (up < lower) up = lower;
+        }
+      }
+      if (keep) {
+        if (has_up && until != MZGPU_FRONTIER_EMPTY && up >= until) has_up = false;
+        if (!(has_up && up == lower)) {
+          t0 = lower;
+          t1 = up;
+          n_upd = has_up ? 2 : 1;
+        }
+      }
+    }
+    // route: ready (time < upper) or held
+    const bool r0 = n_upd >= 1 && (upper == MZGPU_FRONTIER_EMPTY || t0 < upper);
+    const bool r1 = n_upd >= 2 && (upper == MZGPU_FRONTIER_EMPTY || t1 < upper);
+    const u32 c_ready = (u32)r0 + (u32)r1, c_held = n_upd - c_ready;
+    const u64 p_ready = warp_reserve(c_ready, (unsigned long long*)(ready + 1));
+    const u64 p_held = warp_reserve(c_held, (unsigned long long*)(held + 1));
+    const u64 p_err = warp_reserve(e_code ? 1u : 0u, (unsigned long long*)err_len);
+    u64 o[3] = {0, 0, 0};
+#pragma unroll
+    for (int k = 0; k < ONW - 2; ++k) {
+      u64 acc = 0;
+      for (u32 f = 0; f < pl.plan.n_fields[k]; ++f) {
+        const mzgpu_field fd = pl.plan.fields[k][f];
+        u64 a = w[fd.src] >> fd.shift;
+        if (fd.bits < 64) a &= (1ull << fd.bits) - 1;
+        acc |= a << fd.dst_shift;
+      }
+      o[k] = acc;
+    }
+    u64 kr = p_ready, kh = p_held;
+    for (u32 u = 0; u < n_upd; ++u) {
+      const u64 t = u == 0 ? t0 : t1;
+      const bool rd = u == 0 ? r0 : r1;
+      u64* dst = (rd ? ready : held) + MZ_MFP_HDR + (rd ? kr++ : kh++) * ONW;
+#pragma unroll
+      for (int k = 0; k < ONW - 2; ++k) dst[k] = o[k];
+      dst[ONW - 2] = t;
+      dst[ONW - 1] = u == 0 ? diff : (u64)0 - diff;
+    }
+    if (e_code) {
+      u64* dst = errs + p_err * 4;
+      dst[0] = e_code;
+      dst[1] = e_pay;
+      dst[2] = time;
+      dst[3] = diff;
+    }
+  }
+}
+
+// the slot of time t among bounds b[0..nb): (# bounds <= t) - 1, at least 0
+__device__ __forceinline__ u32 mfp_slot(const MfpBounds& b, u64 t) {
+  u32 lo = 0, hi = b.nb;
+  while (lo < hi) {
+    const u32 mid = (lo + hi) >> 1;
+    if (b.v[mid] <= t) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo ? lo - 1 : 0;
+}
+
+// pass 1 of a partition: per-slot histogram of the source slices' rows
+template <int NW>
+__global__ void __launch_bounds__(ET) k_mfp_count(const MfpSlices s, const __grid_constant__ MfpBounds b,
+                                                   u64* __restrict__ hist, u64* __restrict__ touched) {
+  __shared__ u32 h[MZ_MFP_MAX_SLOTS];
+  __shared__ unsigned long long seen_blk;
+  for (u32 j = threadIdx.x; j < b.nb; j += ET) h[j] = 0;
+  if (threadIdx.x == 0) seen_blk = 0;
+  __syncthreads();
+  const u64 gtid = (u64)blockIdx.x * ET + threadIdx.x, stride = (u64)gridDim.x * ET;
+  u64 seen = 0;
+  for (u32 k = 0; k < s.n; ++k) {
+    const u64* seg = s.base[k];
+    const u64 lo = seg[s.idx[k]], hi = seg[s.idx[k] + 1];
+    const u64* rows = seg + MZ_MFP_HDR;
+    for (u64 i = lo + gtid; i < hi; i += stride) {
+      atomicAdd(&h[mfp_slot(b, rows[i * NW + NW - 2])], 1u);
+      ++seen;
+    }
+  }
+  __syncthreads();
+  if (seen) atomicAdd(&seen_blk, (unsigned long long)seen);
+  __syncthreads();
+  for (u32 j = threadIdx.x; j < b.nb; j += ET)
+    if (h[j]) atomicAdd((unsigned long long*)&hist[j], (unsigned long long)h[j]);
+  if (threadIdx.x == 0 && seen_blk) atomicAdd((unsigned long long*)touched, seen_blk);  // one global add per block
+}
+
+// pass 2: scatter every row to its slot of the destination segment (order within a slot is arbitrary:
+// every release is consolidated); block 0 writes the segment header and the total
+template <int NW>
+__global__ void __launch_bounds__(ET) k_mfp_scatter(const MfpSlices s, const __grid_constant__ MfpBounds b,
+                                                     const u64* __restrict__ hist, u64* __restrict__ cursor,
+                                                     u64* __restrict__ dst, u64* __restrict__ total,
+                                                     u64* __restrict__ touched) {
+  __shared__ u64 off[MZ_MFP_MAX_SLOTS + 1];
+  __shared__ unsigned long long moved_blk;
+  if (threadIdx.x == 0) {
+    moved_blk = 0;
+    u64 a = 0;
+    for (u32 j = 0; j < b.nb; ++j) {
+      off[j] = a;
+      a += hist[j];
+    }
+    off[b.nb] = a;
+    if (blockIdx.x == 0) {
+      for (u32 j = 0; j <= b.nb; ++j) dst[j] = off[j];
+      if (total) *total = a;
+    }
+  }
+  __syncthreads();
+  const u64 gtid = (u64)blockIdx.x * ET + threadIdx.x, stride = (u64)gridDim.x * ET;
+  u64 moved = 0;
+  u64* out = dst + MZ_MFP_HDR;
+  for (u32 k = 0; k < s.n; ++k) {
+    const u64* seg = s.base[k];
+    const u64 lo = seg[s.idx[k]], hi = seg[s.idx[k] + 1];
+    const u64* rows = seg + MZ_MFP_HDR;
+    for (u64 i = lo + gtid; i < hi; i += stride) {
+      const u64* r = rows + i * NW;
+      const u32 j = mfp_slot(b, r[NW - 2]);
+      // one cursor reservation per warp and slot (a split has 2 slots, a gather 1: per-row atomics on one
+      // address would serialise)
+      const unsigned act = __activemask();
+      const unsigned peers = __match_any_sync(act, j);
+      const int leader = __ffs(peers) - 1;
+      const unsigned lane = threadIdx.x & 31;
+      unsigned long long base = 0;
+      if ((int)lane == leader) base = atomicAdd((unsigned long long*)&cursor[j], (unsigned long long)__popc(peers));
+      base = __shfl_sync(peers, base, leader);
+      const u64 p = off[j] + base + __popc(peers & ((1u << lane) - 1));
+#pragma unroll
+      for (int q = 0; q < NW; ++q) out[p * NW + q] = r[q];
+      ++moved;
+    }
+  }
+  if (moved) atomicAdd(&moved_blk, (unsigned long long)moved);
+  __syncthreads();
+  if (threadIdx.x == 0 && moved_blk) atomicAdd((unsigned long long*)touched, moved_blk);
+}
+
+// the least time of the source slices' rows (atomicMin into *m, which starts at u64::MAX)
+template <int NW>
+__global__ void __launch_bounds__(ET) k_mfp_min_time(const MfpSlices s, u64* __restrict__ m) {
+  const u64 gtid = (u64)blockIdx.x * ET + threadIdx.x, stride = (u64)gridDim.x * ET;
+  u64 best = ~0ull;
+  for (u32 k = 0; k < s.n; ++k) {
+    const u64* seg = s.base[k];
+    const u64 lo = seg[s.idx[k]], hi = seg[s.idx[k] + 1];
+    const u64* rows = seg + MZ_MFP_HDR;
+    for (u64 i = lo + gtid; i < hi; i += stride) best = min(best, rows[i * NW + NW - 2]);
+  }
+  if (best != ~0ull) atomicMin((unsigned long long*)m, (unsigned long long)best);
+}
+
+static unsigned mfp_grid(mzgpu_ctx* ctx, u64 n_ub) {
+  u64 g = (n_ub + ET - 1) / ET;
+  const u64 maxg = (u64)ctx->num_sms * 8;
+  if (g > maxg) g = maxg;
+  return g == 0 ? 1u : (unsigned)g;
+}
+
+}  // namespace
+
+int32_t mz_mfp_eval(mzgpu_ctx* ctx, const MfpDevPlan& pl, const u64* d_rows, DLen n, u64 n_ub, u64 upper, u64 until,
+                    u64* ready, u64* held, u64* errs, u64* err_len) {
+  const int iw = (int)pl.plan.in_row_bytes, ow = (int)pl.plan.out_row_bytes;
+  const unsigned grid = mfp_grid(ctx, n_ub);
+  MZ_BYTES(ctx, n.p == nullptr ? n.imm * (u64)(iw + 2 * ow) : 0);
+  if (iw == 32 && ow == 32) MZ_LAUNCH(ctx, (k_mfp_eval<32, 32>), grid, ET, 0, d_rows, n, pl, upper, until, ready, held, errs, err_len);
+  else if (iw == 32) MZ_LAUNCH(ctx, (k_mfp_eval<32, 40>), grid, ET, 0, d_rows, n, pl, upper, until, ready, held, errs, err_len);
+  else if (ow == 32) MZ_LAUNCH(ctx, (k_mfp_eval<40, 32>), grid, ET, 0, d_rows, n, pl, upper, until, ready, held, errs, err_len);
+  else MZ_LAUNCH(ctx, (k_mfp_eval<40, 40>), grid, ET, 0, d_rows, n, pl, upper, until, ready, held, errs, err_len);
+  return MZGPU_OK;
+}
+
+int32_t mz_mfp_partition(mzgpu_ctx* ctx, int rb, const MfpSlices* chunks, u32 n_chunks, u64 rows_ub,
+                         const MfpBounds& b, u64* hist, u64* cursor, u64* dst, u64* total, u64* touched) {
+  const unsigned grid = mfp_grid(ctx, rows_ub);
+  MZ_CUDA(ctx, cudaMemsetAsync(hist, 0, 2 * MZ_MFP_MAX_SLOTS * sizeof(u64), ctx->stream));  // hist + cursor
+  for (u32 c = 0; c < n_chunks; ++c) {
+    if (rb == 32) MZ_LAUNCH(ctx, k_mfp_count<4>, grid, ET, 0, chunks[c], b, hist, touched);
+    else MZ_LAUNCH(ctx, k_mfp_count<5>, grid, ET, 0, chunks[c], b, hist, touched);
+  }
+  for (u32 c = 0; c < n_chunks; ++c) {
+    MZ_BYTES(ctx, 0);
+    if (rb == 32) MZ_LAUNCH(ctx, k_mfp_scatter<4>, grid, ET, 0, chunks[c], b, hist, cursor, dst, total, touched);
+    else MZ_LAUNCH(ctx, k_mfp_scatter<5>, grid, ET, 0, chunks[c], b, hist, cursor, dst, total, touched);
+  }
+  return MZGPU_OK;
+}
+
+int32_t mz_mfp_min_time(mzgpu_ctx* ctx, int rb, const MfpSlices* chunks, u32 n_chunks, u64 rows_ub, u64* d_min) {
+  const unsigned grid = mfp_grid(ctx, rows_ub);
+  MZ_CUDA(ctx, cudaMemsetAsync(d_min, 0xff, sizeof(u64), ctx->stream));
+  for (u32 c = 0; c < n_chunks; ++c) {
+    if (rb == 32) MZ_LAUNCH(ctx, k_mfp_min_time<4>, grid, ET, 0, chunks[c], d_min);
+    else MZ_LAUNCH(ctx, k_mfp_min_time<5>, grid, ET, 0, chunks[c], d_min);
+  }
+  return MZGPU_OK;
+}

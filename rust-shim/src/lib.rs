@@ -12,6 +12,7 @@ pub mod correction;
 pub mod delta_join;
 pub mod exchange;
 pub mod linear_join;
+pub mod mfp;
 pub mod reduce;
 pub mod sys;
 pub mod trace;

@@ -91,6 +91,38 @@ pub struct Having {
 pub const COMM_ID_BYTES: usize = 128;
 pub const P2P_HANDLE_BYTES: usize = 64;
 
+/// A temporal filter operator (mzgpu_mfp_op), created from an `Mfp` plan.
+pub enum MfpOp {}
+pub const MFP_MAX_PREDICATES: usize = 4;
+pub const MFP_MAX_TEMPORAL: usize = 4;
+pub const MFP_MAX_OPS: usize = 16;
+pub const MFP_MAX_CONSTS: usize = 8;
+pub const HOP_COL_MZTS: u8 = 15;
+pub const HOP_INT_TO_MZTS: u8 = 16;
+pub const HOP_COL_TS: u8 = 17;
+pub const HOP_COL_DATE: u8 = 18;
+pub const HOP_TS_ADD_IV: u8 = 19;
+pub const HOP_TS_TO_MZTS: u8 = 20;
+pub const HOP_DATE_TO_MZTS: u8 = 21;
+pub const HOP_COL_F64: u8 = 22;
+/// A temporal filter's plan (mzgpu_mfp): projection fields, predicates and `mz_now() CMP expr` programs.
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct Mfp {
+    pub in_row_bytes: u32,
+    pub out_row_bytes: u32,
+    pub n_fields: [u32; 3],
+    pub fields: [[Field; 6]; 3],
+    pub n_predicates: u32,
+    pub n_temporal: u32,
+    pub n_consts: u32,
+    pub temporal_cmp: [u32; MFP_MAX_TEMPORAL],
+    pub n_ops: [u32; MFP_MAX_PREDICATES],
+    pub n_temporal_ops: [u32; MFP_MAX_TEMPORAL],
+    pub ops: [[HavingOp; MFP_MAX_OPS]; MFP_MAX_PREDICATES],
+    pub temporal_ops: [[HavingOp; MFP_MAX_OPS]; MFP_MAX_TEMPORAL],
+    pub consts: [HavingConst; MFP_MAX_CONSTS],
+}
+
 #[link(name = "mzgpu")]
 extern "C" {
     pub fn mzgpu_ctx_create(device: i32, worker_index: i32, peers: i32, out: *mut *mut Ctx) -> i32;
@@ -221,6 +253,12 @@ extern "C" {
     pub fn mzgpu_topk_basic(r: *mut Reduce, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_topk_basic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_topk_basic_negatives_trace(r: *mut Reduce) -> *mut Spine;
+    pub fn mzgpu_mfp_new(ctx: *mut Ctx, plan: *const Mfp, until: u64, out: *mut *mut MfpOp) -> i32;
+    pub fn mzgpu_mfp_free(op: *mut MfpOp);
+    pub fn mzgpu_mfp_step(op: *mut MfpOp, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_mfp_step_buf(op: *mut MfpOp, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_mfp_frontier(op: *mut MfpOp, out: *mut u64) -> i32;
+    pub fn mzgpu_mfp_stats(op: *mut MfpOp, out: *mut u64) -> i32;
     pub fn mzgpu_rowkey_pack(row_bytes: *const u8, len: u64, key_out: *mut u64) -> i32;
     pub fn mzgpu_rowkeys_pack(data: *const u8, offsets: *const u64, n: u64, keys_out: *mut u64, n_done: *mut u64) -> i32;
     pub fn mzgpu_rowkey_unpack(key: u64, row_bytes_out: *mut u8, len_out: *mut u64) -> i32;
