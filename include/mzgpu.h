@@ -983,9 +983,8 @@ mzgpu_spine* mzgpu_topk_basic_negatives_trace(mzgpu_reduce* r); /* borrowed, for
  * src/compute/src/extensions/temporal_bucket.rs, over BucketChain, src/timely-util/src/temporal.rs:59-211).
  *
  * Input: R32 or R40 rows with any diffs.  Output: R32 or R40 rows whose words (key, val1 and, for R40, val2)
- * are each an OR of up to MZGPU_MAX_FIELDS input bit-fields (mzgpu_field, src MZGPU_SRC_KEY / VAL1 / VAL2, where
- * VAL2 is the R40 input's second value word).  Map expressions are not projected: as with HAVING, the map part
- * stays with the caller, and an expression a predicate reads is written inline in it.
+ * are each an OR of up to MZGPU_MAX_FIELDS bit-fields (mzgpu_field, src MZGPU_SRC_KEY / VAL1 / VAL2, where
+ * VAL2 is the R40 input's second value word, or MZGPU_SRC_MAP(i), map expression i of mzgpu_mfp_new_map).
  *
  * Non-temporal predicates (0..MZGPU_MFP_MAX_PREDICATES) are programs of the HAVING interpreter
  * (mzgpu_having_op; same types, width rules, errors and three-valued AND / OR / NOT) evaluated in order as
@@ -1094,6 +1093,70 @@ typedef struct mzgpu_mfp {
 } mzgpu_mfp;
 typedef struct mzgpu_mfp_op mzgpu_mfp_op;
 int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t until, mzgpu_mfp_op** out);
+
+/* ---- map expressions of the device MfpPlan: the `expressions` of a MapFilterProject, computed per row, read by
+ * the predicates and the temporal bounds and projected into the output (SafeMfpPlan::evaluate_inner,
+ * src/expr/src/linear.rs:1680-1700).
+ *
+ * mzgpu_mfp_new_map(ctx, plan, map, until, out) is mzgpu_mfp_new with map->n_exprs expressions appended to the
+ * input columns; map == NULL or n_exprs == 0 is exactly mzgpu_mfp_new (which is that call).  Each expression is a
+ * postfix program of the same interpreter that leaves one value of any type (INT, BOOL, MZTS, TS or DATE); its
+ * constants index map->consts, not plan->consts.  The opcodes beyond those of the predicates:
+ *   MZGPU_HOP_MAP arg         push the value of expression `arg`, with its type.  Inside expression i only
+ *                             arg < i; predicates and temporal programs may read any expression
+ *   MZGPU_HOP_NEG / ABS       INT -> INT at width arg (neg_int32/64, abs_int32/64): the width's minimum is
+ *                             Int32OutOfRange / Int64OutOfRange with the operand as payload
+ *   MZGPU_HOP_MOD             INT, INT -> INT at width arg (mod_int32/64): a zero divisor is DivisionByZero,
+ *                             MIN % -1 is 0
+ *   MZGPU_HOP_INT64_TO_INT32  INT -> int32 (cast_int64_to_int32): out of range is Int32OutOfRange with the
+ *                             operand as payload
+ *   MZGPU_HOP_IF              BOOL, T, T -> T (MirScalarExpr::If; both branches of one type, or both INT): an
+ *                             error in the condition is the result, otherwise the taken branch's value or error;
+ *                             an error in the branch not taken never surfaces
+ * A MZGPU_HOP_MAP value never carries an error: an expression's error stops the row before anything reads it.
+ * AND / OR do not take an operand that may carry an error whose payload varies with the data (from
+ * MZGPU_HOP_INT64_TO_INT32 or an mz_timestamp cast): the reference orders two such errors by their message
+ * strings.  Such a program is MZGPU_E_UNSUPPORTED.  When AND / OR meet two errors of one code, the payload-0 one
+ * (a division's "a / b" message) wins over NEG / ABS's operand, as the longer string does.
+ *
+ * Per input row, in the order of SafeMfpPlan::evaluate_inner and MfpPlan::evaluate:
+ *   1. the support of predicate p is 1 + the highest MZGPU_HOP_MAP index it reads (0 if none);
+ *   2. before p runs, the expressions not yet evaluated below its support are evaluated in index order; an
+ *      expression error stops the row and becomes an error update at the row's (time, diff); a predicate that is
+ *      not TRUE drops the row;
+ *   3. once every predicate has passed, every remaining expression is evaluated, projected or not: its errors
+ *      count;
+ *   4. the temporal bounds are evaluated as for mzgpu_mfp_new, and may read expressions (MZTS-typed ones);
+ *   5. the output row is the projection over the input words and the expression values: a field with src
+ *      MZGPU_SRC_MAP(i) takes bits [shift, shift + bits) of expression i's value (an INT as two's-complement
+ *      i64, a BOOL as 0 / 1, an MZTS, TS or DATE as its u64 bits).
+ * Errors are the R32 error rows of mzgpu_mfp_new with its codes.
+ *
+ * Refused on the host before any launch, leaving no operator and the context usable: MZGPU_E_INVALID for a
+ * forward MZGPU_HOP_MAP reference, type errors, a wrong stack depth, more than MZGPU_MFP_MAX_MAPS expressions,
+ * MZGPU_MFP_MAX_OPS ops or MZGPU_MFP_MAX_CONSTS constants, and a projected expression index >= n_exprs;
+ * MZGPU_E_UNSUPPORTED for everything mzgpu_mfp_new refuses as unsupported (MZTS / TS / DATE values in a
+ * non-temporal predicate, which includes an expression of those types read by one) and the AND / OR rule above.
+ * Not supported: float64 columns and arithmetic, numeric, NULLs, variable-width values.  Step, frontier, stats
+ * and free are those of mzgpu_mfp_new. */
+#define MZGPU_MFP_MAX_MAPS 8
+#define MZGPU_SRC_MAP0 16 /* mzgpu_field.src of expression 0 (above every MZGPU_SRC_*) */
+#define MZGPU_SRC_MAP(i) (MZGPU_SRC_MAP0 + (i))
+#define MZGPU_HOP_MAP 23
+#define MZGPU_HOP_NEG 24
+#define MZGPU_HOP_ABS 25
+#define MZGPU_HOP_MOD 26
+#define MZGPU_HOP_INT64_TO_INT32 27
+#define MZGPU_HOP_IF 28
+typedef struct mzgpu_mfp_map {
+  uint32_t n_exprs; /* 0..MZGPU_MFP_MAX_MAPS */
+  uint32_t n_consts;
+  uint32_t n_ops[MZGPU_MFP_MAX_MAPS];
+  mzgpu_having_op ops[MZGPU_MFP_MAX_MAPS][MZGPU_MFP_MAX_OPS];
+  mzgpu_having_const consts[MZGPU_MFP_MAX_CONSTS];
+} mzgpu_mfp_map;
+int32_t mzgpu_mfp_new_map(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map, uint64_t until,
+                          mzgpu_mfp_op** out);
 void mzgpu_mfp_free(mzgpu_mfp_op* op);
 int32_t mzgpu_mfp_step(mzgpu_mfp_op* op, const void* rows, uint64_t n, int32_t mem, uint64_t upper, mzgpu_buf* out,
                        mzgpu_buf* errs);

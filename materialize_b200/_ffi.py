@@ -200,6 +200,21 @@ class Mfp(C.Structure):
     ]
 
 
+# map expressions of the MfpPlan (mzgpu_mfp_map, include/mzgpu.h)
+MFP_MAX_MAPS, SRC_MAP0 = 8, 16
+HOP_MAP, HOP_NEG, HOP_ABS, HOP_MOD, HOP_INT64_TO_INT32, HOP_IF = 23, 24, 25, 26, 27, 28
+
+
+class MfpMap(C.Structure):
+    _fields_ = [
+        ("n_exprs", C.c_uint32),
+        ("n_consts", C.c_uint32),
+        ("n_ops", C.c_uint32 * MFP_MAX_MAPS),
+        ("ops", (HavingOp * MFP_MAX_OPS) * MFP_MAX_MAPS),
+        ("consts", HavingConst * MFP_MAX_CONSTS),
+    ]
+
+
 class Filter(C.Structure):
     _fields_ = [("field", Field), ("op", C.c_uint32), ("rhs", C.c_uint64)]
 
@@ -349,6 +364,7 @@ SIGNATURES = {
     "mzgpu_topk_basic_buf": (i32, [vp, vp, u64, vp, vp]),
     "mzgpu_topk_basic_negatives_trace": (vp, [vp]),
     "mzgpu_mfp_new": (i32, [vp, C.POINTER(Mfp), u64, PV]),
+    "mzgpu_mfp_new_map": (i32, [vp, C.POINTER(Mfp), C.POINTER(MfpMap), u64, PV]),
     "mzgpu_mfp_free": (None, [vp]),
     "mzgpu_mfp_step": (i32, [vp, vp, u64, i32, u64, vp, vp]),
     "mzgpu_mfp_step_buf": (i32, [vp, vp, u64, vp, vp]),

@@ -894,6 +894,16 @@ def col(src, shift=0, bits=64, signed=False, code=F.HOP_COL):
     return hop(code, src, shift, bits, 1 if signed else 0)
 
 
+def map_ref(i):
+    """Push the value of map expression `i` (HOP_MAP)."""
+    return hop(F.HOP_MAP, i)
+
+
+def field_map(i, shift=0, bits=64, dst_shift=0):
+    """An output field taking bits [shift, shift + bits) of map expression `i`, placed at `dst_shift`."""
+    return (F.SRC_MAP0 + i, shift, bits, dst_shift)
+
+
 def interval_const(micros=0, days=0, months=0):
     """An interval constant for HOP_TS_ADD_IV: (lo, hi) with lo = microseconds, hi = days | months << 32."""
     return (micros & (2**64 - 1), (days & 0xFFFFFFFF) | ((months & 0xFFFFFFFF) << 32))
@@ -904,10 +914,12 @@ class Mfp:
     output words (key, val1, val2) as lists of (src, shift, bits, dst_shift); `predicates` are op lists (hop());
     `temporal` is a list of (cmp, ops) for `mz_now() cmp expr`; `consts` are (lo, hi) pairs.  step() returns
     (updates, errors): the updates of time < upper, consolidated, and R32 error rows (code, payload, time, diff);
-    future updates are held until an upper passes them."""
+    future updates are held until an upper passes them.  `maps` are the map expressions (op lists over
+    `map_consts`, mzgpu_mfp_new_map): predicates and temporal programs read them with map_ref(), output fields with
+    field_map()."""
 
     def __init__(self, ctx, fields, predicates=(), temporal=(), consts=(), in_row_bytes=32, out_row_bytes=32,
-                 until=F.FRONTIER_EMPTY):
+                 until=F.FRONTIER_EMPTY, maps=(), map_consts=()):
         self.ctx, self.in_row_bytes, self.out_row_bytes = ctx, in_row_bytes, out_row_bytes
         m = F.Mfp()
         m.in_row_bytes, m.out_row_bytes = in_row_bytes, out_row_bytes
@@ -931,7 +943,18 @@ class Mfp:
         for k, (lo, hi) in enumerate(consts[:F.MFP_MAX_CONSTS]):
             m.consts[k].lo, m.consts[k].hi = lo & (2**64 - 1), hi & (2**64 - 1)
         h = C.c_void_p()
-        ctx.check(F.lib.mzgpu_mfp_new(ctx.h, C.byref(m), until, C.byref(h)))
+        if not maps:
+            ctx.check(F.lib.mzgpu_mfp_new(ctx.h, C.byref(m), until, C.byref(h)))
+            self.h = h
+            return
+        mp = F.MfpMap()
+        mp.n_exprs, mp.n_consts = len(maps), len(map_consts)
+        for e, ops in enumerate(maps[:F.MFP_MAX_MAPS]):
+            mp.n_ops[e] = len(ops)
+            put(mp.ops[e], ops)
+        for k, (lo, hi) in enumerate(map_consts[:F.MFP_MAX_CONSTS]):
+            mp.consts[k].lo, mp.consts[k].hi = lo & (2**64 - 1), hi & (2**64 - 1)
+        ctx.check(F.lib.mzgpu_mfp_new_map(ctx.h, C.byref(m), C.byref(mp), until, C.byref(h)))
         self.h = h
 
     def step(self, rows, upper):

@@ -1224,13 +1224,19 @@ int32_t mz_partition(mzgpu_ctx* ctx, int row_bytes, const void* d_rows, DLen n, 
 
 // mfp.cu: the temporal filter (mzgpu_mfp_new).  A plan as the kernels read it: the caller's descriptor plus
 // the derived bound lists (program index in bits 0-2, bit 3: wrapped in step_mz_timestamp), in the order of
-// MfpPlan::create_from.
+// MfpPlan::create_from; and the map expressions (mzgpu_mfp_new_map) with each predicate's support.
 struct MfpDevPlan {
   mzgpu_mfp plan;
   u32 n_lower, n_upper;
   u32 lower[MZGPU_MFP_MAX_TEMPORAL], upper[MZGPU_MFP_MAX_TEMPORAL];
   i64 iv_us[MZGPU_MFP_MAX_CONSTS];  // interval constants folded to microseconds (MZGPU_HOP_TS_ADD_IV)
+  mzgpu_mfp_map map;                // n_exprs == 0 without expressions
+  i64 map_iv_us[MZGPU_MFP_MAX_CONSTS];
+  u32 support[MZGPU_MFP_MAX_PREDICATES];  // expressions evaluated before predicate p
 };
+// k_mfp_eval takes the plan as a __grid_constant__ parameter beside 80 bytes of others: within the 4 KB of
+// kernel parameters every CUDA 12 driver accepts
+static_assert(sizeof(MfpDevPlan) + 80 <= 4096, "MfpDevPlan exceeds the kernel parameter limit");
 // a segment: MZ_MFP_HDR header words (slice j's rows are [hdr[j], hdr[j + 1])), then the rows
 #define MZ_MFP_HDR 72
 #define MZ_MFP_MAX_SLOTS 65  // 64 bucket bounds and the overflow slot of an insert round

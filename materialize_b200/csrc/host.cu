@@ -4968,121 +4968,188 @@ static int32_t mfp_step_dev(mzgpu_mfp_op* op, const u64* d_rows, DLen n, u64 n_u
   return MZGPU_OK;
 }
 
-// The checks of one program (include/mzgpu.h): a type per stack slot, simulated op by op.  MZGPU_E_INVALID is
-// returned at once; a well-formed construct outside the subset is noted in *unsupported (the first one).
-static int32_t validate_mfp_program(mzgpu_ctx* ctx, const mzgpu_mfp& m, const mzgpu_having_op* ops, uint32_t n_ops,
-                                    bool temporal, uint32_t p, i64* iv_us, const char** unsupported) {
-  enum Ty { INT32, INT64, BOOL, MZTS, TS, DATE };
-  const char* what = temporal ? "temporal predicate" : "predicate";
+// The checks of one program (include/mzgpu.h): a type per stack slot, simulated op by op, and whether the slot may
+// carry an error whose payload varies with the data (kept out of AND / OR).  MZGPU_E_INVALID is returned at once; a
+// well-formed construct outside the subset is noted in *unsupported (the first one).
+enum MfpTy { MFP_INT32, MFP_INT64, MFP_BOOL, MFP_MZTS, MFP_TS, MFP_DATE };
+enum MfpKind { MFP_PREDICATE, MFP_TEMPORAL, MFP_MAP };
+struct MfpProgram {
+  MfpKind kind;
+  uint32_t index;  // predicate / temporal predicate / expression number
+  const mzgpu_having_op* ops;
+  uint32_t n_ops;
+  const mzgpu_having_const* consts;  // the program's constant pool
+  uint32_t n_consts;
+  i64* iv_us;                // its folded intervals
+  const MfpTy* map_ty;       // the types of the expressions it may read: [0, n_readable)
+  uint32_t n_readable;
+};
+static int32_t validate_mfp_program(mzgpu_ctx* ctx, uint32_t in_row_bytes, const MfpProgram& g, MfpTy* result,
+                                    uint32_t* support, const char** unsupported) {
+  const char* what = g.kind == MFP_TEMPORAL ? "temporal predicate" : g.kind == MFP_MAP ? "expression" : "predicate";
+  const bool predicate = g.kind == MFP_PREDICATE;
   auto bad = [&](uint32_t i, const char* why) {
-    MZ_SET_ERR(ctx, "mfp: %s %u, op %u: %s", what, p, i, why);
+    MZ_SET_ERR(ctx, "mfp: %s %u, op %u: %s", what, g.index, i, why);
     return MZGPU_E_INVALID;
   };
   auto outside = [&](uint32_t i, const char* why) {
     if (*unsupported == nullptr) {
-      MZ_SET_ERR(ctx, "mfp: %s %u, op %u: %s", what, p, i, why);
+      MZ_SET_ERR(ctx, "mfp: %s %u, op %u: %s", what, g.index, i, why);
       *unsupported = why;
     }
   };
-  const uint32_t max_src = m.in_row_bytes == 40 ? MZGPU_SRC_VAL2 : MZGPU_SRC_VAL1;
-  if (n_ops == 0 || n_ops > MZGPU_MFP_MAX_OPS) return bad(0, "op count (1..16)");
-  Ty ty[MZGPU_HAVING_MAX_STACK];
+  const uint32_t max_src = in_row_bytes == 40 ? MZGPU_SRC_VAL2 : MZGPU_SRC_VAL1;
+  if (g.n_ops == 0 || g.n_ops > MZGPU_MFP_MAX_OPS) return bad(0, "op count (1..16)");
+  MfpTy ty[MZGPU_HAVING_MAX_STACK];
+  bool varying[MZGPU_HAVING_MAX_STACK];
   int sp = 0;
-  for (uint32_t i = 0; i < n_ops; ++i) {
-    const mzgpu_having_op& o = ops[i];
+  *support = 0;
+  for (uint32_t i = 0; i < g.n_ops; ++i) {
+    const mzgpu_having_op& o = g.ops[i];
     const uint32_t code = o.code;
     const bool col = code == MZGPU_HOP_COL || code == MZGPU_HOP_COL_MZTS || code == MZGPU_HOP_COL_TS ||
                      code == MZGPU_HOP_COL_DATE || code == MZGPU_HOP_COL_F64;
-    if (col || code == MZGPU_HOP_INT) {
+    if (col || code == MZGPU_HOP_INT || code == MZGPU_HOP_MAP) {
       if (sp == MZGPU_HAVING_MAX_STACK) return bad(i, "stack overflow (depth 8)");
-      Ty t = INT64;
+      MfpTy t = MFP_INT64;
       if (col) {
         if (o.arg > max_src) return bad(i, "column word out of range");
         if (o.bits == 0 || o.bits > 64 || (uint32_t)o.shift + o.bits > 64 || o.sign_extend > 1)
           return bad(i, "column field is empty or out of range");
-        if (code == MZGPU_HOP_COL) t = (o.bits < 32 || (o.bits == 32 && o.sign_extend)) ? INT32 : INT64;
+        if (code == MZGPU_HOP_COL) t = (o.bits < 32 || (o.bits == 32 && o.sign_extend)) ? MFP_INT32 : MFP_INT64;
         if (code == MZGPU_HOP_COL_MZTS) {
           if (o.sign_extend) return bad(i, "an mz_timestamp column is unsigned");
-          t = MZTS;
+          t = MFP_MZTS;
         }
-        if (code == MZGPU_HOP_COL_TS) t = TS;
+        if (code == MZGPU_HOP_COL_TS) t = MFP_TS;
         if (code == MZGPU_HOP_COL_DATE) {
           if (o.bits > 32 || (o.bits == 32 && !o.sign_extend)) return bad(i, "a date column is at most an i32");
-          t = DATE;
+          t = MFP_DATE;
         }
         if (code == MZGPU_HOP_COL_F64) {
           if (o.bits != 64) return bad(i, "a float64 column is a whole word");
           outside(i, "float64 columns");
         }
+      } else if (code == MZGPU_HOP_MAP) {
+        if (o.arg >= g.n_readable)
+          return bad(i, g.kind == MFP_MAP ? "reads an expression at or after its own" : "expression index out of range");
+        t = g.map_ty[o.arg];
+        if (o.arg + 1u > *support) *support = o.arg + 1u;
       } else {
-        if (o.konst >= m.n_consts) return bad(i, "constant index out of range");
-        const mzgpu_having_const& k = m.consts[o.konst];
+        if (o.konst >= g.n_consts) return bad(i, "constant index out of range");
+        const mzgpu_having_const& k = g.consts[o.konst];
         if (k.hi != ((int64_t)k.lo < 0 ? ~0ull : 0ull)) return bad(i, "INT constant outside i64");
-        t = (int64_t)k.lo >= INT32_MIN && (int64_t)k.lo <= INT32_MAX ? INT32 : INT64;
+        t = (int64_t)k.lo >= INT32_MIN && (int64_t)k.lo <= INT32_MAX ? MFP_INT32 : MFP_INT64;
       }
-      if (!temporal && (t == MZTS || t == TS || t == DATE)) outside(i, "mz_timestamp values in a non-temporal predicate");
+      if (predicate && (t == MFP_MZTS || t == MFP_TS || t == MFP_DATE))
+        outside(i, "mz_timestamp values in a non-temporal predicate");
+      varying[sp] = false;  // an expression read here has been evaluated without error
       ty[sp++] = t;
       continue;
     }
-    if (code >= MZGPU_HOP_INT_TO_MZTS && code <= MZGPU_HOP_DATE_TO_MZTS) {  // unary (COL_TS / COL_DATE above)
+    const bool unary_int = code == MZGPU_HOP_NEG || code == MZGPU_HOP_ABS || code == MZGPU_HOP_INT64_TO_INT32;
+    if ((code >= MZGPU_HOP_INT_TO_MZTS && code <= MZGPU_HOP_DATE_TO_MZTS) || unary_int) {  // (COL_TS / COL_DATE above)
       if (sp < 1) return bad(i, "stack underflow");
-      Ty& a = ty[sp - 1];
+      MfpTy& a = ty[sp - 1];
+      const bool ia = a == MFP_INT32 || a == MFP_INT64;
+      if (unary_int) {
+        if (!ia) return bad(i, "integer function of a non-integer");
+        if (code == MZGPU_HOP_INT64_TO_INT32) {
+          a = MFP_INT32;
+          varying[sp - 1] = true;  // Int32OutOfRange carries the operand
+        } else {
+          if (o.arg != 32 && o.arg != 64) return bad(i, "width is not 32 or 64");
+          if (o.arg == 32 && a != MFP_INT32) return bad(i, "32-bit operation on an operand that is not int32");
+          a = o.arg == 32 ? MFP_INT32 : MFP_INT64;
+        }
+        continue;
+      }
       if (code == MZGPU_HOP_INT_TO_MZTS) {
-        if (a != INT32 && a != INT64) return bad(i, "cast to mz_timestamp of a non-integer");
-        a = MZTS;
+        if (!ia) return bad(i, "cast to mz_timestamp of a non-integer");
+        a = MFP_MZTS;
+        varying[sp - 1] = true;
       } else if (code == MZGPU_HOP_TS_TO_MZTS) {
-        if (a != TS) return bad(i, "timestamp cast of a non-timestamp");
-        a = MZTS;
+        if (a != MFP_TS) return bad(i, "timestamp cast of a non-timestamp");
+        a = MFP_MZTS;
+        varying[sp - 1] = true;
       } else if (code == MZGPU_HOP_DATE_TO_MZTS) {
-        if (a != DATE) return bad(i, "date cast of a non-date");
-        a = MZTS;
+        if (a != MFP_DATE) return bad(i, "date cast of a non-date");
+        a = MFP_MZTS;
+        varying[sp - 1] = true;
       } else {  // MZGPU_HOP_TS_ADD_IV
-        if (a != TS) return bad(i, "interval added to a non-timestamp");
-        if (o.konst >= m.n_consts) return bad(i, "constant index out of range");
-        const mzgpu_having_const& k = m.consts[o.konst];
+        if (a != MFP_TS) return bad(i, "interval added to a non-timestamp");
+        if (o.konst >= g.n_consts) return bad(i, "constant index out of range");
+        const mzgpu_having_const& k = g.consts[o.konst];
         const int32_t days = (int32_t)(uint32_t)k.hi, months = (int32_t)(uint32_t)(k.hi >> 32);
         const __int128 us = (__int128)days * 86400000000ll + (__int128)(int64_t)k.lo;
         if (months != 0) outside(i, "intervals with months");
         else if (us < (__int128)INT64_MIN || us > (__int128)INT64_MAX) outside(i, "interval beyond i64 microseconds");
-        else iv_us[o.konst] = (i64)us;
+        else g.iv_us[o.konst] = (i64)us;
       }
-      if (!temporal) outside(i, "mz_timestamp values in a non-temporal predicate");
+      if (predicate) outside(i, "mz_timestamp values in a non-temporal predicate");
       continue;
     }
     if (code == MZGPU_HOP_NOT) {
       if (sp < 1) return bad(i, "stack underflow");
-      if (ty[sp - 1] != BOOL) return bad(i, "NOT of a non-BOOL");
+      if (ty[sp - 1] != MFP_BOOL) return bad(i, "NOT of a non-BOOL");
       continue;
     }
-    if (code < MZGPU_HOP_ADD || code > MZGPU_HOP_OR) return bad(i, "unknown opcode");
+    if (code == MZGPU_HOP_IF) {
+      if (sp < 3) return bad(i, "stack underflow");
+      const MfpTy c = ty[sp - 3], t = ty[sp - 2], e = ty[sp - 1];
+      const bool it = t == MFP_INT32 || t == MFP_INT64, ie = e == MFP_INT32 || e == MFP_INT64;
+      if (c != MFP_BOOL) return bad(i, "IF on a non-BOOL condition");
+      if (t != e && !(it && ie)) return bad(i, "IF branches of different types");
+      ty[sp - 3] = t == e ? t : MFP_INT64;
+      varying[sp - 3] = varying[sp - 3] || varying[sp - 2] || varying[sp - 1];
+      sp -= 2;
+      continue;
+    }
+    const bool arith = (code >= MZGPU_HOP_ADD && code <= MZGPU_HOP_DIV) || code == MZGPU_HOP_MOD;
+    if (!arith && code != MZGPU_HOP_CMP && code != MZGPU_HOP_AND && code != MZGPU_HOP_OR) return bad(i, "unknown opcode");
     if (sp < 2) return bad(i, "stack underflow");
-    const Ty a = ty[sp - 2], b = ty[sp - 1];
+    const MfpTy a = ty[sp - 2], b = ty[sp - 1];
+    const bool va = varying[sp - 2], vb = varying[sp - 1];
     --sp;
-    const bool ia = a == INT32 || a == INT64, ib = b == INT32 || b == INT64;
+    const bool ia = a == MFP_INT32 || a == MFP_INT64, ib = b == MFP_INT32 || b == MFP_INT64;
+    varying[sp - 1] = va || vb;
     if (code == MZGPU_HOP_AND || code == MZGPU_HOP_OR) {
-      if (a != BOOL || b != BOOL) return bad(i, "AND / OR of a non-BOOL");
+      if (a != MFP_BOOL || b != MFP_BOOL) return bad(i, "AND / OR of a non-BOOL");
+      if (va || vb) outside(i, "AND / OR over an error whose payload varies with the data");
     } else if (code == MZGPU_HOP_CMP) {
       if (o.arg > MZGPU_CMP_GE) return bad(i, "unknown compare op");
-      if ((a == BOOL) != (b == BOOL)) return bad(i, "BOOL compared with a value");
-      if (a == BOOL) outside(i, "BOOL comparisons");
+      if ((a == MFP_BOOL) != (b == MFP_BOOL)) return bad(i, "BOOL compared with a value");
+      if (a == MFP_BOOL) outside(i, "BOOL comparisons");
       else if (!ia || !ib) outside(i, "comparisons of mz_timestamp, timestamp or date values");
-      ty[sp - 1] = BOOL;
+      ty[sp - 1] = MFP_BOOL;
     } else {
       if (o.arg != 32 && o.arg != 64) return bad(i, "width is not 32 or 64");
       if (!ia || !ib) return bad(i, "arithmetic on a non-integer");
-      if (o.arg == 32 && (a != INT32 || b != INT32)) return bad(i, "32-bit operation on an operand that is not int32");
-      ty[sp - 1] = o.arg == 32 ? INT32 : INT64;
+      if (o.arg == 32 && (a != MFP_INT32 || b != MFP_INT32))
+        return bad(i, "32-bit operation on an operand that is not int32");
+      ty[sp - 1] = o.arg == 32 ? MFP_INT32 : MFP_INT64;
     }
   }
-  if (sp != 1 || ty[0] != (temporal ? MZTS : BOOL))
-    return bad(n_ops, temporal ? "the program does not leave one mz_timestamp" : "the predicate does not leave one BOOL");
+  if (g.kind == MFP_MAP) {
+    if (sp != 1) return bad(g.n_ops, "the expression does not leave one value");
+  } else if (sp != 1 || ty[0] != (g.kind == MFP_TEMPORAL ? MFP_MZTS : MFP_BOOL)) {
+    return bad(g.n_ops, g.kind == MFP_TEMPORAL ? "the program does not leave one mz_timestamp"
+                                               : "the predicate does not leave one BOOL");
+  }
+  *result = ty[0];
   return MZGPU_OK;
 }
 
 extern "C" int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t until, mzgpu_mfp_op** out) {
+  return mzgpu_mfp_new_map(ctx, plan, nullptr, until, out);
+}
+
+extern "C" int32_t mzgpu_mfp_new_map(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map, uint64_t until,
+                                     mzgpu_mfp_op** out) {
   MZ_CHECK_CTX(ctx);
   if (plan == nullptr || out == nullptr) return MZGPU_E_INVALID;
   const mzgpu_mfp& m = *plan;
+  if (map != nullptr && map->n_exprs == 0) map = nullptr;  // exactly mzgpu_mfp_new
   if ((m.in_row_bytes != 32 && m.in_row_bytes != 40) || (m.out_row_bytes != 32 && m.out_row_bytes != 40)) {
     MZ_SET_ERR(ctx, "mfp: rows are 32 or 40 bytes (in %u, out %u)", m.in_row_bytes, m.out_row_bytes);
     return MZGPU_E_INVALID;
@@ -5093,6 +5160,11 @@ extern "C" int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t
                m.n_temporal, m.n_consts);
     return MZGPU_E_INVALID;
   }
+  if (map && (map->n_exprs > MZGPU_MFP_MAX_MAPS || map->n_consts > MZGPU_MFP_MAX_CONSTS)) {
+    MZ_SET_ERR(ctx, "mfp: %u expressions (0..8), %u expression constants (0..8)", map->n_exprs, map->n_consts);
+    return MZGPU_E_INVALID;
+  }
+  const uint32_t n_exprs = map ? map->n_exprs : 0;
   const uint32_t max_src = m.in_row_bytes == 40 ? MZGPU_SRC_VAL2 : MZGPU_SRC_VAL1;
   for (int k = 0; k < 3; ++k) {
     if (m.n_fields[k] > MZGPU_MAX_FIELDS || (k == 2 && m.out_row_bytes == 32 && m.n_fields[2] != 0)) {
@@ -5100,8 +5172,16 @@ extern "C" int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t
       return MZGPU_E_INVALID;
     }
     for (uint32_t f = 0; f < m.n_fields[k]; ++f) {
-      MZ_TRY(validate_field(ctx, m.fields[k][f], true));
-      if (m.fields[k][f].src > max_src || (uint32_t)m.fields[k][f].shift + m.fields[k][f].bits > 64) {
+      mzgpu_field fd = m.fields[k][f];
+      const bool is_map = fd.src >= MZGPU_SRC_MAP0;
+      if (is_map && fd.src - MZGPU_SRC_MAP0 >= n_exprs) {
+        MZ_SET_ERR(ctx, "mfp: output word %d, field %u reads expression %u of %u", k, f, fd.src - MZGPU_SRC_MAP0,
+                   n_exprs);
+        return MZGPU_E_INVALID;
+      }
+      if (is_map) fd.src = MZGPU_SRC_KEY;  // the bit-field checks of an input field
+      MZ_TRY(validate_field(ctx, fd, true));
+      if ((!is_map && fd.src > max_src) || (uint32_t)fd.shift + fd.bits > 64) {
         MZ_SET_ERR(ctx, "mfp: output word %d, field %u reads past the input row", k, f);
         return MZGPU_E_INVALID;
       }
@@ -5110,10 +5190,20 @@ extern "C" int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t
   MfpDevPlan pl;
   memset(&pl, 0, sizeof(pl));
   pl.plan = m;
+  if (map) pl.map = *map;
   const char* unsupported = nullptr;
   std::string unsupported_msg;
+  MfpTy map_ty[MZGPU_MFP_MAX_MAPS];
+  for (uint32_t e = 0; e < n_exprs; ++e) {
+    const MfpProgram g{MFP_MAP, e, map->ops[e], map->n_ops[e], map->consts, map->n_consts, pl.map_iv_us, map_ty, e};
+    uint32_t support;
+    MZ_TRY(validate_mfp_program(ctx, m.in_row_bytes, g, &map_ty[e], &support, &unsupported));
+    if (unsupported && unsupported_msg.empty()) unsupported_msg = ctx->last_error;
+  }
   for (uint32_t p = 0; p < m.n_predicates; ++p) {
-    MZ_TRY(validate_mfp_program(ctx, m, m.ops[p], m.n_ops[p], false, p, pl.iv_us, &unsupported));
+    const MfpProgram g{MFP_PREDICATE, p, m.ops[p], m.n_ops[p], m.consts, m.n_consts, pl.iv_us, map_ty, n_exprs};
+    MfpTy t;
+    MZ_TRY(validate_mfp_program(ctx, m.in_row_bytes, g, &t, &pl.support[p], &unsupported));
     if (unsupported && unsupported_msg.empty()) unsupported_msg = ctx->last_error;
   }
   for (uint32_t p = 0; p < m.n_temporal; ++p) {
@@ -5126,7 +5216,11 @@ extern "C" int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t
       MZ_SET_ERR(ctx, "mfp: temporal predicate %u: mz_now() <> expr is not a temporal filter", p);
       unsupported = "<>";
     }
-    MZ_TRY(validate_mfp_program(ctx, m, m.temporal_ops[p], m.n_temporal_ops[p], true, p, pl.iv_us, &unsupported));
+    const MfpProgram g{MFP_TEMPORAL, p, m.temporal_ops[p], m.n_temporal_ops[p], m.consts, m.n_consts, pl.iv_us,
+                       map_ty, n_exprs};
+    MfpTy t;
+    uint32_t support;
+    MZ_TRY(validate_mfp_program(ctx, m.in_row_bytes, g, &t, &support, &unsupported));
     if (unsupported && unsupported_msg.empty()) unsupported_msg = ctx->last_error;
     // MfpPlan::create_from (src/expr/src/linear.rs:1772-1804)
     if (c == MZGPU_CMP_EQ) {

@@ -22,6 +22,7 @@ struct MVal {
 };
 
 __device__ __forceinline__ u32 mfp_arith(u32 code, int w, i64 a, i64 b, i64* r) {
+  const i64 lo = w == 32 ? (i64)(-2147483647 - 1) : (i64)0x8000000000000000ull;
   i64 x;
   bool ovf = false;
   if (code == MZGPU_HOP_ADD) {
@@ -33,10 +34,12 @@ __device__ __forceinline__ u32 mfp_arith(u32 code, int w, i64 a, i64 b, i64* r) 
   } else if (code == MZGPU_HOP_MUL) {
     x = (i64)((u64)a * (u64)b);
     ovf = __mul64hi((long long)a, (long long)b) != (x >> 63);
+  } else if (code == MZGPU_HOP_MOD) {  // checked_rem(b).unwrap_or(0): MIN % -1 is 0
+    if (b == 0) return MZGPU_HAVING_ERR_DIVISION_BY_ZERO;
+    x = b == -1 ? 0 : a % b;
   } else {
     if (b == 0) return MZGPU_HAVING_ERR_DIVISION_BY_ZERO;
-    if (b == -1 && a == (w == 32 ? (i64)(-2147483647 - 1) : (i64)0x8000000000000000ull))
-      return w == 32 ? MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE : MZGPU_HAVING_ERR_INT64_OUT_OF_RANGE;
+    if (b == -1 && a == lo) return w == 32 ? MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE : MZGPU_HAVING_ERR_INT64_OUT_OF_RANGE;
     x = a / b;
   }
   if (w == 32 && x != (i64)(int)x) ovf = true;
@@ -58,8 +61,10 @@ __device__ __forceinline__ u64 mfp_field(const u64* w, const mzgpu_having_op& o)
   return a;
 }
 
-// Runs one program; returns the value left on the stack.
-__device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, const MfpDevPlan& pl, const u64* w) {
+// Runs one program over the input words w and the expression values mv (every one a MZGPU_HOP_MAP may read is
+// evaluated, without error); its constants are consts / iv_us.  Returns the value left on the stack.
+__device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, const mzgpu_having_const* consts,
+                                     const i64* iv_us, const u64* w, const u64* mv) {
   constexpr int D = MZGPU_HAVING_MAX_STACK;
   u64 v[D], pay[D];
   u32 err[D];
@@ -68,8 +73,8 @@ __device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, cons
     const mzgpu_having_op o = ops[i];
     const u32 code = o.code;
     if (code == MZGPU_HOP_COL || code == MZGPU_HOP_COL_MZTS || code == MZGPU_HOP_COL_TS ||
-        code == MZGPU_HOP_COL_DATE || code == MZGPU_HOP_INT) {
-      v[sp] = code == MZGPU_HOP_INT ? pl.plan.consts[o.konst].lo : mfp_field(w, o);
+        code == MZGPU_HOP_COL_DATE || code == MZGPU_HOP_INT || code == MZGPU_HOP_MAP) {
+      v[sp] = code == MZGPU_HOP_INT ? consts[o.konst].lo : code == MZGPU_HOP_MAP ? mv[o.arg] : mfp_field(w, o);
       err[sp] = 0;
       pay[sp] = 0;
       ++sp;
@@ -80,7 +85,8 @@ __device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, cons
       if (err[y] == 0) v[y] ^= 1;
       continue;
     }
-    if (code >= MZGPU_HOP_INT_TO_MZTS) {  // the unary casts and TS + interval
+    if ((code >= MZGPU_HOP_INT_TO_MZTS && code <= MZGPU_HOP_DATE_TO_MZTS) || code == MZGPU_HOP_NEG ||
+        code == MZGPU_HOP_ABS || code == MZGPU_HOP_INT64_TO_INT32) {  // the unary ops and TS + interval
       if (err[y] != 0) continue;
       const i64 a = (i64)v[y];
       if (code == MZGPU_HOP_INT_TO_MZTS || code == MZGPU_HOP_TS_TO_MZTS || code == MZGPU_HOP_DATE_TO_MZTS) {
@@ -94,7 +100,7 @@ __device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, cons
           v[y] = (u64)r;
         }
       } else if (code == MZGPU_HOP_TS_ADD_IV) {  // the interval is folded to i64 microseconds on the host
-        const i64 b = pl.iv_us[o.konst];
+        const i64 b = iv_us[o.konst];
         const i64 r = (i64)((u64)a + (u64)b);
         if ((((a ^ r) & (b ^ r)) < 0) || r < TS_LOW_US || r > TS_HIGH_US) {
           err[y] = MZGPU_MFP_ERR_TIMESTAMP_OUT_OF_RANGE;
@@ -102,6 +108,30 @@ __device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, cons
         } else {
           v[y] = (u64)r;
         }
+      } else if (code == MZGPU_HOP_INT64_TO_INT32) {
+        if (a != (i64)(int)a) {
+          err[y] = MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE;
+          pay[y] = (u64)a;
+        }
+      } else {  // NEG / ABS: checked_neg / checked_abs at width arg
+        const i64 lo = o.arg == 32 ? (i64)(-2147483647 - 1) : (i64)0x8000000000000000ull;
+        if (a == lo) {
+          err[y] = o.arg == 32 ? MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE : MZGPU_HAVING_ERR_INT64_OUT_OF_RANGE;
+          pay[y] = (u64)a;
+        } else if (code == MZGPU_HOP_NEG || a < 0) {
+          v[y] = (u64)0 - (u64)a;
+        }
+      }
+      continue;
+    }
+    if (code == MZGPU_HOP_IF) {  // c, t, e: the condition's error, else the taken branch's value or error
+      sp -= 2;
+      const int c = sp - 1, t = sp, e = sp + 1;
+      if (err[c] == 0) {
+        const int k = v[c] == 1 ? t : e;
+        v[c] = v[k];
+        err[c] = err[k];
+        pay[c] = pay[k];
       }
       continue;
     }
@@ -109,12 +139,13 @@ __device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, cons
     const int x = sp - 1;
     const u32 ex = err[x], ey = err[y];
     if (code == MZGPU_HOP_AND || code == MZGPU_HOP_OR) {
-      // variadic And / Or: the dominant value wins over an error, else the larger error
+      // variadic And / Or: the dominant value wins over an error, else the larger error (of one code, the
+      // payload-0 one: a division's "a / b" message orders after NEG / ABS's operand)
       const u64 dom = code == MZGPU_HOP_AND ? 0 : 1;
       if ((ex == 0 && v[x] == dom) || (ey == 0 && v[y] == dom)) {
         v[x] = dom;
         err[x] = 0;
-      } else if (ey > ex) {
+      } else if (ey > ex || (ey != 0 && ey == ex && pay[y] == 0)) {
         err[x] = ey;
         pay[x] = pay[y];
       }
@@ -180,7 +211,8 @@ __device__ __forceinline__ u64 warp_reserve(u32 c, unsigned long long* cursor) {
   return base + ex;
 }
 
-// k_mfp_eval<IW, OW>: every input row through MfpPlan::evaluate (include/mzgpu.h).  An output update at a
+// k_mfp_eval<IW, OW>: every input row through MfpPlan::evaluate (include/mzgpu.h), its map expressions evaluated
+// lazily in SafeMfpPlan::evaluate_inner's order (mzgpu_mfp_new_map).  An output update at a
 // time < upper (any time, if upper is MZGPU_FRONTIER_EMPTY) goes to the `ready` segment, any other to
 // `held`; errors to `errs` (R32).  Each segment's count is header word 1, the error count *err_len.
 template <int IW, int OW>
@@ -194,6 +226,8 @@ __global__ void __launch_bounds__(ET) k_mfp_eval(const u64* __restrict__ in, con
   for (u64 base = (u64)blockIdx.x * ET; base < n; base += stride) {  // warp-uniform trip count
     const u64 i = base + threadIdx.x;
     u64 w[3] = {0, 0, 0};
+    u64 mv[MZGPU_MFP_MAX_MAPS];  // expression values [0, ne)
+    u32 ne = 0;
     u64 time = 0, diff = 0;
     // outputs: up to two updates (time, diff) and one error (code, payload)
     u32 n_upd = 0, e_code = 0;
@@ -206,19 +240,35 @@ __global__ void __launch_bounds__(ET) k_mfp_eval(const u64* __restrict__ in, con
       time = r[INW - 2];
       diff = r[INW - 1];
       bool keep = true;
+      // the expressions below `support`, in index order; an error stops the row
+      auto eval_maps = [&](u32 support) {
+        for (; ne < support && keep; ++ne) {
+          const MVal m = mfp_run(pl.map.ops[ne], pl.map.n_ops[ne], pl.map.consts, pl.map_iv_us, w, mv);
+          if (m.err) {
+            e_code = m.err;
+            e_pay = m.pay;
+            keep = false;
+          }
+          mv[ne] = m.v;
+        }
+      };
       for (u32 p = 0; p < pl.plan.n_predicates && keep; ++p) {
-        const MVal m = mfp_run(pl.plan.ops[p], pl.plan.n_ops[p], pl, w);
+        eval_maps(pl.support[p]);
+        if (!keep) break;
+        const MVal m = mfp_run(pl.plan.ops[p], pl.plan.n_ops[p], pl.plan.consts, pl.iv_us, w, mv);
         if (m.err) {
           e_code = m.err;
+          e_pay = m.pay;
           keep = false;
         } else if (m.v == 0) {
           keep = false;
         }
       }
+      eval_maps(pl.map.n_exprs);
       u64 lower = time;
       for (u32 b = 0; b < pl.n_lower && keep; ++b) {
         const int q = pl.lower[b] & 7;
-        MVal m = mfp_run(pl.plan.temporal_ops[q], pl.plan.n_temporal_ops[q], pl, w);
+        MVal m = mfp_run(pl.plan.temporal_ops[q], pl.plan.n_temporal_ops[q], pl.plan.consts, pl.iv_us, w, mv);
         if (!m.err && (pl.lower[b] & 8)) {  // step_mz_timestamp
           if (m.v == ~0ull) m.err = MZGPU_MFP_ERR_MZ_TIMESTAMP_STEP_OVERFLOW;
           else m.v += 1;
@@ -238,7 +288,7 @@ __global__ void __launch_bounds__(ET) k_mfp_eval(const u64* __restrict__ in, con
       for (u32 b = 0; b < pl.n_upper && keep; ++b) {
         if (has_up && up == lower) break;  // cannot be produced: later bounds are not evaluated
         const int q = pl.upper[b] & 7;
-        MVal m = mfp_run(pl.plan.temporal_ops[q], pl.plan.n_temporal_ops[q], pl, w);
+        MVal m = mfp_run(pl.plan.temporal_ops[q], pl.plan.n_temporal_ops[q], pl.plan.consts, pl.iv_us, w, mv);
         if (!m.err && (pl.upper[b] & 8)) {
           if (m.v == ~0ull) m.err = MZGPU_MFP_ERR_MZ_TIMESTAMP_STEP_OVERFLOW;
           else m.v += 1;
@@ -275,7 +325,7 @@ __global__ void __launch_bounds__(ET) k_mfp_eval(const u64* __restrict__ in, con
       u64 acc = 0;
       for (u32 f = 0; f < pl.plan.n_fields[k]; ++f) {
         const mzgpu_field fd = pl.plan.fields[k][f];
-        u64 a = w[fd.src] >> fd.shift;
+        u64 a = (fd.src >= MZGPU_SRC_MAP0 ? mv[fd.src - MZGPU_SRC_MAP0] : w[fd.src]) >> fd.shift;
         if (fd.bits < 64) a &= (1ull << fd.bits) - 1;
         acc |= a << fd.dst_shift;
       }

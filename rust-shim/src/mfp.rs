@@ -13,6 +13,14 @@ impl GpuMfp {
         unsafe { sys::check(worker_ctx(), sys::mzgpu_mfp_new(worker_ctx(), plan, until, &mut h))?; }
         Ok(GpuMfp { h })
     }
+    /// The plan with map expressions (`MapFilterProject::expressions`, or a `KeyValPlan`'s key and value
+    /// expressions): predicates, temporal programs and output fields read them.  MZGPU_E_UNSUPPORTED: keep the
+    /// Rust operator for this plan.
+    pub fn new_map(plan: &sys::Mfp, map: &sys::MfpMap, until: u64) -> Result<Self, (i32, String)> {
+        let mut h = std::ptr::null_mut();
+        unsafe { sys::check(worker_ctx(), sys::mzgpu_mfp_new_map(worker_ctx(), plan, map, until, &mut h))?; }
+        Ok(GpuMfp { h })
+    }
     /// One activation: updates due before `upper` (new and held) are appended to `out`, consolidated; errors
     /// (R32: code, payload, time, diff) to `errs`.
     pub fn step(&mut self, rows: *mut sys::Buf, upper: u64, out: *mut sys::Buf, errs: *mut sys::Buf) -> Result<(), (i32, String)> {

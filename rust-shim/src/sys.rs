@@ -122,6 +122,24 @@ pub struct Mfp {
     pub temporal_ops: [[HavingOp; MFP_MAX_OPS]; MFP_MAX_TEMPORAL],
     pub consts: [HavingConst; MFP_MAX_CONSTS],
 }
+pub const MFP_MAX_MAPS: usize = 8;
+/// `Field::src` of map expression i is `SRC_MAP0 + i`.
+pub const SRC_MAP0: u8 = 16;
+pub const HOP_MAP: u8 = 23;
+pub const HOP_NEG: u8 = 24;
+pub const HOP_ABS: u8 = 25;
+pub const HOP_MOD: u8 = 26;
+pub const HOP_INT64_TO_INT32: u8 = 27;
+pub const HOP_IF: u8 = 28;
+/// The map expressions of an `Mfp` plan (mzgpu_mfp_map): postfix programs over their own constant pool.
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct MfpMap {
+    pub n_exprs: u32,
+    pub n_consts: u32,
+    pub n_ops: [u32; MFP_MAX_MAPS],
+    pub ops: [[HavingOp; MFP_MAX_OPS]; MFP_MAX_MAPS],
+    pub consts: [HavingConst; MFP_MAX_CONSTS],
+}
 
 #[link(name = "mzgpu")]
 extern "C" {
@@ -254,6 +272,7 @@ extern "C" {
     pub fn mzgpu_topk_basic_buf(r: *mut Reduce, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_topk_basic_negatives_trace(r: *mut Reduce) -> *mut Spine;
     pub fn mzgpu_mfp_new(ctx: *mut Ctx, plan: *const Mfp, until: u64, out: *mut *mut MfpOp) -> i32;
+    pub fn mzgpu_mfp_new_map(ctx: *mut Ctx, plan: *const Mfp, map: *const MfpMap, until: u64, out: *mut *mut MfpOp) -> i32;
     pub fn mzgpu_mfp_free(op: *mut MfpOp);
     pub fn mzgpu_mfp_step(op: *mut MfpOp, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_mfp_step_buf(op: *mut MfpOp, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
