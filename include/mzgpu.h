@@ -1164,6 +1164,103 @@ int32_t mzgpu_mfp_step_buf(mzgpu_mfp_op* op, mzgpu_buf* rows, uint64_t upper, mz
 int32_t mzgpu_mfp_frontier(mzgpu_mfp_op* op, uint64_t* out);
 int32_t mzgpu_mfp_stats(mzgpu_mfp_op* op, uint64_t out[3]);
 
+/* ---- FlatMap: a table function per input row, its rows appended to the input and run through the MfpPlan
+ * (render_flat_map and drain_through_mfp, src/compute/src/render/flat_map.rs:29-200), for the table functions of
+ * the fixed-width subset (TableFunc::eval, src/expr/src/relation/func.rs:3520-3620):
+ *   MZGPU_TF_GENERATE_SERIES_INT32 / _INT64   args start, stop, step (INT32 programs / INT programs read as i64);
+ *                        values start, start + step, ... while <= stop (step > 0) or >= stop (step < 0), stopping
+ *                        on a checked-add overflow (num::range_step_inclusive, restated line for line by
+ *                        TimestampRangeStepInclusive, func.rs:2884-2923).  The count is floor((stop - start) / step)
+ *                        + 1 when the direction matches, else 0 (up to 2^64 rows for one input row); step == 0 is
+ *                        InvalidParameterValue with payload 0.  One column: the value (int32 / int64).
+ *   MZGPU_TF_GENERATE_SERIES_TIMESTAMP       args start, stop (TS programs); the step is the constant step_iv
+ *                        (lo = microseconds as i64, hi = days in bits 0-31 | months in bits 32-63).  The same
+ *                        series over i64 microseconds (generate_series_ts, func.rs:2925-2948); a zero step
+ *                        (as_microseconds) is InvalidParameterValue with payload 0.  One column: the timestamp.
+ *   MZGPU_TF_REPEAT_ROW                      arg n (INT): one row with diff n if n != 0 (func.rs:3283-3290).
+ *   MZGPU_TF_REPEAT_ROW_NON_NEGATIVE         arg n (INT): n < 0 is InvalidParameterValue with payload n; 0 gives
+ *                        nothing, otherwise one row with diff n (func.rs:3292-3306).
+ *   MZGPU_TF_GUARD_SUBQUERY_SIZE             arg count (INT): 1 gives nothing, above 1 MultipleRowsFromSubquery,
+ *                        below 0 NegativeRowsFromSubquery, 0 Internal (func.rs:3588-3606).  No rows, ever.
+ * with_ordinality (WithOrdinality::eval, func.rs:3912-3960; allowed as TableFunc::with_ordinality allows it,
+ * func.rs:3482-3517, so MZGPU_TF_REPEAT_ROW with it is MZGPU_E_INVALID): every function row with diff d >= 0
+ * becomes d rows of diff 1, with an int64 ordinal from 1 as one more column.  So repeat_row_non_negative(n) with
+ * ordinality yields n rows, with ordinals 1..n.
+ *
+ * The function's columns are extension columns 0, 1 of the row the MfpPlan sees: a program's MZGPU_HOP_COL /
+ * COL_TS / COL_MZTS op or a projection field reads column i as source word MZGPU_SRC_FN0 + i (a series value as a
+ * sign-extended i64 word, the ordinal as an i64).  An extension index at or beyond the function's column count
+ * is MZGPU_E_INVALID.  The argument programs (n_ops[a] ops each, constants from `consts`, an interval in
+ * MZGPU_HOP_TS_ADD_IV folded as in the MfpPlan) read the input row only: MZGPU_HOP_MAP and MZGPU_SRC_FN0 are
+ * MZGPU_E_INVALID there.
+ *
+ * Per input row (words, time, diff), in order:
+ *   1. the argument programs, in order; the first error becomes an error row at the input's (time, diff) and the
+ *      row produces nothing more (flat_map.rs:75-85);
+ *   2. the function; its error likewise becomes an error row at (time, diff);
+ *   3. each function row (columns, d) is the row input ++ columns run through the MfpPlan exactly as
+ *      mzgpu_mfp_new_map does (predicates, map expressions, temporal bounds, until, error rows, ready / held),
+ *      at the input's time with diff d * diff, wrapping (flat_map.rs:168-199).
+ * The new error codes follow MZGPU_MFP_ERR_TIMESTAMP_OUT_OF_RANGE.  They are raised by the function only and
+ * never meet AND / OR, so their place in the numbering does not matter.
+ *
+ * An activation is mzgpu_flat_map_step[_buf] and then mzgpu_flat_map_work until *done.  The function rows of an
+ * activation are numbered in input-row order, then series order; each call expands the next `fuel` of them
+ * (fuel counts function rows before the MfpPlan; 0 is MZGPU_E_INVALID) and appends to `out`, consolidated, the
+ * resulting updates with time < upper together with every held update that has become due, exactly as
+ * mzgpu_mfp_step does; errors go to `errs`, consolidated.  `upper` belongs to the activation (the rules of
+ * mzgpu_mfp_step apply).  What `out` and `errs` accumulate over an activation does not depend on `fuel`.  The
+ * reference yields between input containers only (flat_map.rs:44-48, COMPUTE_FLAT_MAP_FUEL = 10^6,
+ * src/compute-types/src/dyncfgs.rs:247-251); a device activation bounds each call's buffers by `fuel` instead.
+ * The rows are copied when the activation starts, so the caller's buffer is free at once.  A step while an
+ * activation is unfinished is MZGPU_E_FRONTIER and changes nothing; work with no activation pending is a no-op
+ * that sets *done.  A step waits for the device once (for the 128-bit count of the activation's function rows,
+ * counted in mzgpu_stats.host_syncs); work never waits for its own sake.
+ *
+ * mzgpu_flat_map_frontier(op, &t): the least held time or, while an activation is unfinished, the least input
+ * time among the rows not yet fully expanded if that is lower; MZGPU_FRONTIER_EMPTY if neither exists.
+ * mzgpu_flat_map_stats(op, out): out[0..2] as mzgpu_mfp_stats, out[3] = function rows still to expand in the
+ * activation (saturating at u64::MAX).  Both wait for the device.
+ *
+ * Refused on the host, leaving no operator and the context usable: MZGPU_E_INVALID for a wrong argument count or
+ * argument types, MZGPU_HOP_MAP in an argument program, an extension column at or beyond the function's column
+ * count, MZGPU_TF_REPEAT_ROW with ordinality, and everything mzgpu_mfp_new_map refuses as invalid;
+ * MZGPU_E_UNSUPPORTED for a timestamp step with months or beyond i64 microseconds, any other table function
+ * (JSON, arrays, lists, maps, regexes, CSV, Wrap, timestamptz series, ROWS FROM) and everything mzgpu_mfp_new_map
+ * refuses as unsupported. */
+#define MZGPU_TF_GENERATE_SERIES_INT32 1
+#define MZGPU_TF_GENERATE_SERIES_INT64 2
+#define MZGPU_TF_GENERATE_SERIES_TIMESTAMP 3
+#define MZGPU_TF_REPEAT_ROW 4
+#define MZGPU_TF_REPEAT_ROW_NON_NEGATIVE 5
+#define MZGPU_TF_GUARD_SUBQUERY_SIZE 6
+#define MZGPU_SRC_FN0 8 /* mzgpu_field.src / MZGPU_HOP_COL* arg of extension column 0 */
+#define MZGPU_SRC_FN(i) (MZGPU_SRC_FN0 + (i))
+#define MZGPU_TF_ERR_INVALID_PARAMETER_VALUE 8
+#define MZGPU_TF_ERR_MULTIPLE_ROWS_FROM_SUBQUERY 9
+#define MZGPU_TF_ERR_NEGATIVE_ROWS_FROM_SUBQUERY 10
+#define MZGPU_TF_ERR_INTERNAL 11
+typedef struct mzgpu_table_func {
+  uint32_t kind; /* MZGPU_TF_* */
+  uint32_t with_ordinality;
+  uint32_t n_consts;
+  uint32_t n_ops[3]; /* argument programs; unused arguments have 0 ops */
+  mzgpu_having_op ops[3][MZGPU_MFP_MAX_OPS];
+  mzgpu_having_const consts[MZGPU_MFP_MAX_CONSTS];
+  mzgpu_having_const step_iv; /* MZGPU_TF_GENERATE_SERIES_TIMESTAMP: the step interval */
+} mzgpu_table_func;
+typedef struct mzgpu_flat_map_op mzgpu_flat_map_op;
+int32_t mzgpu_flat_map_new(mzgpu_ctx* ctx, const mzgpu_table_func* func, const mzgpu_mfp* plan,
+                           const mzgpu_mfp_map* map, uint64_t until, mzgpu_flat_map_op** out);
+void mzgpu_flat_map_free(mzgpu_flat_map_op* op);
+int32_t mzgpu_flat_map_step(mzgpu_flat_map_op* op, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                            uint64_t fuel, mzgpu_buf* out, mzgpu_buf* errs, int32_t* done);
+int32_t mzgpu_flat_map_step_buf(mzgpu_flat_map_op* op, mzgpu_buf* rows, uint64_t upper, uint64_t fuel,
+                                mzgpu_buf* out, mzgpu_buf* errs, int32_t* done);
+int32_t mzgpu_flat_map_work(mzgpu_flat_map_op* op, uint64_t fuel, mzgpu_buf* out, mzgpu_buf* errs, int32_t* done);
+int32_t mzgpu_flat_map_frontier(mzgpu_flat_map_op* op, uint64_t* out);
+int32_t mzgpu_flat_map_stats(mzgpu_flat_map_op* op, uint64_t out[4]);
+
 /* ------------------------------ f1 (first step): Row keys as fixed-width words */
 /* A `Row` orders by byte length first, then by its bytes (RowRef::cmp,
  * src/repr/src/row.rs:704-722; the arrangement key order of RowRowSpine,

@@ -215,6 +215,26 @@ class MfpMap(C.Structure):
     ]
 
 
+# FlatMap (mzgpu_table_func, include/mzgpu.h)
+TF_GENERATE_SERIES_INT32, TF_GENERATE_SERIES_INT64, TF_GENERATE_SERIES_TIMESTAMP = 1, 2, 3
+TF_REPEAT_ROW, TF_REPEAT_ROW_NON_NEGATIVE, TF_GUARD_SUBQUERY_SIZE = 4, 5, 6
+SRC_FN0 = 8
+TF_ERR_INVALID_PARAMETER_VALUE, TF_ERR_MULTIPLE_ROWS_FROM_SUBQUERY = 8, 9
+TF_ERR_NEGATIVE_ROWS_FROM_SUBQUERY, TF_ERR_INTERNAL = 10, 11
+
+
+class TableFunc(C.Structure):
+    _fields_ = [
+        ("kind", C.c_uint32),
+        ("with_ordinality", C.c_uint32),
+        ("n_consts", C.c_uint32),
+        ("n_ops", C.c_uint32 * 3),
+        ("ops", (HavingOp * MFP_MAX_OPS) * 3),
+        ("consts", HavingConst * MFP_MAX_CONSTS),
+        ("step_iv", HavingConst),
+    ]
+
+
 class Filter(C.Structure):
     _fields_ = [("field", Field), ("op", C.c_uint32), ("rhs", C.c_uint64)]
 
@@ -370,6 +390,13 @@ SIGNATURES = {
     "mzgpu_mfp_step_buf": (i32, [vp, vp, u64, vp, vp]),
     "mzgpu_mfp_frontier": (i32, [vp, C.POINTER(u64)]),
     "mzgpu_mfp_stats": (i32, [vp, C.POINTER(u64)]),
+    "mzgpu_flat_map_new": (i32, [vp, C.POINTER(TableFunc), C.POINTER(Mfp), C.POINTER(MfpMap), u64, PV]),
+    "mzgpu_flat_map_free": (None, [vp]),
+    "mzgpu_flat_map_step": (i32, [vp, vp, u64, i32, u64, u64, vp, vp, C.POINTER(i32)]),
+    "mzgpu_flat_map_step_buf": (i32, [vp, vp, u64, u64, vp, vp, C.POINTER(i32)]),
+    "mzgpu_flat_map_work": (i32, [vp, u64, vp, vp, C.POINTER(i32)]),
+    "mzgpu_flat_map_frontier": (i32, [vp, C.POINTER(u64)]),
+    "mzgpu_flat_map_stats": (i32, [vp, C.POINTER(u64)]),
     "mzgpu_comm_unique_id": (i32, [C.POINTER(C.c_uint8)]),
     "mzgpu_comm_init": (i32, [vp, C.POINTER(C.c_uint8)]),
     "mzgpu_exchange": (i32, [vp, vp, vp]),

@@ -909,6 +909,44 @@ def interval_const(micros=0, days=0, months=0):
     return (micros & (2**64 - 1), (days & 0xFFFFFFFF) | ((months & 0xFFFFFFFF) << 32))
 
 
+def _put_ops(dst, ops):
+    for i, o in enumerate(ops[:F.MFP_MAX_OPS]):
+        dst[i].code, dst[i].arg, dst[i].shift, dst[i].bits, dst[i].sign_extend, dst[i].konst = o
+
+
+def _put_consts(dst, consts):
+    for k, (lo, hi) in enumerate(consts[:F.MFP_MAX_CONSTS]):
+        dst[k].lo, dst[k].hi = lo & (2**64 - 1), hi & (2**64 - 1)
+
+
+def _mfp_structs(fields, predicates, temporal, consts, in_row_bytes, out_row_bytes, maps, map_consts):
+    """The mzgpu_mfp and (None without expressions) mzgpu_mfp_map of a plan."""
+    m = F.Mfp()
+    m.in_row_bytes, m.out_row_bytes = in_row_bytes, out_row_bytes
+    for w, fl in enumerate(fields):
+        m.n_fields[w] = len(fl)
+        for i, f in enumerate(fl[:6]):
+            m.fields[w][i] = F.Field(*f)
+    m.n_predicates, m.n_temporal, m.n_consts = len(predicates), len(temporal), len(consts)
+    for p, ops in enumerate(predicates[:F.MFP_MAX_PREDICATES]):
+        m.n_ops[p] = len(ops)
+        _put_ops(m.ops[p], ops)
+    for p, (cmp, ops) in enumerate(temporal[:F.MFP_MAX_TEMPORAL]):
+        m.temporal_cmp[p] = cmp
+        m.n_temporal_ops[p] = len(ops)
+        _put_ops(m.temporal_ops[p], ops)
+    _put_consts(m.consts, consts)
+    if not maps:
+        return m, None
+    mp = F.MfpMap()
+    mp.n_exprs, mp.n_consts = len(maps), len(map_consts)
+    for e, ops in enumerate(maps[:F.MFP_MAX_MAPS]):
+        mp.n_ops[e] = len(ops)
+        _put_ops(mp.ops[e], ops)
+    _put_consts(mp.consts, map_consts)
+    return m, mp
+
+
 class Mfp:
     """A temporal filter (mzgpu_mfp_new): the MfpPlan of a `WHERE mz_now() ...` query.  `fields` gives the
     output words (key, val1, val2) as lists of (src, shift, bits, dst_shift); `predicates` are op lists (hop());
@@ -921,40 +959,12 @@ class Mfp:
     def __init__(self, ctx, fields, predicates=(), temporal=(), consts=(), in_row_bytes=32, out_row_bytes=32,
                  until=F.FRONTIER_EMPTY, maps=(), map_consts=()):
         self.ctx, self.in_row_bytes, self.out_row_bytes = ctx, in_row_bytes, out_row_bytes
-        m = F.Mfp()
-        m.in_row_bytes, m.out_row_bytes = in_row_bytes, out_row_bytes
-        for w, fl in enumerate(fields):
-            m.n_fields[w] = len(fl)
-            for i, f in enumerate(fl[:6]):
-                m.fields[w][i] = F.Field(*f)
-        m.n_predicates, m.n_temporal, m.n_consts = len(predicates), len(temporal), len(consts)
-
-        def put(dst, ops):
-            for i, o in enumerate(ops[:F.MFP_MAX_OPS]):
-                dst[i].code, dst[i].arg, dst[i].shift, dst[i].bits, dst[i].sign_extend, dst[i].konst = o
-
-        for p, ops in enumerate(predicates[:F.MFP_MAX_PREDICATES]):
-            m.n_ops[p] = len(ops)
-            put(m.ops[p], ops)
-        for p, (cmp, ops) in enumerate(temporal[:F.MFP_MAX_TEMPORAL]):
-            m.temporal_cmp[p] = cmp
-            m.n_temporal_ops[p] = len(ops)
-            put(m.temporal_ops[p], ops)
-        for k, (lo, hi) in enumerate(consts[:F.MFP_MAX_CONSTS]):
-            m.consts[k].lo, m.consts[k].hi = lo & (2**64 - 1), hi & (2**64 - 1)
+        m, mp = _mfp_structs(fields, predicates, temporal, consts, in_row_bytes, out_row_bytes, maps, map_consts)
         h = C.c_void_p()
-        if not maps:
+        if mp is None:
             ctx.check(F.lib.mzgpu_mfp_new(ctx.h, C.byref(m), until, C.byref(h)))
-            self.h = h
-            return
-        mp = F.MfpMap()
-        mp.n_exprs, mp.n_consts = len(maps), len(map_consts)
-        for e, ops in enumerate(maps[:F.MFP_MAX_MAPS]):
-            mp.n_ops[e] = len(ops)
-            put(mp.ops[e], ops)
-        for k, (lo, hi) in enumerate(map_consts[:F.MFP_MAX_CONSTS]):
-            mp.consts[k].lo, mp.consts[k].hi = lo & (2**64 - 1), hi & (2**64 - 1)
-        ctx.check(F.lib.mzgpu_mfp_new_map(ctx.h, C.byref(m), C.byref(mp), until, C.byref(h)))
+        else:
+            ctx.check(F.lib.mzgpu_mfp_new_map(ctx.h, C.byref(m), C.byref(mp), until, C.byref(h)))
         self.h = h
 
     def step(self, rows, upper):
@@ -985,6 +995,80 @@ class Mfp:
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:
             F.lib.mzgpu_mfp_free(self.h)
+            self.h = None
+
+
+def field_fn(i, shift=0, bits=64, dst_shift=0):
+    """An output field taking bits [shift, shift + bits) of FlatMap extension column `i`, placed at `dst_shift`."""
+    return (F.SRC_FN0 + i, shift, bits, dst_shift)
+
+
+class FlatMap:
+    """FlatMap (mzgpu_flat_map_new): table function `kind` (TF_*) over each input row, its rows appended to the
+    input and run through an MfpPlan (the arguments of Mfp).  `args` are the argument programs (op lists over
+    `arg_consts`, reading the input row); `step_iv` the timestamp series step (interval_const()).  Extension column
+    i is col(SRC_FN0 + i) in programs and field_fn(i) in the output.  step(rows, upper, fuel) starts an activation
+    and expands its first `fuel` function rows, work(fuel) the next ones: each returns (updates, errors, done)."""
+
+    def __init__(self, ctx, kind, args, fields, with_ordinality=False, arg_consts=(), step_iv=(0, 0), predicates=(),
+                 temporal=(), consts=(), in_row_bytes=32, out_row_bytes=32, until=F.FRONTIER_EMPTY, maps=(),
+                 map_consts=()):
+        self.ctx, self.in_row_bytes, self.out_row_bytes = ctx, in_row_bytes, out_row_bytes
+        tf = F.TableFunc()
+        tf.kind, tf.with_ordinality, tf.n_consts = kind, 1 if with_ordinality else 0, len(arg_consts)
+        for a, ops in enumerate(args[:3]):
+            tf.n_ops[a] = len(ops)
+            _put_ops(tf.ops[a], ops)
+        _put_consts(tf.consts, arg_consts)
+        tf.step_iv.lo, tf.step_iv.hi = step_iv[0] & (2**64 - 1), step_iv[1] & (2**64 - 1)
+        m, mp = _mfp_structs(fields, predicates, temporal, consts, in_row_bytes, out_row_bytes, maps, map_consts)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_flat_map_new(ctx.h, C.byref(tf), C.byref(m), C.byref(mp) if mp is not None else None,
+                                           until, C.byref(h)))
+        self.h = h
+
+    def step(self, rows, upper, fuel=F.MFP_RESTORE_FUEL):
+        rows = np.ascontiguousarray(rows)
+        out, errs, done = DeviceRows(self.ctx, self.out_row_bytes), DeviceRows(self.ctx, 32), C.c_int32(0)
+        self.ctx.check(F.lib.mzgpu_flat_map_step(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, fuel, out.h,
+                                                 errs.h, C.byref(done)))
+        return out.download(), errs.download(), bool(done.value)
+
+    def step_dev(self, dev_rows, upper, fuel=F.MFP_RESTORE_FUEL, out=None, errs=None):
+        """step() over device-resident rows; updates and errors are appended on the device: (out, errs, done)."""
+        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
+        errs = errs if errs is not None else DeviceRows(self.ctx, 32)
+        done = C.c_int32(0)
+        self.ctx.check(F.lib.mzgpu_flat_map_step_buf(self.h, dev_rows.h, upper, fuel, out.h, errs.h, C.byref(done)))
+        return out, errs, bool(done.value)
+
+    def work(self, fuel=F.MFP_RESTORE_FUEL, out=None, errs=None):
+        """The next `fuel` function rows of the activation: (updates, errors, done); with `out` / `errs`
+        (DeviceRows) they are appended there and returned as they are."""
+        dev = out is not None
+        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
+        errs = errs if errs is not None else DeviceRows(self.ctx, 32)
+        done = C.c_int32(0)
+        self.ctx.check(F.lib.mzgpu_flat_map_work(self.h, fuel, out.h, errs.h, C.byref(done)))
+        if dev:
+            return out, errs, bool(done.value)
+        return out.download(), errs.download(), bool(done.value)
+
+    def frontier(self):
+        """The least held time or, during an activation, unexpanded input time; FRONTIER_EMPTY if none."""
+        t = C.c_uint64(0)
+        self.ctx.check(F.lib.mzgpu_flat_map_frontier(self.h, C.byref(t)))
+        return t.value
+
+    def stats(self):
+        """(held rows, buckets, rows the store touched in the last page, function rows still to expand)."""
+        a = (C.c_uint64 * 4)()
+        self.ctx.check(F.lib.mzgpu_flat_map_stats(self.h, a))
+        return tuple(int(x) for x in a)
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_flat_map_free(self.h)
             self.h = None
 
 

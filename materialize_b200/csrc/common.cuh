@@ -1257,3 +1257,31 @@ int32_t mz_mfp_eval(mzgpu_ctx* ctx, const MfpDevPlan& pl, const u64* d_rows, DLe
 int32_t mz_mfp_partition(mzgpu_ctx* ctx, int rb, const MfpSlices* chunks, u32 n_chunks, u64 rows_ub,
                          const MfpBounds& b, u64* hist, u64* cursor, u64* dst, u64* total, u64* touched);
 int32_t mz_mfp_min_time(mzgpu_ctx* ctx, int rb, const MfpSlices* chunks, u32 n_chunks, u64 rows_ub, u64* d_min);
+
+// mfp.cu: FlatMap (mzgpu_flat_map_new).  The table function as the kernels read it beside the MfpPlan: its
+// descriptor, its folded intervals, the timestamp step in microseconds and its number of arguments.
+struct FlatMapDevPlan {
+  MfpDevPlan mfp;
+  mzgpu_table_func tf;
+  i64 iv_us[MZGPU_MFP_MAX_CONSTS];
+  i64 step_us;
+  u32 n_args;
+};
+// k_fm_expand takes the plan as a __grid_constant__ parameter beside 96 bytes of others
+static_assert(sizeof(FlatMapDevPlan) + 96 <= 4096, "FlatMapDevPlan exceeds the kernel parameter limit");
+#define MZ_FM_TILE 1024  // input rows per tile of the count-and-scan kernel
+// Per input row: the function's record (start, step, diff multiplier) and the inclusive 128-bit prefix of the
+// function-row counts; the look-back state is 3 words per tile (flag, lo, hi), zeroed before the launch, with a
+// tile ticket after it.  d_total gets (total lo, total hi, input rows).
+struct FmRec {
+  i64 start, step, mult;
+};
+int32_t mz_fm_count(mzgpu_ctx* ctx, const FlatMapDevPlan& pl, const u64* d_rows, DLen n, u64 n_ub, FmRec* rec,
+                    ulonglong2* incl, u64* lb_state, u64* d_total, u64* errs, u64* err_len);
+// one page: function rows [g, g + page) of the activation, through the MfpPlan into ready / held / errs
+int32_t mz_fm_expand(mzgpu_ctx* ctx, const FlatMapDevPlan& pl, const u64* d_rows, const FmRec* rec,
+                     const ulonglong2* incl, u64 n, unsigned __int128 g, u64 page, u64 upper, u64 until, u64* ready,
+                     u64* held, u64* errs, u64* err_len);
+// the least time of the input rows whose function rows are not all below ordinal g (atomicMin into *d_min)
+int32_t mz_fm_min_time(mzgpu_ctx* ctx, int iw, const u64* d_rows, const ulonglong2* incl, u64 n,
+                       unsigned __int128 g, u64* d_min);

@@ -4900,8 +4900,8 @@ static int32_t mfp_emit(mzgpu_ctx* ctx, int rb, const u64* d_rows, DLen n, u64 u
   return buf_append_dev(dst, cons.p, dlen_of(len, 0), std::min(cap, ub));
 }
 
-static int32_t mfp_step_dev(mzgpu_mfp_op* op, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
-                            mzgpu_buf* errs) {
+// the checks of a step, before it changes anything
+static int32_t mfp_step_check(mzgpu_mfp_op* op, u64 upper, mzgpu_buf* out, mzgpu_buf* errs) {
   mzgpu_ctx* ctx = op->ctx;
   if (out == nullptr || errs == nullptr || out == errs || (int)out->rb != op->ow || errs->rb != 32) {
     MZ_SET_ERR(ctx, "mfp_step: out must hold %d-byte rows and errs 32-byte rows (distinct buffers)", op->ow);
@@ -4912,32 +4912,23 @@ static int32_t mfp_step_dev(mzgpu_mfp_op* op, const u64* d_rows, DLen n, u64 n_u
                (unsigned long long)op->upper);
     return MZGPU_E_FRONTIER;
   }
+  return MZGPU_OK;
+}
+
+// A step's start: the held rows of earlier steps into the chain.
+static int32_t mfp_step_begin(mzgpu_mfp_op* op) {
   MZ_TRY(mfp_poll(op, false));
   op->step_seq++;
-  MZ_CUDA(ctx, cudaMemsetAsync(op->touched(), 0, 8, ctx->stream));
-  MZ_TRY(mfp_flush_pending(op));
-  const int onw = op->ow / 8;
-  // 1. evaluate the new rows: ready, held and error rows
-  auto ready = std::make_shared<MfpSeg>(), held = std::make_shared<MfpSeg>();
-  ready->ub = held->ub = 2 * n_ub;
-  DevMem err_rows;
-  Lazy4 err_len;
-  if (n_ub > 0) {
-    MZ_TRY(ready->mem.alloc(ctx, (MZ_MFP_HDR + 2 * n_ub * (u64)onw) * 8));
-    MZ_TRY(held->mem.alloc(ctx, (MZ_MFP_HDR + 2 * n_ub * (u64)onw) * 8));
-    MZ_TRY(err_rows.alloc(ctx, n_ub * 32));
-    MZ_TRY(err_len.make_pending(ctx));
-    MZ_CUDA(ctx, cudaMemsetAsync(ready->mem.p, 0, 16, ctx->stream));
-    MZ_CUDA(ctx, cudaMemsetAsync(held->mem.p, 0, 16, ctx->stream));
-    MZ_CUDA(ctx, cudaMemsetAsync(err_len.dptr(), 0, 8, ctx->stream));
-    MZ_TRY(mz_mfp_eval(ctx, op->pl, d_rows, n, n_ub, upper, op->until, ready->base(), held->base(),
-                       (u64*)err_rows.p, err_len.dptr()));
-    err_len.mark_written();
-  } else {
-    ready->known = held->known = true;
-    memset(ready->off, 0, sizeof(ready->off));
-    memset(held->off, 0, sizeof(held->off));
-  }
+  MZ_CUDA(op->ctx, cudaMemsetAsync(op->touched(), 0, 8, op->ctx->stream));
+  return mfp_flush_pending(op);
+}
+
+// A step's end, once its new updates are in `ready` and `held` (bounds ub) and its errors in err_rows (count
+// err_len on the device, bound err_ub): steps 2-6 below.
+static int32_t mfp_step_end(mzgpu_mfp_op* op, const std::shared_ptr<MfpSeg>& ready, const std::shared_ptr<MfpSeg>& held,
+                            const u64* err_rows, DLen err_len, u64 err_ub, u64 upper, mzgpu_buf* out,
+                            mzgpu_buf* errs) {
+  mzgpu_ctx* ctx = op->ctx;
   // 2. peel the due buckets; 3. release them with the ready rows, consolidated
   std::vector<MfpSlice> rel;
   MZ_TRY(mfp_peel(op, upper, &rel));
@@ -4954,18 +4945,58 @@ static int32_t mfp_step_dev(mzgpu_mfp_op* op, const u64* d_rows, DLen n, u64 n_u
   rel.clear();
   // 4. restore the chain; 5. hold the rest (inserted by the next step or read)
   MZ_TRY(mfp_restore(op));
-  if (n_ub > 0) {
+  if (held->ub > 0) {
     MZ_TRY(mfp_mirror(op, held));
     op->pending.push_back(held);
   }
   // 6. errors
-  if (n_ub > 0) MZ_TRY(mfp_emit(ctx, 32, (const u64*)err_rows.p, dlen_of(err_len, 0), n_ub, errs));
+  if (err_ub > 0) MZ_TRY(mfp_emit(ctx, 32, err_rows, err_len, err_ub, errs));
   cudaEvent_t ev;
   MZ_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   MZ_CUDA(ctx, cudaEventRecord(ev, ctx->stream));
   op->events.emplace_back(op->step_seq, ev);
   op->upper = upper;
   return MZGPU_OK;
+}
+
+// ready / held segments for up to `ub` updates (empty and known when ub == 0), their counts zeroed
+static int32_t mfp_segments(mzgpu_mfp_op* op, u64 ub, std::shared_ptr<MfpSeg>* ready, std::shared_ptr<MfpSeg>* held) {
+  mzgpu_ctx* ctx = op->ctx;
+  *ready = std::make_shared<MfpSeg>();
+  *held = std::make_shared<MfpSeg>();
+  for (MfpSeg* s : {ready->get(), held->get()}) {
+    s->ub = ub;
+    if (ub > 0) {
+      MZ_TRY(s->mem.alloc(ctx, (MZ_MFP_HDR + ub * (u64)(op->ow / 8)) * 8));
+      MZ_CUDA(ctx, cudaMemsetAsync(s->mem.p, 0, 16, ctx->stream));
+    } else {
+      s->known = true;
+      memset(s->off, 0, sizeof(s->off));
+    }
+  }
+  return MZGPU_OK;
+}
+
+static int32_t mfp_step_dev(mzgpu_mfp_op* op, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                            mzgpu_buf* errs) {
+  mzgpu_ctx* ctx = op->ctx;
+  MZ_TRY(mfp_step_check(op, upper, out, errs));
+  MZ_TRY(mfp_step_begin(op));
+  // 1. evaluate the new rows: ready, held and error rows
+  std::shared_ptr<MfpSeg> ready, held;
+  MZ_TRY(mfp_segments(op, 2 * n_ub, &ready, &held));
+  DevMem err_rows;
+  Lazy4 err_len;
+  if (n_ub > 0) {
+    MZ_TRY(err_rows.alloc(ctx, n_ub * 32));
+    MZ_TRY(err_len.make_pending(ctx));
+    MZ_CUDA(ctx, cudaMemsetAsync(err_len.dptr(), 0, 8, ctx->stream));
+    MZ_TRY(mz_mfp_eval(ctx, op->pl, d_rows, n, n_ub, upper, op->until, ready->base(), held->base(),
+                       (u64*)err_rows.p, err_len.dptr()));
+    err_len.mark_written();
+  }
+  return mfp_step_end(op, ready, held, (const u64*)err_rows.p, n_ub > 0 ? dlen_of(err_len, 0) : dlen_imm(0), n_ub,
+                      upper, out, errs);
 }
 
 // The checks of one program (include/mzgpu.h): a type per stack slot, simulated op by op, and whether the slot may
@@ -4983,6 +5014,7 @@ struct MfpProgram {
   i64* iv_us;                // its folded intervals
   const MfpTy* map_ty;       // the types of the expressions it may read: [0, n_readable)
   uint32_t n_readable;
+  uint32_t n_fn;             // FlatMap extension columns it may read (MZGPU_SRC_FN0 + i, i < n_fn)
 };
 static int32_t validate_mfp_program(mzgpu_ctx* ctx, uint32_t in_row_bytes, const MfpProgram& g, MfpTy* result,
                                     uint32_t* support, const char** unsupported) {
@@ -5013,7 +5045,8 @@ static int32_t validate_mfp_program(mzgpu_ctx* ctx, uint32_t in_row_bytes, const
       if (sp == MZGPU_HAVING_MAX_STACK) return bad(i, "stack overflow (depth 8)");
       MfpTy t = MFP_INT64;
       if (col) {
-        if (o.arg > max_src) return bad(i, "column word out of range");
+        if (o.arg > max_src && !(o.arg >= MZGPU_SRC_FN0 && o.arg < MZGPU_SRC_FN0 + g.n_fn))
+        return bad(i, "column word out of range");
         if (o.bits == 0 || o.bits > 64 || (uint32_t)o.shift + o.bits > 64 || o.sign_extend > 1)
           return bad(i, "column field is empty or out of range");
         if (code == MZGPU_HOP_COL) t = (o.bits < 32 || (o.bits == 32 && o.sign_extend)) ? MFP_INT32 : MFP_INT64;
@@ -5144,10 +5177,10 @@ extern "C" int32_t mzgpu_mfp_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, uint64_t
   return mzgpu_mfp_new_map(ctx, plan, nullptr, until, out);
 }
 
-extern "C" int32_t mzgpu_mfp_new_map(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map, uint64_t until,
-                                     mzgpu_mfp_op** out) {
-  MZ_CHECK_CTX(ctx);
-  if (plan == nullptr || out == nullptr) return MZGPU_E_INVALID;
+// The plan of mzgpu_mfp_new_map, checked, over input rows with n_fn FlatMap extension columns.
+static int32_t mfp_build_plan(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map, uint32_t n_fn,
+                              MfpDevPlan* out_pl) {
+  if (plan == nullptr) return MZGPU_E_INVALID;
   const mzgpu_mfp& m = *plan;
   if (map != nullptr && map->n_exprs == 0) map = nullptr;  // exactly mzgpu_mfp_new
   if ((m.in_row_bytes != 32 && m.in_row_bytes != 40) || (m.out_row_bytes != 32 && m.out_row_bytes != 40)) {
@@ -5179,7 +5212,8 @@ extern "C" int32_t mzgpu_mfp_new_map(mzgpu_ctx* ctx, const mzgpu_mfp* plan, cons
                    n_exprs);
         return MZGPU_E_INVALID;
       }
-      if (is_map) fd.src = MZGPU_SRC_KEY;  // the bit-field checks of an input field
+      const bool is_fn = fd.src >= MZGPU_SRC_FN0 && fd.src < MZGPU_SRC_FN0 + n_fn;
+      if (is_map || is_fn) fd.src = MZGPU_SRC_KEY;  // the bit-field checks of an input field
       MZ_TRY(validate_field(ctx, fd, true));
       if ((!is_map && fd.src > max_src) || (uint32_t)fd.shift + fd.bits > 64) {
         MZ_SET_ERR(ctx, "mfp: output word %d, field %u reads past the input row", k, f);
@@ -5195,13 +5229,15 @@ extern "C" int32_t mzgpu_mfp_new_map(mzgpu_ctx* ctx, const mzgpu_mfp* plan, cons
   std::string unsupported_msg;
   MfpTy map_ty[MZGPU_MFP_MAX_MAPS];
   for (uint32_t e = 0; e < n_exprs; ++e) {
-    const MfpProgram g{MFP_MAP, e, map->ops[e], map->n_ops[e], map->consts, map->n_consts, pl.map_iv_us, map_ty, e};
+    const MfpProgram g{MFP_MAP, e, map->ops[e], map->n_ops[e], map->consts, map->n_consts, pl.map_iv_us, map_ty, e,
+                       n_fn};
     uint32_t support;
     MZ_TRY(validate_mfp_program(ctx, m.in_row_bytes, g, &map_ty[e], &support, &unsupported));
     if (unsupported && unsupported_msg.empty()) unsupported_msg = ctx->last_error;
   }
   for (uint32_t p = 0; p < m.n_predicates; ++p) {
-    const MfpProgram g{MFP_PREDICATE, p, m.ops[p], m.n_ops[p], m.consts, m.n_consts, pl.iv_us, map_ty, n_exprs};
+    const MfpProgram g{MFP_PREDICATE, p, m.ops[p], m.n_ops[p], m.consts, m.n_consts, pl.iv_us, map_ty, n_exprs,
+                       n_fn};
     MfpTy t;
     MZ_TRY(validate_mfp_program(ctx, m.in_row_bytes, g, &t, &pl.support[p], &unsupported));
     if (unsupported && unsupported_msg.empty()) unsupported_msg = ctx->last_error;
@@ -5217,7 +5253,7 @@ extern "C" int32_t mzgpu_mfp_new_map(mzgpu_ctx* ctx, const mzgpu_mfp* plan, cons
       unsupported = "<>";
     }
     const MfpProgram g{MFP_TEMPORAL, p, m.temporal_ops[p], m.n_temporal_ops[p], m.consts, m.n_consts, pl.iv_us,
-                       map_ty, n_exprs};
+                       map_ty, n_exprs, n_fn};
     MfpTy t;
     uint32_t support;
     MZ_TRY(validate_mfp_program(ctx, m.in_row_bytes, g, &t, &support, &unsupported));
@@ -5240,16 +5276,34 @@ extern "C" int32_t mzgpu_mfp_new_map(mzgpu_ctx* ctx, const mzgpu_mfp* plan, cons
     ctx->last_error = unsupported_msg;
     return MZGPU_E_UNSUPPORTED;
   }
+  *out_pl = pl;
+  return MZGPU_OK;
+}
+
+static int32_t mfp_op_create(mzgpu_ctx* ctx, const MfpDevPlan& pl, uint64_t until,
+                             std::unique_ptr<mzgpu_mfp_op>* out) {
   auto op = std::unique_ptr<mzgpu_mfp_op>(new mzgpu_mfp_op());
   op->ctx = ctx;
   op->pl = pl;
-  op->ow = (int)m.out_row_bytes;
+  op->ow = (int)pl.plan.out_row_bytes;
   op->until = until;
   MZ_TRY(op->scratch.alloc(ctx, (2 * MZ_MFP_MAX_SLOTS + 2) * 8));
   MZ_CUDA(ctx, cudaMemsetAsync(op->scratch.p, 0, (2 * MZ_MFP_MAX_SLOTS + 2) * 8, ctx->stream));
   MZ_CUDA(ctx, cudaMallocHost((void**)&op->h_mirror, (size_t)MZ_MFP_MIRROR * MZ_MFP_HDR * 8));
   for (int s = MZ_MFP_MIRROR - 1; s >= 0; --s) op->free_slots.push_back(s);
   op->chain.emplace(0, MfpBucket{64, {}});  // BucketChain::new: one bucket over the whole domain
+  *out = std::move(op);
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_mfp_new_map(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map, uint64_t until,
+                                     mzgpu_mfp_op** out) {
+  MZ_CHECK_CTX(ctx);
+  if (plan == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  MfpDevPlan pl;
+  MZ_TRY(mfp_build_plan(ctx, plan, map, 0, &pl));
+  std::unique_ptr<mzgpu_mfp_op> op;
+  MZ_TRY(mfp_op_create(ctx, pl, until, &op));
   *out = op.release();
   return MZGPU_OK;
 }
@@ -5327,5 +5381,234 @@ extern "C" int32_t mzgpu_mfp_stats(mzgpu_mfp_op* op, uint64_t out[3]) {
   out[0] = held;
   out[1] = op->chain.size();
   MZ_TRY(copy_out(op->ctx, &out[2], op->touched(), 8, MZGPU_MEM_HOST));
+  return MZGPU_OK;
+}
+
+// ========================================================== FlatMap
+// mzgpu_flat_map_new (include/mzgpu.h): a table function per input row, expanded in pages through the MfpPlan of
+// an mzgpu_mfp_op, whose bucket chain holds the future updates.  An activation's rows are copied, their function
+// records and inclusive 128-bit counts computed in one pass (mfp.cu: k_fm_count), and the count of function rows
+// read back once; every page is one load-balanced expansion (k_fm_expand) followed by steps 2-6 of a mfp step.
+typedef unsigned __int128 u128;
+struct mzgpu_flat_map_op {
+  std::unique_ptr<mzgpu_mfp_op> mfp;
+  FlatMapDevPlan pl;
+  // the activation in progress
+  bool active = false;
+  DevMem rows, rec, incl, lb, first_errs;
+  u64 n = 0, n_first_errs = 0, upper = 0;
+  u128 total = 0, g = 0;  // function rows, and the first not yet expanded
+  DevMem d_total;         // total lo, hi, input rows, argument / function errors
+};
+
+static int32_t fm_fail(mzgpu_ctx* ctx, int32_t st, const char* what) {
+  MZ_SET_ERR(ctx, "flat_map: %s", what);
+  return st;
+}
+
+extern "C" int32_t mzgpu_flat_map_new(mzgpu_ctx* ctx, const mzgpu_table_func* func, const mzgpu_mfp* plan,
+                                      const mzgpu_mfp_map* map, uint64_t until, mzgpu_flat_map_op** out) {
+  MZ_CHECK_CTX(ctx);
+  if (func == nullptr || plan == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  const mzgpu_table_func& tf = *func;
+  if (tf.kind < MZGPU_TF_GENERATE_SERIES_INT32 || tf.kind > MZGPU_TF_GUARD_SUBQUERY_SIZE)
+    return fm_fail(ctx, MZGPU_E_UNSUPPORTED, "table function outside the fixed-width subset");
+  if (tf.with_ordinality > 1) return fm_fail(ctx, MZGPU_E_INVALID, "with_ordinality is 0 or 1");
+  if (tf.kind == MZGPU_TF_REPEAT_ROW && tf.with_ordinality)
+    return fm_fail(ctx, MZGPU_E_INVALID, "repeat_row WITH ORDINALITY (its diffs may be negative)");
+  if (tf.n_consts > MZGPU_MFP_MAX_CONSTS) return fm_fail(ctx, MZGPU_E_INVALID, "argument constants (0..8)");
+  const bool series = tf.kind <= MZGPU_TF_GENERATE_SERIES_TIMESTAMP;
+  const bool ts = tf.kind == MZGPU_TF_GENERATE_SERIES_TIMESTAMP;
+  const uint32_t n_args = ts ? 2 : series ? 3 : 1;
+  // the function's columns: the series value, then the ordinal
+  const uint32_t n_fn = (series ? 1u : 0u) + tf.with_ordinality;
+  FlatMapDevPlan pl;
+  memset(&pl, 0, sizeof(pl));
+  pl.tf = tf;
+  pl.n_args = n_args;
+  for (uint32_t a = 0; a < 3; ++a)
+    if ((a < n_args) != (tf.n_ops[a] != 0)) return fm_fail(ctx, MZGPU_E_INVALID, "argument count");
+  const char* unsupported = nullptr;
+  std::string unsupported_msg;
+  for (uint32_t a = 0; a < n_args; ++a) {
+    const MfpProgram g{MFP_MAP, a, tf.ops[a], tf.n_ops[a], tf.consts, tf.n_consts, pl.iv_us, nullptr, 0, 0};
+    MfpTy t;
+    uint32_t support;
+    MZ_TRY(validate_mfp_program(ctx, plan->in_row_bytes, g, &t, &support, &unsupported));
+    if (unsupported && unsupported_msg.empty()) unsupported_msg = ctx->last_error;
+    const bool ok = ts ? t == MFP_TS
+                       : tf.kind == MZGPU_TF_GENERATE_SERIES_INT32 ? t == MFP_INT32 : t == MFP_INT32 || t == MFP_INT64;
+    if (!ok) {
+      MZ_SET_ERR(ctx, "flat_map: argument %u has the wrong type", a);
+      return MZGPU_E_INVALID;
+    }
+  }
+  if (ts) {
+    const mzgpu_having_const& k = tf.step_iv;
+    const int32_t days = (int32_t)(uint32_t)k.hi, months = (int32_t)(uint32_t)(k.hi >> 32);
+    const __int128 us = (__int128)days * 86400000000ll + (__int128)(int64_t)k.lo;
+    if (months != 0 && !unsupported) {
+      MZ_SET_ERR(ctx, "flat_map: a timestamp series step with months");
+      unsupported = "months";
+      unsupported_msg = ctx->last_error;
+    } else if ((us < (__int128)INT64_MIN || us > (__int128)INT64_MAX) && !unsupported) {
+      MZ_SET_ERR(ctx, "flat_map: a timestamp series step beyond i64 microseconds");
+      unsupported = "step";
+      unsupported_msg = ctx->last_error;
+    } else {
+      pl.step_us = (i64)us;
+    }
+  }
+  const int32_t st = mfp_build_plan(ctx, plan, map, n_fn, &pl.mfp);
+  if (st == MZGPU_E_INVALID) return st;
+  if (unsupported) {
+    ctx->last_error = unsupported_msg;
+    return MZGPU_E_UNSUPPORTED;
+  }
+  MZ_TRY(st);
+  auto op = std::unique_ptr<mzgpu_flat_map_op>(new mzgpu_flat_map_op());
+  MZ_TRY(mfp_op_create(ctx, pl.mfp, until, &op->mfp));
+  op->pl = pl;
+  MZ_TRY(op->d_total.alloc(ctx, 4 * 8));
+  *out = op.release();
+  return MZGPU_OK;
+}
+
+extern "C" void mzgpu_flat_map_free(mzgpu_flat_map_op* op) { delete op; }
+
+// One page: the next `fuel` function rows of the activation through the MfpPlan (the first page also carries the
+// argument and function errors), then steps 2-6 of a mfp step.
+static int32_t fm_page(mzgpu_flat_map_op* op, uint64_t fuel, mzgpu_buf* out, mzgpu_buf* errs, int32_t* done) {
+  mzgpu_mfp_op* m = op->mfp.get();
+  mzgpu_ctx* ctx = m->ctx;
+  const u128 left = op->total - op->g;
+  const u64 page = left < (u128)fuel ? (u64)left : fuel;
+  MZ_TRY(mfp_step_begin(m));
+  std::shared_ptr<MfpSeg> ready, held;
+  MZ_TRY(mfp_segments(m, 2 * page, &ready, &held));
+  const u64 err_ub = op->n_first_errs + page;
+  DevMem err_rows;
+  Lazy4 err_len;
+  if (err_ub > 0) {
+    MZ_TRY(err_rows.alloc(ctx, err_ub * 32));
+    MZ_TRY(err_len.make_pending(ctx));
+    const u64 k = op->n_first_errs;
+    if (k) {
+      MZ_TRY(copy_out(ctx, err_len.dptr(), (const u64*)op->d_total.p + 3, 8, MZGPU_MEM_DEVICE));
+      MZ_TRY(copy_out(ctx, err_rows.p, op->first_errs.p, k * 32, MZGPU_MEM_DEVICE));
+    } else {
+      MZ_CUDA(ctx, cudaMemsetAsync(err_len.dptr(), 0, 8, ctx->stream));
+    }
+  }
+  if (page > 0)
+    MZ_TRY(mz_fm_expand(ctx, op->pl, (const u64*)op->rows.p, (const FmRec*)op->rec.p, (const ulonglong2*)op->incl.p,
+                        op->n, op->g, page, op->upper, m->until, ready->base(), held->base(), (u64*)err_rows.p,
+                        err_len.dptr()));
+  if (err_ub > 0) err_len.mark_written();
+  MZ_TRY(mfp_step_end(m, ready, held, (const u64*)err_rows.p, err_ub > 0 ? dlen_of(err_len, 0) : dlen_imm(0), err_ub,
+                      op->upper, out, errs));
+  op->g += page;
+  op->n_first_errs = 0;
+  op->first_errs.release();
+  if (op->g == op->total) {
+    op->active = false;
+    op->rows.release();
+    op->rec.release();
+    op->incl.release();
+    op->lb.release();
+  }
+  *done = op->active ? 0 : 1;
+  return MZGPU_OK;
+}
+
+static int32_t fm_step_dev(mzgpu_flat_map_op* op, const void* d_rows, int32_t mem, DLen n, u64 n_ub, uint64_t upper,
+                           uint64_t fuel, mzgpu_buf* out, mzgpu_buf* errs, int32_t* done) {
+  mzgpu_mfp_op* m = op->mfp.get();
+  mzgpu_ctx* ctx = m->ctx;
+  if (done == nullptr || fuel == 0) return fm_fail(ctx, MZGPU_E_INVALID, "step needs fuel > 0 and a done flag");
+  if (op->active) return fm_fail(ctx, MZGPU_E_FRONTIER, "step while an activation is unfinished (call work)");
+  MZ_TRY(mfp_step_check(m, upper, out, errs));
+  const u64 irb = op->pl.mfp.plan.in_row_bytes;
+  op->total = op->g = 0;
+  op->n = op->n_first_errs = 0;
+  if (n_ub > 0) {
+    // the rows are copied: the caller's buffer is free once the step returns
+    MZ_TRY(op->rows.alloc(ctx, n_ub * irb));
+    MZ_TRY(copy_in(ctx, op->rows.p, d_rows, n_ub * irb, mem));
+    const u64 n_tiles = (n_ub + MZ_FM_TILE - 1) / MZ_FM_TILE;
+    MZ_TRY(op->rec.alloc(ctx, n_ub * sizeof(FmRec)));
+    MZ_TRY(op->incl.alloc(ctx, n_ub * 16));
+    MZ_TRY(op->lb.alloc(ctx, (n_tiles * 5 + 1) * 8));
+    MZ_TRY(op->first_errs.alloc(ctx, n_ub * 32));
+    u64* tot = (u64*)op->d_total.p;
+    MZ_CUDA(ctx, cudaMemsetAsync(tot, 0, 4 * 8, ctx->stream));
+    MZ_TRY(mz_fm_count(ctx, op->pl, (const u64*)op->rows.p, n, n_ub, (FmRec*)op->rec.p, (ulonglong2*)op->incl.p,
+                       (u64*)op->lb.p, tot, (u64*)op->first_errs.p, tot + 3));
+    u64 h[4];
+    MZ_TRY(copy_out(ctx, h, tot, sizeof(h), MZGPU_MEM_HOST));  // the activation's one wait
+    op->total = ((u128)h[1] << 64) | h[0];
+    op->n = h[2];
+    op->n_first_errs = h[3];
+  }
+  op->active = true;
+  op->upper = upper;
+  return fm_page(op, fuel, out, errs, done);
+}
+
+extern "C" int32_t mzgpu_flat_map_step(mzgpu_flat_map_op* op, const void* rows, uint64_t n, int32_t mem,
+                                       uint64_t upper, uint64_t fuel, mzgpu_buf* out, mzgpu_buf* errs, int32_t* done) {
+  if (op == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(op->mfp->ctx);
+  op->mfp->ctx->stats.rows_in += n;
+  return fm_step_dev(op, rows, mem, dlen_imm(n), n, upper, fuel, out, errs, done);
+}
+
+extern "C" int32_t mzgpu_flat_map_step_buf(mzgpu_flat_map_op* op, mzgpu_buf* rows, uint64_t upper, uint64_t fuel,
+                                           mzgpu_buf* out, mzgpu_buf* errs, int32_t* done) {
+  if (op == nullptr || rows == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(op->mfp->ctx);
+  if (rows->rb != op->pl.mfp.plan.in_row_bytes || rows == out || rows == errs)
+    return fm_fail(op->mfp->ctx, MZGPU_E_INVALID, "step_buf: input rows of the plan's width, not an output buffer");
+  return fm_step_dev(op, rows->mem.p, MZGPU_MEM_DEVICE, buf_dlen(rows), rows->ub, upper, fuel, out, errs, done);
+}
+
+extern "C" int32_t mzgpu_flat_map_work(mzgpu_flat_map_op* op, uint64_t fuel, mzgpu_buf* out, mzgpu_buf* errs,
+                                       int32_t* done) {
+  if (op == nullptr || done == nullptr) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = op->mfp->ctx;
+  MZ_CHECK_CTX(ctx);
+  if (fuel == 0) return fm_fail(ctx, MZGPU_E_INVALID, "work needs fuel > 0");
+  if (!op->active) {
+    *done = 1;
+    return MZGPU_OK;
+  }
+  MZ_TRY(mfp_step_check(op->mfp.get(), op->upper, out, errs));
+  return fm_page(op, fuel, out, errs, done);
+}
+
+extern "C" int32_t mzgpu_flat_map_frontier(mzgpu_flat_map_op* op, uint64_t* out) {
+  if (op == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  mzgpu_ctx* ctx = op->mfp->ctx;
+  MZ_CHECK_CTX(ctx);
+  u64 t = MZGPU_FRONTIER_EMPTY;
+  MZ_TRY(mzgpu_mfp_frontier(op->mfp.get(), &t));
+  if (op->active && op->n > 0) {
+    u64* dmin = op->mfp->dmin();
+    MZ_CUDA(ctx, cudaMemsetAsync(dmin, 0xff, 8, ctx->stream));
+    MZ_TRY(mz_fm_min_time(ctx, (int)op->pl.mfp.plan.in_row_bytes, (const u64*)op->rows.p,
+                          (const ulonglong2*)op->incl.p, op->n, op->g, dmin));
+    u64 pend;
+    MZ_TRY(copy_out(ctx, &pend, dmin, 8, MZGPU_MEM_HOST));
+    if (pend != ~0ull && (t == MZGPU_FRONTIER_EMPTY || pend < t)) t = pend;
+  }
+  *out = t;
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_flat_map_stats(mzgpu_flat_map_op* op, uint64_t out[4]) {
+  if (op == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  MZ_TRY(mzgpu_mfp_stats(op->mfp.get(), out));
+  const u128 left = op->active ? op->total - op->g : 0;
+  out[3] = left > (u128)~0ull ? ~0ull : (u64)left;
   return MZGPU_OK;
 }

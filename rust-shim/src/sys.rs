@@ -140,6 +140,27 @@ pub struct MfpMap {
     pub ops: [[HavingOp; MFP_MAX_OPS]; MFP_MAX_MAPS],
     pub consts: [HavingConst; MFP_MAX_CONSTS],
 }
+/// A FlatMap operator (mzgpu_flat_map_op), created from a `TableFunc` and an `Mfp` plan.
+pub enum FlatMapOp {}
+pub const TF_GENERATE_SERIES_INT32: u32 = 1;
+pub const TF_GENERATE_SERIES_INT64: u32 = 2;
+pub const TF_GENERATE_SERIES_TIMESTAMP: u32 = 3;
+pub const TF_REPEAT_ROW: u32 = 4;
+pub const TF_REPEAT_ROW_NON_NEGATIVE: u32 = 5;
+pub const TF_GUARD_SUBQUERY_SIZE: u32 = 6;
+/// `Field::src` / a column op's `arg` of FlatMap extension column i is `SRC_FN0 + i`.
+pub const SRC_FN0: u8 = 8;
+/// A table function (mzgpu_table_func): its kind, WITH ORDINALITY and argument programs over the input row.
+#[repr(C)] #[derive(Clone, Copy, Debug, Default)]
+pub struct TableFunc {
+    pub kind: u32,
+    pub with_ordinality: u32,
+    pub n_consts: u32,
+    pub n_ops: [u32; 3],
+    pub ops: [[HavingOp; MFP_MAX_OPS]; 3],
+    pub consts: [HavingConst; MFP_MAX_CONSTS],
+    pub step_iv: HavingConst,
+}
 
 #[link(name = "mzgpu")]
 extern "C" {
@@ -278,6 +299,13 @@ extern "C" {
     pub fn mzgpu_mfp_step_buf(op: *mut MfpOp, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_mfp_frontier(op: *mut MfpOp, out: *mut u64) -> i32;
     pub fn mzgpu_mfp_stats(op: *mut MfpOp, out: *mut u64) -> i32;
+    pub fn mzgpu_flat_map_new(ctx: *mut Ctx, func: *const TableFunc, plan: *const Mfp, map: *const MfpMap, until: u64, out: *mut *mut FlatMapOp) -> i32;
+    pub fn mzgpu_flat_map_free(op: *mut FlatMapOp);
+    pub fn mzgpu_flat_map_step(op: *mut FlatMapOp, rows: *const c_void, n: u64, mem: i32, upper: u64, fuel: u64, out: *mut Buf, errs: *mut Buf, done: *mut i32) -> i32;
+    pub fn mzgpu_flat_map_step_buf(op: *mut FlatMapOp, rows: *mut Buf, upper: u64, fuel: u64, out: *mut Buf, errs: *mut Buf, done: *mut i32) -> i32;
+    pub fn mzgpu_flat_map_work(op: *mut FlatMapOp, fuel: u64, out: *mut Buf, errs: *mut Buf, done: *mut i32) -> i32;
+    pub fn mzgpu_flat_map_frontier(op: *mut FlatMapOp, out: *mut u64) -> i32;
+    pub fn mzgpu_flat_map_stats(op: *mut FlatMapOp, out: *mut u64) -> i32;
     pub fn mzgpu_rowkey_pack(row_bytes: *const u8, len: u64, key_out: *mut u64) -> i32;
     pub fn mzgpu_rowkeys_pack(data: *const u8, offsets: *const u64, n: u64, keys_out: *mut u64, n_done: *mut u64) -> i32;
     pub fn mzgpu_rowkey_unpack(key: u64, row_bytes_out: *mut u8, len_out: *mut u64) -> i32;
