@@ -592,41 +592,88 @@ def map_rows(ctx, rows, closure):
     return out.download()
 
 
-class ReduceAccumulable:
-    """One-column reduce (mzgpu_reduce_new).  The operator is freed with this object, and a Spine from
-    input_trace() borrows the operator's arrangement: it must not outlive the operator."""
+class _Reduce:
+    """What every reduce operator shares.  A subclass sets step and step_dev with _steps(), and _out_rb and
+    _arr_rb, the row bytes of its output and of its input arrangement.  The operator is freed with this object,
+    and a Spine from input_trace() borrows the operator's arrangement: it must not outlive the operator."""
 
-    # the input arrangement's rows: exploded accumulators (mzgpu_racc), or the (key, value) rows
-    # themselves for MIN / MAX / TopK
-    row_bytes = 80
-
-    def __init__(self, ctx, agg_kind=F.AGG_COUNT_SUM_I64):
+    def _create(self, ctx, new, *args):
         self.ctx = ctx
-        if agg_kind in (F.AGG_MIN, F.AGG_MAX):
-            self.row_bytes = 32
         h = C.c_void_p()
-        ctx.check(F.lib.mzgpu_reduce_new(ctx.h, agg_kind, C.byref(h)))
+        ctx.check(new(ctx.h, *args, C.byref(h)))
         self.h = h
 
-    def step(self, rows, upper):
-        rows = np.ascontiguousarray(rows)
-        out = DeviceRows(self.ctx, 64)
-        self.ctx.check(F.lib.mzgpu_reduce_accumulable(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h))
-        return out.download()
-
-    def step_dev(self, dev_rows, upper, out=None):
-        """One activation over device-resident rows; corrections are appended to `out` on the device."""
-        out = out if out is not None else DeviceRows(self.ctx, 64)
-        self.ctx.check(F.lib.mzgpu_reduce_accumulable_buf(self.h, dev_rows.h, upper, out.h))
-        return out
-
     def input_trace(self):
-        return Spine(self.ctx, self.row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+        return Spine(self.ctx, self._arr_rb, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
 
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:
             F.lib.mzgpu_reduce_free(self.h)
             self.h = None
+
+
+def _steps(host_fn, buf_fn, errs_rb=None):
+    """step() and step_dev() of a reduce operator class: its host-form and buffer-form step functions, and the row
+    bytes of its error rows (None: the operator has no error rows).  They call the class's own entry points
+    whatever operator they are given, so the library refuses an operator of another kind."""
+    host, buf = getattr(F.lib, host_fn), getattr(F.lib, buf_fn)
+
+    def outs(self, out=None, errs=None):
+        out = out if out is not None else DeviceRows(self.ctx, self._out_rb)
+        if errs_rb is None:
+            return (out,)
+        return out, errs if errs is not None else DeviceRows(self.ctx, errs_rb)
+
+    def step(self, rows, upper):
+        """One activation over host rows: the output rows, or (output, errors) for an operator with error rows."""
+        rows = np.ascontiguousarray(rows)
+        o = outs(self)
+        self.ctx.check(host(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, *(x.h for x in o)))
+        got = tuple(x.download() for x in o)
+        return got if errs_rb else got[0]
+
+    def step_dev(self, dev_rows, upper, out=None, errs=None):
+        """One activation over device-resident rows; its output (and errors, for an operator with error rows) are
+        appended on the device."""
+        o = outs(self, out, errs)
+        self.ctx.check(buf(self.h, dev_rows.h, upper, *(x.h for x in o)))
+        return o if errs_rb else o[0]
+
+    return step, step_dev
+
+
+def _accum_lanes(lanes):
+    arr = (F.AccumLane * max(1, len(lanes)))()
+    for i, (kind, src, shift, bits, sx) in enumerate(lanes):
+        arr[i].kind = kind
+        arr[i].sign_extend = 1 if sx else 0
+        arr[i].field = F.Field(src, shift, bits, 0)
+    return arr
+
+
+def _order_lanes(order):
+    arr = (F.OrderLane * max(1, len(order)))()
+    for i, (src, shift, bits, sx, desc, f64) in enumerate(order):
+        arr[i].sign_extend = 1 if sx else 0
+        arr[i].descending = 1 if desc else 0
+        arr[i].flags = F.ORDER_F64 if f64 else 0
+        arr[i].field = F.Field(src, shift, bits, 0)
+    return arr
+
+
+class ReduceAccumulable(_Reduce):
+    """One-column reduce (mzgpu_reduce_new)."""
+
+    step, step_dev = _steps("mzgpu_reduce_accumulable", "mzgpu_reduce_accumulable_buf")
+    _out_rb = 64
+    # the input arrangement's rows: exploded accumulators (mzgpu_racc), or the (key, value) rows
+    # themselves for MIN / MAX / TopK
+    row_bytes = _arr_rb = 80
+
+    def __init__(self, ctx, agg_kind=F.AGG_COUNT_SUM_I64):
+        if agg_kind in (F.AGG_MIN, F.AGG_MAX):
+            self.row_bytes = self._arr_rb = 32
+        self._create(ctx, F.lib.mzgpu_reduce_new, agg_kind)
 
 
 def accum_lane(kind, src=SRC_VAL1, shift=0, bits=64, sign_extend=False):
@@ -740,147 +787,71 @@ def having(*predicates):
     return hv
 
 
-class ReduceLanes:
+class ReduceLanes(_Reduce):
     """COUNT / SUM of several value columns per key in one arrangement (mzgpu_reduce_lanes_new).
     `lanes` is a list of accum_lane(...) tuples; input rows are R32 (in_row_bytes=32) or R40 (40).
     Output rows have the dtype ROUT_LANES[class] (lane l in ["lanes"][:, l]).  `having`: a HAVING
     filter, having(...) or an F.Having (mzgpu_reduce_lanes_new_having); its errors are in bits
     16-18 of "flags" (ROUT_HAVING_ERR_SHIFT)."""
 
+    _step, step_dev = _steps("mzgpu_reduce_lanes", "mzgpu_reduce_lanes_buf")
+
     def __init__(self, ctx, lanes, in_row_bytes=32, having=None):
-        self.ctx = ctx
         self.n_lanes = len(lanes)
         self.in_row_bytes = in_row_bytes
-        arr = (F.AccumLane * max(1, len(lanes)))()
-        for i, (kind, src, shift, bits, sx) in enumerate(lanes):
-            arr[i].kind = kind
-            arr[i].sign_extend = 1 if sx else 0
-            arr[i].field = F.Field(src, shift, bits, 0)
-        h = C.c_void_p()
+        args = (in_row_bytes, _accum_lanes(lanes), len(lanes))
         if having is None:
-            ctx.check(F.lib.mzgpu_reduce_lanes_new(ctx.h, in_row_bytes, arr, len(lanes), C.byref(h)))
+            self._create(ctx, F.lib.mzgpu_reduce_lanes_new, *args)
         else:
-            ctx.check(F.lib.mzgpu_reduce_lanes_new_having(ctx.h, in_row_bytes, arr, len(lanes), C.byref(having), C.byref(h)))
-        self.h = h
+            self._create(ctx, F.lib.mzgpu_reduce_lanes_new_having, *args, C.byref(having))
         self.lane_class = F.lane_class(self.n_lanes)
-        self.arr_row_bytes, self.out_row_bytes = F.LANE_ROW_BYTES[self.lane_class]
+        self.arr_row_bytes, self.out_row_bytes = self._arr_rb, self._out_rb = F.LANE_ROW_BYTES[self.lane_class]
 
     def step(self, rows, upper):
-        rows = np.ascontiguousarray(rows)
-        out = DeviceRows(self.ctx, self.out_row_bytes)
-        self.ctx.check(F.lib.mzgpu_reduce_lanes(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h))
-        return out.download().view(F.ROUT_LANES[self.lane_class])
-
-    def step_dev(self, dev_rows, upper, out=None):
-        """One activation over device-resident rows; corrections are appended to `out` on the device."""
-        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
-        self.ctx.check(F.lib.mzgpu_reduce_lanes_buf(self.h, dev_rows.h, upper, out.h))
-        return out
-
-    def input_trace(self):
-        return Spine(self.ctx, self.arr_row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+        return ReduceLanes._step(self, rows, upper).view(F.ROUT_LANES[self.lane_class])
 
     def distinct_trace(self, lane):
         """The (key, value) pair arrangement (R32 rows) of distinct lane `lane`; None for any other lane."""
         h = F.lib.mzgpu_reduce_lanes_distinct_trace(self.h, lane)
         return Spine(self.ctx, 32, _borrowed=h) if h else None
 
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            F.lib.mzgpu_reduce_free(self.h)
-            self.h = None
 
-
-class TopKMonotonic:
+class TopKMonotonic(_Reduce):
     """MonotonicTop1 / MonotonicTopK over append-only input (mzgpu_topk_monotonic_new): the first `limit`
     rows per key in the order of `order` (order_lane() tuples, at most 3; ties by val1, then val2), with only
     that window arranged.  Top1 is limit=1; LIMIT NULL is TOPK_NO_LIMIT.  Input rows are R32
     (in_row_bytes=32) or R40 (40).  step() returns (changes, errors): the window's changes as rows of the
-    input width, and R16 error rows (key = time, diff = rows with diff <= 0 at that time)."""
+    input width, and R16 error rows (key = time, diff = rows with diff <= 0 at that time).  input_trace() is the
+    window arrangement (RTOPK rows)."""
+
+    step, step_dev = _steps("mzgpu_topk_monotonic", "mzgpu_topk_monotonic_buf", 16)
+    _arr_rb = 72
 
     def __init__(self, ctx, order, limit, in_row_bytes=32, must_consolidate=False):
-        self.ctx = ctx
-        self.in_row_bytes = in_row_bytes
-        arr = (F.OrderLane * max(1, len(order)))()
-        for i, (src, shift, bits, sx, desc, f64) in enumerate(order):
-            arr[i].sign_extend = 1 if sx else 0
-            arr[i].descending = 1 if desc else 0
-            arr[i].flags = F.ORDER_F64 if f64 else 0
-            arr[i].field = F.Field(src, shift, bits, 0)
-        h = C.c_void_p()
-        ctx.check(F.lib.mzgpu_topk_monotonic_new(ctx.h, in_row_bytes, arr, len(order), int(limit),
-                                                 1 if must_consolidate else 0, C.byref(h)))
-        self.h = h
-
-    def step(self, rows, upper):
-        rows = np.ascontiguousarray(rows)
-        out, errs = DeviceRows(self.ctx, self.in_row_bytes), DeviceRows(self.ctx, 16)
-        self.ctx.check(F.lib.mzgpu_topk_monotonic(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
-        return out.download(), errs.download()
-
-    def step_dev(self, dev_rows, upper, out=None, errs=None):
-        """One activation over device-resident rows; changes and errors are appended on the device."""
-        out = out if out is not None else DeviceRows(self.ctx, self.in_row_bytes)
-        errs = errs if errs is not None else DeviceRows(self.ctx, 16)
-        self.ctx.check(F.lib.mzgpu_topk_monotonic_buf(self.h, dev_rows.h, upper, out.h, errs.h))
-        return out, errs
-
-    def input_trace(self):
-        """The window arrangement (RTOPK rows)."""
-        return Spine(self.ctx, 72, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
-
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            F.lib.mzgpu_reduce_free(self.h)
-            self.h = None
+        self.in_row_bytes = self._out_rb = in_row_bytes
+        self._create(ctx, F.lib.mzgpu_topk_monotonic_new, in_row_bytes, _order_lanes(order), len(order), int(limit),
+                     1 if must_consolidate else 0)
 
 
-class TopKBasic:
+class TopKBasic(_Reduce):
     """BasicTopKPlan over input with retractions (mzgpu_topk_basic_new): per key the units in positions
     [offset, offset + limit) of its live rows in the order of `order` (order_lane() tuples, at most 3; ties by
     val1, then val2).  LIMIT NULL is TOPK_NO_LIMIT.  Input rows are R32 (in_row_bytes=32) or R40 (40), with any
     diffs.  step() returns (changes, errors): the window's changes as rows of the input width, and R32 error rows
-    (key, 0, time, +1 entering / -1 leaving the negative-count state)."""
+    (key, 0, time, +1 entering / -1 leaving the negative-count state).  input_trace() is the whole live input
+    (RTOPK rows)."""
+
+    step, step_dev = _steps("mzgpu_topk_basic", "mzgpu_topk_basic_buf", 32)
+    _arr_rb = 72
 
     def __init__(self, ctx, order, limit, offset=0, in_row_bytes=32):
-        self.ctx = ctx
-        self.in_row_bytes = in_row_bytes
-        arr = (F.OrderLane * max(1, len(order)))()
-        for i, (src, shift, bits, sx, desc, f64) in enumerate(order):
-            arr[i].sign_extend = 1 if sx else 0
-            arr[i].descending = 1 if desc else 0
-            arr[i].flags = F.ORDER_F64 if f64 else 0
-            arr[i].field = F.Field(src, shift, bits, 0)
-        h = C.c_void_p()
-        ctx.check(F.lib.mzgpu_topk_basic_new(ctx.h, in_row_bytes, arr, len(order), int(limit), int(offset),
-                                             C.byref(h)))
-        self.h = h
-
-    def step(self, rows, upper):
-        rows = np.ascontiguousarray(rows)
-        out, errs = DeviceRows(self.ctx, self.in_row_bytes), DeviceRows(self.ctx, 32)
-        self.ctx.check(F.lib.mzgpu_topk_basic(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
-        return out.download(), errs.download()
-
-    def step_dev(self, dev_rows, upper, out=None, errs=None):
-        """One activation over device-resident rows; changes and errors are appended on the device."""
-        out = out if out is not None else DeviceRows(self.ctx, self.in_row_bytes)
-        errs = errs if errs is not None else DeviceRows(self.ctx, 32)
-        self.ctx.check(F.lib.mzgpu_topk_basic_buf(self.h, dev_rows.h, upper, out.h, errs.h))
-        return out, errs
-
-    def input_trace(self):
-        """The whole live input (RTOPK rows)."""
-        return Spine(self.ctx, 72, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
+        self.in_row_bytes = self._out_rb = in_row_bytes
+        self._create(ctx, F.lib.mzgpu_topk_basic_new, in_row_bytes, _order_lanes(order), len(order), int(limit),
+                     int(offset))
 
     def negatives_trace(self):
         """The negatives arrangement: R32 rows (key, 0, time, delta), summed per key its negative-count rows."""
         return Spine(self.ctx, 32, _borrowed=F.lib.mzgpu_topk_basic_negatives_trace(self.h))
-
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            F.lib.mzgpu_reduce_free(self.h)
-            self.h = None
 
 
 def hop(code, arg=0, shift=0, bits=0, sign_extend=0, konst=0):
@@ -1072,107 +1043,50 @@ class FlatMap:
             self.h = None
 
 
-class ReduceMonotonic:
+class ReduceMonotonic(_Reduce):
     """MIN / MAX of several value columns per key over append-only input (mzgpu_reduce_monotonic_new,
     build_monotonic).  `lanes` are accum_lane(AGG_MIN | AGG_MAX, ...) tuples; sign_extend=True makes a lane
     an int64 aggregate (signed order), False an unsigned one.  Input rows are R32 (in_row_bytes=32) or R40
     (40).  step() returns (corrections, errors): corrections of dtype MONO_OUT[class] (lane l in
     ["vals"][:, l]), errors R16 rows (key = time, diff = rows with diff <= 0 at that time)."""
 
+    step, step_dev = _steps("mzgpu_reduce_monotonic", "mzgpu_reduce_monotonic_buf", 16)
+
     def __init__(self, ctx, lanes, in_row_bytes=32, must_consolidate=False):
-        self.ctx = ctx
         self.n_lanes = len(lanes)
         self.in_row_bytes = in_row_bytes
-        arr = (F.AccumLane * max(1, len(lanes)))()
-        for i, (kind, src, shift, bits, sx) in enumerate(lanes):
-            arr[i].kind = kind
-            arr[i].sign_extend = 1 if sx else 0
-            arr[i].field = F.Field(src, shift, bits, 0)
-        h = C.c_void_p()
-        ctx.check(F.lib.mzgpu_reduce_monotonic_new(ctx.h, in_row_bytes, arr, len(lanes), 1 if must_consolidate else 0,
-                                                   C.byref(h)))
-        self.h = h
+        self._create(ctx, F.lib.mzgpu_reduce_monotonic_new, in_row_bytes, _accum_lanes(lanes), len(lanes),
+                     1 if must_consolidate else 0)
         self.lane_class = F.mono_class(self.n_lanes)
-        self.arr_row_bytes, self.out_row_bytes = F.MONO_ROW_BYTES[self.lane_class]
-
-    def step(self, rows, upper):
-        rows = np.ascontiguousarray(rows)
-        out, errs = DeviceRows(self.ctx, self.out_row_bytes), DeviceRows(self.ctx, 16)
-        self.ctx.check(F.lib.mzgpu_reduce_monotonic(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
-        return out.download(), errs.download()
-
-    def step_dev(self, dev_rows, upper, out=None, errs=None):
-        """One activation over device-resident rows; corrections and errors are appended on the device."""
-        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
-        errs = errs if errs is not None else DeviceRows(self.ctx, 16)
-        self.ctx.check(F.lib.mzgpu_reduce_monotonic_buf(self.h, dev_rows.h, upper, out.h, errs.h))
-        return out, errs
-
-    def input_trace(self):
-        return Spine(self.ctx, self.arr_row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
-
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            F.lib.mzgpu_reduce_free(self.h)
-            self.h = None
+        self.arr_row_bytes, self.out_row_bytes = self._arr_rb, self._out_rb = F.MONO_ROW_BYTES[self.lane_class]
 
 
-class ReduceHierarchical:
+class ReduceHierarchical(_Reduce):
     """MIN / MAX of several value columns per key over input with retractions (mzgpu_reduce_hierarchical_new,
     build_bucketed).  `lanes` are accum_lane(AGG_MIN | AGG_MAX, ...) tuples, as for ReduceMonotonic.  Input rows
     are R32 (in_row_bytes=32) or R40 (40).  step() returns (corrections, errors): corrections of dtype
     MONO_OUT[class] (lane l in ["vals"][:, l]), errors R32 rows (key, 0, time, +1 entering / -1 leaving the
     non-positive-accumulation state).  The arrangement (input_trace) holds the masked input rows."""
 
+    step, step_dev = _steps("mzgpu_reduce_hierarchical", "mzgpu_reduce_hierarchical_buf", 32)
+
     def __init__(self, ctx, lanes, in_row_bytes=32):
-        self.ctx = ctx
         self.n_lanes = len(lanes)
-        self.in_row_bytes = in_row_bytes
-        arr = (F.AccumLane * max(1, len(lanes)))()
-        for i, (kind, src, shift, bits, sx) in enumerate(lanes):
-            arr[i].kind = kind
-            arr[i].sign_extend = 1 if sx else 0
-            arr[i].field = F.Field(src, shift, bits, 0)
-        h = C.c_void_p()
-        ctx.check(F.lib.mzgpu_reduce_hierarchical_new(ctx.h, in_row_bytes, arr, len(lanes), C.byref(h)))
-        self.h = h
+        self.in_row_bytes = self._arr_rb = in_row_bytes
+        self._create(ctx, F.lib.mzgpu_reduce_hierarchical_new, in_row_bytes, _accum_lanes(lanes), len(lanes))
         self.lane_class = F.mono_class(self.n_lanes)
-        self.out_row_bytes = F.MONO_ROW_BYTES[self.lane_class][1]
-
-    def step(self, rows, upper):
-        rows = np.ascontiguousarray(rows)
-        out, errs = DeviceRows(self.ctx, self.out_row_bytes), DeviceRows(self.ctx, 32)
-        self.ctx.check(F.lib.mzgpu_reduce_hierarchical(self.h, _ptr(rows), len(rows), F.MEM_HOST, upper, out.h, errs.h))
-        return out.download(), errs.download()
-
-    def step_dev(self, dev_rows, upper, out=None, errs=None):
-        """One activation over device-resident rows; corrections and errors are appended on the device."""
-        out = out if out is not None else DeviceRows(self.ctx, self.out_row_bytes)
-        errs = errs if errs is not None else DeviceRows(self.ctx, 32)
-        self.ctx.check(F.lib.mzgpu_reduce_hierarchical_buf(self.h, dev_rows.h, upper, out.h, errs.h))
-        return out, errs
-
-    def input_trace(self):
-        return Spine(self.ctx, self.in_row_bytes, _borrowed=F.lib.mzgpu_reduce_input_trace(self.h))
-
-    def __del__(self):
-        if getattr(self, "h", None) and self.ctx.h:
-            F.lib.mzgpu_reduce_free(self.h)
-            self.h = None
+        self.out_row_bytes = self._out_rb = F.MONO_ROW_BYTES[self.lane_class][1]
 
 
 class TopK(ReduceAccumulable):
     """TopK per key over (key, value) rows (BasicTopKPlan, src/compute/src/render/top_k.rs:215-248,
     521-673): `limit` < 0 or None = no limit; stepped like every other reduce kind."""
 
-    row_bytes = 32
+    row_bytes = _arr_rb = 32
 
     def __init__(self, ctx, limit, offset=0, descending=False):
-        self.ctx = ctx
-        h = C.c_void_p()
         lim = -1 if limit is None else int(limit)
-        ctx.check(F.lib.mzgpu_topk_new(ctx.h, lim, int(offset), 1 if descending else 0, C.byref(h)))
-        self.h = h
+        self._create(ctx, F.lib.mzgpu_topk_new, lim, int(offset), 1 if descending else 0)
 
 
 def route(key, peers):

@@ -667,6 +667,16 @@ static int32_t consolidate_dev(mzgpu_ctx* ctx, int rb, const void* d_in, DLen n,
   return MZGPU_OK;
 }
 
+// append `n` device rows (count possibly on the device, bound ub) to `dst`, consolidated
+static int32_t append_consolidated(mzgpu_ctx* ctx, int rb, const void* d_rows, DLen n, u64 ub, mzgpu_buf* dst) {
+  if (ub == 0) return MZGPU_OK;
+  DevMem cons;
+  u64 cap = 0;
+  Lazy4 len;
+  MZ_TRY(consolidate_dev(ctx, rb, d_rows, n, ub, &cons, &cap, &len));
+  return buf_append_dev(dst, cons.p, dlen_of(len, 0), len.known ? len.v[0] : std::min(cap, ub));
+}
+
 static int32_t consolidate_ptr(mzgpu_ctx* ctx, int rb, void* rows, u64 n, int32_t mem, u64* n_out) {
   MZ_CHECK_CTX(ctx);
   if ((rows == nullptr && n) || n_out == nullptr) return MZGPU_E_INVALID;
@@ -1924,6 +1934,12 @@ static int32_t trace_view(mzgpu_ctx* ctx, const std::vector<mzgpu_batch*>& batch
   }
   return MZGPU_OK;
 }
+// The view of every batch of a spine.
+static int32_t trace_view_of(mzgpu_spine* s, TraceView* tv) {
+  std::vector<mzgpu_batch*> batches;
+  s->all_batches(batches);
+  return trace_view(s->ctx, batches, tv);
+}
 // Upper bound on the matches of one probe row: the sum over batches of the
 // longest key run.  *exact is false if some run length saturated.
 static int32_t trace_fanout(const std::vector<mzgpu_batch*>& batches, u64* fan, bool* exact) {
@@ -2503,39 +2519,46 @@ extern "C" int32_t mzgpu_map_rows(mzgpu_ctx* ctx, const mzgpu_r32* rows, uint64_
 }
 
 // =================================================================== reduce
+// Which operator a mzgpu_reduce is; each pair of step entry points takes one shape.
+enum class ReduceShape {
+  ACCUM,           // mzgpu_reduce_new and mzgpu_topk_new, told apart by agg_kind
+  LANES,           // mzgpu_reduce_lanes_new[_having]
+  MONOTONIC,       // mzgpu_reduce_monotonic_new
+  HIERARCHICAL,    // mzgpu_reduce_hierarchical_new
+  TOPK_MONOTONIC,  // mzgpu_topk_monotonic_new
+  TOPK_BASIC,      // mzgpu_topk_basic_new
+};
 struct mzgpu_reduce {
   mzgpu_ctx* ctx;
-  int agg_kind;
-  TopKParams topk = {-1, 0, 0};
-  // mzgpu_reduce_lanes_new: lane class (1, 2, 4, 8) and descriptors; 0 for every other operator
-  int lane_class = 0;
-  LaneSet lanes = {};
+  ReduceShape shape;
+  // LANES: the lane class (1, 2, 4, 8); MONOTONIC / HIERARCHICAL: the mono class (4, 8)
+  int cls = 0;
   mzgpu_batcher* batcher = nullptr;
   mzgpu_spine* input = nullptr;
-  // distinct lanes (MZGPU_ACCUM_DISTINCT), in lane order: the lane index, and the batcher and R32 pair
-  // arrangement of its (key, value) pairs
+  // ACCUM: the aggregate kind, and mzgpu_topk_new's parameters.  LANES: the first lane's kind without the
+  // DISTINCT bit, which class 1 runs the one-column kernels with.
+  int agg_kind = 0;
+  TopKParams topk = {-1, 0, 0};
+  // LANES, MONOTONIC, HIERARCHICAL: the lane descriptors
+  LaneSet lanes = {};
+  // LANES: the distinct lanes (MZGPU_ACCUM_DISTINCT), in lane order: the lane index, and the batcher and R32
+  // pair arrangement of its (key, value) pairs
   int n_distinct = 0;
   u32 distinct_lane[MZGPU_MAX_ACCUM_LANES] = {};
   mzgpu_batcher* pair_batcher[MZGPU_MAX_ACCUM_LANES] = {};
   mzgpu_spine* pairs[MZGPU_MAX_ACCUM_LANES] = {};
-  // mzgpu_reduce_lanes_new_having: the validated HAVING program, run by the corrections kernels
+  // LANES from mzgpu_reduce_lanes_new_having: the validated HAVING program, run by the corrections kernels
   bool has_having = false;
   mzgpu_having having = {};
-  // mzgpu_reduce_monotonic_new: lane class (4, 8; 0 for every other operator), the lanes' encodings, and
-  // consolidate_named_if's flag with the value bits the lanes read
-  int mono_class = 0;
+  // MONOTONIC, HIERARCHICAL: the lanes' encodings and the value bits they read
   MonoXor mono = {};
-  bool must_consolidate = false;
   u64 mono_mask[2] = {0, 0};
-  // mzgpu_reduce_hierarchical_new: lane class (4, 8; 0 for every other operator); lanes, mono and mono_mask
-  // above hold its lanes, their encodings and the value bits they read
-  int hier_class = 0;
-  // mzgpu_topk_monotonic_new: the order lanes and limit (must_consolidate above is its flag too)
-  bool topk_mono = false;
+  // MONOTONIC, TOPK_MONOTONIC: consolidate_named_if's flag
+  bool must_consolidate = false;
+  // TOPK_MONOTONIC, TOPK_BASIC: the order lanes and limit
   TopKOrder tko = {};
-  // mzgpu_topk_basic_new (tko above holds its order lanes and limit): the offset (clamped to INT64_MAX), and the
-  // batcher and R32 arrangement of the negatives, (key, 0, time, change in the key's negative-count rows)
-  bool topk_basic = false;
+  // TOPK_BASIC: the offset (clamped to INT64_MAX), and the batcher and R32 arrangement of the negatives,
+  // (key, 0, time, change in the key's negative-count rows)
   i64 topk_offset = 0;
   mzgpu_batcher* neg_batcher = nullptr;
   mzgpu_spine* negs = nullptr;
@@ -2553,16 +2576,25 @@ struct mzgpu_reduce {
   }
 };
 
+// A new operator of `shape` with its input batcher and arrangement of arr_rb-byte rows.
+static int32_t reduce_alloc(mzgpu_ctx* ctx, ReduceShape shape, uint32_t arr_rb, std::unique_ptr<mzgpu_reduce>* out) {
+  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
+  r->ctx = ctx;
+  r->shape = shape;
+  MZ_TRY(mzgpu_batcher_new(ctx, arr_rb, &r->batcher));
+  MZ_TRY(mzgpu_spine_new(ctx, arr_rb, 1, &r->input));
+  *out = std::move(r);
+  return MZGPU_OK;
+}
+
 extern "C" int32_t mzgpu_reduce_new(mzgpu_ctx* ctx, int32_t agg_kind, mzgpu_reduce** out) {
   MZ_CHECK_CTX(ctx);
   if (out == nullptr || agg_kind < MZGPU_AGG_COUNT_SUM_I64 || agg_kind > MZGPU_AGG_MAX) return MZGPU_E_INVALID;
-  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
-  r->ctx = ctx;
-  r->agg_kind = agg_kind;
   // accumulable kinds arrange exploded diffs (RACC); MIN/MAX arranges the (key, value) rows themselves
   const uint32_t rb = (agg_kind == MZGPU_AGG_MIN || agg_kind == MZGPU_AGG_MAX) ? 32 : 80;
-  MZ_TRY(mzgpu_batcher_new(ctx, rb, &r->batcher));
-  MZ_TRY(mzgpu_spine_new(ctx, rb, 1, &r->input));
+  std::unique_ptr<mzgpu_reduce> r;
+  MZ_TRY(reduce_alloc(ctx, ReduceShape::ACCUM, rb, &r));
+  r->agg_kind = agg_kind;
   *out = r.release();
   return MZGPU_OK;
 }
@@ -2570,14 +2602,12 @@ extern "C" int32_t mzgpu_topk_new(mzgpu_ctx* ctx, int64_t limit, uint64_t offset
                                   mzgpu_reduce** out) {
   MZ_CHECK_CTX(ctx);
   if (out == nullptr) return MZGPU_E_INVALID;
-  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
-  r->ctx = ctx;
+  std::unique_ptr<mzgpu_reduce> r;
+  MZ_TRY(reduce_alloc(ctx, ReduceShape::ACCUM, 32, &r));
   r->agg_kind = MZGPU_AGG_TOPK;
   r->topk.limit = limit < 0 ? -1 : limit;
   r->topk.offset = offset;
   r->topk.descending = descending != 0;
-  MZ_TRY(mzgpu_batcher_new(ctx, 32, &r->batcher));
-  MZ_TRY(mzgpu_spine_new(ctx, 32, 1, &r->input));
   *out = r.release();
   return MZGPU_OK;
 }
@@ -2631,9 +2661,8 @@ static int32_t distinct_step(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_u
   if (cap == 0) return MZGPU_OK;
   // at most one presence change per new pair row
   Seg s;
-  const int c = r->lane_class;
-  MZ_TRY(s.rows.alloc(ctx, cap * mz_lane_arr_bytes(c)));
-  MZ_TRY(mz_distinct_presence(ctx, c, d, jobs, s.rows.as<u64>(), cap, &s.len, &s.word));
+  MZ_TRY(s.rows.alloc(ctx, cap * mz_lane_arr_bytes(r->cls)));
+  MZ_TRY(mz_distinct_presence(ctx, r->cls, d, jobs, s.rows.as<u64>(), cap, &s.len, &s.word));
   s.ub = cap;
   return batcher_push_seg(r->batcher, std::move(s));
 }
@@ -2682,6 +2711,21 @@ static bool single_pass_fits(u64 n, u64 per_row) {
   return (n + 255) / 256 <= MZ_LB_TILES && per_row * n <= MZ_BOUND_MAX_ROWS;
 }
 
+// A segment of the input's length: the same count as the input rows, shared with nothing (a device-resident
+// count is copied on the device).
+static int32_t seg_len_of_input(mzgpu_ctx* ctx, DLen n, u64 n_ub, Seg* s) {
+  if (n.p == nullptr) {
+    s->len.set(ctx, n.imm);
+    s->ub = n.imm;
+    return MZGPU_OK;
+  }
+  MZ_TRY(s->len.make_pending(ctx));
+  MZ_CUDA(ctx, cudaMemcpyAsync(s->len.dptr(), n.p, 8, cudaMemcpyDeviceToDevice, ctx->stream));
+  s->len.mark_written();
+  s->ub = n_ub;
+  return MZGPU_OK;
+}
+
 static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
                            bool minmax, u64 per_row);
 static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out) {
@@ -2723,45 +2767,34 @@ static int32_t reduce_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, 
 static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
                            bool minmax, u64 per_row) {
   mzgpu_ctx* ctx = r->ctx;
+  const bool lanes = r->shape == ReduceShape::LANES;
   // a lanes operator whose lanes are all distinct has no plain explode
-  const bool plain = r->lane_class == 0 || r->lanes.distinct_mask != (1u << r->lanes.n) - 1;
+  const bool plain = !lanes || r->lanes.distinct_mask != (1u << r->lanes.n) - 1;
   if (n_ub && plain) {
     Seg s;
     if (minmax) {
       MZ_TRY(s.rows.alloc(ctx, n_ub * 32));
       MZ_CUDA(ctx, cudaMemcpyAsync(s.rows.p, d_rows, n_ub * 32, cudaMemcpyDeviceToDevice, ctx->stream));
     } else {
-      const int c = r->lane_class;
-      MZ_TRY(s.rows.alloc(ctx, n_ub * (c ? mz_lane_arr_bytes(c) : 80)));
-      if (c)
-        MZ_TRY(mz_explode_lanes(ctx, c, d_rows, n, n_ub, r->lanes, s.rows.as<u64>()));
+      MZ_TRY(s.rows.alloc(ctx, n_ub * (lanes ? mz_lane_arr_bytes(r->cls) : 80)));
+      if (lanes)
+        MZ_TRY(mz_explode_lanes(ctx, r->cls, d_rows, n, n_ub, r->lanes, s.rows.as<u64>()));
       else
         MZ_TRY(mz_explode(ctx, d_rows, n, n_ub, r->agg_kind, s.rows.as<u64>()));
     }
-    if (n.p == nullptr) {
-      s.len.set(ctx, n.imm);
-      s.ub = n.imm;
-    } else {
-      // same count as the input rows: share nothing, copy the word on the device
-      MZ_TRY(s.len.make_pending(ctx));
-      MZ_CUDA(ctx, cudaMemcpyAsync(s.len.dptr(), n.p, 8, cudaMemcpyDeviceToDevice, ctx->stream));
-      s.len.mark_written();
-      s.ub = n_ub;
-    }
+    MZ_TRY(seg_len_of_input(ctx, n, n_ub, &s));
     MZ_TRY(batcher_push_seg(r->batcher, std::move(s)));
   }
   // arrange: seal the accumulable arrangement's batch at the new frontier
   mzgpu_batch* batch = nullptr;
   MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
   // reduce_abelian over the keys of the new batch
-  std::vector<mzgpu_batch*> prior;
-  r->input->all_batches(prior);
   TraceView tv;
-  int32_t st = trace_view(ctx, prior, &tv);
+  int32_t st = trace_view_of(r->input, &tv);
   const u64 b_ub = batch->len_ub;
-  const int lc = r->lane_class ? r->lane_class : 1;
+  const int lc = lanes ? r->cls : 1;
   const u64 out_rb = (u64)mz_lane_out_bytes(lc);
-  const LaneSet* ls = r->lane_class ? &r->lanes : nullptr;
+  const LaneSet* ls = lanes ? &r->lanes : nullptr;
   const mzgpu_having* hv = r->has_having ? &r->having : nullptr;
   // The single-pass bound is checked against the batch's length bound; when that is loose (a
   // device-resident input buffer's capacity), the length is read back and checked again before the
@@ -2773,9 +2806,8 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
   }
   if (st == MZGPU_OK && s_ub > 0) {
     if (single_pass_fits(s_ub, per_row)) {
-      DevMem corr, cons;
-      Lazy4 clen, flen;
-      u64 ccap = 0;
+      DevMem corr;
+      Lazy4 clen;
       st = corr.alloc(ctx, per_row * s_ub * out_rb);
       if (st == MZGPU_OK) st = clen.make_pending(ctx);
       if (st == MZGPU_OK) {
@@ -2791,16 +2823,12 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
         // the accumulable kinds' corrections leave the kernel consolidated (reduce.cu:
         // sort_key_corrections): keys ascending, each key's few rows sorted by its thread
         st = buf_append_dev(out, corr.p, dlen_of(clen, 0), per_row * s_ub);
-      } else {
-        if (st == MZGPU_OK)
-          st = consolidate_dev(ctx, 64, corr.p, dlen_of(clen, 0), per_row * s_ub, &cons, &ccap, &flen);
-        if (st == MZGPU_OK)
-          st = buf_append_dev(out, cons.p, dlen_of(flen, 0), flen.known ? flen.v[0] : per_row * s_ub);
+      } else if (st == MZGPU_OK) {
+        st = append_consolidated(ctx, 64, corr.p, dlen_of(clen, 0), per_row * s_ub, out);
       }
     } else {
-      DevMem corr, cons;
-      u64 n_corr = 0, ccap = 0;
-      Lazy4 flen;
+      DevMem corr;
+      u64 n_corr = 0;
       if (minmax) {
         MZ_SET_ERR(ctx, "MIN/MAX/TopK reduce: batch of %llu rows exceeds the single-pass bound",
                    (unsigned long long)s_ub);
@@ -2812,51 +2840,12 @@ static int32_t reduce_main(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub,
       if (st == MZGPU_OK && n_corr && lc > 1) {
         // consolidated by construction, as in the single-pass form (and no RowT for these widths)
         st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
-      } else {
-        if (st == MZGPU_OK && n_corr)
-          st = consolidate_dev(ctx, 64, corr.p, dlen_imm(n_corr), n_corr, &cons, &ccap, &flen);
-        if (st == MZGPU_OK && n_corr)
-          st = buf_append_dev(out, cons.p, dlen_of(flen, 0), flen.known ? flen.v[0] : n_corr);
+      } else if (st == MZGPU_OK) {
+        st = append_consolidated(ctx, 64, corr.p, dlen_imm(n_corr), n_corr, out);
       }
     }
   }
   return reduce_seal_tail(r, batch, st);
-}
-
-// The rows of a host-form reduce entry point (n rows of in_rb bytes) counted into rows_in and, when they are in
-// host memory, uploaded into `in`; *d_rows is where the activation reads them.
-static int32_t reduce_rows_in(mzgpu_ctx* ctx, const void* rows, uint64_t n, int32_t mem, uint32_t in_rb, DevMem* in,
-                              const u64** d_rows) {
-  ctx->stats.rows_in += n;
-  *d_rows = (const u64*)rows;
-  if (mem == MZGPU_MEM_HOST && n) {
-    MZ_TRY(in->alloc(ctx, n * in_rb));
-    MZ_TRY(copy_in(ctx, in->p, rows, n * in_rb, mem));
-    *d_rows = in->as<u64>();
-  }
-  return MZGPU_OK;
-}
-
-extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_t n,
-                                            int32_t mem, uint64_t upper, mzgpu_buf* out) {
-  if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->lane_class || r->mono_class ||
-      r->topk_mono || r->hier_class || r->topk_basic)
-    return MZGPU_E_INVALID;
-  mzgpu_ctx* ctx = r->ctx;
-  MZ_CHECK_CTX(ctx);
-  DevMem in;
-  const u64* d_rows;
-  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, 32, &in, &d_rows));
-  return reduce_dev(r, d_rows, dlen_imm(n), n, upper, out);
-}
-extern "C" int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
-                                                mzgpu_buf* out) {
-  if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64 || r->lane_class ||
-      r->mono_class || r->topk_mono || r->hier_class || r->topk_basic)
-    return MZGPU_E_INVALID;
-  MZ_CHECK_CTX(r->ctx);
-  r->ctx->stats.rows_in += rows->ub;
-  return reduce_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out);
 }
 
 // ------------------------------------------------------- reduce over several value columns
@@ -2868,13 +2857,27 @@ extern "C" int32_t mzgpu_reduce_lanes_row_bytes(uint32_t n_lanes, uint32_t* arr_
   return MZGPU_OK;
 }
 
+// The checks every lane constructor starts with: an output pointer, the lanes (n of them) and R32 / R40 input.
+static int32_t lane_args_check(mzgpu_ctx* ctx, const char* name, uint32_t in_row_bytes, const void* lanes, uint32_t n,
+                               mzgpu_reduce** out) {
+  if (out == nullptr || (lanes == nullptr && n) || (in_row_bytes != 32 && in_row_bytes != 40)) {
+    MZ_SET_ERR(ctx, "%s: bad arguments (input rows of %u bytes)", name, in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  return MZGPU_OK;
+}
+// Why a lane's field is not a bit-field of a value word of the input rows, or null when it is.
+static const char* value_field_bad(const mzgpu_field& f, uint32_t in_row_bytes) {
+  if (f.src != MZGPU_SRC_VAL1 && !(f.src == MZGPU_SRC_VAL2 && in_row_bytes == 40))
+    return "source word is not a value word of the input row";
+  if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64) return "field is empty or out of range";
+  return nullptr;
+}
+
 extern "C" int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
                                           uint32_t n_lanes, mzgpu_reduce** out) {
   MZ_CHECK_CTX(ctx);
-  if (out == nullptr || (lanes == nullptr && n_lanes) || (in_row_bytes != 32 && in_row_bytes != 40)) {
-    MZ_SET_ERR(ctx, "reduce_lanes: bad arguments (input rows of %u bytes)", in_row_bytes);
-    return MZGPU_E_INVALID;
-  }
+  MZ_TRY(lane_args_check(ctx, "reduce_lanes", in_row_bytes, lanes, n_lanes, out));
   if (n_lanes == 0 || n_lanes > MZGPU_MAX_ACCUM_LANES) {
     MZ_SET_ERR(ctx, "reduce_lanes: %u lanes (1..%d)", n_lanes, MZGPU_MAX_ACCUM_LANES);
     return MZGPU_E_INVALID;
@@ -2886,14 +2889,10 @@ extern "C" int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes,
     const int32_t base = L.kind & ~MZGPU_ACCUM_DISTINCT;
     const bool distinct = (L.kind & MZGPU_ACCUM_DISTINCT) != 0;
     const bool f64 = base == MZGPU_AGG_COUNT_SUM_F64;
-    const char* bad = nullptr;
+    const char* bad = value_field_bad(f, in_row_bytes);
     if (base != MZGPU_AGG_COUNT_SUM_I64 && !f64)
       bad = "kind is not COUNT_SUM_I64 / COUNT_SUM_F64, optionally | MZGPU_ACCUM_DISTINCT";
-    else if (f.src != MZGPU_SRC_VAL1 && !(f.src == MZGPU_SRC_VAL2 && in_row_bytes == 40))
-      bad = "source word is not a value word of the input row";
-    else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
-      bad = "field is empty or out of range";
-    else if (f64 && (f.shift != 0 || f.bits != 64))
+    else if (bad == nullptr && f64 && (f.shift != 0 || f.bits != 64))
       bad = "a float64 lane must pick a whole word";
     if (bad != nullptr) {
       MZ_SET_ERR(ctx, "reduce_lanes: lane %u: %s", l, bad);
@@ -2910,16 +2909,12 @@ extern "C" int32_t mzgpu_reduce_lanes_new(mzgpu_ctx* ctx, uint32_t in_row_bytes,
   }
   ls.n = n_lanes;
   ls.in_words = in_row_bytes / 8;
-  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
-  r->ctx = ctx;
-  r->lane_class = mz_lane_class(n_lanes);
+  const int c = mz_lane_class(n_lanes);
+  std::unique_ptr<mzgpu_reduce> r;
+  MZ_TRY(reduce_alloc(ctx, ReduceShape::LANES, (uint32_t)mz_lane_arr_bytes(c), &r));
+  r->cls = c;
   r->lanes = ls;
-  // class 1 runs the one-column kernels, which take the lane's kind (without the DISTINCT bit) as the
-  // aggregate kind
   r->agg_kind = (ls.f64_mask & 1u) ? MZGPU_AGG_COUNT_SUM_F64 : MZGPU_AGG_COUNT_SUM_I64;
-  const uint32_t rb = (uint32_t)mz_lane_arr_bytes(r->lane_class);
-  MZ_TRY(mzgpu_batcher_new(ctx, rb, &r->batcher));
-  MZ_TRY(mzgpu_spine_new(ctx, rb, 1, &r->input));
   for (uint32_t l = 0; l < n_lanes; ++l) {
     if (((ls.distinct_mask >> l) & 1u) == 0) continue;
     const int j = r->n_distinct++;
@@ -3053,35 +3048,6 @@ extern "C" mzgpu_spine* mzgpu_reduce_lanes_distinct_trace(mzgpu_reduce* r, uint3
   return nullptr;
 }
 
-static bool lanes_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out) {
-  return r->lane_class != 0 && in_rb == r->lanes.in_words * 8 && out->rb == (uint32_t)mz_lane_out_bytes(r->lane_class);
-}
-extern "C" int32_t mzgpu_reduce_lanes(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
-                                      mzgpu_buf* out) {
-  if (r == nullptr || out == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
-  mzgpu_ctx* ctx = r->ctx;
-  MZ_CHECK_CTX(ctx);
-  const uint32_t in_rb = r->lanes.in_words * 8;
-  if (!lanes_io_ok(r, in_rb, out)) {
-    MZ_SET_ERR(ctx, "reduce_lanes: output buffer of %u-byte rows", out->rb);
-    return MZGPU_E_INVALID;
-  }
-  DevMem in;
-  const u64* d_rows;
-  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
-  return reduce_dev(r, d_rows, dlen_imm(n), n, upper, out);
-}
-extern "C" int32_t mzgpu_reduce_lanes_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out) {
-  if (r == nullptr || rows == nullptr || out == nullptr) return MZGPU_E_INVALID;
-  MZ_CHECK_CTX(r->ctx);
-  if (!lanes_io_ok(r, rows->rb, out)) {
-    MZ_SET_ERR(r->ctx, "reduce_lanes: input rows of %u bytes / output rows of %u bytes", rows->rb, out->rb);
-    return MZGPU_E_INVALID;
-  }
-  r->ctx->stats.rows_in += rows->ub;
-  return reduce_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out);
-}
-
 // ------------------------------------------------------- monotonic MIN / MAX reduce
 extern "C" int32_t mzgpu_reduce_monotonic_row_bytes(uint32_t n_lanes, uint32_t* arr_row_bytes,
                                                     uint32_t* out_row_bytes) {
@@ -3096,11 +3062,8 @@ extern "C" int32_t mzgpu_reduce_monotonic_row_bytes(uint32_t n_lanes, uint32_t* 
 // in the messages): MZGPU_E_INVALID for a malformed descriptor, then MZGPU_E_UNSUPPORTED for a float64 lane.
 // Fills the lanes, their encodings (value ^ xm: every lane an unsigned max) and the value bits they read.
 static int32_t minmax_lanes(mzgpu_ctx* ctx, const char* what, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
-                            uint32_t n_lanes, LaneSet* ls_out, MonoXor* mx_out, u64* mask) {
-  if (in_row_bytes != 32 && in_row_bytes != 40) {
-    MZ_SET_ERR(ctx, "%s: bad arguments (input rows of %u bytes)", what, in_row_bytes);
-    return MZGPU_E_INVALID;
-  }
+                            uint32_t n_lanes, mzgpu_reduce** out, LaneSet* ls_out, MonoXor* mx_out, u64* mask) {
+  MZ_TRY(lane_args_check(ctx, what, in_row_bytes, lanes, n_lanes, out));
   if (n_lanes == 0 || n_lanes > MZGPU_MAX_ACCUM_LANES) {
     MZ_SET_ERR(ctx, "%s: %u lanes (1..%d)", what, n_lanes, MZGPU_MAX_ACCUM_LANES);
     return MZGPU_E_INVALID;
@@ -3113,13 +3076,9 @@ static int32_t minmax_lanes(mzgpu_ctx* ctx, const char* what, uint32_t in_row_by
     const mzgpu_accum_lane& L = lanes[l];
     const mzgpu_field& f = L.field;
     const int32_t base = L.kind & ~MZGPU_MONO_F64;
-    const char* bad = nullptr;
+    const char* bad = value_field_bad(f, in_row_bytes);
     if (base != MZGPU_AGG_MIN && base != MZGPU_AGG_MAX)
       bad = "kind is not MZGPU_AGG_MIN / MZGPU_AGG_MAX, optionally | MZGPU_MONO_F64";
-    else if (f.src != MZGPU_SRC_VAL1 && !(f.src == MZGPU_SRC_VAL2 && in_row_bytes == 40))
-      bad = "source word is not a value word of the input row";
-    else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
-      bad = "field is empty or out of range";
     if (bad != nullptr) {
       MZ_SET_ERR(ctx, "%s: lane %u: %s", what, l, bad);
       return MZGPU_E_INVALID;
@@ -3145,26 +3104,19 @@ static int32_t minmax_lanes(mzgpu_ctx* ctx, const char* what, uint32_t in_row_by
 extern "C" int32_t mzgpu_reduce_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
                                               uint32_t n_lanes, int32_t must_consolidate, mzgpu_reduce** out) {
   MZ_CHECK_CTX(ctx);
-  if (out == nullptr || (lanes == nullptr && n_lanes)) {
-    MZ_SET_ERR(ctx, "reduce_monotonic: bad arguments (input rows of %u bytes)", in_row_bytes);
-    return MZGPU_E_INVALID;
-  }
   LaneSet ls;
   MonoXor mx;
   u64 mask[2];
-  MZ_TRY(minmax_lanes(ctx, "reduce_monotonic", in_row_bytes, lanes, n_lanes, &ls, &mx, mask));
-  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
-  r->ctx = ctx;
-  r->agg_kind = -1;
-  r->mono_class = mz_mono_class(n_lanes);
+  MZ_TRY(minmax_lanes(ctx, "reduce_monotonic", in_row_bytes, lanes, n_lanes, out, &ls, &mx, mask));
+  const int c = mz_mono_class(n_lanes);
+  std::unique_ptr<mzgpu_reduce> r;
+  MZ_TRY(reduce_alloc(ctx, ReduceShape::MONOTONIC, (uint32_t)mz_mono_arr_bytes(c), &r));
+  r->cls = c;
   r->lanes = ls;
   r->mono = mx;
   r->must_consolidate = must_consolidate != 0;
   r->mono_mask[0] = mask[0];
   r->mono_mask[1] = mask[1];
-  const uint32_t rb = (uint32_t)mz_mono_arr_bytes(r->mono_class);
-  MZ_TRY(mzgpu_batcher_new(ctx, rb, &r->batcher));
-  MZ_TRY(mzgpu_spine_new(ctx, rb, 1, &r->input));
   *out = r.release();
   return MZGPU_OK;
 }
@@ -3174,7 +3126,7 @@ static int32_t monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_u
                              mzgpu_buf* errs) {
   mzgpu_ctx* ctx = r->ctx;
   MZ_TRY(reduce_begin(r));
-  const int c = r->mono_class;
+  const int c = r->cls;
   if (n_ub) {
     const u32 iw = r->lanes.in_words;
     DevMem masked, cons;
@@ -3190,9 +3142,7 @@ static int32_t monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_u
       if (clen.known) n_ub = clen.v[0];
     }
     Seg s;
-    DevMem erows, econs;
-    Lazy4 elen;
-    u64 ecap = 0;
+    DevMem erows;
     MZ_TRY(s.rows.alloc(ctx, n_ub * mz_mono_arr_bytes(c)));
     MZ_TRY(erows.alloc(ctx, n_ub * 16));
     MZ_TRY(s.len.make_pending(ctx));
@@ -3201,16 +3151,13 @@ static int32_t monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_u
     s.len.mark_written();
     s.ub = n_ub;
     // the rejected rows' error collection: (time, number of rejected rows)
-    MZ_TRY(consolidate_dev(ctx, 16, erows.p, dlen_of(s.len, 1), n_ub, &econs, &ecap, &elen));
-    MZ_TRY(buf_append_dev(errs, econs.p, dlen_of(elen, 0), elen.known ? elen.v[0] : n_ub));
+    MZ_TRY(append_consolidated(ctx, 16, erows.p, dlen_of(s.len, 1), n_ub, errs));
     MZ_TRY(batcher_push_seg(r->batcher, std::move(s)));
   }
   mzgpu_batch* batch = nullptr;
   MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
-  std::vector<mzgpu_batch*> prior;
-  r->input->all_batches(prior);
   TraceView tv;
-  int32_t st = trace_view(ctx, prior, &tv);
+  int32_t st = trace_view_of(r->input, &tv);
   const u64 b_ub = batch->len_ub;
   const u64 out_rb = (u64)mz_mono_out_bytes(c);
   if (st == MZGPU_OK && b_ub > 0) {
@@ -3238,62 +3185,22 @@ static int32_t monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_u
   return reduce_seal_tail(r, batch, st);
 }
 
-static bool monotonic_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
-  return r->mono_class != 0 && in_rb == r->lanes.in_words * 8 && out->rb == (uint32_t)mz_mono_out_bytes(r->mono_class) &&
-         errs->rb == 16 && out != errs;
-}
-extern "C" int32_t mzgpu_reduce_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
-                                          mzgpu_buf* out, mzgpu_buf* errs) {
-  if (r == nullptr || out == nullptr || errs == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
-  mzgpu_ctx* ctx = r->ctx;
-  MZ_CHECK_CTX(ctx);
-  const uint32_t in_rb = r->lanes.in_words * 8;
-  if (!monotonic_io_ok(r, in_rb, out, errs)) {
-    MZ_SET_ERR(ctx, "reduce_monotonic: output buffer of %u-byte rows / error buffer of %u-byte rows", out->rb,
-               errs->rb);
-    return MZGPU_E_INVALID;
-  }
-  DevMem in;
-  const u64* d_rows;
-  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
-  return monotonic_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
-}
-extern "C" int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
-                                              mzgpu_buf* errs) {
-  if (r == nullptr || rows == nullptr || out == nullptr || errs == nullptr) return MZGPU_E_INVALID;
-  MZ_CHECK_CTX(r->ctx);
-  if (!monotonic_io_ok(r, rows->rb, out, errs)) {
-    MZ_SET_ERR(r->ctx, "reduce_monotonic: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes",
-               rows->rb, out->rb, errs->rb);
-    return MZGPU_E_INVALID;
-  }
-  r->ctx->stats.rows_in += rows->ub;
-  return monotonic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
-}
-
 // ------------------------------------------------------- hierarchical MIN / MAX reduce
 extern "C" int32_t mzgpu_reduce_hierarchical_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_accum_lane* lanes,
                                                  uint32_t n_lanes, mzgpu_reduce** out) {
   MZ_CHECK_CTX(ctx);
-  if (out == nullptr || (lanes == nullptr && n_lanes)) {
-    MZ_SET_ERR(ctx, "reduce_hierarchical: bad arguments (input rows of %u bytes)", in_row_bytes);
-    return MZGPU_E_INVALID;
-  }
   LaneSet ls;
   MonoXor mx;
   u64 mask[2];
-  MZ_TRY(minmax_lanes(ctx, "reduce_hierarchical", in_row_bytes, lanes, n_lanes, &ls, &mx, mask));
-  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
-  r->ctx = ctx;
-  r->agg_kind = -1;
-  r->hier_class = mz_mono_class(n_lanes);
+  MZ_TRY(minmax_lanes(ctx, "reduce_hierarchical", in_row_bytes, lanes, n_lanes, out, &ls, &mx, mask));
+  std::unique_ptr<mzgpu_reduce> r;
+  // the arrangement holds the masked input rows themselves, with ordinary SUM diffs
+  MZ_TRY(reduce_alloc(ctx, ReduceShape::HIERARCHICAL, in_row_bytes, &r));
+  r->cls = mz_mono_class(n_lanes);
   r->lanes = ls;
   r->mono = mx;
   r->mono_mask[0] = mask[0];
   r->mono_mask[1] = mask[1];
-  // the arrangement holds the masked input rows themselves, with ordinary SUM diffs
-  MZ_TRY(mzgpu_batcher_new(ctx, in_row_bytes, &r->batcher));
-  MZ_TRY(mzgpu_spine_new(ctx, in_row_bytes, 1, &r->input));
   *out = r.release();
   return MZGPU_OK;
 }
@@ -3304,35 +3211,25 @@ static int32_t hierarchical_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 
                                 mzgpu_buf* errs) {
   mzgpu_ctx* ctx = r->ctx;
   MZ_TRY(reduce_begin(r));
-  const int c = r->hier_class;
+  const int c = r->cls;
   const u32 iw = r->lanes.in_words;
   if (n_ub) {
     // (key, the bits the lanes read, time, diff): rows that differ only in unread bits are one value row
     Seg s;
     MZ_TRY(s.rows.alloc(ctx, n_ub * iw * 8));
     MZ_TRY(mz_monotonic_mask(ctx, d_rows, n, n_ub, iw, r->mono_mask[0], r->mono_mask[1], s.rows.as<u64>()));
-    if (n.p == nullptr) {
-      s.len.set(ctx, n.imm);
-      s.ub = n.imm;
-    } else {
-      MZ_TRY(s.len.make_pending(ctx));
-      MZ_CUDA(ctx, cudaMemcpyAsync(s.len.dptr(), n.p, 8, cudaMemcpyDeviceToDevice, ctx->stream));
-      s.len.mark_written();
-      s.ub = n_ub;
-    }
+    MZ_TRY(seg_len_of_input(ctx, n, n_ub, &s));
     MZ_TRY(batcher_push_seg(r->batcher, std::move(s)));
   }
   mzgpu_batch* batch = nullptr;
   MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
-  std::vector<mzgpu_batch*> prior;
-  r->input->all_batches(prior);
   TraceView tv;
-  int32_t st = trace_view(ctx, prior, &tv);
+  int32_t st = trace_view_of(r->input, &tv);
   const u64 b_ub = batch->len_ub;
   if (st == MZGPU_OK && b_ub > 0) {
-    DevMem corr, erows, econs;
-    Lazy4 elen, eflen;
-    u64 ecap = 0, e_ub = b_ub;
+    DevMem corr, erows;
+    Lazy4 elen;
+    u64 e_ub = b_ub;
     st = elen.make_pending(ctx);
     if (single_pass_fits(b_ub, 2)) {  // (the bound alone: a loose one takes the two-pass form)
       Lazy4 clen;
@@ -3360,45 +3257,9 @@ static int32_t hierarchical_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 
       if (st == MZGPU_OK && n_corr) st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
     }
     // the error rows leave the kernel unordered: (key, 0, time, +-1), at most one per key and time
-    if (st == MZGPU_OK && e_ub > 0) st = consolidate_dev(ctx, 32, erows.p, dlen_of(elen, 0), e_ub, &econs, &ecap, &eflen);
-    if (st == MZGPU_OK && e_ub > 0)
-      st = buf_append_dev(errs, econs.p, dlen_of(eflen, 0), eflen.known ? eflen.v[0] : e_ub);
+    if (st == MZGPU_OK) st = append_consolidated(ctx, 32, erows.p, dlen_of(elen, 0), e_ub, errs);
   }
   return reduce_seal_tail(r, batch, st);
-}
-
-static bool hierarchical_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
-  return r->hier_class != 0 && in_rb == r->lanes.in_words * 8 && out->rb == (uint32_t)mz_mono_out_bytes(r->hier_class) &&
-         errs->rb == 32 && out != errs;
-}
-extern "C" int32_t mzgpu_reduce_hierarchical(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem,
-                                             uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs) {
-  if (r == nullptr || out == nullptr || errs == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
-  mzgpu_ctx* ctx = r->ctx;
-  MZ_CHECK_CTX(ctx);
-  const uint32_t in_rb = r->lanes.in_words * 8;
-  if (!hierarchical_io_ok(r, in_rb, out, errs)) {
-    MZ_SET_ERR(ctx, "reduce_hierarchical: output buffer of %u-byte rows / error buffer of %u-byte rows", out->rb,
-               errs->rb);
-    return MZGPU_E_INVALID;
-  }
-  DevMem in;
-  const u64* d_rows;
-  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
-  return hierarchical_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
-}
-extern "C" int32_t mzgpu_reduce_hierarchical_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
-                                                 mzgpu_buf* errs) {
-  if (r == nullptr || rows == nullptr || out == nullptr || errs == nullptr) return MZGPU_E_INVALID;
-  MZ_CHECK_CTX(r->ctx);
-  if (!hierarchical_io_ok(r, rows->rb, out, errs)) {
-    MZ_SET_ERR(r->ctx,
-               "reduce_hierarchical: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes",
-               rows->rb, out->rb, errs->rb);
-    return MZGPU_E_INVALID;
-  }
-  r->ctx->stats.rows_in += rows->ub;
-  return hierarchical_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
 }
 
 // ------------------------------------------------------- monotonic TopK
@@ -3406,10 +3267,7 @@ extern "C" int32_t mzgpu_reduce_hierarchical_buf(mzgpu_reduce* r, mzgpu_buf* row
 // descriptor, then MZGPU_E_UNSUPPORTED for a float64 lane or a negative limit) into *to.
 static int32_t topk_order(mzgpu_ctx* ctx, const char* name, uint32_t in_row_bytes, const mzgpu_order_lane* order,
                           uint32_t n_order, int64_t limit, mzgpu_reduce** out, TopKOrder* to_out) {
-  if (out == nullptr || (order == nullptr && n_order) || (in_row_bytes != 32 && in_row_bytes != 40)) {
-    MZ_SET_ERR(ctx, "%s: bad arguments (input rows of %u bytes)", name, in_row_bytes);
-    return MZGPU_E_INVALID;
-  }
+  MZ_TRY(lane_args_check(ctx, name, in_row_bytes, order, n_order, out));
   if (n_order > MZGPU_MAX_ORDER_LANES) {
     MZ_SET_ERR(ctx, "%s: %u order lanes (0..%d)", name, n_order, MZGPU_MAX_ORDER_LANES);
     return MZGPU_E_INVALID;
@@ -3419,13 +3277,8 @@ static int32_t topk_order(mzgpu_ctx* ctx, const char* name, uint32_t in_row_byte
   for (uint32_t j = 0; j < n_order; ++j) {
     const mzgpu_order_lane& L = order[j];
     const mzgpu_field& f = L.field;
-    const char* bad = nullptr;
-    if ((L.flags & ~(uint32_t)MZGPU_ORDER_F64) != 0)
-      bad = "unknown flag bits";
-    else if (f.src != MZGPU_SRC_VAL1 && !(f.src == MZGPU_SRC_VAL2 && in_row_bytes == 40))
-      bad = "source word is not a value word of the input row";
-    else if (f.bits == 0 || f.bits > 64 || f.shift > 63 || (u32)f.shift + f.bits > 64)
-      bad = "field is empty or out of range";
+    const char* bad = value_field_bad(f, in_row_bytes);
+    if ((L.flags & ~(uint32_t)MZGPU_ORDER_F64) != 0) bad = "unknown flag bits";
     if (bad != nullptr) {
       MZ_SET_ERR(ctx, "%s: order lane %u: %s", name, j, bad);
       return MZGPU_E_INVALID;
@@ -3457,14 +3310,10 @@ extern "C" int32_t mzgpu_topk_monotonic_new(mzgpu_ctx* ctx, uint32_t in_row_byte
   MZ_CHECK_CTX(ctx);
   TopKOrder to;
   MZ_TRY(topk_order(ctx, "topk_monotonic", in_row_bytes, order, n_order, limit, out, &to));
-  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
-  r->ctx = ctx;
-  r->agg_kind = -1;
-  r->topk_mono = true;
+  std::unique_ptr<mzgpu_reduce> r;
+  MZ_TRY(reduce_alloc(ctx, ReduceShape::TOPK_MONOTONIC, MZGPU_ROW_RTOPK, &r));
   r->tko = to;
   r->must_consolidate = must_consolidate != 0;
-  MZ_TRY(mzgpu_batcher_new(ctx, MZGPU_ROW_RTOPK, &r->batcher));
-  MZ_TRY(mzgpu_spine_new(ctx, MZGPU_ROW_RTOPK, 1, &r->input));
   *out = r.release();
   return MZGPU_OK;
 }
@@ -3488,25 +3337,22 @@ static int32_t topk_monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u6
       n = dlen_of(clen, 0);
       if (clen.known) n_ub = clen.v[0];
     }
-    DevMem arr, erows, econs, sorted;
-    Lazy4 alen, elen, slen;
-    u64 ecap = 0, scap = 0;
+    DevMem arr, erows, sorted;
+    Lazy4 alen, slen;
+    u64 scap = 0;
     MZ_TRY(arr.alloc(ctx, n_ub * RB));
     MZ_TRY(erows.alloc(ctx, n_ub * 16));
     MZ_TRY(alen.make_pending(ctx));
     MZ_TRY(mz_topk_explode(ctx, d_rows, n, n_ub, to, arr.as<u64>(), erows.as<u64>(), alen.dptr()));
     alen.mark_written();
     // the rejected rows' error collection: (time, number of rejected rows)
-    MZ_TRY(consolidate_dev(ctx, 16, erows.p, dlen_of(alen, 1), n_ub, &econs, &ecap, &elen));
-    MZ_TRY(buf_append_dev(errs, econs.p, dlen_of(elen, 0), elen.known ? elen.v[0] : n_ub));
+    MZ_TRY(append_consolidated(ctx, 16, erows.p, dlen_of(alen, 1), n_ub, errs));
     // the kept rows sorted and consolidated by (key, order, row, time); never arranged themselves
     MZ_TRY(consolidate_dev(ctx, (int)RB, arr.p, dlen_of(alen, 0), n_ub, &sorted, &scap, &slen));
     arr.release();
     const u64 s_ub = slen.known ? slen.v[0] : n_ub;
-    std::vector<mzgpu_batch*> prior;
-    r->input->all_batches(prior);
     TraceView tv;
-    MZ_TRY(trace_view(ctx, prior, &tv));
+    MZ_TRY(trace_view_of(r->input, &tv));
     // Output bound of one new row of multiplicity m: it enters at most once, and the units it adds evict or
     // cut at most min(m, limit) rows, so 1 + limit rows per new row (exactly one without a limit).
     const i64 L = to.limit;
@@ -3549,38 +3395,6 @@ static int32_t topk_monotonic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u6
   return reduce_seal_tail(r, batch, MZGPU_OK);
 }
 
-static bool topk_monotonic_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
-  return r->topk_mono && in_rb == r->tko.in_words * 8 && out->rb == in_rb && errs->rb == 16 && out != errs;
-}
-extern "C" int32_t mzgpu_topk_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
-                                        mzgpu_buf* out, mzgpu_buf* errs) {
-  if (r == nullptr || out == nullptr || errs == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
-  mzgpu_ctx* ctx = r->ctx;
-  MZ_CHECK_CTX(ctx);
-  const uint32_t in_rb = r->tko.in_words * 8;
-  if (!topk_monotonic_io_ok(r, in_rb, out, errs)) {
-    MZ_SET_ERR(ctx, "topk_monotonic: output buffer of %u-byte rows / error buffer of %u-byte rows", out->rb,
-               errs->rb);
-    return MZGPU_E_INVALID;
-  }
-  DevMem in;
-  const u64* d_rows;
-  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
-  return topk_monotonic_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
-}
-extern "C" int32_t mzgpu_topk_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
-                                            mzgpu_buf* errs) {
-  if (r == nullptr || rows == nullptr || out == nullptr || errs == nullptr) return MZGPU_E_INVALID;
-  MZ_CHECK_CTX(r->ctx);
-  if (!topk_monotonic_io_ok(r, rows->rb, out, errs)) {
-    MZ_SET_ERR(r->ctx, "topk_monotonic: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes",
-               rows->rb, out->rb, errs->rb);
-    return MZGPU_E_INVALID;
-  }
-  r->ctx->stats.rows_in += rows->ub;
-  return topk_monotonic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
-}
-
 // ------------------------------------------------------- basic TopK
 extern "C" int32_t mzgpu_topk_basic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, const mzgpu_order_lane* order,
                                         uint32_t n_order, int64_t limit, uint64_t offset, mzgpu_reduce** out) {
@@ -3592,15 +3406,11 @@ extern "C" int32_t mzgpu_topk_basic_new(mzgpu_ctx* ctx, uint32_t in_row_bytes, c
                (unsigned long long)offset, (long long)limit);
     return MZGPU_E_UNSUPPORTED;
   }
-  std::unique_ptr<mzgpu_reduce> r(new mzgpu_reduce());
-  r->ctx = ctx;
-  r->agg_kind = -1;
-  r->topk_basic = true;
+  std::unique_ptr<mzgpu_reduce> r;
+  MZ_TRY(reduce_alloc(ctx, ReduceShape::TOPK_BASIC, MZGPU_ROW_RTOPK, &r));
   r->tko = to;
   // (no count reaches 2^63: an offset past it leaves every window empty, as INT64_MAX does)
   r->topk_offset = (i64)std::min<u64>(offset, (u64)INT64_MAX);
-  MZ_TRY(mzgpu_batcher_new(ctx, MZGPU_ROW_RTOPK, &r->batcher));
-  MZ_TRY(mzgpu_spine_new(ctx, MZGPU_ROW_RTOPK, 1, &r->input));
   MZ_TRY(mzgpu_batcher_new(ctx, 32, &r->neg_batcher));
   MZ_TRY(mzgpu_spine_new(ctx, 32, 1, &r->negs));
   *out = r.release();
@@ -3620,31 +3430,20 @@ static int32_t topk_basic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_
     Seg s;
     MZ_TRY(s.rows.alloc(ctx, n_ub * MZGPU_ROW_RTOPK));
     MZ_TRY(mz_topk_basic_explode(ctx, d_rows, n, n_ub, to, s.rows.as<u64>()));
-    if (n.p == nullptr) {
-      s.len.set(ctx, n.imm);
-      s.ub = n.imm;
-    } else {
-      MZ_TRY(s.len.make_pending(ctx));
-      MZ_CUDA(ctx, cudaMemcpyAsync(s.len.dptr(), n.p, 8, cudaMemcpyDeviceToDevice, ctx->stream));
-      s.len.mark_written();
-      s.ub = n_ub;
-    }
+    MZ_TRY(seg_len_of_input(ctx, n, n_ub, &s));
     MZ_TRY(batcher_push_seg(r->batcher, std::move(s)));
   }
   mzgpu_batch* batch = nullptr;
   MZ_TRY(batcher_seal(r->batcher, upper, &batch, nullptr));
-  std::vector<mzgpu_batch*> prior, nprior;
-  r->input->all_batches(prior);
-  r->negs->all_batches(nprior);
   TraceView tv, nv;
-  int32_t st = trace_view(ctx, prior, &tv);
-  if (st == MZGPU_OK) st = trace_view(ctx, nprior, &nv);
+  int32_t st = trace_view_of(r->input, &tv);
+  if (st == MZGPU_OK) st = trace_view_of(r->negs, &nv);
   const u64 b_ub = batch->len_ub;
   Seg ns;  // the negatives deltas: the negatives batcher's new rows
   if (st == MZGPU_OK && b_ub > 0) {
-    DevMem corr, erows, econs;
-    Lazy4 slen, eflen;  // slen: [0] error rows, [1] negatives rows
-    u64 ecap = 0, s_ub = b_ub;
+    DevMem corr, erows;
+    Lazy4 slen;  // [0] error rows, [1] negatives rows
+    u64 s_ub = b_ub;
     st = slen.make_pending(ctx);
     // Output rows per new row, finite limit: a change at one new time of a key is a row whose share of the
     // window differs between the previous and the current time, so it holds a unit of the old window or of the
@@ -3681,10 +3480,7 @@ static int32_t topk_basic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_
       if (st == MZGPU_OK && n_corr) st = buf_append_dev(out, corr.p, dlen_imm(n_corr), n_corr);
     }
     // the error rows leave the kernel unordered: (key, 0, time, +-1), at most one per key and time
-    if (st == MZGPU_OK && s_ub > 0)
-      st = consolidate_dev(ctx, 32, erows.p, dlen_of(slen, 0), s_ub, &econs, &ecap, &eflen);
-    if (st == MZGPU_OK && s_ub > 0)
-      st = buf_append_dev(errs, econs.p, dlen_of(eflen, 0), eflen.known ? eflen.v[0] : s_ub);
+    if (st == MZGPU_OK) st = append_consolidated(ctx, 32, erows.p, dlen_of(slen, 0), s_ub, errs);
     // the negatives deltas, unordered too: the seal below sorts and consolidates them
     if (st == MZGPU_OK && s_ub > 0) {
       ns.len = std::move(slen);
@@ -3705,35 +3501,152 @@ static int32_t topk_basic_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_
   return reduce_seal_tail(r, batch, nst);
 }
 
-static bool topk_basic_io_ok(mzgpu_reduce* r, uint32_t in_rb, mzgpu_buf* out, mzgpu_buf* errs) {
-  return r->topk_basic && in_rb == r->tko.in_words * 8 && out->rb == in_rb && errs->rb == 32 && out != errs;
+// ------------------------------------------------------- step entry points
+// The rows one step of an operator of `shape` takes: its name in messages, the input and output row bytes (r's
+// own; meaningful when r has that shape) and the error row bytes (0: no error buffer).
+struct ReduceIo {
+  const char* name;
+  uint32_t in_rb, out_rb, errs_rb;
+};
+static ReduceIo reduce_io(ReduceShape shape, const mzgpu_reduce* r) {
+  const uint32_t lanes_in = r->lanes.in_words * 8, order_in = r->tko.in_words * 8;
+  switch (shape) {
+    case ReduceShape::ACCUM: return {"reduce_accumulable", 32, 64, 0};
+    case ReduceShape::LANES: return {"reduce_lanes", lanes_in, (uint32_t)mz_lane_out_bytes(r->cls), 0};
+    case ReduceShape::MONOTONIC: return {"reduce_monotonic", lanes_in, (uint32_t)mz_mono_out_bytes(r->cls), 16};
+    case ReduceShape::HIERARCHICAL: return {"reduce_hierarchical", lanes_in, (uint32_t)mz_mono_out_bytes(r->cls), 32};
+    case ReduceShape::TOPK_MONOTONIC: return {"topk_monotonic", order_in, order_in, 16};
+    case ReduceShape::TOPK_BASIC: return {"topk_basic", order_in, order_in, 32};
+  }
+  return {};
+}
+
+// MZGPU_E_INVALID with the entry point's message unless r has `shape` and the input rows, out and errs (a second
+// buffer) have its widths.  `rows` is the buffer form's input, null in the host form (rows of the operator's
+// own width).
+static int32_t reduce_io_check(const ReduceIo& io, ReduceShape shape, mzgpu_reduce* r, const mzgpu_buf* rows,
+                               const mzgpu_buf* out, const mzgpu_buf* errs) {
+  if (r->shape == shape && (rows == nullptr || rows->rb == io.in_rb) && out->rb == io.out_rb &&
+      (io.errs_rb == 0 || (errs->rb == io.errs_rb && out != errs)))
+    return MZGPU_OK;
+  mzgpu_ctx* ctx = r->ctx;
+  if (rows == nullptr && io.errs_rb)
+    MZ_SET_ERR(ctx, "%s: output buffer of %u-byte rows / error buffer of %u-byte rows", io.name, out->rb, errs->rb);
+  else if (rows == nullptr)
+    MZ_SET_ERR(ctx, "%s: output buffer of %u-byte rows", io.name, out->rb);
+  else if (io.errs_rb)
+    MZ_SET_ERR(ctx, "%s: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes", io.name,
+               rows->rb, out->rb, errs->rb);
+  else
+    MZ_SET_ERR(ctx, "%s: input rows of %u bytes / output rows of %u bytes", io.name, rows->rb, out->rb);
+  return MZGPU_E_INVALID;
+}
+
+// One activation of r over device rows, by its shape.
+static int32_t reduce_step_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n_ub, u64 upper, mzgpu_buf* out,
+                               mzgpu_buf* errs) {
+  switch (r->shape) {
+    case ReduceShape::ACCUM:
+    case ReduceShape::LANES: return reduce_dev(r, d_rows, n, n_ub, upper, out);
+    case ReduceShape::MONOTONIC: return monotonic_dev(r, d_rows, n, n_ub, upper, out, errs);
+    case ReduceShape::HIERARCHICAL: return hierarchical_dev(r, d_rows, n, n_ub, upper, out, errs);
+    case ReduceShape::TOPK_MONOTONIC: return topk_monotonic_dev(r, d_rows, n, n_ub, upper, out, errs);
+    case ReduceShape::TOPK_BASIC: return topk_basic_dev(r, d_rows, n, n_ub, upper, out, errs);
+  }
+  return MZGPU_E_INVALID;
+}
+
+// The rows of a host-form reduce entry point (n rows of in_rb bytes) counted into rows_in and, when they are in
+// host memory, uploaded into `in`; *d_rows is where the activation reads them.
+static int32_t reduce_rows_in(mzgpu_ctx* ctx, const void* rows, uint64_t n, int32_t mem, uint32_t in_rb, DevMem* in,
+                              const u64** d_rows) {
+  ctx->stats.rows_in += n;
+  *d_rows = (const u64*)rows;
+  if (mem == MZGPU_MEM_HOST && n) {
+    MZ_TRY(in->alloc(ctx, n * in_rb));
+    MZ_TRY(copy_in(ctx, in->p, rows, n * in_rb, mem));
+    *d_rows = in->as<u64>();
+  }
+  return MZGPU_OK;
+}
+
+// The host form of a step: n rows of the operator's input width in `mem`.
+static int32_t reduce_step(ReduceShape shape, mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem,
+                           uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs) {
+  if (r == nullptr || out == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
+  const ReduceIo io = reduce_io(shape, r);
+  if (io.errs_rb && errs == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(r->ctx);
+  MZ_TRY(reduce_io_check(io, shape, r, nullptr, out, errs));
+  DevMem in;
+  const u64* d_rows;
+  MZ_TRY(reduce_rows_in(r->ctx, rows, n, mem, io.in_rb, &in, &d_rows));
+  return reduce_step_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
+}
+// The buffer form of a step: the rows of a device buffer, read without waiting for its length.
+static int32_t reduce_step_buf(ReduceShape shape, mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                               mzgpu_buf* errs) {
+  if (r == nullptr || rows == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  const ReduceIo io = reduce_io(shape, r);
+  if (io.errs_rb && errs == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(r->ctx);
+  MZ_TRY(reduce_io_check(io, shape, r, rows, out, errs));
+  r->ctx->stats.rows_in += rows->ub;
+  return reduce_step_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
+}
+
+// The accumulable forms refuse a misuse without a message, and before a sticky context reports its own status.
+extern "C" int32_t mzgpu_reduce_accumulable(mzgpu_reduce* r, const mzgpu_r32* rows, uint64_t n,
+                                            int32_t mem, uint64_t upper, mzgpu_buf* out) {
+  if (r == nullptr || out == nullptr || (rows == nullptr && n) || out->rb != 64 || r->shape != ReduceShape::ACCUM)
+    return MZGPU_E_INVALID;
+  return reduce_step(ReduceShape::ACCUM, r, rows, n, mem, upper, out, nullptr);
+}
+extern "C" int32_t mzgpu_reduce_accumulable_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper,
+                                                mzgpu_buf* out) {
+  if (r == nullptr || rows == nullptr || out == nullptr || rows->rb != 32 || out->rb != 64 ||
+      r->shape != ReduceShape::ACCUM)
+    return MZGPU_E_INVALID;
+  return reduce_step_buf(ReduceShape::ACCUM, r, rows, upper, out, nullptr);
+}
+extern "C" int32_t mzgpu_reduce_lanes(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                      mzgpu_buf* out) {
+  return reduce_step(ReduceShape::LANES, r, rows, n, mem, upper, out, nullptr);
+}
+extern "C" int32_t mzgpu_reduce_lanes_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out) {
+  return reduce_step_buf(ReduceShape::LANES, r, rows, upper, out, nullptr);
+}
+extern "C" int32_t mzgpu_reduce_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                          mzgpu_buf* out, mzgpu_buf* errs) {
+  return reduce_step(ReduceShape::MONOTONIC, r, rows, n, mem, upper, out, errs);
+}
+extern "C" int32_t mzgpu_reduce_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                              mzgpu_buf* errs) {
+  return reduce_step_buf(ReduceShape::MONOTONIC, r, rows, upper, out, errs);
+}
+extern "C" int32_t mzgpu_reduce_hierarchical(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem,
+                                             uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs) {
+  return reduce_step(ReduceShape::HIERARCHICAL, r, rows, n, mem, upper, out, errs);
+}
+extern "C" int32_t mzgpu_reduce_hierarchical_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                                 mzgpu_buf* errs) {
+  return reduce_step_buf(ReduceShape::HIERARCHICAL, r, rows, upper, out, errs);
+}
+extern "C" int32_t mzgpu_topk_monotonic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
+                                        mzgpu_buf* out, mzgpu_buf* errs) {
+  return reduce_step(ReduceShape::TOPK_MONOTONIC, r, rows, n, mem, upper, out, errs);
+}
+extern "C" int32_t mzgpu_topk_monotonic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
+                                            mzgpu_buf* errs) {
+  return reduce_step_buf(ReduceShape::TOPK_MONOTONIC, r, rows, upper, out, errs);
 }
 extern "C" int32_t mzgpu_topk_basic(mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem, uint64_t upper,
                                     mzgpu_buf* out, mzgpu_buf* errs) {
-  if (r == nullptr || out == nullptr || errs == nullptr || (rows == nullptr && n)) return MZGPU_E_INVALID;
-  mzgpu_ctx* ctx = r->ctx;
-  MZ_CHECK_CTX(ctx);
-  const uint32_t in_rb = r->tko.in_words * 8;
-  if (!topk_basic_io_ok(r, in_rb, out, errs)) {
-    MZ_SET_ERR(ctx, "topk_basic: output buffer of %u-byte rows / error buffer of %u-byte rows", out->rb, errs->rb);
-    return MZGPU_E_INVALID;
-  }
-  DevMem in;
-  const u64* d_rows;
-  MZ_TRY(reduce_rows_in(ctx, rows, n, mem, in_rb, &in, &d_rows));
-  return topk_basic_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
+  return reduce_step(ReduceShape::TOPK_BASIC, r, rows, n, mem, upper, out, errs);
 }
 extern "C" int32_t mzgpu_topk_basic_buf(mzgpu_reduce* r, mzgpu_buf* rows, uint64_t upper, mzgpu_buf* out,
                                         mzgpu_buf* errs) {
-  if (r == nullptr || rows == nullptr || out == nullptr || errs == nullptr) return MZGPU_E_INVALID;
-  MZ_CHECK_CTX(r->ctx);
-  if (!topk_basic_io_ok(r, rows->rb, out, errs)) {
-    MZ_SET_ERR(r->ctx, "topk_basic: input rows of %u bytes / output rows of %u bytes / error rows of %u bytes",
-               rows->rb, out->rb, errs->rb);
-    return MZGPU_E_INVALID;
-  }
-  r->ctx->stats.rows_in += rows->ub;
-  return topk_basic_dev(r, rows->mem.as<u64>(), buf_dlen(rows), rows->ub, upper, out, errs);
+  return reduce_step_buf(ReduceShape::TOPK_BASIC, r, rows, upper, out, errs);
 }
 
 // ============================================================ Row keys as words (f1, first step)
@@ -4890,16 +4803,6 @@ static int32_t mfp_flush_pending(mzgpu_mfp_op* op) {
   return MZGPU_OK;
 }
 
-// append `n` device rows (count on the device, bound ub) to `dst`, consolidated
-static int32_t mfp_emit(mzgpu_ctx* ctx, int rb, const u64* d_rows, DLen n, u64 ub, mzgpu_buf* dst) {
-  if (ub == 0) return MZGPU_OK;
-  DevMem cons;
-  u64 cap = 0;
-  Lazy4 len;
-  MZ_TRY(consolidate_dev(ctx, rb, d_rows, n, ub, &cons, &cap, &len));
-  return buf_append_dev(dst, cons.p, dlen_of(len, 0), std::min(cap, ub));
-}
-
 // the checks of a step, before it changes anything
 static int32_t mfp_step_check(mzgpu_mfp_op* op, u64 upper, mzgpu_buf* out, mzgpu_buf* errs) {
   mzgpu_ctx* ctx = op->ctx;
@@ -4940,7 +4843,7 @@ static int32_t mfp_step_end(mzgpu_mfp_op* op, const std::shared_ptr<MfpSeg>& rea
     const u64 zero = 0;
     MZ_TRY(mfp_partition(op, rel, &zero, 1, &all, tot.dptr(), false));
     tot.mark_written();
-    MZ_TRY(mfp_emit(ctx, op->ow, all->base() + MZ_MFP_HDR, dlen_of(tot, 0), all->ub, out));
+    MZ_TRY(append_consolidated(ctx, op->ow, all->base() + MZ_MFP_HDR, dlen_of(tot, 0), all->ub, out));
   }
   rel.clear();
   // 4. restore the chain; 5. hold the rest (inserted by the next step or read)
@@ -4950,7 +4853,7 @@ static int32_t mfp_step_end(mzgpu_mfp_op* op, const std::shared_ptr<MfpSeg>& rea
     op->pending.push_back(held);
   }
   // 6. errors
-  if (err_ub > 0) MZ_TRY(mfp_emit(ctx, 32, err_rows, err_len, err_ub, errs));
+  if (err_ub > 0) MZ_TRY(append_consolidated(ctx, 32, err_rows, err_len, err_ub, errs));
   cudaEvent_t ev;
   MZ_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   MZ_CUDA(ctx, cudaEventRecord(ev, ctx->stream));
