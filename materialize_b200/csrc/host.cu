@@ -382,6 +382,20 @@ static int32_t copy_out(mzgpu_ctx* ctx, void* dst, const void* d_src, size_t byt
   return MZGPU_OK;
 }
 
+// The rows of a host-form entry point (n rows of in_rb bytes) counted into rows_in and, when they are in host
+// memory, uploaded into `in`; *d_rows is where the operator reads them.
+static int32_t entry_rows_in(mzgpu_ctx* ctx, const void* rows, uint64_t n, int32_t mem, uint32_t in_rb, DevMem* in,
+                             const u64** d_rows) {
+  ctx->stats.rows_in += n;
+  *d_rows = (const u64*)rows;
+  if (mem == MZGPU_MEM_HOST && n) {
+    MZ_TRY(in->alloc(ctx, n * in_rb));
+    MZ_TRY(copy_in(ctx, in->p, rows, n * in_rb, mem));
+    *d_rows = in->as<u64>();
+  }
+  return MZGPU_OK;
+}
+
 // Closure descriptors come from the caller: everything the device code indexes or shifts by is
 // checked here, once, at plan time (include/mzgpu.h: richer plans are MZGPU_E_UNSUPPORTED, malformed
 // descriptors MZGPU_E_INVALID; nothing undefined reaches a kernel).
@@ -636,15 +650,24 @@ extern "C" int32_t mzgpu_buf_download(mzgpu_buf* b, void* rows, uint64_t cap, in
 }
 
 // ============================================================ consolidation
+// a row count on the host: when it is on the device, every count enqueued so far is read back (one wait)
+static int32_t dlen_read(mzgpu_ctx* ctx, DLen n, u64* out) {
+  *out = n.imm;
+  if (n.p != nullptr) {
+    MZ_TRY(mz_resolve_counters(ctx));
+    *out = ctx->h_cnt[n.p - ctx->d_cnt];  // the block is part of the arena mirror
+  }
+  return MZGPU_OK;
+}
+
 // rows (device, count possibly device resident) -> consolidated rows; the fused
 // kernel for small / medium inputs, the multi-kernel path beyond.
 static int32_t consolidate_dev(mzgpu_ctx* ctx, int rb, const void* d_in, DLen n, u64 n_ub, DevMem* out,
                                u64* out_cap, Lazy4* out_len) {
   if (n.p != nullptr && !mz_use_fused(false, n_ub)) {
     // bound too loose to size buffers by: read the count back
-    MZ_TRY(mz_resolve_counters(ctx));
-    n = dlen_imm(ctx->h_cnt[n.p - ctx->d_cnt]);  // the block is part of the arena mirror
-    n_ub = n.imm;
+    MZ_TRY(dlen_read(ctx, n, &n_ub));
+    n = dlen_imm(n_ub);
   }
   if (mz_use_fused(n.p == nullptr, n_ub)) {
     FusedJob job;
@@ -1995,6 +2018,94 @@ extern "C" int32_t mzgpu_spine_export(mzgpu_spine* s, mzgpu_buf* out) {
 }
 
 // ================================================================ join_core
+// The trace side of a probe, planned once for any stream: the view of the trace's batches (in the caller's
+// storage: it is large), the kernel parameters, and the fan-out bound that decides the form a stream takes.
+struct ProbePlan {
+  TraceView* tv;
+  ProbeParams pp;
+  u64 fan;       // matches of one probe row at most: the sum over batches of the longest key run
+  bool exact;    // no batch's longest run saturated
+  u64 max_rows;  // the largest output bound the caller lets the bounded form take
+  // n_ub probe rows yield at most n_ub x fan rows, and that bound is within the caller's limit
+  bool within(u64 n_ub) const { return exact && fan > 0 && n_ub <= max_rows / fan; }
+  // Bounded fan-out: one pass into a buffer of n_ub x fan rows -- the probe walks the trace once
+  // instead of twice (count, write) and needs no read-back.  Otherwise the exact two-pass form runs.
+  bool bounded(u64 n_ub) const { return within(n_ub) && mz_probe_tiles(n_ub, tv->n_batches) <= MZ_LB_TILES; }
+};
+// `mode` MZ_PROBE_HALF_LE / _LT or MZ_PROBE_JOIN.  Without a closure a half join writes (key, val2) -- the
+// lookup value replaces the stream value -- and join_core the R40 row (key, val1, val2).
+static int32_t probe_plan(mzgpu_ctx* ctx, const std::vector<mzgpu_batch*>& batches, int mode,
+                          const mzgpu_closure* closure, u64 meet, bool swap_vals, u64 max_rows, TraceView* tv,
+                          ProbePlan* p) {
+  MZ_TRY(trace_fanout(batches, &p->fan, &p->exact));
+  MZ_TRY(trace_view(ctx, batches, tv));
+  p->tv = tv;
+  p->max_rows = max_rows;
+  memset(&p->pp, 0, sizeof(p->pp));
+  p->pp.mode = mode;
+  p->pp.meet = meet;
+  p->pp.swap_vals = swap_vals ? 1 : 0;
+  p->pp.has_closure = closure != nullptr || mode != MZ_PROBE_JOIN ? 1 : 0;
+  if (closure != nullptr) {
+    p->pp.closure = *closure;
+  } else if (mode != MZ_PROBE_JOIN) {
+    p->pp.closure.n_key_fields = 1;
+    p->pp.closure.key_fields[0] = mzgpu_field{MZGPU_SRC_KEY, 0, 64, 0};
+    p->pp.closure.n_val_fields = 1;
+    p->pp.closure.val_fields[0] = mzgpu_field{MZGPU_SRC_VAL2, 0, 64, 0};
+  }
+  return MZGPU_OK;
+}
+
+// What becomes of a probe's output: appended to `out` as it is, appended consolidated, or consolidated and
+// appended with its exact row count returned (join_core's fuel accounting reads it back anyway).
+enum class ProbeOut { APPEND, APPEND_CONSOLIDATED, CONSOLIDATE_COUNT };
+// A plan run over n stream rows (count possibly on the device, bound n_ub).
+static int32_t probe_run(mzgpu_ctx* ctx, const ProbePlan& p, const u64* d_stream, DLen n, u64 n_ub, ProbeOut how,
+                         mzgpu_buf* out, u64* n_out = nullptr) {
+  if (n_out != nullptr) *n_out = 0;
+  if (n_ub == 0 || p.tv->n_batches == 0) return MZGPU_OK;
+  const int rb = p.pp.has_closure ? 32 : 40;
+  DevMem res;
+  Lazy4 rlen;
+  DLen r_len;
+  u64 r_ub = 0;
+  if (p.bounded(n_ub)) {
+    const u64 bound = n_ub * p.fan;
+    if (how == ProbeOut::APPEND) {
+      MZ_TRY(buf_reserve(out, out->ub + bound, true));
+      Append a;
+      MZ_TRY(buf_begin_append(out, &a));
+      MZ_TRY(mz_probe_async(ctx, d_stream, n, n_ub, *p.tv, p.pp, out->mem.as<u64>(), a.base, out->cap, a.out_len));
+      buf_end_append(out, a, bound);
+      return MZGPU_OK;
+    }
+    MZ_TRY(res.alloc(ctx, bound * rb));
+    MZ_TRY(rlen.make_pending(ctx));
+    MZ_TRY(mz_probe_async(ctx, d_stream, n, n_ub, *p.tv, p.pp, res.as<u64>(), dlen_imm(0), bound, rlen.dptr()));
+    rlen.mark_written();
+    if (how == ProbeOut::CONSOLIDATE_COUNT) MZ_TRY(rlen.resolve());
+    r_len = dlen_of(rlen, 0);
+    r_ub = rlen.known ? rlen.v[0] : bound;
+  } else {
+    u64 nn = 0;
+    MZ_TRY(dlen_read(ctx, n, &nn));
+    if (nn == 0) return MZGPU_OK;
+    MZ_TRY(mz_probe(ctx, d_stream, nn, *p.tv, p.pp, &res, &r_ub));
+    r_len = dlen_imm(r_ub);
+  }
+  if (how == ProbeOut::APPEND) return buf_append_dev(out, res.p, r_len, r_ub);
+  if (how == ProbeOut::APPEND_CONSOLIDATED) return append_consolidated(ctx, rb, res.p, r_len, r_ub, out);
+  if (r_ub == 0) return MZGPU_OK;
+  DevMem cons;
+  u64 ccap = 0;
+  Lazy4 clen;
+  MZ_TRY(consolidate_dev(ctx, rb, res.p, r_len, r_ub, &cons, &ccap, &clen));
+  MZ_TRY(clen.resolve());
+  *n_out = clen.v[0];
+  return buf_append_dev(out, cons.p, dlen_imm(*n_out), *n_out);
+}
+
 struct mzgpu_join {
   mzgpu_ctx* ctx;
   mzgpu_spine *t1, *t2;
@@ -2102,64 +2213,25 @@ extern "C" int32_t mzgpu_join_core_work_until(mzgpu_join* j, uint64_t fuel_rows,
     // the item leaves the queue only once its output has been appended: a failure below (more
     // batches than a trace view holds, counter arena, ...) leaves it queued, so no join work is lost
     mzgpu_join::Work& w = j->todo.front();
-    TraceView tv;
-    int32_t st = MZGPU_OK;
-    for (auto* b : w.others)
-      if (st == MZGPU_OK) st = batch_resolve(b);
-    if (st == MZGPU_OK) st = batch_ready(w.batch);
-    if (st == MZGPU_OK) st = batch_resolve(w.batch);
-    if (st == MZGPU_OK) st = trace_view(j->ctx, w.others, &tv);
-    DevMem res, cons;
-    u64 n_res = 0, ccap = 0;
-    Lazy4 clen;
+    for (auto* b : w.others) MZ_TRY(batch_resolve(b));
+    MZ_TRY(batch_ready(w.batch));
+    MZ_TRY(batch_resolve(w.batch));
     // this slice: rows [w.pos, w.pos + n_probe) of the work item's batch
-    const u64 n_total = st == MZGPU_OK ? w.batch->st.v[0] : 0;
+    const u64 n_total = w.batch->st.v[0];
     // a caller that gave no deadline and has fuel left for more than one slice is not asking to be
     // yielded to: it gets slices as large as its fuel allows (up to 16M rows), which take the bulk
     // sort for the slice's output instead of ten 1M-row fused launches (BASELINE config 2)
     u64 slice = MZ_JOIN_SLICE_ROWS;
     if (deadline_ns == 0) slice = std::max<u64>(slice, std::min<u64>(fuel_rows - produced, 16ull << 20));
     const u64 n_probe = std::min<u64>(n_total - std::min(n_total, w.pos), slice);
-    const u64* d_probe = w.batch->rows.as<u64>() + w.pos * 4;
-    if (st == MZGPU_OK && n_probe > 0) {
-      ProbeParams pp;
-      memset(&pp, 0, sizeof(pp));
-      pp.mode = MZ_PROBE_JOIN;
-      pp.meet = w.cap;
-      pp.has_closure = j->has_closure ? 1 : 0;
-      pp.swap_vals = w.side == 1 ? 1 : 0;
-      pp.closure = j->closure;
-      // Bounded fan-out: one pass into a buffer of n x (sum of the longest key runs) rows -- the
-      // probe walks the trace once instead of twice (count, write) and the only read-back is the
-      // result count that the fuel accounting needs anyway.
-      u64 fan = 0;
-      bool exact = true;
-      st = trace_fanout(w.others, &fan, &exact);
-      const bool bounded = st == MZGPU_OK && exact && fan > 0 &&
-                           n_probe <= MZ_BULK_BOUND_BYTES / (fan * out_rb) && mz_probe_tiles(n_probe, tv.n_batches) <= MZ_LB_TILES;
-      if (st == MZGPU_OK && bounded) {
-        Lazy4 rlen;
-        const u64 bound = n_probe * fan;
-        st = res.alloc(j->ctx, bound * out_rb);
-        if (st == MZGPU_OK) st = rlen.make_pending(j->ctx);
-        if (st == MZGPU_OK) {
-          st = mz_probe_async(j->ctx, d_probe, dlen_imm(n_probe), n_probe, tv, pp, res.as<u64>(), dlen_imm(0), bound,
-                              rlen.dptr());
-          rlen.mark_written();
-        }
-        if (st == MZGPU_OK) st = rlen.resolve();
-        if (st == MZGPU_OK) n_res = rlen.v[0];
-      } else if (st == MZGPU_OK) {
-        st = mz_probe(j->ctx, d_probe, n_probe, tv, pp, &res, &n_res);
-      }
-    }
+    TraceView tv;
+    ProbePlan plan;
+    MZ_TRY(probe_plan(j->ctx, w.others, MZ_PROBE_JOIN, j->has_closure ? &j->closure : nullptr, w.cap, w.side == 1,
+                      MZ_BULK_BOUND_BYTES / out_rb, &tv, &plan));
     // Work::process consolidates each work item's output buffer before sending
-    if (st == MZGPU_OK && n_res)
-      st = consolidate_dev(j->ctx, out_rb, res.p, dlen_imm(n_res), n_res, &cons, &ccap, &clen);
-    if (st == MZGPU_OK && n_res) st = clen.resolve();
-    const u64 n_cons = n_res ? clen.v[0] : 0;
-    if (st == MZGPU_OK && n_cons) st = buf_append_dev(out, cons.p, dlen_imm(n_cons), n_cons);
-    if (st != MZGPU_OK) return st;
+    u64 n_cons = 0;
+    MZ_TRY(probe_run(j->ctx, plan, w.batch->rows.as<u64>() + w.pos * 4, dlen_imm(n_probe), n_probe,
+                     ProbeOut::CONSOLIDATE_COUNT, out, &n_cons));
     w.pos += n_probe;
     if (w.pos >= n_total) {
       j->release_work(w);
@@ -2176,106 +2248,11 @@ extern "C" int32_t mzgpu_join_core_work(mzgpu_join* j, uint64_t fuel_rows, mzgpu
 }
 
 // ================================================================ half_join
-// Bounded probes run in one pass with no host round trip: the capacity
-// n_ub x (sum over batches of the longest key run) cannot be exceeded.  Beyond
-// MZ_BOUND_MAX_ROWS (heavy skew) the exact two-pass form (count, read back,
-// write) is used.
+// half joins: the bounded single-pass form may take this many output rows; beyond it (heavy skew) the
+// exact two-pass form runs
 #define MZ_BOUND_MAX_ROWS (48ull << 20)
 
-static int32_t half_join_dev(mzgpu_ctx* ctx, const u64* d_stream, DLen n, u64 n_ub, mzgpu_spine* trace,
-                             int32_t cmp_mode, const mzgpu_closure* closure, int32_t consolidate_output,
-                             mzgpu_buf* out) {
-  if (n_ub == 0) return MZGPU_OK;
-  std::vector<mzgpu_batch*> all;
-  spine_readable(trace, all);
-  u64 fan = 0;
-  bool exact = true;
-  MZ_TRY(trace_fanout(all, &fan, &exact));
-  TraceView tv;
-  MZ_TRY(trace_view(ctx, all, &tv));
-  if (tv.n_batches == 0) return MZGPU_OK;
-  ProbeParams pp;
-  memset(&pp, 0, sizeof(pp));
-  pp.mode = cmp_mode == MZGPU_HALFJOIN_LE ? MZ_PROBE_HALF_LE : MZ_PROBE_HALF_LT;
-  pp.has_closure = 1;
-  if (closure) {
-    pp.closure = *closure;
-  } else {
-    // identity on (key, val2): the lookup value replaces the stream value
-    pp.closure.n_key_fields = 1;
-    pp.closure.key_fields[0] = mzgpu_field{MZGPU_SRC_KEY, 0, 64, 0};
-    pp.closure.n_val_fields = 1;
-    pp.closure.val_fields[0] = mzgpu_field{MZGPU_SRC_VAL2, 0, 64, 0};
-  }
-  const bool bounded = exact && fan > 0 && n_ub <= MZ_BOUND_MAX_ROWS / fan &&
-                       mz_probe_tiles(n_ub, tv.n_batches) <= MZ_LB_TILES;
-  if (bounded) {
-    const u64 bound = n_ub * fan;
-    if (!consolidate_output) {
-      MZ_TRY(buf_reserve(out, out->ub + bound, true));
-      Append a;
-      MZ_TRY(buf_begin_append(out, &a));
-      MZ_TRY(mz_probe_async(ctx, d_stream, n, n_ub, tv, pp, out->mem.as<u64>(), a.base, out->cap, a.out_len));
-      buf_end_append(out, a, bound);
-      return MZGPU_OK;
-    }
-    // probe into a scratch array, consolidate that, append
-    DevMem res, cons;
-    Lazy4 rlen, clen;
-    u64 ccap = 0;
-    MZ_TRY(res.alloc(ctx, bound * 32));
-    MZ_TRY(rlen.make_pending(ctx));
-    MZ_TRY(mz_probe_async(ctx, d_stream, n, n_ub, tv, pp, res.as<u64>(), dlen_imm(0), bound, rlen.dptr()));
-    rlen.mark_written();
-    MZ_TRY(consolidate_dev(ctx, 32, res.p, dlen_of(rlen, 0), bound, &cons, &ccap, &clen));
-    return buf_append_dev(out, cons.p, dlen_of(clen, 0), clen.known ? clen.v[0] : bound);
-  }
-  // exact two-pass form
-  u64 nn = n.imm;
-  if (n.p != nullptr) {
-    MZ_TRY(mz_resolve_counters(ctx));
-    nn = ctx->h_cnt[n.p - ctx->d_cnt];
-  }
-  if (nn == 0) return MZGPU_OK;
-  DevMem res;
-  u64 n_res = 0;
-  MZ_TRY(mz_probe(ctx, d_stream, nn, tv, pp, &res, &n_res));
-  if (consolidate_output && n_res) {
-    DevMem cons;
-    Lazy4 clen;
-    u64 ccap = 0;
-    MZ_TRY(consolidate_dev(ctx, 32, res.p, dlen_imm(n_res), n_res, &cons, &ccap, &clen));
-    MZ_TRY(buf_append_dev(out, cons.p, dlen_of(clen, 0), clen.known ? clen.v[0] : n_res));
-  } else if (n_res) {
-    MZ_TRY(buf_append_dev(out, res.p, dlen_imm(n_res), n_res));
-  }
-  return MZGPU_OK;
-}
-
-extern "C" int32_t mzgpu_half_join(mzgpu_ctx* ctx, const mzgpu_r32* stream, uint64_t n, int32_t mem,
-                                   mzgpu_spine* trace, int32_t cmp_mode, const mzgpu_closure* closure,
-                                   int32_t consolidate_output, mzgpu_buf* out) {
-  MZ_CHECK_CTX(ctx);
-  if (trace == nullptr || out == nullptr || (stream == nullptr && n) || trace->rb != 32 || out->rb != 32 ||
-      (cmp_mode != MZGPU_HALFJOIN_LE && cmp_mode != MZGPU_HALFJOIN_LT))
-    return MZGPU_E_INVALID;
-  MZ_TRY(validate_closure(ctx, closure));
-  if (n == 0) return MZGPU_OK;
-  ctx->stats.rows_in += n;
-  DevMem in;
-  const u64* d_stream = (const u64*)stream;
-  if (mem == MZGPU_MEM_HOST) {
-    MZ_TRY(in.alloc(ctx, n * 32));
-    MZ_TRY(copy_in(ctx, in.p, stream, n * 32, mem));
-    d_stream = in.as<u64>();
-  }
-  return half_join_dev(ctx, d_stream, dlen_imm(n), n, trace, cmp_mode, closure, consolidate_output, out);
-}
-// k half joins in one launch (mz_probe_async_many).  Requests whose output buffers coincide must
-// be adjacent: they form a chain whose results are appended in request order -- the last stage of
-// the delta paths, whose outputs are concatenated (delta_join.rs:302-308).  Anything the single
-// launch cannot take (unbounded fan-out, an empty stream or trace, a buffer named twice apart)
-// runs request by request; the results are the same either way.
+// One half join: a stream probes a trace, the results are appended to `out`.
 struct HalfJoinReq {
   mzgpu_buf* stream;  // the stream to probe with, or ...
   mzgpu_spine* trace;
@@ -2288,26 +2265,87 @@ struct HalfJoinReq {
   const mzgpu_closure* pre = nullptr;
   u64 skip_time = MZGPU_FRONTIER_EMPTY;
 };
-static int32_t map_rows_into(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const mzgpu_closure* closure,
-                             u64 skip_time, mzgpu_buf* out);
 static const u64* req_rows(const HalfJoinReq& r) { return r.src ? r.src->rows.as<u64>() : r.stream->mem.as<u64>(); }
 static DLen req_dlen(const HalfJoinReq& r) { return r.src ? batch_dlen(r.src) : buf_dlen(r.stream); }
 static u64 req_ub(const HalfJoinReq& r) { return r.src ? r.src->len_ub : r.stream->ub; }
+// a source batch of 32-byte rows, or a buffer of them other than the output
+static bool req_stream_ok(const HalfJoinReq& r) {
+  return r.src != nullptr ? r.src->rb == 32 : r.stream != nullptr && r.stream != r.out && r.stream->rb == 32;
+}
+// The argument check every half-join entry point makes of each request; `stream_ok` is its check of the rows
+// the request probes with.  Refusals set no message; a malformed closure sets its own.
+static int32_t half_join_check(mzgpu_ctx* ctx, bool stream_ok, const HalfJoinReq& r) {
+  if (!stream_ok || r.trace == nullptr || r.out == nullptr || r.trace->rb != 32 || r.out->rb != 32 ||
+      (r.cmp_mode != MZGPU_HALFJOIN_LE && r.cmp_mode != MZGPU_HALFJOIN_LT))
+    return MZGPU_E_INVALID;
+  MZ_TRY(validate_closure(ctx, r.pre));
+  return validate_closure(ctx, r.closure);
+}
+static int32_t half_join_plan(mzgpu_ctx* ctx, const HalfJoinReq& r, TraceView* tv, ProbePlan* p) {
+  std::vector<mzgpu_batch*> all;
+  spine_readable(r.trace, all);
+  return probe_plan(ctx, all, r.cmp_mode == MZGPU_HALFJOIN_LE ? MZ_PROBE_HALF_LE : MZ_PROBE_HALF_LT, r.closure, 0,
+                    false, MZ_BOUND_MAX_ROWS, tv, p);
+}
+static int32_t half_join_dev(mzgpu_ctx* ctx, const HalfJoinReq& r, const u64* d_stream, DLen n, u64 n_ub,
+                             int32_t consolidate_output) {
+  if (n_ub == 0) return MZGPU_OK;
+  TraceView tv;
+  ProbePlan plan;
+  MZ_TRY(half_join_plan(ctx, r, &tv, &plan));
+  return probe_run(ctx, plan, d_stream, n, n_ub, consolidate_output ? ProbeOut::APPEND_CONSOLIDATED : ProbeOut::APPEND,
+                   r.out);
+}
+
+extern "C" int32_t mzgpu_half_join(mzgpu_ctx* ctx, const mzgpu_r32* stream, uint64_t n, int32_t mem,
+                                   mzgpu_spine* trace, int32_t cmp_mode, const mzgpu_closure* closure,
+                                   int32_t consolidate_output, mzgpu_buf* out) {
+  MZ_CHECK_CTX(ctx);
+  const HalfJoinReq r{nullptr, trace, cmp_mode, closure, out};
+  MZ_TRY(half_join_check(ctx, stream != nullptr || n == 0, r));
+  DevMem in;
+  const u64* d_stream;
+  MZ_TRY(entry_rows_in(ctx, stream, n, mem, 32, &in, &d_stream));
+  return half_join_dev(ctx, r, d_stream, dlen_imm(n), n, consolidate_output);
+}
+extern "C" int32_t mzgpu_half_join_buf(mzgpu_ctx* ctx, mzgpu_buf* stream, mzgpu_spine* trace, int32_t cmp_mode,
+                                       const mzgpu_closure* closure, int32_t consolidate_output, mzgpu_buf* out) {
+  MZ_CHECK_CTX(ctx);
+  const HalfJoinReq r{stream, trace, cmp_mode, closure, out};
+  MZ_TRY(half_join_check(ctx, req_stream_ok(r), r));
+  ctx->stats.rows_in += stream->ub;
+  return half_join_dev(ctx, r, stream->mem.as<u64>(), buf_dlen(stream), stream->ub, consolidate_output);
+}
+
+static int32_t map_rows_into(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const mzgpu_closure* closure,
+                             u64 skip_time, mzgpu_buf* out);
+// k <= MZ_PROBE_MANY_MAX half joins in one launch (mz_probe_async_many).  Requests whose output buffers
+// coincide must be adjacent: they form a chain whose results are appended in request order -- the last stage
+// of the delta paths, whose outputs are concatenated (delta_join.rs:302-308).  Anything the single launch
+// cannot take (unbounded fan-out, an empty stream or trace, a buffer named twice apart) runs request by
+// request; the results are the same either way.
 static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs) {
+  static thread_local TraceView tvs[MZ_PROBE_MANY_MAX];  // large: kept off the stack
+  ProbePlan plans[MZ_PROBE_MANY_MAX];
+  int planned = 0;  // requests [0, planned) have their trace side planned
   auto one_by_one = [&]() -> int32_t {
     for (int j = 0; j < k; ++j) {
       const HalfJoinReq& r = reqs[j];
+      mzgpu_buf tmp;
+      const mzgpu_buf* s = r.stream;
       if (r.src != nullptr) {
         // the separate operators: update stream into a scratch buffer, then the half join
-        mzgpu_buf tmp;
         tmp.ctx = ctx;
         tmp.rb = 32;
         tmp.len.set(ctx, 0);
         MZ_TRY(map_rows_into(ctx, req_rows(r), req_dlen(r), req_ub(r), r.pre, r.skip_time, &tmp));
-        MZ_TRY(half_join_dev(ctx, tmp.mem.as<u64>(), buf_dlen(&tmp), tmp.ub, r.trace, r.cmp_mode, r.closure, 0, r.out));
-      } else {
-        MZ_TRY(half_join_dev(ctx, req_rows(r), req_dlen(r), req_ub(r), r.trace, r.cmp_mode, r.closure, 0, r.out));
+        s = &tmp;
       }
+      // the stream is read now, not when the chain was planned: it may be an earlier request's output
+      if (s->ub == 0) continue;
+      // nothing between planning and running changes a spine: the chain's plan of this trace still holds
+      if (j >= planned) MZ_TRY(half_join_plan(ctx, r, &tvs[j], &plans[j]));
+      MZ_TRY(probe_run(ctx, plans[j], s->mem.as<u64>(), buf_dlen(s), s->ub, ProbeOut::APPEND, r.out));
     }
     return MZGPU_OK;
   };
@@ -2315,10 +2353,7 @@ static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs
     if (reqs[j].src != nullptr) MZ_TRY(batch_ready(reqs[j].src));
   bool any_src = false;
   for (int j = 0; j < k; ++j) any_src = any_src || reqs[j].src != nullptr;
-  if ((k < 2 && !any_src) || k > MZ_PROBE_MANY_MAX) return one_by_one();
-  static thread_local TraceView tvs[MZ_PROBE_MANY_MAX];  // large: kept off the stack
-  ProbeParams pps[MZ_PROBE_MANY_MAX];
-  u64 bound[MZ_PROBE_MANY_MAX];
+  if (k < 2 && !any_src) return one_by_one();
   u64 tiles = 0;
   for (int j = 0; j < k; ++j) {
     const HalfJoinReq& r = reqs[j];
@@ -2327,51 +2362,30 @@ static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs
     for (int i = 0; i < k; ++i)
       if (reqs[i].stream != nullptr && reqs[i].stream == r.out) return one_by_one();
     if (req_ub(r) == 0) return one_by_one();
-    std::vector<mzgpu_batch*> all;
-    spine_readable(r.trace, all);
-    u64 fan = 0;
-    bool exact = true;
-    MZ_TRY(trace_fanout(all, &fan, &exact));
-    MZ_TRY(trace_view(ctx, all, &tvs[j]));
-    if (tvs[j].n_batches == 0 || !exact || fan == 0 || req_ub(r) > MZ_BOUND_MAX_ROWS / fan) return one_by_one();
-    bound[j] = req_ub(r) * fan;
+    MZ_TRY(half_join_plan(ctx, r, &tvs[j], &plans[j]));
+    planned = j + 1;
+    if (tvs[j].n_batches == 0 || !plans[j].within(req_ub(r))) return one_by_one();
     tiles += mz_probe_tiles(req_ub(r), tvs[j].n_batches);
-    memset(&pps[j], 0, sizeof(ProbeParams));
-    pps[j].mode = r.cmp_mode == MZGPU_HALFJOIN_LE ? MZ_PROBE_HALF_LE : MZ_PROBE_HALF_LT;
-    pps[j].has_closure = 1;
-    if (r.closure) {
-      pps[j].closure = *r.closure;
-    } else {
-      pps[j].closure.n_key_fields = 1;
-      pps[j].closure.key_fields[0] = mzgpu_field{MZGPU_SRC_KEY, 0, 64, 0};
-      pps[j].closure.n_val_fields = 1;
-      pps[j].closure.val_fields[0] = mzgpu_field{MZGPU_SRC_VAL2, 0, 64, 0};
-    }
   }
+  // the requests share the look-back state: their tiles together must fit
   if (tiles > MZ_LB_TILES) return one_by_one();
   // chains: reserve each output for the sum of its requests' bounds, open one append per chain
   ProbeJobHost jobs[MZ_PROBE_MANY_MAX];
   Append app[MZ_PROBE_MANY_MAX];
-  u64 chain_bound[MZ_PROBE_MANY_MAX];
-  int chain_first[MZ_PROBE_MANY_MAX];
+  u64 chain_bound[MZ_PROBE_MANY_MAX] = {};
+  mzgpu_buf* chain_out[MZ_PROBE_MANY_MAX];
   int nc = 0;
   for (int j = 0; j < k; ++j) {
-    if (j == 0 || reqs[j].out != reqs[j - 1].out) {
-      chain_first[nc] = j;
-      chain_bound[nc] = 0;
-      ++nc;
-    }
-    chain_bound[nc - 1] += bound[j];
+    if (j == 0 || reqs[j].out != reqs[j - 1].out) chain_out[nc++] = reqs[j].out;
+    jobs[j].chain = nc - 1;
+    chain_bound[nc - 1] += req_ub(reqs[j]) * plans[j].fan;
   }
   for (int c = 0; c < nc; ++c) {
-    mzgpu_buf* out = reqs[chain_first[c]].out;
-    MZ_TRY(buf_reserve(out, out->ub + chain_bound[c], true));
-    MZ_TRY(buf_begin_append(out, &app[c]));
+    MZ_TRY(buf_reserve(chain_out[c], chain_out[c]->ub + chain_bound[c], true));
+    MZ_TRY(buf_begin_append(chain_out[c], &app[c]));
   }
-  int c = -1;
   for (int j = 0; j < k; ++j) {
-    if (j == 0 || reqs[j].out != reqs[j - 1].out) ++c;
-    mzgpu_buf* out = reqs[j].out;
+    const int c = jobs[j].chain;
     jobs[j].d_stream = req_rows(reqs[j]);
     jobs[j].n = req_dlen(reqs[j]);
     jobs[j].n_ub = req_ub(reqs[j]);
@@ -2379,92 +2393,52 @@ static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs
     jobs[j].pre = reqs[j].pre;
     jobs[j].skip_time = reqs[j].skip_time;
     jobs[j].trace = &tvs[j];
-    jobs[j].pp = &pps[j];
-    jobs[j].chain = c;
-    jobs[j].d_out = out->mem.as<u64>();
+    jobs[j].pp = &plans[j].pp;
+    jobs[j].d_out = chain_out[c]->mem.as<u64>();
     jobs[j].out_base = app[c].base;
-    jobs[j].out_cap = out->cap;
+    jobs[j].out_cap = chain_out[c]->cap;
     jobs[j].d_out_len = app[c].out_len;
   }
   MZ_TRY(mz_probe_async_many(ctx, k, jobs));
-  for (int cc = 0; cc < nc; ++cc) buf_end_append(reqs[chain_first[cc]].out, app[cc], chain_bound[cc]);
+  for (int cc = 0; cc < nc; ++cc) buf_end_append(chain_out[cc], app[cc], chain_bound[cc]);
   return MZGPU_OK;
 }
-
+// The *_many entry points: request j is built by req(j), checked and its rows counted before request j + 1 is
+// checked; then groups of at most MZ_PROBE_MANY_MAX run, never splitting a chain's adjacency.
+template <class Req>
+static int32_t half_join_many_entry(mzgpu_ctx* ctx, uint32_t k, bool arrays_ok, Req req) {
+  MZ_CHECK_CTX(ctx);
+  if (k == 0) return MZGPU_OK;
+  if (!arrays_ok || k > 64) return MZGPU_E_INVALID;
+  std::vector<HalfJoinReq> reqs(k);
+  for (uint32_t j = 0; j < k; ++j) {
+    reqs[j] = req(j);
+    MZ_TRY(half_join_check(ctx, req_stream_ok(reqs[j]), reqs[j]));
+    ctx->stats.rows_in += req_ub(reqs[j]);
+  }
+  for (uint32_t at = 0; at < k; at += MZ_PROBE_MANY_MAX)
+    MZ_TRY(half_join_many_dev(ctx, (int)std::min<uint32_t>(MZ_PROBE_MANY_MAX, k - at), reqs.data() + at));
+  return MZGPU_OK;
+}
 extern "C" int32_t mzgpu_half_join_many(mzgpu_ctx* ctx, uint32_t k, mzgpu_buf* const* streams,
                                         mzgpu_spine* const* traces, const int32_t* cmp_modes,
                                         const mzgpu_closure* const* closures, mzgpu_buf* const* outs) {
-  MZ_CHECK_CTX(ctx);
-  if (k == 0) return MZGPU_OK;
-  if (streams == nullptr || traces == nullptr || cmp_modes == nullptr || outs == nullptr || k > 64)
-    return MZGPU_E_INVALID;
-  std::vector<HalfJoinReq> reqs(k);
-  for (uint32_t j = 0; j < k; ++j) {
-    if (streams[j] == nullptr || traces[j] == nullptr || outs[j] == nullptr || streams[j] == outs[j] ||
-        streams[j]->rb != 32 || traces[j]->rb != 32 || outs[j]->rb != 32 ||
-        (cmp_modes[j] != MZGPU_HALFJOIN_LE && cmp_modes[j] != MZGPU_HALFJOIN_LT))
-      return MZGPU_E_INVALID;
-    reqs[j].stream = streams[j];
-    reqs[j].trace = traces[j];
-    reqs[j].cmp_mode = cmp_modes[j];
-    reqs[j].closure = closures ? closures[j] : nullptr;
-    MZ_TRY(validate_closure(ctx, reqs[j].closure));
-    reqs[j].out = outs[j];
-    ctx->stats.rows_in += streams[j]->ub;
-  }
-  // groups of at most MZ_PROBE_MANY_MAX, never splitting a chain's adjacency
-  for (uint32_t at = 0; at < k; at += MZ_PROBE_MANY_MAX) {
-    const int g = (int)std::min<uint32_t>(MZ_PROBE_MANY_MAX, k - at);
-    MZ_TRY(half_join_many_dev(ctx, g, reqs.data() + at));
-  }
-  return MZGPU_OK;
+  const bool arrays_ok = streams != nullptr && traces != nullptr && cmp_modes != nullptr && outs != nullptr;
+  return half_join_many_entry(ctx, k, arrays_ok, [&](uint32_t j) {
+    return HalfJoinReq{streams[j], traces[j], cmp_modes[j], closures ? closures[j] : nullptr, outs[j]};
+  });
 }
-
 extern "C" int32_t mzgpu_delta_first_stage_many(mzgpu_ctx* ctx, uint32_t k, mzgpu_batch* const* batches,
                                                 const mzgpu_closure* const* initial_closures,
                                                 const uint64_t* skip_times, mzgpu_spine* const* traces,
                                                 const int32_t* cmp_modes, const mzgpu_closure* const* closures,
                                                 mzgpu_buf* const* outs) {
-  MZ_CHECK_CTX(ctx);
-  if (k == 0) return MZGPU_OK;
-  if (batches == nullptr || skip_times == nullptr || traces == nullptr || cmp_modes == nullptr || outs == nullptr ||
-      k > 64)
-    return MZGPU_E_INVALID;
-  std::vector<HalfJoinReq> reqs(k);
-  for (uint32_t j = 0; j < k; ++j) {
-    if (batches[j] == nullptr || traces[j] == nullptr || outs[j] == nullptr || batches[j]->rb != 32 ||
-        traces[j]->rb != 32 || outs[j]->rb != 32 ||
-        (cmp_modes[j] != MZGPU_HALFJOIN_LE && cmp_modes[j] != MZGPU_HALFJOIN_LT))
-      return MZGPU_E_INVALID;
-    reqs[j].stream = nullptr;
-    reqs[j].src = batches[j];
-    reqs[j].pre = initial_closures ? initial_closures[j] : nullptr;
-    reqs[j].skip_time = skip_times[j];
-    reqs[j].trace = traces[j];
-    reqs[j].cmp_mode = cmp_modes[j];
-    reqs[j].closure = closures ? closures[j] : nullptr;
-    MZ_TRY(validate_closure(ctx, reqs[j].pre));
-    MZ_TRY(validate_closure(ctx, reqs[j].closure));
-    reqs[j].out = outs[j];
-    ctx->stats.rows_in += batches[j]->len_ub;
-  }
-  for (uint32_t at = 0; at < k; at += MZ_PROBE_MANY_MAX) {
-    const int g = (int)std::min<uint32_t>(MZ_PROBE_MANY_MAX, k - at);
-    MZ_TRY(half_join_many_dev(ctx, g, reqs.data() + at));
-  }
-  return MZGPU_OK;
-}
-
-extern "C" int32_t mzgpu_half_join_buf(mzgpu_ctx* ctx, mzgpu_buf* stream, mzgpu_spine* trace, int32_t cmp_mode,
-                                       const mzgpu_closure* closure, int32_t consolidate_output, mzgpu_buf* out) {
-  MZ_CHECK_CTX(ctx);
-  if (stream == nullptr || trace == nullptr || out == nullptr || stream == out || stream->rb != 32 ||
-      trace->rb != 32 || out->rb != 32 || (cmp_mode != MZGPU_HALFJOIN_LE && cmp_mode != MZGPU_HALFJOIN_LT))
-    return MZGPU_E_INVALID;
-  MZ_TRY(validate_closure(ctx, closure));
-  ctx->stats.rows_in += stream->ub;
-  return half_join_dev(ctx, stream->mem.as<u64>(), buf_dlen(stream), stream->ub, trace, cmp_mode, closure,
-                       consolidate_output, out);
+  const bool arrays_ok = batches != nullptr && skip_times != nullptr && traces != nullptr && cmp_modes != nullptr &&
+                         outs != nullptr;
+  return half_join_many_entry(ctx, k, arrays_ok, [&](uint32_t j) {
+    return HalfJoinReq{nullptr, traces[j], cmp_modes[j], closures ? closures[j] : nullptr, outs[j], batches[j],
+                       initial_closures ? initial_closures[j] : nullptr, skip_times[j]};
+  });
 }
 
 // rows -> closure(rows) appended to `out`; at most one output row per input row
@@ -2472,11 +2446,8 @@ static int32_t map_rows_into(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub
                              u64 skip_time, mzgpu_buf* out) {
   if (n_ub == 0) return MZGPU_OK;
   if ((n_ub + 255) / 256 > MZ_LB_TILES) {
-    u64 nn = n.imm;
-    if (n.p != nullptr) {
-      MZ_TRY(mz_resolve_counters(ctx));
-      nn = ctx->h_cnt[n.p - ctx->d_cnt];
-    }
+    u64 nn = 0;
+    MZ_TRY(dlen_read(ctx, n, &nn));
     DevMem res;
     u64 n_res = 0;
     MZ_TRY(mz_map_rows_dev(ctx, d_rows, nn, closure, skip_time, &res, &n_res));
@@ -3556,20 +3527,6 @@ static int32_t reduce_step_dev(mzgpu_reduce* r, const u64* d_rows, DLen n, u64 n
   return MZGPU_E_INVALID;
 }
 
-// The rows of a host-form reduce entry point (n rows of in_rb bytes) counted into rows_in and, when they are in
-// host memory, uploaded into `in`; *d_rows is where the activation reads them.
-static int32_t reduce_rows_in(mzgpu_ctx* ctx, const void* rows, uint64_t n, int32_t mem, uint32_t in_rb, DevMem* in,
-                              const u64** d_rows) {
-  ctx->stats.rows_in += n;
-  *d_rows = (const u64*)rows;
-  if (mem == MZGPU_MEM_HOST && n) {
-    MZ_TRY(in->alloc(ctx, n * in_rb));
-    MZ_TRY(copy_in(ctx, in->p, rows, n * in_rb, mem));
-    *d_rows = in->as<u64>();
-  }
-  return MZGPU_OK;
-}
-
 // The host form of a step: n rows of the operator's input width in `mem`.
 static int32_t reduce_step(ReduceShape shape, mzgpu_reduce* r, const void* rows, uint64_t n, int32_t mem,
                            uint64_t upper, mzgpu_buf* out, mzgpu_buf* errs) {
@@ -3580,7 +3537,7 @@ static int32_t reduce_step(ReduceShape shape, mzgpu_reduce* r, const void* rows,
   MZ_TRY(reduce_io_check(io, shape, r, nullptr, out, errs));
   DevMem in;
   const u64* d_rows;
-  MZ_TRY(reduce_rows_in(r->ctx, rows, n, mem, io.in_rb, &in, &d_rows));
+  MZ_TRY(entry_rows_in(r->ctx, rows, n, mem, io.in_rb, &in, &d_rows));
   return reduce_step_dev(r, d_rows, dlen_imm(n), n, upper, out, errs);
 }
 // The buffer form of a step: the rows of a device buffer, read without waiting for its length.
