@@ -1164,6 +1164,57 @@ int32_t mzgpu_mfp_step_buf(mzgpu_mfp_op* op, mzgpu_buf* rows, uint64_t upper, mz
 int32_t mzgpu_mfp_frontier(mzgpu_mfp_op* op, uint64_t* out);
 int32_t mzgpu_mfp_stats(mzgpu_mfp_op* op, uint64_t out[3]);
 
+/* ---- join closures: the device MfpPlan as the closure of the probe operators (JoinClosure,
+ * src/compute-types/src/plan/join.rs:50-82, applied by every half join, delta_join.rs:383-591, and every join_core
+ * stage of a linear join, linear_join.rs:460-500).
+ *
+ * mzgpu_join_closure_new(ctx, plan, map, out) checks the plan once, with the validation and plan build of
+ * mzgpu_mfp_new_map, and keeps it in device memory.  The plan reads three input words: plan->in_row_bytes is 40,
+ * source word MZGPU_SRC_KEY is the key, MZGPU_SRC_VAL1 the stream row's value and MZGPU_SRC_VAL2 the lookup row's
+ * value (for join_core: trace1's value and trace2's value, whichever side pushed).  out_row_bytes is 32 or 40.
+ * Predicates, map expressions, projection, types, error codes and error order are those of mzgpu_mfp_new_map.
+ * Refused, leaving no handle and the context usable: in_row_bytes != 40 and n_temporal != 0 (a JoinClosure's plan
+ * is a SafeMfpPlan) with MZGPU_E_INVALID, and everything mzgpu_mfp_new_map refuses, with its status.  A join or
+ * a call using the handle must not outlive it.
+ *
+ * ready_equivalences are lowered by the caller into leading predicates: a class [e0, e1, ..., en] becomes
+ * CMP_EQ(e0, e1), ..., CMP_EQ(e0, en), placed before the plan's own predicates, within the same limit of
+ * MZGPU_MFP_MAX_PREDICATES.  This is JoinClosure::apply: e0's error wins (it is evaluated first), a mismatch stops
+ * evaluation before later expressions, and no map expression runs before them (their support is 0).
+ *
+ * Per match (key, va, vb) at time t and diff d (half join: the stream row's time and d1 * d2, wrapping; join_core:
+ * max(t1, t2, meet)): at most one output row, the projection, once every predicate is TRUE and every map
+ * expression has been evaluated without error; or one error row (code, payload, t, d), R32, in `errs`.  `out`
+ * follows the rules of the bit-field closure entry points (probe order, consolidated when asked).  The half joins
+ * append `errs` consolidated over the call; join_core appends them consolidated per slice, as it does its output.
+ * The single-pass probe holds room for one error row per match, so no error row is ever dropped; with an MfpPlan
+ * closure a half join takes that form within the same bytes as without one (an output and an error row per match).
+ *
+ * mzgpu_half_join_mfp[_buf] and mzgpu_half_join_many_mfp are mzgpu_half_join[_buf] and mzgpu_half_join_many with
+ * the closure `jc` (jcs[j] for request j, none NULL); out rows are jc's out_row_bytes wide.  `errs` (R32) is not
+ * any stream or output of the call.  mzgpu_join_new_mfp is mzgpu_join_new with `jc`; its work entry point is
+ * mzgpu_join_core_work_mfp (deadline_ns as mzgpu_join_core_work_until, 0 = none), where fuel counts output and
+ * error rows together (mz_join_core.rs:718-770); mzgpu_join_core_work[_until] on such a join is MZGPU_E_INVALID.
+ * Out of scope: mzgpu_linear_join_new's plan, the fused initial closure of mzgpu_delta_first_stage_many and
+ * mzgpu_update_stream (run mzgpu_mfp_step with a non-temporal plan, then mzgpu_half_join_many_mfp). */
+typedef struct mzgpu_join_closure mzgpu_join_closure;
+int32_t mzgpu_join_closure_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map,
+                               mzgpu_join_closure** out);
+void mzgpu_join_closure_free(mzgpu_join_closure* jc);
+int32_t mzgpu_half_join_mfp(mzgpu_ctx* ctx, const mzgpu_r32* stream, uint64_t n, int32_t mem, mzgpu_spine* trace,
+                            int32_t cmp_mode, const mzgpu_join_closure* jc, int32_t consolidate_output,
+                            mzgpu_buf* out, mzgpu_buf* errs);
+int32_t mzgpu_half_join_mfp_buf(mzgpu_ctx* ctx, mzgpu_buf* stream, mzgpu_spine* trace, int32_t cmp_mode,
+                                const mzgpu_join_closure* jc, int32_t consolidate_output, mzgpu_buf* out,
+                                mzgpu_buf* errs);
+int32_t mzgpu_half_join_many_mfp(mzgpu_ctx* ctx, uint32_t k, mzgpu_buf* const* streams, mzgpu_spine* const* traces,
+                                 const int32_t* cmp_modes, const mzgpu_join_closure* const* jcs,
+                                 mzgpu_buf* const* outs, mzgpu_buf* errs);
+int32_t mzgpu_join_new_mfp(mzgpu_ctx* ctx, mzgpu_spine* trace1, mzgpu_spine* trace2, const mzgpu_join_closure* jc,
+                           mzgpu_join** out);
+int32_t mzgpu_join_core_work_mfp(mzgpu_join* j, uint64_t fuel_rows, uint64_t deadline_ns, mzgpu_buf* out,
+                                 mzgpu_buf* errs, int32_t* done);
+
 /* ---- FlatMap: a table function per input row, its rows appended to the input and run through the MfpPlan
  * (render_flat_map and drain_through_mfp, src/compute/src/render/flat_map.rs:29-200), for the table functions of
  * the fixed-width subset (TableFunc::eval, src/expr/src/relation/func.rs:3520-3620):

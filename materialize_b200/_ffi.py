@@ -386,6 +386,13 @@ SIGNATURES = {
     "mzgpu_mfp_new": (i32, [vp, C.POINTER(Mfp), u64, PV]),
     "mzgpu_mfp_new_map": (i32, [vp, C.POINTER(Mfp), C.POINTER(MfpMap), u64, PV]),
     "mzgpu_mfp_free": (None, [vp]),
+    "mzgpu_join_closure_new": (i32, [vp, C.POINTER(Mfp), C.POINTER(MfpMap), PV]),
+    "mzgpu_join_closure_free": (None, [vp]),
+    "mzgpu_half_join_mfp": (i32, [vp, vp, u64, i32, vp, i32, vp, i32, vp, vp]),
+    "mzgpu_half_join_mfp_buf": (i32, [vp, vp, vp, i32, vp, i32, vp, vp]),
+    "mzgpu_half_join_many_mfp": (i32, [vp, u32, vp, vp, vp, vp, vp, vp]),
+    "mzgpu_join_new_mfp": (i32, [vp, vp, vp, vp, PV]),
+    "mzgpu_join_core_work_mfp": (i32, [vp, u64, u64, vp, vp, PI32]),
     "mzgpu_mfp_step": (i32, [vp, vp, u64, i32, u64, vp, vp]),
     "mzgpu_mfp_step_buf": (i32, [vp, vp, u64, vp, vp]),
     "mzgpu_mfp_frontier": (i32, [vp, C.POINTER(u64)]),

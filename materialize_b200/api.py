@@ -443,27 +443,46 @@ class Spine:
 
 
 class JoinCore:
-    """mz_join_core over two arrangements."""
+    """mz_join_core over two arrangements.  `closure` is a bit-field closure (F.Closure) or a JoinClosure; with a
+    JoinClosure, work() and work_until() also append the error rows to self.errs (R32)."""
 
     def __init__(self, ctx, trace1, trace2, closure=None):
         self.ctx, self.closure = ctx, closure
-        self._keep = (trace1, trace2)
+        self._keep = (trace1, trace2, closure)
         h = C.c_void_p()
-        ctx.check(F.lib.mzgpu_join_new(ctx.h, trace1.h, trace2.h, _clp(closure), C.byref(h)))
+        self.errs = None
+        if isinstance(closure, JoinClosure):
+            ctx.check(F.lib.mzgpu_join_new_mfp(ctx.h, trace1.h, trace2.h, closure.h, C.byref(h)))
+            self.out, self.errs = DeviceRows(ctx, closure.out_row_bytes), DeviceRows(ctx, 32)
+        else:
+            ctx.check(F.lib.mzgpu_join_new(ctx.h, trace1.h, trace2.h, _clp(closure), C.byref(h)))
+            self.out = DeviceRows(ctx, 32 if closure is not None else 40)
         self.h = h
-        self.out = DeviceRows(ctx, 32 if closure is not None else 40)
 
     def push(self, side, batch, cap):
         self.ctx.check(F.lib.mzgpu_join_core_push(self.h, side, batch.h, cap))
 
     def work(self, fuel_rows=1 << 62):
+        if self.errs is not None:
+            return self.work_until(fuel_rows, 0)
         done = C.c_int32(0)
         self.ctx.check(F.lib.mzgpu_join_core_work(self.h, fuel_rows, self.out.h, C.byref(done)))
+        return bool(done.value)
+
+    def work_mfp(self, fuel_rows, deadline_ns=0, out=None, errs=None):
+        """mzgpu_join_core_work_mfp into `out` / `errs` (default: self.out / self.errs); returns done."""
+        done = C.c_int32(0)
+        out = out if out is not None else self.out
+        errs = errs if errs is not None else self.errs
+        self.ctx.check(F.lib.mzgpu_join_core_work_mfp(self.h, fuel_rows, deadline_ns, out.h, errs.h if errs is not None
+                                                      else None, C.byref(done)))
         return bool(done.value)
 
     def work_until(self, fuel_rows, deadline_ns):
         """Work::process with the reference's yield function: stop after fuel_rows of results or at the
         first yield point after deadline_ns (time.monotonic_ns() clock; 0 = no deadline)."""
+        if self.errs is not None:
+            return self.work_mfp(fuel_rows, deadline_ns)
         done = C.c_int32(0)
         self.ctx.check(F.lib.mzgpu_join_core_work_until(self.h, fuel_rows, deadline_ns, self.out.h, C.byref(done)))
         return bool(done.value)
@@ -550,6 +569,38 @@ def half_join_many(ctx, requests):
     cls = (C.c_void_p * k)(*[C.cast(C.pointer(r[3]), C.c_void_p) if r[3] is not None else None for r in requests])
     outs = (C.c_void_p * k)(*[r[4].h for r in requests])
     ctx.check(F.lib.mzgpu_half_join_many(ctx.h, k, streams, traces, cmps, cls, outs))
+
+
+def half_join_mfp(ctx, stream, trace, cmp_mode, jc, consolidate_output=True):
+    """half_join with a JoinClosure: returns (rows, errors), the errors R32 (code, payload, time, diff)."""
+    stream = np.ascontiguousarray(stream)
+    out, errs = DeviceRows(ctx, jc.out_row_bytes), DeviceRows(ctx, 32)
+    ctx.check(F.lib.mzgpu_half_join_mfp(ctx.h, _ptr(stream), len(stream), F.MEM_HOST, trace.h, cmp_mode, jc.h,
+                                        1 if consolidate_output else 0, out.h, errs.h))
+    return out.download(), errs.download()
+
+
+def half_join_mfp_dev(ctx, dev_stream, trace, cmp_mode, jc, consolidate_output=False, out=None, errs=None):
+    """half_join_mfp over a device-resident stream; (out, errs) stay on the device."""
+    out = out if out is not None else DeviceRows(ctx, jc.out_row_bytes)
+    errs = errs if errs is not None else DeviceRows(ctx, 32)
+    ctx.check(F.lib.mzgpu_half_join_mfp_buf(ctx.h, dev_stream.h, trace.h, cmp_mode, jc.h,
+                                            1 if consolidate_output else 0, out.h, errs.h))
+    return out, errs
+
+
+def half_join_many_mfp(ctx, requests, errs=None):
+    """mzgpu_half_join_many_mfp.  requests: (dev_stream, trace, cmp_mode, JoinClosure, out DeviceRows); returns
+    `errs` (a new DeviceRows unless given) with the errors of every request, consolidated."""
+    errs = errs if errs is not None else DeviceRows(ctx, 32)
+    k = len(requests)
+    streams = (C.c_void_p * max(1, k))(*[r[0].h for r in requests])
+    traces = (C.c_void_p * max(1, k))(*[r[1].h for r in requests])
+    cmps = (C.c_int32 * max(1, k))(*[r[2] for r in requests])
+    jcs = (C.c_void_p * max(1, k))(*[r[3].h for r in requests])
+    outs = (C.c_void_p * max(1, k))(*[r[4].h for r in requests])
+    ctx.check(F.lib.mzgpu_half_join_many_mfp(ctx.h, k, streams, traces, cmps, jcs, outs, errs.h))
+    return errs
 
 
 def delta_first_stage_many(ctx, requests):
@@ -966,6 +1017,34 @@ class Mfp:
     def __del__(self):
         if getattr(self, "h", None) and self.ctx.h:
             F.lib.mzgpu_mfp_free(self.h)
+            self.h = None
+
+
+def lower_equivalences(classes):
+    """JoinClosure's ready_equivalences as leading predicates: a class [e0, e1, ..., en] of expressions (op lists)
+    becomes CMP_EQ(e0, e1), ..., CMP_EQ(e0, en)."""
+    return [list(c[0]) + list(e) + [hop(F.HOP_CMP, _CMP["eq"])] for c in classes for e in c[1:]]
+
+
+class JoinClosure:
+    """The closure of the probe operators as a device MfpPlan (mzgpu_join_closure_new): JoinClosure
+    { ready_equivalences, before } over the words (key, stream value, lookup value) = SRC_KEY / SRC_VAL1 / SRC_VAL2.
+    `equivalences` are lowered ahead of `predicates` (lower_equivalences); the other arguments are those of Mfp
+    without temporal predicates.  Pass it to half_join_mfp*, half_join_many_mfp or JoinCore."""
+
+    def __init__(self, ctx, fields, predicates=(), consts=(), out_row_bytes=32, maps=(), map_consts=(),
+                 equivalences=(), in_row_bytes=40, temporal=()):
+        self.ctx, self.out_row_bytes = ctx, out_row_bytes
+        preds = lower_equivalences(equivalences) + list(predicates)
+        m, mp = _mfp_structs(fields, preds, temporal, consts, in_row_bytes, out_row_bytes, maps, map_consts)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_join_closure_new(ctx.h, C.byref(m), C.byref(mp) if mp is not None else None,
+                                               C.byref(h)))
+        self.h = h
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_join_closure_free(self.h)
             self.h = None
 
 

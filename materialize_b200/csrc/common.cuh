@@ -1031,6 +1031,17 @@ struct ProbeParams {
   int swap_vals;    // join_core side 1: probe rows are val2, lookup rows are val1
   mzgpu_closure closure;
 };
+// An MfpPlan closure on a probe (mzgpu_join_closure): the plan in device memory and the output row width.  The
+// single-pass forms write the R32 error rows at errs[(*err_len)++] (err_cap rows; *err_len zeroed by the caller);
+// the two-pass form allocates them.
+struct MfpDevPlan;
+struct MfpProbe {
+  const MfpDevPlan* pl;
+  int out_rb;
+  u64* errs;
+  u64 err_cap;
+  u64* err_len;
+};
 #define MZ_PROBE_MANY_MAX 3
 struct ProbeJobHost {
   const u64* d_stream;
@@ -1046,6 +1057,7 @@ struct ProbeJobHost {
   DLen out_base;
   u64 out_cap;
   u64* d_out_len;
+  const MfpProbe* mfp = nullptr;  // an MfpPlan closure instead of pp's (every job of a launch, or none)
 };
 int32_t mz_probe_async_many(mzgpu_ctx* ctx, int k, const ProbeJobHost* jobs);
 // tiles the single-pass probe cuts `n_ub` probe rows into (rows per tile shrink with the trace's
@@ -1062,14 +1074,17 @@ static inline u64 mz_probe_tiles(u64 n_ub, u32 n_batches) {
 }
 // Probe `n` R32 stream rows against the trace; appends results to d_out
 // (allocated here) and returns the count.  One sync (to size the output).
+// With an MfpPlan closure (`mfp`) the error rows go to `errs` (allocated here), *n_errs of them.
 int32_t mz_probe(mzgpu_ctx* ctx, const u64* d_stream, u64 n, const TraceView& trace,
-                 const ProbeParams& pp, DevMem* out, u64* n_out);
+                 const ProbeParams& pp, DevMem* out, u64* n_out, const MfpProbe* mfp = nullptr,
+                 DevMem* errs = nullptr, u64* n_errs = nullptr);
 // Single-pass form: `n` is read on the device, results are written at
 // d_out[out_base ...] (capacity out_cap rows: the caller guarantees it with a
 // bound, ctx->d_status records a violation) and the new length is left in
 // *d_out_len.  No host round trip.
 int32_t mz_probe_async(mzgpu_ctx* ctx, const u64* d_stream, DLen n, u64 n_ub, const TraceView& trace,
-                       const ProbeParams& pp, u64* d_out, DLen out_base, u64 out_cap, u64* d_out_len);
+                       const ProbeParams& pp, u64* d_out, DLen out_base, u64 out_cap, u64* d_out_len,
+                       const MfpProbe* mfp = nullptr);
 int32_t mz_map_rows_async(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const mzgpu_closure* closure,
                           u64 skip_time, u64* d_out, DLen out_base, u64 out_cap, u64* d_out_len);
 // Apply a closure to R32 rows (val2 = 0); optional skip of rows at `skip_time`.
@@ -1285,3 +1300,261 @@ int32_t mz_fm_expand(mzgpu_ctx* ctx, const FlatMapDevPlan& pl, const u64* d_rows
 // the least time of the input rows whose function rows are not all below ordinal g (atomicMin into *d_min)
 int32_t mz_fm_min_time(mzgpu_ctx* ctx, int iw, const u64* d_rows, const ulonglong2* incl, u64 n,
                        unsigned __int128 g, u64* d_min);
+
+#ifdef __CUDACC__
+// ---------------------------------------------------------- the MfpPlan interpreter (mfp.cu, probe.cu)
+namespace {
+
+// A stack value: v (an INT as i64, a BOOL as 0 / 1, an MZTS as u64 bits, a TS as i64 microseconds,
+// a DATE as i64 days), err (0 or an MZGPU_*_ERR_* code, ordered as the EvalError variants) and the
+// error payload.  No value is NULL (no nullable column is in the subset).  Types are host-checked
+// (host.cu: validate_mfp_program), so the device only follows the opcodes.
+struct MVal {
+  u64 v;
+  u32 err;
+  u64 pay;
+};
+
+__device__ __forceinline__ u32 mfp_arith(u32 code, int w, i64 a, i64 b, i64* r) {
+  const i64 lo = w == 32 ? (i64)(-2147483647 - 1) : (i64)0x8000000000000000ull;
+  i64 x;
+  bool ovf = false;
+  if (code == MZGPU_HOP_ADD) {
+    x = (i64)((u64)a + (u64)b);
+    ovf = ((a ^ x) & (b ^ x)) < 0;
+  } else if (code == MZGPU_HOP_SUB) {
+    x = (i64)((u64)a - (u64)b);
+    ovf = ((a ^ b) & (a ^ x)) < 0;
+  } else if (code == MZGPU_HOP_MUL) {
+    x = (i64)((u64)a * (u64)b);
+    ovf = __mul64hi((long long)a, (long long)b) != (x >> 63);
+  } else if (code == MZGPU_HOP_MOD) {  // checked_rem(b).unwrap_or(0): MIN % -1 is 0
+    if (b == 0) return MZGPU_HAVING_ERR_DIVISION_BY_ZERO;
+    x = b == -1 ? 0 : a % b;
+  } else {
+    if (b == 0) return MZGPU_HAVING_ERR_DIVISION_BY_ZERO;
+    if (b == -1 && a == lo) return w == 32 ? MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE : MZGPU_HAVING_ERR_INT64_OUT_OF_RANGE;
+    x = a / b;
+  }
+  if (w == 32 && x != (i64)(int)x) ovf = true;
+  if (ovf) return MZGPU_HAVING_ERR_NUMERIC_FIELD_OVERFLOW;
+  *r = x;
+  return 0;
+}
+
+// [LOW_DATE, HIGH_DATE + 1 day) in microseconds since 1970-01-01 (src/repr/src/adt/timestamp.rs:577-592)
+constexpr i64 TS_LOW_US = -210863692800000000ll;
+constexpr i64 TS_HIGH_US = 8210266876799999999ll;
+
+__device__ __forceinline__ u64 mfp_field(const u64* w, const mzgpu_having_op& o) {
+  u64 a = w[o.arg] >> o.shift;
+  if (o.bits < 64) {
+    a &= (1ull << o.bits) - 1;
+    if (o.sign_extend && ((a >> (o.bits - 1)) & 1)) a |= ~0ull << o.bits;
+  }
+  return a;
+}
+
+// Runs one program over the input words w and the expression values mv (every one a MZGPU_HOP_MAP may read is
+// evaluated, without error); its constants are consts / iv_us.  Returns the value left on the stack.
+__device__ __noinline__ MVal mfp_run(const mzgpu_having_op* ops, u32 n_ops, const mzgpu_having_const* consts,
+                                     const i64* iv_us, const u64* w, const u64* mv) {
+  constexpr int D = MZGPU_HAVING_MAX_STACK;
+  u64 v[D], pay[D];
+  u32 err[D];
+  int sp = 0;
+  for (u32 i = 0; i < n_ops; ++i) {
+    const mzgpu_having_op o = ops[i];
+    const u32 code = o.code;
+    if (code == MZGPU_HOP_COL || code == MZGPU_HOP_COL_MZTS || code == MZGPU_HOP_COL_TS ||
+        code == MZGPU_HOP_COL_DATE || code == MZGPU_HOP_INT || code == MZGPU_HOP_MAP) {
+      v[sp] = code == MZGPU_HOP_INT ? consts[o.konst].lo : code == MZGPU_HOP_MAP ? mv[o.arg] : mfp_field(w, o);
+      err[sp] = 0;
+      pay[sp] = 0;
+      ++sp;
+      continue;
+    }
+    const int y = sp - 1;
+    if (code == MZGPU_HOP_NOT) {
+      if (err[y] == 0) v[y] ^= 1;
+      continue;
+    }
+    if ((code >= MZGPU_HOP_INT_TO_MZTS && code <= MZGPU_HOP_DATE_TO_MZTS) || code == MZGPU_HOP_NEG ||
+        code == MZGPU_HOP_ABS || code == MZGPU_HOP_INT64_TO_INT32) {  // the unary ops and TS + interval
+      if (err[y] != 0) continue;
+      const i64 a = (i64)v[y];
+      if (code == MZGPU_HOP_INT_TO_MZTS || code == MZGPU_HOP_TS_TO_MZTS || code == MZGPU_HOP_DATE_TO_MZTS) {
+        i64 r = a;
+        if (code == MZGPU_HOP_TS_TO_MZTS) r = a >= 0 ? a / 1000 : -((-(a + 1)) / 1000) - 1;  // toward -inf
+        if (code == MZGPU_HOP_DATE_TO_MZTS) r = a * 86400000ll;                             // i32 days: no overflow
+        if (r < 0) {
+          err[y] = MZGPU_MFP_ERR_MZ_TIMESTAMP_OUT_OF_RANGE;
+          pay[y] = (u64)a;
+        } else {
+          v[y] = (u64)r;
+        }
+      } else if (code == MZGPU_HOP_TS_ADD_IV) {  // the interval is folded to i64 microseconds on the host
+        const i64 b = iv_us[o.konst];
+        const i64 r = (i64)((u64)a + (u64)b);
+        if ((((a ^ r) & (b ^ r)) < 0) || r < TS_LOW_US || r > TS_HIGH_US) {
+          err[y] = MZGPU_MFP_ERR_TIMESTAMP_OUT_OF_RANGE;
+          pay[y] = 0;
+        } else {
+          v[y] = (u64)r;
+        }
+      } else if (code == MZGPU_HOP_INT64_TO_INT32) {
+        if (a != (i64)(int)a) {
+          err[y] = MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE;
+          pay[y] = (u64)a;
+        }
+      } else {  // NEG / ABS: checked_neg / checked_abs at width arg
+        const i64 lo = o.arg == 32 ? (i64)(-2147483647 - 1) : (i64)0x8000000000000000ull;
+        if (a == lo) {
+          err[y] = o.arg == 32 ? MZGPU_HAVING_ERR_INT32_OUT_OF_RANGE : MZGPU_HAVING_ERR_INT64_OUT_OF_RANGE;
+          pay[y] = (u64)a;
+        } else if (code == MZGPU_HOP_NEG || a < 0) {
+          v[y] = (u64)0 - (u64)a;
+        }
+      }
+      continue;
+    }
+    if (code == MZGPU_HOP_IF) {  // c, t, e: the condition's error, else the taken branch's value or error
+      sp -= 2;
+      const int c = sp - 1, t = sp, e = sp + 1;
+      if (err[c] == 0) {
+        const int k = v[c] == 1 ? t : e;
+        v[c] = v[k];
+        err[c] = err[k];
+        pay[c] = pay[k];
+      }
+      continue;
+    }
+    --sp;
+    const int x = sp - 1;
+    const u32 ex = err[x], ey = err[y];
+    if (code == MZGPU_HOP_AND || code == MZGPU_HOP_OR) {
+      // variadic And / Or: the dominant value wins over an error, else the larger error (of one code, the
+      // payload-0 one: a division's "a / b" message orders after NEG / ABS's operand)
+      const u64 dom = code == MZGPU_HOP_AND ? 0 : 1;
+      if ((ex == 0 && v[x] == dom) || (ey == 0 && v[y] == dom)) {
+        v[x] = dom;
+        err[x] = 0;
+      } else if (ey > ex || (ey != 0 && ey == ex && pay[y] == 0)) {
+        err[x] = ey;
+        pay[x] = pay[y];
+      }
+      continue;
+    }
+    if (ex != 0 || ey != 0) {  // the first operand's error, else the second's
+      if (ex == 0) {
+        err[x] = ey;
+        pay[x] = pay[y];
+      }
+      continue;
+    }
+    if (code == MZGPU_HOP_CMP) {
+      const i64 a = (i64)v[x], b = (i64)v[y];
+      bool r;
+      switch (o.arg) {
+        case MZGPU_CMP_EQ: r = a == b; break;
+        case MZGPU_CMP_NE: r = a != b; break;
+        case MZGPU_CMP_LT: r = a < b; break;
+        case MZGPU_CMP_LE: r = a <= b; break;
+        case MZGPU_CMP_GT: r = a > b; break;
+        default: r = a >= b; break;
+      }
+      v[x] = r ? 1 : 0;
+      continue;
+    }
+    i64 r = 0;
+    const u32 e = mfp_arith(code, o.arg, (i64)v[x], (i64)v[y], &r);
+    if (e != 0) {
+      err[x] = e;
+      pay[x] = 0;
+    } else {
+      v[x] = (u64)r;
+    }
+  }
+  MVal out;
+  out.v = v[0];
+  out.err = err[0];
+  out.pay = pay[0];
+  return out;
+}
+
+// inclusive warp scan of small counts; returns the exclusive prefix, *total = the warp's sum
+__device__ __forceinline__ u32 warp_excl(u32 c, u32* total) {
+  const int lane = threadIdx.x & 31;
+  u32 s = c;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const u32 t = __shfl_up_sync(0xffffffffu, s, d);
+    if (lane >= d) s += t;
+  }
+  *total = __shfl_sync(0xffffffffu, s, 31);
+  return s - c;
+}
+
+// one warp-aggregated reservation of `c` rows at *cursor
+__device__ __forceinline__ u64 warp_reserve(u32 c, unsigned long long* cursor) {
+  u32 total;
+  const u32 ex = warp_excl(c, &total);
+  u64 base = 0;
+  if ((threadIdx.x & 31) == 31 && total) base = atomicAdd(cursor, (unsigned long long)total);
+  base = __shfl_sync(0xffffffffu, base, 31);
+  return base + ex;
+}
+
+// The non-temporal half of MfpPlan::evaluate over the words w (SafeMfpPlan::evaluate_inner): each predicate after
+// the expressions below its support, in order, then every remaining expression; mv receives the expression values.
+// Returns whether the row survives; an error stops evaluation and is left in *e_code / *e_pay.
+__device__ __forceinline__ bool mfp_filter_map(const MfpDevPlan& pl, const u64* w, u64* mv, u32* e_code,
+                                               u64* e_pay) {
+  bool keep = true;
+  u32 ne = 0;
+  // the expressions below `support`, in index order; an error stops the row
+  auto eval_maps = [&](u32 support) {
+    for (; ne < support && keep; ++ne) {
+      const MVal m = mfp_run(pl.map.ops[ne], pl.map.n_ops[ne], pl.map.consts, pl.map_iv_us, w, mv);
+      if (m.err) {
+        *e_code = m.err;
+        *e_pay = m.pay;
+        keep = false;
+      }
+      mv[ne] = m.v;
+    }
+  };
+  for (u32 p = 0; p < pl.plan.n_predicates && keep; ++p) {
+    eval_maps(pl.support[p]);
+    if (!keep) break;
+    const MVal m = mfp_run(pl.plan.ops[p], pl.plan.n_ops[p], pl.plan.consts, pl.iv_us, w, mv);
+    if (m.err) {
+      *e_code = m.err;
+      *e_pay = m.pay;
+      keep = false;
+    } else if (m.v == 0) {
+      keep = false;
+    }
+  }
+  eval_maps(pl.map.n_exprs);
+  return keep;
+}
+
+// The projection: the first ONW - 2 output words over the words w and the expression values mv.
+template <int ONW>
+__device__ __forceinline__ void mfp_project(const MfpDevPlan& pl, const u64* w, const u64* mv, u64* o) {
+#pragma unroll
+  for (int k = 0; k < ONW - 2; ++k) {
+    u64 acc = 0;
+    for (u32 f = 0; f < pl.plan.n_fields[k]; ++f) {
+      const mzgpu_field fd = pl.plan.fields[k][f];
+      u64 a = (fd.src >= MZGPU_SRC_MAP0 ? mv[fd.src - MZGPU_SRC_MAP0] : w[fd.src]) >> fd.shift;
+      if (fd.bits < 64) a &= (1ull << fd.bits) - 1;
+      acc |= a << fd.dst_shift;
+    }
+    o[k] = acc;
+  }
+}
+
+}  // namespace
+#endif  // __CUDACC__

@@ -2017,12 +2017,106 @@ extern "C" int32_t mzgpu_spine_export(mzgpu_spine* s, mzgpu_buf* out) {
   return MZGPU_OK;
 }
 
+// ============================================================ join closures
+// An MfpPlan closure of the probe operators (mzgpu_join_closure_new): the checked plan, and its copy in device
+// memory that the probe kernels read (warp-uniform loads; the plan is too large for the kernel parameters).
+struct mzgpu_join_closure {
+  mzgpu_ctx* ctx;
+  MfpDevPlan pl;
+  DevMem dev;
+  int out_rb() const { return (int)pl.plan.out_row_bytes; }
+};
+static int32_t mfp_build_plan(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map, uint32_t n_fn,
+                              MfpDevPlan* out_pl);
+extern "C" int32_t mzgpu_join_closure_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map,
+                                          mzgpu_join_closure** out) {
+  MZ_CHECK_CTX(ctx);
+  if (plan == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  if (plan->in_row_bytes != 40) {
+    MZ_SET_ERR(ctx, "join closure: the input is (key, stream value, lookup value), in_row_bytes 40, not %u",
+               plan->in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  if (plan->n_temporal != 0) {
+    MZ_SET_ERR(ctx, "join closure: %u temporal predicates (a JoinClosure's plan has none)", plan->n_temporal);
+    return MZGPU_E_INVALID;
+  }
+  auto jc = std::unique_ptr<mzgpu_join_closure>(new mzgpu_join_closure());
+  jc->ctx = ctx;
+  MZ_TRY(mfp_build_plan(ctx, plan, map, 0, &jc->pl));
+  MZ_TRY(jc->dev.alloc(ctx, sizeof(MfpDevPlan)));
+  MZ_TRY(copy_in(ctx, jc->dev.p, &jc->pl, sizeof(MfpDevPlan), MZGPU_MEM_HOST));
+  *out = jc.release();
+  return MZGPU_OK;
+}
+extern "C" void mzgpu_join_closure_free(mzgpu_join_closure* jc) { delete jc; }
+
+// The error rows of one call's probes with an MfpPlan closure: each probe leaves its raw rows as a chunk, and
+// errs_flush appends them all to the caller's buffer, consolidated once.
+struct ErrSink {
+  struct Chunk {
+    DevMem rows;
+    Lazy4 len;
+    u64 ub;
+  };
+  std::vector<Chunk> chunks;
+};
+// `n_out` set: the exact count of the appended rows is returned (join_core's fuel counts them)
+static int32_t errs_flush(mzgpu_ctx* ctx, ErrSink& s, mzgpu_buf* errs, u64* n_out = nullptr) {
+  if (n_out != nullptr) *n_out = 0;
+  u64 ub = 0;
+  for (auto& c : s.chunks) ub += c.ub;
+  if (ub == 0) {
+    s.chunks.clear();
+    return MZGPU_OK;
+  }
+  mzgpu_buf all;
+  const void* rows = s.chunks[0].rows.p;
+  DLen n = dlen_of(s.chunks[0].len, 0);
+  if (s.chunks.size() > 1) {
+    all.ctx = ctx;
+    all.rb = 32;
+    all.len.set(ctx, 0);
+    for (auto& c : s.chunks) MZ_TRY(buf_append_dev(&all, c.rows.p, dlen_of(c.len, 0), c.ub));
+    rows = all.mem.p;
+    n = buf_dlen(&all);
+  }
+  int32_t st;
+  if (n_out == nullptr) {
+    st = append_consolidated(ctx, 32, rows, n, ub, errs);
+  } else {
+    DevMem cons;
+    u64 ccap = 0;
+    Lazy4 clen;
+    st = consolidate_dev(ctx, 32, rows, n, ub, &cons, &ccap, &clen);
+    if (st == MZGPU_OK) st = clen.resolve();
+    if (st == MZGPU_OK) {
+      *n_out = clen.v[0];
+      st = buf_append_dev(errs, cons.p, dlen_imm(*n_out), *n_out);
+    }
+  }
+  s.chunks.clear();
+  return st;
+}
+// A chunk of `cap` error rows with a zeroed device count, for a single-pass probe to fill.
+static int32_t errs_chunk(mzgpu_ctx* ctx, const mzgpu_join_closure* jc, u64 cap, ErrSink* s, MfpProbe* mp) {
+  s->chunks.emplace_back();
+  ErrSink::Chunk& c = s->chunks.back();
+  c.ub = cap;
+  MZ_TRY(c.rows.alloc(ctx, cap * 32));
+  MZ_TRY(c.len.make_pending(ctx));
+  MZ_CUDA(ctx, cudaMemsetAsync(c.len.dptr(), 0, 8, ctx->stream));
+  *mp = MfpProbe{(const MfpDevPlan*)jc->dev.p, jc->out_rb(), c.rows.as<u64>(), cap, c.len.dptr()};
+  return MZGPU_OK;
+}
+
 // ================================================================ join_core
 // The trace side of a probe, planned once for any stream: the view of the trace's batches (in the caller's
 // storage: it is large), the kernel parameters, and the fan-out bound that decides the form a stream takes.
 struct ProbePlan {
   TraceView* tv;
   ProbeParams pp;
+  const mzgpu_join_closure* jc;  // an MfpPlan closure instead of pp's
   u64 fan;       // matches of one probe row at most: the sum over batches of the longest key run
   bool exact;    // no batch's longest run saturated
   u64 max_rows;  // the largest output bound the caller lets the bounded form take
@@ -2031,24 +2125,27 @@ struct ProbePlan {
   // Bounded fan-out: one pass into a buffer of n_ub x fan rows -- the probe walks the trace once
   // instead of twice (count, write) and needs no read-back.  Otherwise the exact two-pass form runs.
   bool bounded(u64 n_ub) const { return within(n_ub) && mz_probe_tiles(n_ub, tv->n_batches) <= MZ_LB_TILES; }
+  int rb() const { return jc != nullptr ? jc->out_rb() : pp.has_closure ? 32 : 40; }
 };
 // `mode` MZ_PROBE_HALF_LE / _LT or MZ_PROBE_JOIN.  Without a closure a half join writes (key, val2) -- the
-// lookup value replaces the stream value -- and join_core the R40 row (key, val1, val2).
+// lookup value replaces the stream value -- and join_core the R40 row (key, val1, val2).  `jc` (an MfpPlan
+// closure) takes the place of `closure`.
 static int32_t probe_plan(mzgpu_ctx* ctx, const std::vector<mzgpu_batch*>& batches, int mode,
                           const mzgpu_closure* closure, u64 meet, bool swap_vals, u64 max_rows, TraceView* tv,
-                          ProbePlan* p) {
+                          ProbePlan* p, const mzgpu_join_closure* jc = nullptr) {
   MZ_TRY(trace_fanout(batches, &p->fan, &p->exact));
   MZ_TRY(trace_view(ctx, batches, tv));
   p->tv = tv;
   p->max_rows = max_rows;
+  p->jc = jc;
   memset(&p->pp, 0, sizeof(p->pp));
   p->pp.mode = mode;
   p->pp.meet = meet;
   p->pp.swap_vals = swap_vals ? 1 : 0;
-  p->pp.has_closure = closure != nullptr || mode != MZ_PROBE_JOIN ? 1 : 0;
-  if (closure != nullptr) {
+  p->pp.has_closure = closure != nullptr || (mode != MZ_PROBE_JOIN && jc == nullptr) ? 1 : 0;
+  if (jc == nullptr && closure != nullptr) {
     p->pp.closure = *closure;
-  } else if (mode != MZ_PROBE_JOIN) {
+  } else if (jc == nullptr && mode != MZ_PROBE_JOIN) {
     p->pp.closure.n_key_fields = 1;
     p->pp.closure.key_fields[0] = mzgpu_field{MZGPU_SRC_KEY, 0, 64, 0};
     p->pp.closure.n_val_fields = 1;
@@ -2060,30 +2157,37 @@ static int32_t probe_plan(mzgpu_ctx* ctx, const std::vector<mzgpu_batch*>& batch
 // What becomes of a probe's output: appended to `out` as it is, appended consolidated, or consolidated and
 // appended with its exact row count returned (join_core's fuel accounting reads it back anyway).
 enum class ProbeOut { APPEND, APPEND_CONSOLIDATED, CONSOLIDATE_COUNT };
-// A plan run over n stream rows (count possibly on the device, bound n_ub).
+// A plan run over n stream rows (count possibly on the device, bound n_ub).  With an MfpPlan closure the error
+// rows are left in `es`: the single-pass form gets room for one per match (n_ub x fan), so it cannot run out.
 static int32_t probe_run(mzgpu_ctx* ctx, const ProbePlan& p, const u64* d_stream, DLen n, u64 n_ub, ProbeOut how,
-                         mzgpu_buf* out, u64* n_out = nullptr) {
+                         mzgpu_buf* out, u64* n_out = nullptr, ErrSink* es = nullptr) {
   if (n_out != nullptr) *n_out = 0;
   if (n_ub == 0 || p.tv->n_batches == 0) return MZGPU_OK;
-  const int rb = p.pp.has_closure ? 32 : 40;
+  const int rb = p.rb();
   DevMem res;
   Lazy4 rlen;
   DLen r_len;
   u64 r_ub = 0;
+  MfpProbe mp;
   if (p.bounded(n_ub)) {
     const u64 bound = n_ub * p.fan;
+    if (p.jc != nullptr) MZ_TRY(errs_chunk(ctx, p.jc, bound, es, &mp));
+    const MfpProbe* mpp = p.jc != nullptr ? &mp : nullptr;
     if (how == ProbeOut::APPEND) {
       MZ_TRY(buf_reserve(out, out->ub + bound, true));
       Append a;
       MZ_TRY(buf_begin_append(out, &a));
-      MZ_TRY(mz_probe_async(ctx, d_stream, n, n_ub, *p.tv, p.pp, out->mem.as<u64>(), a.base, out->cap, a.out_len));
+      MZ_TRY(mz_probe_async(ctx, d_stream, n, n_ub, *p.tv, p.pp, out->mem.as<u64>(), a.base, out->cap, a.out_len,
+                            mpp));
       buf_end_append(out, a, bound);
+      if (mpp != nullptr) es->chunks.back().len.mark_written();
       return MZGPU_OK;
     }
     MZ_TRY(res.alloc(ctx, bound * rb));
     MZ_TRY(rlen.make_pending(ctx));
-    MZ_TRY(mz_probe_async(ctx, d_stream, n, n_ub, *p.tv, p.pp, res.as<u64>(), dlen_imm(0), bound, rlen.dptr()));
+    MZ_TRY(mz_probe_async(ctx, d_stream, n, n_ub, *p.tv, p.pp, res.as<u64>(), dlen_imm(0), bound, rlen.dptr(), mpp));
     rlen.mark_written();
+    if (mpp != nullptr) es->chunks.back().len.mark_written();
     if (how == ProbeOut::CONSOLIDATE_COUNT) MZ_TRY(rlen.resolve());
     r_len = dlen_of(rlen, 0);
     r_ub = rlen.known ? rlen.v[0] : bound;
@@ -2091,7 +2195,15 @@ static int32_t probe_run(mzgpu_ctx* ctx, const ProbePlan& p, const u64* d_stream
     u64 nn = 0;
     MZ_TRY(dlen_read(ctx, n, &nn));
     if (nn == 0) return MZGPU_OK;
-    MZ_TRY(mz_probe(ctx, d_stream, nn, *p.tv, p.pp, &res, &r_ub));
+    if (p.jc != nullptr) {
+      mp = MfpProbe{(const MfpDevPlan*)p.jc->dev.p, rb, nullptr, 0, nullptr};
+      es->chunks.emplace_back();
+      ErrSink::Chunk& c = es->chunks.back();
+      MZ_TRY(mz_probe(ctx, d_stream, nn, *p.tv, p.pp, &res, &r_ub, &mp, &c.rows, &c.ub));
+      c.len.set(ctx, c.ub);
+    } else {
+      MZ_TRY(mz_probe(ctx, d_stream, nn, *p.tv, p.pp, &res, &r_ub));
+    }
     r_len = dlen_imm(r_ub);
   }
   if (how == ProbeOut::APPEND) return buf_append_dev(out, res.p, r_len, r_ub);
@@ -2111,6 +2223,7 @@ struct mzgpu_join {
   mzgpu_spine *t1, *t2;
   bool has_closure;
   mzgpu_closure closure;
+  const mzgpu_join_closure* jc = nullptr;  // mzgpu_join_new_mfp (the caller keeps it alive)
   u64 ack1 = 0, ack2 = 0;
   struct Work {
     int side;
@@ -2144,14 +2257,15 @@ static void join_enqueue(mzgpu_join* j, int side, mzgpu_batch* batch, u64 cap) {
   j->todo.push_back(std::move(w));
 }
 
-extern "C" int32_t mzgpu_join_new(mzgpu_ctx* ctx, mzgpu_spine* trace1, mzgpu_spine* trace2,
-                                  const mzgpu_closure* closure, mzgpu_join** out) {
+static int32_t join_create(mzgpu_ctx* ctx, mzgpu_spine* trace1, mzgpu_spine* trace2, const mzgpu_closure* closure,
+                           const mzgpu_join_closure* jc, mzgpu_join** out) {
   MZ_CHECK_CTX(ctx);
   if (trace1 == nullptr || trace2 == nullptr || out == nullptr || trace1->rb != 32 || trace2->rb != 32)
     return MZGPU_E_INVALID;
   MZ_TRY(validate_closure(ctx, closure));
   mzgpu_join* j = new mzgpu_join();
   j->ctx = ctx;
+  j->jc = jc;
   j->t1 = trace1;
   j->t2 = trace2;
   j->has_closure = closure != nullptr;
@@ -2170,6 +2284,16 @@ extern "C" int32_t mzgpu_join_new(mzgpu_ctx* ctx, mzgpu_spine* trace1, mzgpu_spi
   }
   *out = j;
   return MZGPU_OK;
+}
+extern "C" int32_t mzgpu_join_new(mzgpu_ctx* ctx, mzgpu_spine* trace1, mzgpu_spine* trace2,
+                                  const mzgpu_closure* closure, mzgpu_join** out) {
+  return join_create(ctx, trace1, trace2, closure, nullptr, out);
+}
+extern "C" int32_t mzgpu_join_new_mfp(mzgpu_ctx* ctx, mzgpu_spine* trace1, mzgpu_spine* trace2,
+                                      const mzgpu_join_closure* jc, mzgpu_join** out) {
+  MZ_CHECK_CTX(ctx);
+  if (jc == nullptr || jc->ctx != ctx) return MZGPU_E_INVALID;
+  return join_create(ctx, trace1, trace2, nullptr, jc, out);
 }
 extern "C" void mzgpu_join_free(mzgpu_join* j) { delete j; }
 
@@ -2196,11 +2320,11 @@ static u64 mono_ns() {
 // rows of a work item's batch probed per slice: the reference's yield budget is 1M rows of work
 // (linear_join.rs:145-151), so a bulk work item (hydration: 10M x 10M rows) yields ~10 times
 #define MZ_JOIN_SLICE_ROWS (1ull << 20)
-extern "C" int32_t mzgpu_join_core_work_until(mzgpu_join* j, uint64_t fuel_rows, uint64_t deadline_ns,
-                                              mzgpu_buf* out, int32_t* done) {
-  if (j == nullptr || out == nullptr) return MZGPU_E_INVALID;
-  MZ_CHECK_CTX(j->ctx);
-  const uint32_t out_rb = j->has_closure ? 32 : 40;
+// Work::process; `errs` receives an MfpPlan closure's error rows, consolidated per slice, and they count as fuel
+// (mz_join_core.rs:718-770 counts every result of the result function).
+static int32_t join_work(mzgpu_join* j, uint64_t fuel_rows, uint64_t deadline_ns, mzgpu_buf* out, mzgpu_buf* errs,
+                         int32_t* done) {
+  const uint32_t out_rb = j->jc != nullptr ? (uint32_t)j->jc->out_rb() : j->has_closure ? 32 : 40;
   if (out->rb != out_rb) {
     MZ_SET_ERR(j->ctx, "join_core_work: output buffer row width %u, expected %u", out->rb, out_rb);
     return MZGPU_E_INVALID;
@@ -2226,22 +2350,42 @@ extern "C" int32_t mzgpu_join_core_work_until(mzgpu_join* j, uint64_t fuel_rows,
     const u64 n_probe = std::min<u64>(n_total - std::min(n_total, w.pos), slice);
     TraceView tv;
     ProbePlan plan;
+    // (with an MfpPlan closure the bounded form also holds one error row per match)
     MZ_TRY(probe_plan(j->ctx, w.others, MZ_PROBE_JOIN, j->has_closure ? &j->closure : nullptr, w.cap, w.side == 1,
-                      MZ_BULK_BOUND_BYTES / out_rb, &tv, &plan));
+                      MZ_BULK_BOUND_BYTES / (out_rb + (j->jc != nullptr ? 32 : 0)), &tv, &plan, j->jc));
     // Work::process consolidates each work item's output buffer before sending
-    u64 n_cons = 0;
+    u64 n_cons = 0, n_errs = 0;
+    ErrSink es;
     MZ_TRY(probe_run(j->ctx, plan, w.batch->rows.as<u64>() + w.pos * 4, dlen_imm(n_probe), n_probe,
-                     ProbeOut::CONSOLIDATE_COUNT, out, &n_cons));
+                     ProbeOut::CONSOLIDATE_COUNT, out, &n_cons, &es));
+    if (j->jc != nullptr) MZ_TRY(errs_flush(j->ctx, es, errs, &n_errs));
     w.pos += n_probe;
     if (w.pos >= n_total) {
       j->release_work(w);
       j->todo.pop_front();
     }
-    produced += n_cons;
+    produced += n_cons + n_errs;
     j->ctx->stats.rows_out += n_cons;
   }
   if (done) *done = j->todo.empty() ? 1 : 0;
   return MZGPU_OK;
+}
+extern "C" int32_t mzgpu_join_core_work_until(mzgpu_join* j, uint64_t fuel_rows, uint64_t deadline_ns,
+                                              mzgpu_buf* out, int32_t* done) {
+  if (j == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(j->ctx);
+  if (j->jc != nullptr) {
+    MZ_SET_ERR(j->ctx, "join_core_work: a join with an MfpPlan closure works through mzgpu_join_core_work_mfp");
+    return MZGPU_E_INVALID;
+  }
+  return join_work(j, fuel_rows, deadline_ns, out, nullptr, done);
+}
+extern "C" int32_t mzgpu_join_core_work_mfp(mzgpu_join* j, uint64_t fuel_rows, uint64_t deadline_ns, mzgpu_buf* out,
+                                            mzgpu_buf* errs, int32_t* done) {
+  if (j == nullptr || out == nullptr || errs == nullptr || j->jc == nullptr || errs->rb != 32 || errs == out)
+    return MZGPU_E_INVALID;
+  MZ_CHECK_CTX(j->ctx);
+  return join_work(j, fuel_rows, deadline_ns, out, errs, done);
 }
 extern "C" int32_t mzgpu_join_core_work(mzgpu_join* j, uint64_t fuel_rows, mzgpu_buf* out, int32_t* done) {
   return mzgpu_join_core_work_until(j, fuel_rows, 0, out, done);
@@ -2264,7 +2408,9 @@ struct HalfJoinReq {
   mzgpu_batch* src = nullptr;
   const mzgpu_closure* pre = nullptr;
   u64 skip_time = MZGPU_FRONTIER_EMPTY;
+  const mzgpu_join_closure* jc = nullptr;  // an MfpPlan closure in place of `closure`
 };
+static uint32_t req_out_rb(const HalfJoinReq& r) { return r.jc != nullptr ? (uint32_t)r.jc->out_rb() : 32; }
 static const u64* req_rows(const HalfJoinReq& r) { return r.src ? r.src->rows.as<u64>() : r.stream->mem.as<u64>(); }
 static DLen req_dlen(const HalfJoinReq& r) { return r.src ? batch_dlen(r.src) : buf_dlen(r.stream); }
 static u64 req_ub(const HalfJoinReq& r) { return r.src ? r.src->len_ub : r.stream->ub; }
@@ -2275,8 +2421,8 @@ static bool req_stream_ok(const HalfJoinReq& r) {
 // The argument check every half-join entry point makes of each request; `stream_ok` is its check of the rows
 // the request probes with.  Refusals set no message; a malformed closure sets its own.
 static int32_t half_join_check(mzgpu_ctx* ctx, bool stream_ok, const HalfJoinReq& r) {
-  if (!stream_ok || r.trace == nullptr || r.out == nullptr || r.trace->rb != 32 || r.out->rb != 32 ||
-      (r.cmp_mode != MZGPU_HALFJOIN_LE && r.cmp_mode != MZGPU_HALFJOIN_LT))
+  if (!stream_ok || r.trace == nullptr || r.out == nullptr || r.trace->rb != 32 || r.out->rb != req_out_rb(r) ||
+      (r.cmp_mode != MZGPU_HALFJOIN_LE && r.cmp_mode != MZGPU_HALFJOIN_LT) || (r.jc != nullptr && r.jc->ctx != ctx))
     return MZGPU_E_INVALID;
   MZ_TRY(validate_closure(ctx, r.pre));
   return validate_closure(ctx, r.closure);
@@ -2284,17 +2430,23 @@ static int32_t half_join_check(mzgpu_ctx* ctx, bool stream_ok, const HalfJoinReq
 static int32_t half_join_plan(mzgpu_ctx* ctx, const HalfJoinReq& r, TraceView* tv, ProbePlan* p) {
   std::vector<mzgpu_batch*> all;
   spine_readable(r.trace, all);
+  // with an MfpPlan closure the bounded form also holds one 32-byte error row per match: the same bytes in all
+  const u64 max_rows = r.jc != nullptr ? MZ_BOUND_MAX_ROWS * 32 / (r.jc->out_rb() + 32) : MZ_BOUND_MAX_ROWS;
   return probe_plan(ctx, all, r.cmp_mode == MZGPU_HALFJOIN_LE ? MZ_PROBE_HALF_LE : MZ_PROBE_HALF_LT, r.closure, 0,
-                    false, MZ_BOUND_MAX_ROWS, tv, p);
+                    false, max_rows, tv, p, r.jc);
 }
 static int32_t half_join_dev(mzgpu_ctx* ctx, const HalfJoinReq& r, const u64* d_stream, DLen n, u64 n_ub,
-                             int32_t consolidate_output) {
+                             int32_t consolidate_output, ErrSink* es = nullptr) {
   if (n_ub == 0) return MZGPU_OK;
   TraceView tv;
   ProbePlan plan;
   MZ_TRY(half_join_plan(ctx, r, &tv, &plan));
   return probe_run(ctx, plan, d_stream, n, n_ub, consolidate_output ? ProbeOut::APPEND_CONSOLIDATED : ProbeOut::APPEND,
-                   r.out);
+                   r.out, nullptr, es);
+}
+// the error buffer of an MfpPlan closure's half joins: R32, apart from every stream and output
+static bool errs_ok(const mzgpu_buf* errs, const mzgpu_buf* stream, const mzgpu_buf* out) {
+  return errs != nullptr && errs->rb == 32 && errs != stream && errs != out;
 }
 
 extern "C" int32_t mzgpu_half_join(mzgpu_ctx* ctx, const mzgpu_r32* stream, uint64_t n, int32_t mem,
@@ -2316,6 +2468,34 @@ extern "C" int32_t mzgpu_half_join_buf(mzgpu_ctx* ctx, mzgpu_buf* stream, mzgpu_
   ctx->stats.rows_in += stream->ub;
   return half_join_dev(ctx, r, stream->mem.as<u64>(), buf_dlen(stream), stream->ub, consolidate_output);
 }
+extern "C" int32_t mzgpu_half_join_mfp(mzgpu_ctx* ctx, const mzgpu_r32* stream, uint64_t n, int32_t mem,
+                                       mzgpu_spine* trace, int32_t cmp_mode, const mzgpu_join_closure* jc,
+                                       int32_t consolidate_output, mzgpu_buf* out, mzgpu_buf* errs) {
+  MZ_CHECK_CTX(ctx);
+  HalfJoinReq r{nullptr, trace, cmp_mode, nullptr, out};
+  r.jc = jc;
+  if (jc == nullptr || !errs_ok(errs, nullptr, out)) return MZGPU_E_INVALID;
+  MZ_TRY(half_join_check(ctx, stream != nullptr || n == 0, r));
+  DevMem in;
+  const u64* d_stream;
+  MZ_TRY(entry_rows_in(ctx, stream, n, mem, 32, &in, &d_stream));
+  ErrSink es;
+  MZ_TRY(half_join_dev(ctx, r, d_stream, dlen_imm(n), n, consolidate_output, &es));
+  return errs_flush(ctx, es, errs);
+}
+extern "C" int32_t mzgpu_half_join_mfp_buf(mzgpu_ctx* ctx, mzgpu_buf* stream, mzgpu_spine* trace, int32_t cmp_mode,
+                                           const mzgpu_join_closure* jc, int32_t consolidate_output, mzgpu_buf* out,
+                                           mzgpu_buf* errs) {
+  MZ_CHECK_CTX(ctx);
+  HalfJoinReq r{stream, trace, cmp_mode, nullptr, out};
+  r.jc = jc;
+  if (jc == nullptr || !errs_ok(errs, stream, out)) return MZGPU_E_INVALID;
+  MZ_TRY(half_join_check(ctx, req_stream_ok(r), r));
+  ctx->stats.rows_in += stream->ub;
+  ErrSink es;
+  MZ_TRY(half_join_dev(ctx, r, stream->mem.as<u64>(), buf_dlen(stream), stream->ub, consolidate_output, &es));
+  return errs_flush(ctx, es, errs);
+}
 
 static int32_t map_rows_into(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub, const mzgpu_closure* closure,
                              u64 skip_time, mzgpu_buf* out);
@@ -2324,7 +2504,7 @@ static int32_t map_rows_into(mzgpu_ctx* ctx, const u64* d_rows, DLen n, u64 n_ub
 // of the delta paths, whose outputs are concatenated (delta_join.rs:302-308).  Anything the single launch
 // cannot take (unbounded fan-out, an empty stream or trace, a buffer named twice apart) runs request by
 // request; the results are the same either way.
-static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs) {
+static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs, ErrSink* es) {
   static thread_local TraceView tvs[MZ_PROBE_MANY_MAX];  // large: kept off the stack
   ProbePlan plans[MZ_PROBE_MANY_MAX];
   int planned = 0;  // requests [0, planned) have their trace side planned
@@ -2345,7 +2525,7 @@ static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs
       if (s->ub == 0) continue;
       // nothing between planning and running changes a spine: the chain's plan of this trace still holds
       if (j >= planned) MZ_TRY(half_join_plan(ctx, r, &tvs[j], &plans[j]));
-      MZ_TRY(probe_run(ctx, plans[j], s->mem.as<u64>(), buf_dlen(s), s->ub, ProbeOut::APPEND, r.out));
+      MZ_TRY(probe_run(ctx, plans[j], s->mem.as<u64>(), buf_dlen(s), s->ub, ProbeOut::APPEND, r.out, nullptr, es));
     }
     return MZGPU_OK;
   };
@@ -2361,7 +2541,7 @@ static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs
       if (reqs[i].out == r.out && reqs[j - 1].out != r.out) return one_by_one();
     for (int i = 0; i < k; ++i)
       if (reqs[i].stream != nullptr && reqs[i].stream == r.out) return one_by_one();
-    if (req_ub(r) == 0) return one_by_one();
+    if (req_ub(r) == 0 || req_out_rb(r) != req_out_rb(reqs[0])) return one_by_one();
     MZ_TRY(half_join_plan(ctx, r, &tvs[j], &plans[j]));
     planned = j + 1;
     if (tvs[j].n_batches == 0 || !plans[j].within(req_ub(r))) return one_by_one();
@@ -2373,12 +2553,24 @@ static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs
   ProbeJobHost jobs[MZ_PROBE_MANY_MAX];
   Append app[MZ_PROBE_MANY_MAX];
   u64 chain_bound[MZ_PROBE_MANY_MAX] = {};
+  MfpProbe mps[MZ_PROBE_MANY_MAX];
   mzgpu_buf* chain_out[MZ_PROBE_MANY_MAX];
   int nc = 0;
   for (int j = 0; j < k; ++j) {
     if (j == 0 || reqs[j].out != reqs[j - 1].out) chain_out[nc++] = reqs[j].out;
     jobs[j].chain = nc - 1;
     chain_bound[nc - 1] += req_ub(reqs[j]) * plans[j].fan;
+  }
+  // MfpPlan closures: one error chunk for the launch, room for one error row per match of every request
+  const bool mfp = reqs[0].jc != nullptr;
+  if (mfp) {
+    u64 err_cap = 0;
+    for (int c = 0; c < nc; ++c) err_cap += chain_bound[c];
+    MZ_TRY(errs_chunk(ctx, reqs[0].jc, err_cap, es, &mps[0]));
+    for (int j = 0; j < k; ++j) {
+      mps[j] = mps[0];
+      mps[j].pl = (const MfpDevPlan*)reqs[j].jc->dev.p;
+    }
   }
   for (int c = 0; c < nc; ++c) {
     MZ_TRY(buf_reserve(chain_out[c], chain_out[c]->ub + chain_bound[c], true));
@@ -2398,27 +2590,33 @@ static int32_t half_join_many_dev(mzgpu_ctx* ctx, int k, const HalfJoinReq* reqs
     jobs[j].out_base = app[c].base;
     jobs[j].out_cap = chain_out[c]->cap;
     jobs[j].d_out_len = app[c].out_len;
+    jobs[j].mfp = mfp ? &mps[j] : nullptr;
   }
   MZ_TRY(mz_probe_async_many(ctx, k, jobs));
   for (int cc = 0; cc < nc; ++cc) buf_end_append(chain_out[cc], app[cc], chain_bound[cc]);
+  if (mfp) es->chunks.back().len.mark_written();
   return MZGPU_OK;
 }
 // The *_many entry points: request j is built by req(j), checked and its rows counted before request j + 1 is
 // checked; then groups of at most MZ_PROBE_MANY_MAX run, never splitting a chain's adjacency.
+// With MfpPlan closures (`errs` set) the errors of all the requests are appended to `errs`, consolidated once.
 template <class Req>
-static int32_t half_join_many_entry(mzgpu_ctx* ctx, uint32_t k, bool arrays_ok, Req req) {
+static int32_t half_join_many_entry(mzgpu_ctx* ctx, uint32_t k, bool arrays_ok, Req req, mzgpu_buf* errs = nullptr) {
   MZ_CHECK_CTX(ctx);
   if (k == 0) return MZGPU_OK;
   if (!arrays_ok || k > 64) return MZGPU_E_INVALID;
+  ErrSink es;
   std::vector<HalfJoinReq> reqs(k);
   for (uint32_t j = 0; j < k; ++j) {
     reqs[j] = req(j);
+    if (errs != nullptr && (reqs[j].jc == nullptr || !errs_ok(errs, reqs[j].stream, reqs[j].out)))
+      return MZGPU_E_INVALID;
     MZ_TRY(half_join_check(ctx, req_stream_ok(reqs[j]), reqs[j]));
     ctx->stats.rows_in += req_ub(reqs[j]);
   }
   for (uint32_t at = 0; at < k; at += MZ_PROBE_MANY_MAX)
-    MZ_TRY(half_join_many_dev(ctx, (int)std::min<uint32_t>(MZ_PROBE_MANY_MAX, k - at), reqs.data() + at));
-  return MZGPU_OK;
+    MZ_TRY(half_join_many_dev(ctx, (int)std::min<uint32_t>(MZ_PROBE_MANY_MAX, k - at), reqs.data() + at, &es));
+  return errs != nullptr ? errs_flush(ctx, es, errs) : MZGPU_OK;
 }
 extern "C" int32_t mzgpu_half_join_many(mzgpu_ctx* ctx, uint32_t k, mzgpu_buf* const* streams,
                                         mzgpu_spine* const* traces, const int32_t* cmp_modes,
@@ -2427,6 +2625,21 @@ extern "C" int32_t mzgpu_half_join_many(mzgpu_ctx* ctx, uint32_t k, mzgpu_buf* c
   return half_join_many_entry(ctx, k, arrays_ok, [&](uint32_t j) {
     return HalfJoinReq{streams[j], traces[j], cmp_modes[j], closures ? closures[j] : nullptr, outs[j]};
   });
+}
+extern "C" int32_t mzgpu_half_join_many_mfp(mzgpu_ctx* ctx, uint32_t k, mzgpu_buf* const* streams,
+                                            mzgpu_spine* const* traces, const int32_t* cmp_modes,
+                                            const mzgpu_join_closure* const* jcs, mzgpu_buf* const* outs,
+                                            mzgpu_buf* errs) {
+  const bool arrays_ok = streams != nullptr && traces != nullptr && cmp_modes != nullptr && jcs != nullptr &&
+                         outs != nullptr && errs != nullptr;
+  return half_join_many_entry(
+      ctx, k, arrays_ok,
+      [&](uint32_t j) {
+        HalfJoinReq r{streams[j], traces[j], cmp_modes[j], nullptr, outs[j]};
+        r.jc = jcs[j];
+        return r;
+      },
+      errs);
 }
 extern "C" int32_t mzgpu_delta_first_stage_many(mzgpu_ctx* ctx, uint32_t k, mzgpu_batch* const* batches,
                                                 const mzgpu_closure* const* initial_closures,

@@ -127,6 +127,21 @@ struct ProbeSmem {
   ProbeWarpSmem w[PT / 32];
 };
 
+// The closure a probe applies to each match: the bit-field closure of ProbeParams (mzgpu_closure, or the R40
+// identity without one), or an MfpPlan (mzgpu_join_closure) over the words (key, va, vb) whose errors become R32
+// rows (code, payload, time, diff) at warp-aggregated slots *err_len++ of `errs` (err_cap rows; the host sizes it
+// so that it cannot fill, a slot past it is reported through the status word and not written).
+struct BitClosure {
+  static constexpr bool MFP = false;
+};
+struct MfpClosure {
+  static constexpr bool MFP = true;
+  const MfpDevPlan* pl;
+  u64* errs;
+  u64 err_cap;
+  unsigned long long* err_len;
+};
+
 struct ProbePre {  // optional map in front of the probe (build_update_stream fused in)
   int has_pre, pre_has_closure;
   u64 skip_time;
@@ -192,13 +207,16 @@ __device__ __forceinline__ u32 warp_exclusive_scan(u32 v, u32* total) {
 // [row0 + w * TRW, + TRW), one per lane.  The warps of the CTA run on their own -- private hit
 // lists, warp scans, no block barrier -- up to the point where the tile's total is needed for the
 // look-back (one barrier), so one warp's memory latency never stalls the other seven.
-template <int OUT_NW>
+template <int OUT_NW, class CL>
 __device__ __forceinline__ void probe_tile(ProbeSmem& S, const u64* __restrict__ stream, u64 n, u64 row0, u32 TRW,
                                            const TraceView& tv, const ProbeParams& pp, const ProbePre& pre,
                                            const LookBack& lb, u32 tile, u64* __restrict__ out, u64 base0,
-                                           u64 out_cap, u64* __restrict__ status, u64* excl_out, u32* total_out) {
+                                           u64 out_cap, u64* __restrict__ status, u64* excl_out, u32* total_out,
+                                           const CL& cl) {
   constexpr int GROUP = 8;
-  constexpr int U = 4;  // candidates per lane and step: their searches and row loads overlap
+  // candidates per lane and step: their searches and row loads overlap (an MfpPlan closure keeps one: the
+  // interpreter's state leaves no registers for more)
+  constexpr int U = CL::MFP ? 1 : 4;
   const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   ProbeWarpSmem& W = S.w[warp];
   // ---- 1. this lane's probe row
@@ -294,7 +312,8 @@ __device__ __forceinline__ void probe_tile(ProbeSmem& S, const u64* __restrict__
   __syncwarp();
   // ---- 3. the candidate walk (pass 0 counts, pass 1 writes).  The first 32 * U candidates --
   // all of them for most warps -- are evaluated once and kept in registers across the look-back.
-  auto eval = [&](u32 c, bool valid, u64* row) -> bool {
+  // An MfpPlan closure's error (*err) leaves its R32 error row in row[0..4); it is written in pass 1 only.
+  auto eval = [&](u32 c, bool valid, u64* row, bool* err) -> bool {
     // the hit this candidate belongs to: last h with hit_pref[h] <= c
     u32 lo = 0, hi = n_hits;
     while (hi - lo > 1) {
@@ -328,7 +347,25 @@ __device__ __forceinline__ void probe_tile(ProbeSmem& S, const u64* __restrict__
     }
     const u64 d = pd * rtd.y;
     const u64 va = pp.swap_vals ? rkv.y : pv, vb = pp.swap_vals ? pv : rkv.y;
-    if (OUT_NW == 4) {
+    if constexpr (CL::MFP) {
+      const u64 w[3] = {pk, va, vb};
+      u64 mv[MZGPU_MFP_MAX_MAPS];
+      u32 e_code = 0;
+      u64 e_pay = 0;
+      keep = mfp_filter_map(*cl.pl, w, mv, &e_code, &e_pay);
+      if (e_code) {
+        *err = true;
+        row[0] = e_code;
+        row[1] = e_pay;
+        row[2] = t;
+        row[3] = d;
+        return false;
+      }
+      if (!keep) return false;
+      mfp_project<OUT_NW>(*cl.pl, w, mv, row);
+      row[OUT_NW - 2] = t;
+      row[OUT_NW - 1] = d;
+    } else if (OUT_NW == 4) {
       u64 k, v;
       keep = closure_eval(pp.closure, pk, va, vb, &k, &v);
       row[0] = k;
@@ -344,19 +381,21 @@ __device__ __forceinline__ void probe_tile(ProbeSmem& S, const u64* __restrict__
     }
     return keep;
   };
-  bool keep0[U];
+  bool keep0[U], err0[U];
   u64 row0r[U][OUT_NW];
   u32 run = 0;
 #pragma unroll
   for (int u = 0; u < U; ++u) {
     const u32 c = (u32)u * 32 + lane;
-    keep0[u] = eval(c, c < n_cand, row0r[u]);
+    err0[u] = false;
+    keep0[u] = eval(c, c < n_cand, row0r[u], &err0[u]);
     run += __popc(__ballot_sync(0xffffffffu, keep0[u]));
   }
 #pragma unroll 1
   for (u32 c0 = 32 * U; c0 < n_cand; c0 += 32) {  // (rare: more than 128 candidates in one warp)
     u64 row[OUT_NW];
-    const bool k = eval(c0 + lane, c0 + lane < n_cand, row);
+    bool err = false;
+    const bool k = eval(c0 + lane, c0 + lane < n_cand, row, &err);
     run += __popc(__ballot_sync(0xffffffffu, k));
   }
   // ---- 4. the tile's total, the look-back
@@ -372,7 +411,17 @@ __device__ __forceinline__ void probe_tile(ProbeSmem& S, const u64* __restrict__
   const u64 excl = lb_exclusive_prefix(lb, tile, (u64)total, &S.bcast);
   u64 pos = base0 + excl + mine;
   // ---- 5. write
-  auto put = [&](bool keep, const u64* row) {
+  auto put = [&](bool keep, bool err, const u64* row) {
+    if constexpr (CL::MFP) {
+      const u64 p = warp_reserve(err ? 1u : 0u, cl.err_len);
+      if (err && p >= cl.err_cap) {
+        atomicMax((unsigned long long*)status, ~0ull);
+      } else if (err) {
+        u64* o = cl.errs + p * 4;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) o[w] = row[w];
+      }
+    }
     const u32 m = __ballot_sync(0xffffffffu, keep);
     if (keep) {
       const u64 p = pos + __popc(m & ((1u << lane) - 1));
@@ -387,23 +436,25 @@ __device__ __forceinline__ void probe_tile(ProbeSmem& S, const u64* __restrict__
     pos += __popc(m);
   };
 #pragma unroll
-  for (int u = 0; u < U; ++u) put(keep0[u], row0r[u]);
+  for (int u = 0; u < U; ++u) put(keep0[u], err0[u], row0r[u]);
 #pragma unroll 1
   for (u32 c0 = 32 * U; c0 < n_cand; c0 += 32) {
     u64 row[OUT_NW];
-    const bool k = eval(c0 + lane, c0 + lane < n_cand, row);
-    put(k, row);
+    bool err = false;
+    const bool k = eval(c0 + lane, c0 + lane < n_cand, row, &err);
+    put(k, err, row);
   }
   *excl_out = excl;
   *total_out = total;
 }
 
-template <int OUT_NW>
+template <int OUT_NW, class CL = BitClosure>
 __global__ void __launch_bounds__(PT, 3) k_probe_lb(const u64* __restrict__ stream, const DLen dn,
                                                  const __grid_constant__ TraceView tv,
                                                  const __grid_constant__ ProbeParams pp, const LookBack lb,
                                                  u64* __restrict__ out, const DLen out_base, u64 out_cap,
-                                                 u64* __restrict__ out_len, u64* __restrict__ status, u32 tile_rows) {
+                                                 u64* __restrict__ out_len, u64* __restrict__ status, u32 tile_rows,
+                                                 const CL cl) {
   __shared__ ProbeSmem S;
   const u64 n = dlen_get(dn);
   const u32 TR = tile_rows;
@@ -422,8 +473,8 @@ __global__ void __launch_bounds__(PT, 3) k_probe_lb(const u64* __restrict__ stre
     }
     u64 excl;
     u32 total;
-    probe_tile<OUT_NW>(S, stream, n, (u64)tile * TR, TR / (PT / 32), tv, pp, pre, lb, tile, out, base0, out_cap, status,
-                       &excl, &total);
+    probe_tile<OUT_NW, CL>(S, stream, n, (u64)tile * TR, TR / (PT / 32), tv, pp, pre, lb, tile, out, base0, out_cap,
+                           status, &excl, &total, cl);
     if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *out_len = base0 + excl + total;
   }
 }
@@ -462,10 +513,16 @@ struct ProbeMany {
   ProbeJobDev job[PROBE_MANY_MAX];
 };
 static_assert(sizeof(ProbeMany) <= 32000, "kernel parameter space");
+// the closure policy of each job of a launch (a job's MfpPlan lives in device memory: three more plans would not fit)
+template <class CL>
+struct ProbeClosures {
+  CL c[PROBE_MANY_MAX];
+};
 
-template <int OUT_NW>
+template <int OUT_NW, class CL = BitClosure>
 __global__ void __launch_bounds__(PT, 3) k_probe_chains(const __grid_constant__ ProbeMany m,
-                                                     u64* __restrict__ status) {
+                                                     u64* __restrict__ status,
+                                                     const __grid_constant__ ProbeClosures<CL> cls) {
   __shared__ ProbeSmem S;
   // The chains of a launch differ in size by an order of magnitude (the lineitem path of a Q3 step
   // carries four times the rows of the orders path, the customer path none): the resident CTAs are
@@ -501,8 +558,8 @@ __global__ void __launch_bounds__(PT, 3) k_probe_chains(const __grid_constant__ 
     pre.pre = &J.pre;
     u64 excl;
     u32 total;
-    probe_tile<OUT_NW>(S, J.stream, nj[q], (u64)(tile - tiles_before[q]) * trj[q], trj[q] / (PT / 32), J.tv, J.pp, pre,
-                       ch.lb, tile, ch.out, base0, ch.out_cap, status, &excl, &total);
+    probe_tile<OUT_NW, CL>(S, J.stream, nj[q], (u64)(tile - tiles_before[q]) * trj[q], trj[q] / (PT / 32), J.tv, J.pp,
+                           pre, ch.lb, tile, ch.out, base0, ch.out_cap, status, &excl, &total, cls.c[ch.first + q]);
     if ((u64)tile == n_tiles - 1 && threadIdx.x == 0) *ch.out_len = base0 + excl + total;
   }
 }
@@ -555,14 +612,16 @@ __global__ void __launch_bounds__(PT) k_map_rows_lb(const u64* __restrict__ rows
   }
 }
 
-template <int OUT_NW, bool WRITE>
+// An MfpPlan closure (CL::MFP): the count pass counts the output rows per probe row and adds the error rows to
+// *cl.err_len; the write pass writes both, the errors at slots *cl.err_len++ (a second counter).
+template <int OUT_NW, bool WRITE, class CL = BitClosure>
 __global__ void __launch_bounds__(PT) k_probe(const u64* __restrict__ stream, u64 n,
                                               const __grid_constant__ TraceView tv,
                                               const __grid_constant__ ProbeParams pp,
                                               u32* __restrict__ tile_counts,
                                               const u32* __restrict__ tile_base,
                                               u32* __restrict__ row_counts,
-                                              u64* __restrict__ out) {
+                                              u64* __restrict__ out, const CL cl) {
   __shared__ u32 sm[34];
   const u64 i = (u64)blockIdx.x * PT + threadIdx.x;
   u64 key = 0, v1 = 0, t1 = 0;
@@ -574,9 +633,23 @@ __global__ void __launch_bounds__(PT) k_probe(const u64* __restrict__ stream, u6
       key = stream[i * 4];
       t1 = stream[i * 4 + 2];
       v1 = pp.has_closure ? stream[i * 4 + 1] : 0;
+      if constexpr (CL::MFP) {
+        v1 = stream[i * 4 + 1];
+        u32 errs = 0;
+        for_each_match<1>(tv, key, t1, pp.mode, [&](u64 v2, u64 t2, i64 d2) {
+          const u64 w[3] = {key, pp.swap_vals ? v2 : v1, pp.swap_vals ? v1 : v2};
+          u64 mv[MZGPU_MFP_MAX_MAPS];
+          u32 e_code = 0;
+          u64 e_pay = 0;
+          if (mfp_filter_map(*cl.pl, w, mv, &e_code, &e_pay)) cnt++;
+          if (e_code) errs++;
+        });
+        if (errs) atomicAdd(cl.err_len, (unsigned long long)errs);
+        row_counts[i] = cnt;
+      }
       u32 runs = 0;
       const bool whole_runs = pp.mode == MZ_PROBE_JOIN && !pp.has_closure;
-      for_each_match<1>(
+      if constexpr (!CL::MFP) for_each_match<1>(
           tv, key, t1, pp.mode,
           [&](u64 v2, u64 t2, i64 d2) {
             if (pp.has_closure) {
@@ -588,7 +661,7 @@ __global__ void __launch_bounds__(PT) k_probe(const u64* __restrict__ stream, u6
           },
           whole_runs ? &runs : nullptr);
       cnt += runs;
-      row_counts[i] = cnt;
+      if constexpr (!CL::MFP) row_counts[i] = cnt;
     } else {
       // the write pass takes the row's count from the count pass: one walk per pass
       cnt = row_counts[i];
@@ -606,7 +679,7 @@ __global__ void __launch_bounds__(PT) k_probe(const u64* __restrict__ stream, u6
     if (threadIdx.x == 0) tile_counts[blockIdx.x] = total;
     return;
   }
-  if (i < n && cnt > 0) {
+  if (i < n && (cnt > 0 || CL::MFP)) {
     u64 pos = (u64)tile_base[blockIdx.x] + ex;
     for_each_match<1>(tv, key, t1, pp.mode, [&](u64 v2, u64 t2, i64 d2) {
       u64 t = t1;
@@ -616,7 +689,26 @@ __global__ void __launch_bounds__(PT) k_probe(const u64* __restrict__ stream, u6
       }
       u64 d = (u64)d1 * (u64)d2;
       u64 a = pp.swap_vals ? v2 : v1, b = pp.swap_vals ? v1 : v2;
-      if (OUT_NW == 4) {
+      if constexpr (CL::MFP) {
+        const u64 w[3] = {key, a, b};
+        u64 mv[MZGPU_MFP_MAX_MAPS];
+        u32 e_code = 0;
+        u64 e_pay = 0;
+        if (mfp_filter_map(*cl.pl, w, mv, &e_code, &e_pay)) {
+          u64 r[OUT_NW];
+          mfp_project<OUT_NW>(*cl.pl, w, mv, r);
+          r[OUT_NW - 2] = t;
+          r[OUT_NW - 1] = d;
+          store_row<OUT_NW>(out, pos, r);
+          pos++;
+        } else if (e_code) {
+          const u64 p = atomicAdd(cl.err_len, 1ull);
+          if (p < cl.err_cap) {
+            u64 e[4] = {e_code, e_pay, t, d};
+            store_row<4>(cl.errs, p, e);
+          }
+        }
+      } else if (OUT_NW == 4) {
         u64 k, v;
         if (closure_eval(pp.closure, key, a, b, &k, &v)) {
           u64 r[4] = {k, v, t, d};
@@ -670,11 +762,24 @@ __global__ void __launch_bounds__(PT) k_map_rows(const u64* __restrict__ rows, u
   if (keep) store_row<4>(out, (u64)tile_base[blockIdx.x] + ex, r);
 }
 
+MfpClosure mfp_closure(const MfpProbe& m, u64* errs, u64 err_cap, u64* err_len) {
+  MfpClosure c;
+  c.pl = m.pl;
+  c.errs = errs;
+  c.err_cap = err_cap;
+  c.err_len = (unsigned long long*)err_len;
+  return c;
+}
+
 }  // namespace
 
+static int32_t mz_probe_mfp(mzgpu_ctx* ctx, const u64* d_stream, u64 n, const TraceView& trace, const ProbeParams& pp,
+                            const MfpProbe& mfp, DevMem* out, u64* n_out, DevMem* errs, u64* n_errs);
+
 int32_t mz_probe(mzgpu_ctx* ctx, const u64* d_stream, u64 n, const TraceView& trace,
-                 const ProbeParams& pp, DevMem* out, u64* n_out) {
+                 const ProbeParams& pp, DevMem* out, u64* n_out, const MfpProbe* mfp, DevMem* errs, u64* n_errs) {
   *n_out = 0;
+  if (mfp != nullptr) return mz_probe_mfp(ctx, d_stream, n, trace, pp, *mfp, out, n_out, errs, n_errs);
   const int out_rb = pp.has_closure ? 32 : 40;
   if (n == 0 || trace.n_batches == 0) return out->alloc(ctx, 16);
   const u64 n_tiles = (n + PT - 1) / PT;
@@ -684,10 +789,10 @@ int32_t mz_probe(mzgpu_ctx* ctx, const u64* d_stream, u64 n, const TraceView& tr
   u64* d_total = ctx->d_scratch + 28;
   if (pp.has_closure) {
     MZ_LAUNCH(ctx, (k_probe<4, false>), (unsigned)n_tiles, PT, 0, d_stream, n, trace, pp, tiles.as<u32>(),
-              (const u32*)nullptr, row_counts.as<u32>(), (u64*)nullptr);
+              (const u32*)nullptr, row_counts.as<u32>(), (u64*)nullptr, BitClosure{});
   } else {
     MZ_LAUNCH(ctx, (k_probe<5, false>), (unsigned)n_tiles, PT, 0, d_stream, n, trace, pp, tiles.as<u32>(),
-              (const u32*)nullptr, row_counts.as<u32>(), (u64*)nullptr);
+              (const u32*)nullptr, row_counts.as<u32>(), (u64*)nullptr, BitClosure{});
   }
   MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
   MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 28, d_total, 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -701,10 +806,58 @@ int32_t mz_probe(mzgpu_ctx* ctx, const u64* d_stream, u64 n, const TraceView& tr
   MZ_BYTES(ctx, n * (32 + 16 * trace.n_batches) + total * (32 + out_rb));
   if (pp.has_closure) {
     MZ_LAUNCH(ctx, (k_probe<4, true>), (unsigned)n_tiles, PT, 0, d_stream, n, trace, pp, (u32*)nullptr,
-              tiles.as<u32>(), row_counts.as<u32>(), out->as<u64>());
+              tiles.as<u32>(), row_counts.as<u32>(), out->as<u64>(), BitClosure{});
   } else {
     MZ_LAUNCH(ctx, (k_probe<5, true>), (unsigned)n_tiles, PT, 0, d_stream, n, trace, pp, (u32*)nullptr,
-              tiles.as<u32>(), row_counts.as<u32>(), out->as<u64>());
+              tiles.as<u32>(), row_counts.as<u32>(), out->as<u64>(), BitClosure{});
+  }
+  return MZGPU_OK;
+}
+
+// The two-pass probe with an MfpPlan closure: the count pass counts output rows per probe row and the error rows
+// in all (one wait reads both totals), the write pass writes the output rows in order and the error rows at
+// atomic slots of an exactly sized array.
+static int32_t mz_probe_mfp(mzgpu_ctx* ctx, const u64* d_stream, u64 n, const TraceView& trace, const ProbeParams& pp,
+                            const MfpProbe& mfp, DevMem* out, u64* n_out, DevMem* errs, u64* n_errs) {
+  *n_errs = 0;
+  if (n == 0 || trace.n_batches == 0) {
+    MZ_TRY(errs->alloc(ctx, 16));
+    return out->alloc(ctx, 16);
+  }
+  const u64 n_tiles = (n + PT - 1) / PT;
+  DevMem tiles, row_counts;
+  MZ_TRY(tiles.alloc(ctx, n_tiles * 4));
+  MZ_TRY(row_counts.alloc(ctx, n * 4));
+  u64* d_total = ctx->d_scratch + 28;  // [0] output rows (k_scan_tiles), [1] error rows
+  u64* d_errs = ctx->d_scratch + 29;
+  MZ_CUDA(ctx, cudaMemsetAsync(d_errs, 0, 8, ctx->stream));
+  const MfpClosure cnt = mfp_closure(mfp, nullptr, 0, d_errs);
+  if (mfp.out_rb == 32) {
+    MZ_LAUNCH(ctx, (k_probe<4, false, MfpClosure>), (unsigned)n_tiles, PT, 0, d_stream, n, trace, pp, tiles.as<u32>(),
+              (const u32*)nullptr, row_counts.as<u32>(), (u64*)nullptr, cnt);
+  } else {
+    MZ_LAUNCH(ctx, (k_probe<5, false, MfpClosure>), (unsigned)n_tiles, PT, 0, d_stream, n, trace, pp, tiles.as<u32>(),
+              (const u32*)nullptr, row_counts.as<u32>(), (u64*)nullptr, cnt);
+  }
+  MZ_LAUNCH(ctx, k_scan_tiles, 1, 1024, 0, tiles.as<u32>(), n_tiles, d_total);
+  MZ_CUDA(ctx, cudaMemcpyAsync(ctx->h_scratch + 28, d_total, 16, cudaMemcpyDeviceToHost, ctx->stream));
+  MZ_SYNC(ctx);
+  ctx->stats.d2h_bytes += 16;
+  const u64 total = ctx->h_scratch[28], n_err = ctx->h_scratch[29];
+  MZ_TRY(out->alloc(ctx, total * mfp.out_rb));
+  MZ_TRY(errs->alloc(ctx, n_err * 32));
+  *n_out = total;
+  *n_errs = n_err;
+  if (total == 0 && n_err == 0) return MZGPU_OK;
+  MZ_BYTES(ctx, n * (32 + 16 * trace.n_batches) + total * (32 + mfp.out_rb) + n_err * 64);
+  MZ_CUDA(ctx, cudaMemsetAsync(d_errs, 0, 8, ctx->stream));
+  const MfpClosure wr = mfp_closure(mfp, errs->as<u64>(), n_err, d_errs);
+  if (mfp.out_rb == 32) {
+    MZ_LAUNCH(ctx, (k_probe<4, true, MfpClosure>), (unsigned)n_tiles, PT, 0, d_stream, n, trace, pp, (u32*)nullptr,
+              tiles.as<u32>(), row_counts.as<u32>(), out->as<u64>(), wr);
+  } else {
+    MZ_LAUNCH(ctx, (k_probe<5, true, MfpClosure>), (unsigned)n_tiles, PT, 0, d_stream, n, trace, pp, (u32*)nullptr,
+              tiles.as<u32>(), row_counts.as<u32>(), out->as<u64>(), wr);
   }
   return MZGPU_OK;
 }
@@ -748,19 +901,29 @@ static unsigned probe_grid(mzgpu_ctx* ctx, u64 tiles) {
 }
 
 int32_t mz_probe_async(mzgpu_ctx* ctx, const u64* d_stream, DLen n, u64 n_ub, const TraceView& trace,
-                       const ProbeParams& pp, u64* d_out, DLen out_base, u64 out_cap, u64* d_out_len) {
+                       const ProbeParams& pp, u64* d_out, DLen out_base, u64 out_cap, u64* d_out_len,
+                       const MfpProbe* mfp) {
   LookBack lb;
   const u64 tiles = mz_probe_tiles(n_ub, trace.n_batches);
   const u32 tr = (u32)mz_probe_tile_rows(n_ub, trace.n_batches);
   MZ_TRY(mz_lookback_begin(ctx, tiles, &lb));
-  const int out_rb = pp.has_closure ? 32 : 40;
+  const int out_rb = mfp != nullptr ? mfp->out_rb : pp.has_closure ? 32 : 40;
   MZ_BYTES(ctx, n.p == nullptr ? n.imm * (32 + 16 * trace.n_batches + 32 + out_rb) : 0);  // exact counts only
-  if (pp.has_closure) {
+  if (mfp != nullptr) {
+    const MfpClosure cl = mfp_closure(*mfp, mfp->errs, mfp->err_cap, mfp->err_len);
+    if (out_rb == 32) {
+      MZ_LAUNCH(ctx, (k_probe_lb<4, MfpClosure>), probe_grid(ctx, tiles), PT, 0, d_stream, n, trace, pp, lb, d_out,
+                out_base, out_cap, d_out_len, ctx->d_status, tr, cl);
+    } else {
+      MZ_LAUNCH(ctx, (k_probe_lb<5, MfpClosure>), probe_grid(ctx, tiles), PT, 0, d_stream, n, trace, pp, lb, d_out,
+                out_base, out_cap, d_out_len, ctx->d_status, tr, cl);
+    }
+  } else if (pp.has_closure) {
     MZ_LAUNCH(ctx, (k_probe_lb<4>), probe_grid(ctx, tiles), PT, 0, d_stream, n, trace, pp, lb, d_out, out_base, out_cap,
-              d_out_len, ctx->d_status, tr);
+              d_out_len, ctx->d_status, tr, BitClosure{});
   } else {
     MZ_LAUNCH(ctx, (k_probe_lb<5>), probe_grid(ctx, tiles), PT, 0, d_stream, n, trace, pp, lb, d_out, out_base, out_cap,
-              d_out_len, ctx->d_status, tr);
+              d_out_len, ctx->d_status, tr, BitClosure{});
   }
   return MZGPU_OK;
 }
@@ -776,6 +939,10 @@ int32_t mz_probe_async_many(mzgpu_ctx* ctx, int k, const ProbeJobHost* jobs) {
   static thread_local ProbeMany m;  // large: kept off the stack
   memset(&m, 0, sizeof(m));
   const bool closure = jobs[0].pp->has_closure != 0;
+  const bool mfp = jobs[0].mfp != nullptr;
+  const int out_rb = mfp ? jobs[0].mfp->out_rb : closure ? 32 : 40;
+  ProbeClosures<MfpClosure> mcl;
+  memset(&mcl, 0, sizeof(mcl));
   if (ctx->profile) {
     // per-kernel profiling: the algorithmic bytes of this launch need the actual stream lengths, which
     // live on the device -- one read-back ahead of the launch (outside its event bracket)
@@ -786,7 +953,8 @@ int32_t mz_probe_async_many(mzgpu_ctx* ctx, int k, const ProbeJobHost* jobs) {
   u64 lb_at = 0, max_grid = 1, bytes = 0, total_tiles = 0, chain_tiles[PROBE_MANY_MAX] = {};
   int nc = 0;
   for (int j = 0; j < k; ++j) {
-    if ((jobs[j].pp->has_closure != 0) != closure) {
+    if ((jobs[j].pp->has_closure != 0) != closure || (jobs[j].mfp != nullptr) != mfp ||
+        (mfp && jobs[j].mfp->out_rb != out_rb)) {
       MZ_SET_ERR(ctx, "probe: jobs of one launch must agree on the output row shape");
       return MZGPU_E_INVALID;
     }
@@ -799,6 +967,7 @@ int32_t mz_probe_async_many(mzgpu_ctx* ctx, int k, const ProbeJobHost* jobs) {
     m.job[j].skip_time = jobs[j].skip_time;
     if (m.job[j].pre_has_closure) m.job[j].pre = *jobs[j].pre;
     m.job[j].tile_rows = (u32)mz_probe_tile_rows(jobs[j].n_ub, jobs[j].trace->n_batches);
+    if (mfp) mcl.c[j] = mfp_closure(*jobs[j].mfp, jobs[j].mfp->errs, jobs[j].mfp->err_cap, jobs[j].mfp->err_len);
     if (j == 0 || jobs[j].chain != jobs[j - 1].chain) {
       ProbeChain& c = m.chain[nc++];
       c.first = (u32)j;
@@ -820,7 +989,7 @@ int32_t mz_probe_async_many(mzgpu_ctx* ctx, int k, const ProbeJobHost* jobs) {
       u64 rows_now = J.n.imm;
       if (J.n.p != nullptr)  // (profiling only: the arena was just read back)
         rows_now = (ctx->profile && J.n.p >= ctx->d_cnt && J.n.p < ctx->d_cnt + (size_t)MZ_CNT_BLOCKS * 4) ? ctx->h_cnt[J.n.p - ctx->d_cnt] : 0;
-      bytes += rows_now * (32 + 16 * J.trace->n_batches + 32 + (closure ? 32 : 40));
+      bytes += rows_now * (32 + 16 * J.trace->n_batches + 32 + out_rb);
     }
     MZ_TRY(mz_lookback_begin_at(ctx, lb_at, tiles, &m.chain[c].lb));
     lb_at += tiles;
@@ -839,10 +1008,18 @@ int32_t mz_probe_async_many(mzgpu_ctx* ctx, int k, const ProbeJobHost* jobs) {
     if (g > max_grid) max_grid = g;
   }
   MZ_BYTES(ctx, bytes);
-  if (closure) {
-    MZ_LAUNCH(ctx, (k_probe_chains<4>), dim3((unsigned)max_grid, (unsigned)nc), PT, 0, m, ctx->d_status);
+  if (mfp && out_rb == 32) {
+    MZ_LAUNCH(ctx, (k_probe_chains<4, MfpClosure>), dim3((unsigned)max_grid, (unsigned)nc), PT, 0, m, ctx->d_status,
+              mcl);
+  } else if (mfp) {
+    MZ_LAUNCH(ctx, (k_probe_chains<5, MfpClosure>), dim3((unsigned)max_grid, (unsigned)nc), PT, 0, m, ctx->d_status,
+              mcl);
+  } else if (closure) {
+    MZ_LAUNCH(ctx, (k_probe_chains<4>), dim3((unsigned)max_grid, (unsigned)nc), PT, 0, m, ctx->d_status,
+              ProbeClosures<BitClosure>{});
   } else {
-    MZ_LAUNCH(ctx, (k_probe_chains<5>), dim3((unsigned)max_grid, (unsigned)nc), PT, 0, m, ctx->d_status);
+    MZ_LAUNCH(ctx, (k_probe_chains<5>), dim3((unsigned)max_grid, (unsigned)nc), PT, 0, m, ctx->d_status,
+              ProbeClosures<BitClosure>{});
   }
   return MZGPU_OK;
 }

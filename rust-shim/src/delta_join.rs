@@ -47,3 +47,17 @@ pub fn first_stage(batches: &[*mut sys::Batch], initial: &[*const Closure], as_o
                                                                    closures.as_ptr(), outs.as_ptr()))
     }
 }
+
+/// The stage-s half joins with `JoinClosure`s outside `mzgpu_closure` (include/mzgpu.h:
+/// `mzgpu_half_join_many_mfp`): `closures[j]` from `mzgpu_join_closure_new`, the error rows of every
+/// request appended to `errs` (R32, consolidated), the input of the error collection.
+pub fn half_join_stage_mfp(streams: &[*mut sys::Buf], traces: &[*mut sys::Spine], less_equal: &[bool],
+                           closures: &[*const sys::JoinClosure], outs: &[*mut sys::Buf], errs: *mut sys::Buf)
+                           -> Result<(), (i32, String)> {
+    let cmps: Vec<_> = less_equal.iter().map(|&le| if le { sys::HALFJOIN_LE } else { sys::HALFJOIN_LT }).collect();
+    unsafe {
+        sys::check(worker_ctx(), sys::mzgpu_half_join_many_mfp(worker_ctx(), streams.len() as u32, streams.as_ptr(),
+                                                               traces.as_ptr(), cmps.as_ptr(), closures.as_ptr(),
+                                                               outs.as_ptr(), errs))
+    }
+}

@@ -48,3 +48,30 @@ impl Drop for GpuLinearJoin {
         unsafe { sys::mzgpu_linear_join_free(self.h); sys::mzgpu_buf_free(self.out); sys::mzgpu_buf_free(self.src); }
     }
 }
+
+/// One join_core stage with a `JoinClosure` outside `mzgpu_closure`, composed by hand (the plan
+/// descriptor takes bit-field closures only): `mzgpu_join_new_mfp` over the stream's and the lookup's
+/// arrangements, then `work` per activation; error rows (R32) go to the error collection.
+pub struct GpuJoinStageMfp { h: *mut sys::Join }
+
+impl GpuJoinStageMfp {
+    /// `jc` must outlive the stage.
+    pub fn new(t1: *mut sys::Spine, t2: *mut sys::Spine, jc: *const sys::JoinClosure) -> Result<Self, (i32, String)> {
+        let mut h = std::ptr::null_mut();
+        unsafe { sys::check(worker_ctx(), sys::mzgpu_join_new_mfp(worker_ctx(), t1, t2, jc, &mut h))?; }
+        Ok(GpuJoinStageMfp { h })
+    }
+
+    /// Work::process with the yield function: output and error rows count as fuel.  Returns done.
+    pub fn work(&mut self, fuel: u64, deadline_ns: u64, out: *mut sys::Buf, errs: *mut sys::Buf) -> Result<bool, (i32, String)> {
+        let mut done = 0i32;
+        unsafe { sys::check(worker_ctx(), sys::mzgpu_join_core_work_mfp(self.h, fuel, deadline_ns, out, errs, &mut done))?; }
+        Ok(done != 0)
+    }
+}
+
+impl Drop for GpuJoinStageMfp {
+    fn drop(&mut self) {
+        unsafe { sys::mzgpu_join_free(self.h); }
+    }
+}

@@ -93,6 +93,7 @@ pub const P2P_HANDLE_BYTES: usize = 64;
 
 /// A temporal filter operator (mzgpu_mfp_op), created from an `Mfp` plan.
 pub enum MfpOp {}
+pub enum JoinClosure {}
 pub const MFP_MAX_PREDICATES: usize = 4;
 pub const MFP_MAX_TEMPORAL: usize = 4;
 pub const MFP_MAX_OPS: usize = 16;
@@ -294,6 +295,14 @@ extern "C" {
     pub fn mzgpu_topk_basic_negatives_trace(r: *mut Reduce) -> *mut Spine;
     pub fn mzgpu_mfp_new(ctx: *mut Ctx, plan: *const Mfp, until: u64, out: *mut *mut MfpOp) -> i32;
     pub fn mzgpu_mfp_new_map(ctx: *mut Ctx, plan: *const Mfp, map: *const MfpMap, until: u64, out: *mut *mut MfpOp) -> i32;
+    // join closures: the device MfpPlan as the closure of the probe operators (mzgpu.h)
+    pub fn mzgpu_join_closure_new(ctx: *mut Ctx, plan: *const Mfp, map: *const MfpMap, out: *mut *mut JoinClosure) -> i32;
+    pub fn mzgpu_join_closure_free(jc: *mut JoinClosure);
+    pub fn mzgpu_half_join_mfp(ctx: *mut Ctx, stream: *const R32, n: u64, mem: i32, trace: *mut Spine, cmp_mode: i32, jc: *const JoinClosure, consolidate_output: i32, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_half_join_mfp_buf(ctx: *mut Ctx, stream: *mut Buf, trace: *mut Spine, cmp_mode: i32, jc: *const JoinClosure, consolidate_output: i32, out: *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_half_join_many_mfp(ctx: *mut Ctx, k: u32, streams: *const *mut Buf, traces: *const *mut Spine, cmp_modes: *const i32, jcs: *const *const JoinClosure, outs: *const *mut Buf, errs: *mut Buf) -> i32;
+    pub fn mzgpu_join_new_mfp(ctx: *mut Ctx, t1: *mut Spine, t2: *mut Spine, jc: *const JoinClosure, out: *mut *mut Join) -> i32;
+    pub fn mzgpu_join_core_work_mfp(j: *mut Join, fuel_rows: u64, deadline_ns: u64, out: *mut Buf, errs: *mut Buf, done: *mut i32) -> i32;
     pub fn mzgpu_mfp_free(op: *mut MfpOp);
     pub fn mzgpu_mfp_step(op: *mut MfpOp, rows: *const c_void, n: u64, mem: i32, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_mfp_step_buf(op: *mut MfpOp, rows: *mut Buf, upper: u64, out: *mut Buf, errs: *mut Buf) -> i32;
