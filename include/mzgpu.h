@@ -1504,6 +1504,109 @@ int32_t mzgpu_exchange_p2p_send(mzgpu_ctx* ctx, uint32_t k, mzgpu_buf** ins);
 int32_t mzgpu_exchange_p2p_recv(mzgpu_ctx* ctx, uint32_t k, mzgpu_buf** outs, const uint64_t* recv_ub);
 /* The routing function itself (for tests and host-side pre-partitioning). */
 uint32_t mzgpu_route(uint64_t key, uint32_t peers);
+/* ---- index peeks: a SELECT against an arrangement at a timestamp (IndexPeek::seek_fulfillment and
+ * collect_finished_data, src/compute/src/compute_state.rs:1433-1673; PeekResultIterator,
+ * src/compute/src/compute_state/peek_result_iterator.rs:40-304; RowSetFinishing, src/expr/src/relation.rs:3526-3646).
+ *
+ * The ok trace is an R32 (key, val) arrangement (mzgpu_spine of 32-byte rows); the optional error trace holds R32
+ * rows (code, payload, time, diff), the error rows every operator here emits, arranged by the caller.
+ *
+ * mzgpu_peek_plan_new(ctx, plan, map, fin, out) checks the plan once with the validation of mzgpu_mfp_new_map and
+ * keeps it, with the finishing, in device memory.  plan->in_row_bytes is 32 (the rows (key, val) the trace holds,
+ * MZGPU_SRC_KEY / VAL1); out_row_bytes is 32 or 40.  Refused, leaving no handle and the context usable:
+ * in_row_bytes != 32 and n_temporal != 0 (a peek's plan is a SafeMfpPlan: the adapter has replaced mz_now() by the
+ * timestamp) with MZGPU_E_INVALID, everything mzgpu_mfp_new_map refuses with its status, and a malformed finishing
+ * (more than MZGPU_MAX_ORDER_LANES lanes, unknown lane flags, a field outside the output row) with MZGPU_E_INVALID;
+ * a float64 order lane and a negative limit with MZGPU_E_UNSUPPORTED.  fin == NULL is no ORDER BY, no LIMIT, no
+ * OFFSET and the identity projection.  A call using the handle must not outlive it.
+ *
+ * mzgpu_finishing: order lanes read the plan's OUTPUT words (field.src MZGPU_SRC_KEY / VAL1 / VAL2 are output words 0,
+ * 1 and 2), encoded as the TopK rows are (signed lanes ^ 2^63, descending lanes complemented); limit (MZGPU_TOPK_NO_LIMIT
+ * = none), offset; and the projection, per output word an OR of bit-fields of the output words (as mzgpu_mfp's
+ * fields; no field for any word = the identity).  Order lanes may read words the projection then drops.
+ *
+ * mzgpu_peek_many(ctx, ok, errs_or_NULL, k, reqs, outs, results): k requests (1..MZGPU_PEEK_MANY_MAX), each with its
+ * plan, as_of, literal keys and max_rows.  literals == NULL is a full scan; otherwise the n_literals keys (in
+ * literals_mem space) are looked up, a duplicate once, so n_literals == 0 finds no rows.  For request i, results[i]:
+ *   MZGPU_PEEK_NOT_READY  the upper of the ok trace or of the error trace is <= as_of (nothing is appended);
+ *   MZGPU_PEEK_ERROR      kind and detail words, in this precedence:
+ *     MZGPU_PEEK_ERR_SINCE            the logical compaction of either trace is beyond as_of: (since, as_of)
+ *     MZGPU_PEEK_ERR_ERRS_ROW         the first (code, payload), in cursor order, of the error trace whose count at
+ *                                     as_of is positive: (code, payload)
+ *     MZGPU_PEEK_ERR_ERRS_RETRACTION  that first non-zero count is negative: (code, payload, count)
+ *     MZGPU_PEEK_ERR_MFP              the first failure in (key, val) order is an MfpPlan error: (code, payload, key, val)
+ *     MZGPU_PEEK_ERR_RETRACTION       ... a pair the plan keeps with a negative count: (key, val, count)
+ *     MZGPU_PEEK_ERR_TOO_LARGE        the finishing keeps more than max_rows rows (0 = no limit): (rows)
+ *   MZGPU_PEEK_ROWS       n_rows rows appended to outs[i] (the plan's out_row_bytes wide): (w0, w1[, w2], as_of,
+ *                         copies) in finishing order, copies clipped by the [offset, offset + limit) cut.
+ * Per pair (key, val) with time <= as_of accumulated to a non-zero count, in (key, val) order: the plan runs; an error
+ * fails the peek, a filtered pair is skipped (its count is never checked), a kept pair with a negative count fails it,
+ * and a kept pair gives its output row with the count as copies.  Output rows equal before the projection are one
+ * row (their copies summed); rows that become equal through the projection are not merged.
+ *
+ * Fixed-width stand-ins, chosen deliberately:
+ *   1. pairs with no count at as_of are not evaluated (the reference also runs the plan on pairs still physically in
+ *      the trace with a zero sum or only future times, which makes its errors depend on compaction state);
+ *   2. rows equal on every order lane are ordered by the output row's words as unsigned (before the projection), as
+ *      the TopK operators document;
+ *   3. LIMIT without ORDER BY keeps the first rows in that word order (the reference takes them in cursor order;
+ *      SQL allows any bag);
+ *   4. max_rows counts the rows the finishing keeps, in place of max_result_size's bytes of variable-width rows;
+ *   5. the literal columns an IndexedFilter appends equal the key by construction: the caller lowers them to
+ *      MZGPU_SRC_KEY.
+ *
+ * No peek modifies a trace: no compaction, no merge work, batches are only read (batches still being built through
+ * their device headers, a merge in flight on the side stream through its inputs).  A trace of more than 64 non-empty
+ * batches is MZGPU_E_UNSUPPORTED, as for the probes.  The call waits for the device once, for all k requests, to read
+ * the results: the answer goes to a client.  It waits before that only where the probes and the consolidation do: a
+ * call with literal requests first reads the row counts of the ok trace's batches still being built (the probe's
+ * fan-out bound needs them), a lookup on key runs longer than 1,024 rows counts its matches first, and more than
+ * 32 Mi gathered rows have their count read back before they are consolidated.  Device memory: the full scans are
+ * gathered once per distinct as_of, (ok trace rows) x (distinct as_of of the full scans) + (error trace rows) x
+ * (distinct as_of) rows of 40 bytes; the finishing rows, 72 bytes each, are at most one per kept pair and request
+ * at that pair's as_of.  mzgpu_peek is mzgpu_peek_many with k = 1.  A refused call (MZGPU_E_INVALID /
+ * _UNSUPPORTED) appends nothing and leaves results unspecified. */
+#define MZGPU_PEEK_MANY_MAX 64
+#define MZGPU_PEEK_ROWS 0
+#define MZGPU_PEEK_NOT_READY 1
+#define MZGPU_PEEK_ERROR 2
+#define MZGPU_PEEK_ERR_SINCE 1
+#define MZGPU_PEEK_ERR_ERRS_ROW 2
+#define MZGPU_PEEK_ERR_ERRS_RETRACTION 3
+#define MZGPU_PEEK_ERR_MFP 4
+#define MZGPU_PEEK_ERR_RETRACTION 5
+#define MZGPU_PEEK_ERR_TOO_LARGE 6
+typedef struct mzgpu_finishing {
+  uint32_t n_order;
+  mzgpu_order_lane order[MZGPU_MAX_ORDER_LANES];
+  int64_t limit;   /* MZGPU_TOPK_NO_LIMIT = none */
+  uint64_t offset;
+  uint32_t n_project[3]; /* fields of projected word 0, 1, 2 (2: 40-byte output only); all 0 = identity */
+  mzgpu_field project[3][MZGPU_MAX_FIELDS];
+} mzgpu_finishing;
+typedef struct mzgpu_peek_plan mzgpu_peek_plan;
+typedef struct mzgpu_peek_req {
+  const mzgpu_peek_plan* plan;
+  uint64_t as_of;
+  const uint64_t* literals; /* NULL = full scan */
+  uint64_t n_literals;
+  int32_t literals_mem;     /* MZGPU_MEM_HOST / MZGPU_MEM_DEVICE */
+  uint64_t max_rows;        /* 0 = none */
+} mzgpu_peek_req;
+typedef struct mzgpu_peek_result {
+  int32_t status;   /* MZGPU_PEEK_ROWS / NOT_READY / ERROR */
+  int32_t err_kind; /* MZGPU_PEEK_ERR_* for MZGPU_PEEK_ERROR, else 0 */
+  uint64_t n_rows;  /* rows appended to the request's output */
+  uint64_t detail[4];
+} mzgpu_peek_result;
+int32_t mzgpu_peek_plan_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map, const mzgpu_finishing* fin,
+                            mzgpu_peek_plan** out);
+void mzgpu_peek_plan_free(mzgpu_peek_plan* p);
+int32_t mzgpu_peek_many(mzgpu_ctx* ctx, mzgpu_spine* ok, mzgpu_spine* errs, uint32_t k, const mzgpu_peek_req* reqs,
+                        mzgpu_buf* const* outs, mzgpu_peek_result* results);
+int32_t mzgpu_peek(mzgpu_ctx* ctx, mzgpu_spine* ok, mzgpu_spine* errs, const mzgpu_peek_req* req, mzgpu_buf* out,
+                   mzgpu_peek_result* result);
+
 /* The device half of an exchange round on its own: the k buffers are bucketed by
  * destination for `peers` workers (any 1 <= peers <= 64, independent of the ctx's
  * own peer count) with the kernels mzgpu_exchange_many runs; outs[e] receives the

@@ -273,6 +273,44 @@ class LinearJoinPlan(C.Structure):
     ]
 
 
+# index peeks (mzgpu_peek_many, include/mzgpu.h)
+PEEK_MANY_MAX = 64
+PEEK_ROWS, PEEK_NOT_READY, PEEK_ERROR = 0, 1, 2
+PEEK_ERR_SINCE, PEEK_ERR_ERRS_ROW, PEEK_ERR_ERRS_RETRACTION = 1, 2, 3
+PEEK_ERR_MFP, PEEK_ERR_RETRACTION, PEEK_ERR_TOO_LARGE = 4, 5, 6
+
+
+class Finishing(C.Structure):
+    _fields_ = [
+        ("n_order", C.c_uint32),
+        ("order", OrderLane * MAX_ORDER_LANES),
+        ("limit", C.c_int64),
+        ("offset", C.c_uint64),
+        ("n_project", C.c_uint32 * 3),
+        ("project", (Field * 6) * 3),
+    ]
+
+
+class PeekReq(C.Structure):
+    _fields_ = [
+        ("plan", C.c_void_p),
+        ("as_of", C.c_uint64),
+        ("literals", C.c_void_p),
+        ("n_literals", C.c_uint64),
+        ("literals_mem", C.c_int32),
+        ("max_rows", C.c_uint64),
+    ]
+
+
+class PeekResult(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("err_kind", C.c_int32),
+        ("n_rows", C.c_uint64),
+        ("detail", C.c_uint64 * 4),
+    ]
+
+
 class Desc(C.Structure):
     _fields_ = [("lower", C.c_uint64), ("upper", C.c_uint64), ("since", C.c_uint64)]
 
@@ -388,6 +426,10 @@ SIGNATURES = {
     "mzgpu_mfp_free": (None, [vp]),
     "mzgpu_join_closure_new": (i32, [vp, C.POINTER(Mfp), C.POINTER(MfpMap), PV]),
     "mzgpu_join_closure_free": (None, [vp]),
+    "mzgpu_peek_plan_new": (i32, [vp, C.POINTER(Mfp), C.POINTER(MfpMap), C.POINTER(Finishing), PV]),
+    "mzgpu_peek_plan_free": (None, [vp]),
+    "mzgpu_peek_many": (i32, [vp, vp, vp, u32, C.POINTER(PeekReq), PV, C.POINTER(PeekResult)]),
+    "mzgpu_peek": (i32, [vp, vp, vp, C.POINTER(PeekReq), vp, C.POINTER(PeekResult)]),
     "mzgpu_half_join_mfp": (i32, [vp, vp, u64, i32, vp, i32, vp, i32, vp, vp]),
     "mzgpu_half_join_mfp_buf": (i32, [vp, vp, vp, i32, vp, i32, vp, vp]),
     "mzgpu_half_join_many_mfp": (i32, [vp, u32, vp, vp, vp, vp, vp, vp]),

@@ -1048,6 +1048,87 @@ class JoinClosure:
             self.h = None
 
 
+class PeekPlan:
+    """The plan of an index peek (mzgpu_peek_plan_new): an MfpPlan without temporal predicates over the trace's
+    (key, val) = SRC_KEY / SRC_VAL1 (the arguments of Mfp), and the finishing: `order` (order_lane() tuples over the
+    plan's OUTPUT words, at most 3), `limit` (None = no limit), `offset`, and `project` (per output word a list of
+    (src, shift, bits, dst_shift) fields over the output words; () = the identity).  Pass it to peek / peek_many."""
+
+    def __init__(self, ctx, fields, predicates=(), consts=(), out_rb=32, maps=(), map_consts=(), order=(), limit=None,
+                 offset=0, project=(), in_row_bytes=32, temporal=()):
+        self.ctx, self.out_row_bytes = ctx, out_rb
+        m, mp = _mfp_structs(fields, predicates, temporal, consts, in_row_bytes, out_rb, maps, map_consts)
+        fin = F.Finishing()
+        fin.n_order = len(order)
+        for i, (src, shift, bits, sx, desc, f64) in enumerate(order[:F.MAX_ORDER_LANES]):
+            fin.order[i].sign_extend, fin.order[i].descending = int(sx), int(desc)
+            fin.order[i].flags = F.ORDER_F64 if f64 else 0
+            fin.order[i].field = F.Field(src, shift, bits, 0)
+        fin.limit = F.TOPK_NO_LIMIT if limit is None else int(limit)
+        fin.offset = int(offset)
+        for w, fl in enumerate(project):
+            fin.n_project[w] = len(fl)
+            for i, f in enumerate(fl[:6]):
+                fin.project[w][i] = F.Field(*f)
+        h = C.c_void_p()
+        ctx.check(F.lib.mzgpu_peek_plan_new(ctx.h, C.byref(m), C.byref(mp) if mp is not None else None,
+                                            C.byref(fin), C.byref(h)))
+        self.h = h
+
+    def __del__(self):
+        if getattr(self, "h", None) and self.ctx.h:
+            F.lib.mzgpu_peek_plan_free(self.h)
+            self.h = None
+
+
+_NO_KEYS = np.zeros(1, dtype=np.uint64)  # the address of an empty literal list
+
+
+def _peek_req(req, plan, as_of, literals, max_rows, keep):
+    """Fill an mzgpu_peek_req; host arrays the call reads are appended to `keep`."""
+    req.plan, req.as_of, req.max_rows, req.literals_mem = plan.h, int(as_of), int(max_rows), F.MEM_HOST
+    if literals is not None:
+        arr = np.ascontiguousarray(np.asarray(literals, dtype=np.uint64).reshape(-1))
+        keep.append(arr)
+        req.literals = (arr if len(arr) else _NO_KEYS).ctypes.data
+        req.n_literals = len(arr)
+
+
+def _peek_result(res, out):
+    if res.status == F.PEEK_ROWS:
+        return ("rows", out.download())
+    if res.status == F.PEEK_NOT_READY:
+        return ("not_ready", None)
+    return ("error", (int(res.err_kind), tuple(int(x) for x in res.detail)))
+
+
+def peek_many(ctx, spine, requests, err_spine=None):
+    """k index peeks in one call (mzgpu_peek_many).  `requests` are dicts with `plan` (PeekPlan), `as_of` and
+    optionally `literals` (None = a full scan; a sequence of keys) and `max_rows` (0 = none).  Returns one result per
+    request, as peek() does."""
+    k = len(requests)
+    reqs, res, keep = (F.PeekReq * k)(), (F.PeekResult * k)(), []
+    outs = [DeviceRows(ctx, r["plan"].out_row_bytes) for r in requests]
+    for i, r in enumerate(requests):
+        _peek_req(reqs[i], r["plan"], r["as_of"], r.get("literals"), r.get("max_rows", 0), keep)
+    out_arr = (C.c_void_p * k)(*[o.h.value for o in outs])
+    ctx.check(F.lib.mzgpu_peek_many(ctx.h, spine.h, err_spine.h if err_spine is not None else None, k, reqs, out_arr,
+                                    res))
+    return [_peek_result(res[i], outs[i]) for i in range(k)]
+
+
+def peek(ctx, plan, spine, as_of, literals=None, err_spine=None, max_rows=0):
+    """One index peek (mzgpu_peek) of `spine` at `as_of`: ("rows", rows) -- (w0, w1[, w2], as_of, copies) in
+    finishing order --, ("not_ready", None) or ("error", (PEEK_ERR_* kind, four detail words)).  `literals` None is a
+    full scan, otherwise the keys to look up."""
+    req, res, keep = F.PeekReq(), F.PeekResult(), []
+    _peek_req(req, plan, as_of, literals, max_rows, keep)
+    out = DeviceRows(ctx, plan.out_row_bytes)
+    ctx.check(F.lib.mzgpu_peek(ctx.h, spine.h, err_spine.h if err_spine is not None else None, C.byref(req), out.h,
+                               C.byref(res)))
+    return _peek_result(res, out)
+
+
 def field_fn(i, shift=0, bits=64, dst_shift=0):
     """An output field taking bits [shift, shift + bits) of FlatMap extension column `i`, placed at `dst_shift`."""
     return (F.SRC_FN0 + i, shift, bits, dst_shift)

@@ -1301,6 +1301,65 @@ int32_t mz_fm_expand(mzgpu_ctx* ctx, const FlatMapDevPlan& pl, const u64* d_rows
 int32_t mz_fm_min_time(mzgpu_ctx* ctx, int iw, const u64* d_rows, const ulonglong2* incl, u64 n,
                        unsigned __int128 g, u64* d_min);
 
+// peek.cu: index peeks (mzgpu_peek_many).  A peek plan as the kernels read it: the MfpPlan over (key, val) and the
+// finishing -- order lanes over the output words (encoded as TopKOrder does), the [offset, end) cut in units and the
+// projection (identity when no word has fields).
+struct PeekFin {
+  mzgpu_field f[3];
+  u32 sign_extend[3];
+  u64 xm[3];
+  u32 n_order;
+  u32 out_words;  // 2 or 3
+  u64 offset, end;  // end = offset + limit, saturating; UINT64_MAX without a limit
+  u32 identity;
+  u32 n_project[3];
+  mzgpu_field project[3][MZGPU_MAX_FIELDS];
+};
+struct PeekDevPlan {
+  MfpDevPlan mfp;
+  PeekFin fin;
+};
+// A request as the kernels see it.  Gathered rows are R40 (slot, key, val, as_of, diff).  Slot i < k holds literal
+// request i's pairs; slot k + j the ok trace at the j-th distinct as_of of the full scans, shared by every full-scan
+// request at that as_of; slot err_base + j the error trace at the j-th distinct as_of.
+#define MZ_PEEK_K 64
+struct PeekScanJobs {  // the full scans of one trace: job j keeps rows with time <= as_of[j] as slot[j]
+  u32 n;
+  u32 slot[MZ_PEEK_K];
+  u64 as_of[MZ_PEEK_K];
+};
+struct PeekLitSegs {  // literal keys [start[s], start[s + 1]) belong to slot[s] at as_of[s]
+  u32 n;
+  u64 start[MZ_PEEK_K + 1];
+  u32 slot[MZ_PEEK_K];
+  u64 as_of[MZ_PEEK_K];
+};
+struct PeekReqs {
+  const PeekDevPlan* pl[MZ_PEEK_K];  // nullptr: the request is not run (decided on the host)
+  u64 as_of[MZ_PEEK_K];
+  u64 reqs[2 * MZ_PEEK_K];   // per ok slot (below err_base): the requests evaluated on its pairs, as a bit set
+  int err_slot[MZ_PEEK_K];  // the request's error-trace slot, -1: no error trace
+  u32 k;
+  u32 err_base;
+};
+struct PeekDevResult {
+  u64 kind;  // 0 or MZGPU_PEEK_ERR_*
+  u64 n_rows;
+  u64 lo;  // the request's rows are at staging byte offset lo * 40
+  u64 d[4];
+};
+int32_t mz_peek_scan(mzgpu_ctx* ctx, const TraceView& tv, const PeekScanJobs& jobs, u64* d_out, u64 cap, u64* d_len);
+int32_t mz_peek_lits(mzgpu_ctx* ctx, const u64* d_keys, const PeekLitSegs& segs, u64* d_rows);
+int32_t mz_peek_unit(mzgpu_ctx* ctx, u64* d_rows, DLen n, u64 n_ub);
+// pairs (consolidated R40 rows) -> 72-byte finishing rows (slot, o0, o1, o2, w0, w1, w2, copies, 0) at d_fin
+// (count at *d_fin_len, zeroed by the caller), one per request of the pair's slot; failures as atomicMin of the row
+// index into d_fail[request], an error-trace slot's first row into d_fail[slot]
+int32_t mz_peek_eval(mzgpu_ctx* ctx, const u64* d_pairs, DLen n, u64 n_ub, u64 fin_cap, const PeekReqs& rq, u64* d_fin,
+                     u64* d_fin_len, u64* d_fail);
+// one block per request: its failure detail, or its cut and projected rows into d_stage
+int32_t mz_peek_finish(mzgpu_ctx* ctx, const PeekReqs& rq, const u64* d_pairs, const u64* d_fail, const u64* d_fin,
+                       DLen n_fin, u64* d_stage, PeekDevResult* d_res);
+
 #ifdef __CUDACC__
 // ---------------------------------------------------------- the MfpPlan interpreter (mfp.cu, probe.cu)
 namespace {

@@ -5685,3 +5685,323 @@ extern "C" int32_t mzgpu_flat_map_stats(mzgpu_flat_map_op* op, uint64_t out[4]) 
   out[3] = left > (u128)~0ull ? ~0ull : (u64)left;
   return MZGPU_OK;
 }
+
+// ============================================================ index peeks
+// mzgpu_peek_many: gather every request's pairs (full scans and literal lookups) into one R40 buffer of rows
+// (slot, key, val, as_of, diff), consolidate it once, evaluate each request's plan per pair, consolidate the
+// finishing rows once (their word order is the finishing order), cut and project per request, and read the k
+// results back with one wait.
+static_assert(MZ_PEEK_K == MZGPU_PEEK_MANY_MAX, "one request slot per request of a call");
+struct mzgpu_peek_plan {
+  mzgpu_ctx* ctx;
+  uint32_t out_rb;
+  DevMem dev;  // PeekDevPlan
+};
+
+// a finishing field: a bit-field of an output word (VAL2 only of 40-byte output)
+static int32_t peek_field_check(mzgpu_ctx* ctx, const char* what, uint32_t i, const mzgpu_field& f, uint32_t out_rb,
+                                bool uses_dst) {
+  const uint32_t max_src = out_rb == 40 ? MZGPU_SRC_VAL2 : MZGPU_SRC_VAL1;
+  if (f.src > max_src || f.bits < 1 || f.bits > 64 || f.shift > 63 || (uint32_t)f.shift + f.bits > 64 ||
+      (uses_dst && f.dst_shift >= 64)) {
+    MZ_SET_ERR(ctx, "peek plan: %s %u is not a bit-field of the %u-byte output row", what, i, out_rb);
+    return MZGPU_E_INVALID;
+  }
+  return MZGPU_OK;
+}
+
+static int32_t peek_finishing(mzgpu_ctx* ctx, const mzgpu_finishing* fin, uint32_t out_rb, PeekFin* F) {
+  F->out_words = out_rb / 8 - 2;
+  F->offset = 0;
+  F->end = ~0ull;
+  F->identity = 1;
+  if (fin == nullptr) return MZGPU_OK;
+  if (fin->n_order > MZGPU_MAX_ORDER_LANES) {
+    MZ_SET_ERR(ctx, "peek plan: %u order lanes (0..%d)", fin->n_order, MZGPU_MAX_ORDER_LANES);
+    return MZGPU_E_INVALID;
+  }
+  int unsupported = -1;
+  for (uint32_t j = 0; j < fin->n_order; ++j) {
+    const mzgpu_order_lane& L = fin->order[j];
+    if ((L.flags & ~(uint32_t)MZGPU_ORDER_F64) != 0) {
+      MZ_SET_ERR(ctx, "peek plan: order lane %u: unknown flag bits", j);
+      return MZGPU_E_INVALID;
+    }
+    MZ_TRY(peek_field_check(ctx, "order lane", j, L.field, out_rb, false));
+    if ((L.flags & MZGPU_ORDER_F64) != 0 && unsupported < 0) unsupported = (int)j;
+    F->f[j] = L.field;
+    F->sign_extend[j] = L.sign_extend != 0;
+    F->xm[j] = (L.sign_extend ? 1ull << 63 : 0) ^ (L.descending ? ~0ull : 0);
+  }
+  for (uint32_t w = 0; w < 3; ++w) {
+    if (fin->n_project[w] > MZGPU_MAX_FIELDS || (w >= F->out_words && fin->n_project[w] != 0)) {
+      MZ_SET_ERR(ctx, "peek plan: %u projection fields for word %u of a %u-byte row", fin->n_project[w], w, out_rb);
+      return MZGPU_E_INVALID;
+    }
+    for (uint32_t i = 0; i < fin->n_project[w]; ++i)
+      MZ_TRY(peek_field_check(ctx, "projection field", i, fin->project[w][i], out_rb, true));
+    F->n_project[w] = fin->n_project[w];
+    for (uint32_t i = 0; i < fin->n_project[w]; ++i) F->project[w][i] = fin->project[w][i];
+    if (fin->n_project[w] != 0) F->identity = 0;
+  }
+  if (unsupported >= 0) {
+    MZ_SET_ERR(ctx, "peek plan: order lane %d: float64 order columns are not supported (OrderedFloat ties -0.0 with "
+                    "+0.0 and NaN payloads)", unsupported);
+    return MZGPU_E_UNSUPPORTED;
+  }
+  if (fin->limit < 0) {
+    MZ_SET_ERR(ctx, "peek plan: negative limit %lld", (long long)fin->limit);
+    return MZGPU_E_UNSUPPORTED;
+  }
+  F->n_order = fin->n_order;
+  F->offset = fin->offset;
+  if (fin->limit != MZGPU_TOPK_NO_LIMIT) {
+    const u64 lim = (u64)fin->limit;
+    F->end = fin->offset > ~0ull - lim ? ~0ull : fin->offset + lim;
+  }
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_peek_plan_new(mzgpu_ctx* ctx, const mzgpu_mfp* plan, const mzgpu_mfp_map* map,
+                                       const mzgpu_finishing* fin, mzgpu_peek_plan** out) {
+  MZ_CHECK_CTX(ctx);
+  if (plan == nullptr || out == nullptr) return MZGPU_E_INVALID;
+  if (plan->in_row_bytes != 32) {
+    MZ_SET_ERR(ctx, "peek plan: the input is the trace's (key, val), in_row_bytes 32, not %u", plan->in_row_bytes);
+    return MZGPU_E_INVALID;
+  }
+  if (plan->n_temporal != 0) {
+    MZ_SET_ERR(ctx, "peek plan: %u temporal predicates (a peek's plan is a SafeMfpPlan)", plan->n_temporal);
+    return MZGPU_E_INVALID;
+  }
+  std::unique_ptr<PeekDevPlan> pd(new PeekDevPlan());
+  memset(pd.get(), 0, sizeof(PeekDevPlan));
+  MZ_TRY(mfp_build_plan(ctx, plan, map, 0, &pd->mfp));
+  MZ_TRY(peek_finishing(ctx, fin, plan->out_row_bytes, &pd->fin));
+  auto p = std::unique_ptr<mzgpu_peek_plan>(new mzgpu_peek_plan());
+  p->ctx = ctx;
+  p->out_rb = plan->out_row_bytes;
+  MZ_TRY(p->dev.alloc(ctx, sizeof(PeekDevPlan)));
+  MZ_TRY(copy_in(ctx, p->dev.p, pd.get(), sizeof(PeekDevPlan), MZGPU_MEM_HOST));
+  *out = p.release();
+  return MZGPU_OK;
+}
+extern "C" void mzgpu_peek_plan_free(mzgpu_peek_plan* p) { delete p; }
+
+// rows of the readable batches (upper bounds for batches still in flight)
+static u64 peek_rows_ub(const std::vector<mzgpu_batch*>& bs) {
+  u64 n = 0;
+  for (auto* b : bs) n += b->st.known ? b->st.v[0] : b->len_ub;
+  return n;
+}
+
+// The literal requests' keys, deduplicated per request, looked up by the half-join probe: the stream rows
+// (key, slot, as_of, +1) under an identity MfpPlan that writes (slot, key, val) appends R40 rows to `g`.
+static int32_t peek_literals(mzgpu_ctx* ctx, const std::vector<mzgpu_batch*>& okb, const mzgpu_peek_req* reqs,
+                             const PeekLitSegs& segs, mzgpu_buf* g) {
+  const u64 n = segs.start[segs.n];
+  DevMem keys, rows, cons;
+  MZ_TRY(keys.alloc(ctx, n * 8));
+  for (u32 s = 0; s < segs.n; ++s) {
+    const mzgpu_peek_req& r = reqs[segs.slot[s]];
+    MZ_TRY(copy_in(ctx, keys.as<u64>() + segs.start[s], r.literals, r.n_literals * 8, r.literals_mem));
+  }
+  MZ_TRY(rows.alloc(ctx, n * 32));
+  MZ_TRY(mz_peek_lits(ctx, keys.as<u64>(), segs, rows.as<u64>()));
+  u64 ccap = 0;
+  Lazy4 clen;
+  MZ_TRY(consolidate_dev(ctx, 32, rows.p, dlen_imm(n), n, &cons, &ccap, &clen));
+  const DLen sn = dlen_of(clen, 0);
+  const u64 s_ub = clen.known ? clen.v[0] : std::min(ccap, n);
+  MZ_TRY(mz_peek_unit(ctx, cons.as<u64>(), sn, s_ub));
+  mzgpu_mfp idp;
+  memset(&idp, 0, sizeof(idp));
+  idp.in_row_bytes = idp.out_row_bytes = 40;
+  idp.n_fields[0] = idp.n_fields[1] = idp.n_fields[2] = 1;
+  idp.fields[0][0] = mzgpu_field{MZGPU_SRC_VAL1, 0, 64, 0};
+  idp.fields[1][0] = mzgpu_field{MZGPU_SRC_KEY, 0, 64, 0};
+  idp.fields[2][0] = mzgpu_field{MZGPU_SRC_VAL2, 0, 64, 0};
+  std::unique_ptr<mzgpu_join_closure> idc(new mzgpu_join_closure());
+  idc->ctx = ctx;
+  MZ_TRY(mfp_build_plan(ctx, &idp, nullptr, 0, &idc->pl));
+  MZ_TRY(idc->dev.alloc(ctx, sizeof(MfpDevPlan)));
+  MZ_TRY(copy_in(ctx, idc->dev.p, &idc->pl, sizeof(MfpDevPlan), MZGPU_MEM_HOST));
+  std::unique_ptr<TraceView> tv(new TraceView());
+  ProbePlan p;
+  MZ_TRY(probe_plan(ctx, okb, MZ_PROBE_HALF_LE, nullptr, 0, false, MZ_BOUND_MAX_ROWS * 32 / (40 + 32), tv.get(), &p,
+                    idc.get()));
+  ErrSink es;  // the identity plan raises no error
+  return probe_run(ctx, p, cons.as<u64>(), sn, s_ub, ProbeOut::APPEND, g, nullptr, &es);
+}
+
+extern "C" int32_t mzgpu_peek_many(mzgpu_ctx* ctx, mzgpu_spine* ok, mzgpu_spine* errs, uint32_t k,
+                                   const mzgpu_peek_req* reqs, mzgpu_buf* const* outs, mzgpu_peek_result* results) {
+  MZ_CHECK_CTX(ctx);
+  if (ok == nullptr || reqs == nullptr || outs == nullptr || results == nullptr || k == 0 || k > MZGPU_PEEK_MANY_MAX) {
+    MZ_SET_ERR(ctx, "peek: bad arguments (k = %u, 1..%d)", k, MZGPU_PEEK_MANY_MAX);
+    return MZGPU_E_INVALID;
+  }
+  if (ok->ctx != ctx || ok->rb != 32 || (errs != nullptr && (errs->ctx != ctx || errs->rb != 32))) {
+    MZ_SET_ERR(ctx, "peek: the ok and error traces are R32 arrangements of this context");
+    return MZGPU_E_INVALID;
+  }
+  for (uint32_t i = 0; i < k; ++i) {
+    const mzgpu_peek_req& r = reqs[i];
+    if (r.plan == nullptr || r.plan->ctx != ctx || outs[i] == nullptr || outs[i]->ctx != ctx ||
+        outs[i]->rb != r.plan->out_rb || (r.literals == nullptr && r.n_literals != 0) ||
+        (r.literals_mem != MZGPU_MEM_HOST && r.literals_mem != MZGPU_MEM_DEVICE)) {
+      MZ_SET_ERR(ctx, "peek: request %u: bad plan, output buffer or literal list", i);
+      return MZGPU_E_INVALID;
+    }
+  }
+  // the frontier checks of seek_fulfillment, on the host
+  const u64 since = std::max(ok->since, errs != nullptr ? errs->since : 0);
+  auto not_ready = [](const mzgpu_spine* s, u64 t) { return s->upper != MZGPU_FRONTIER_EMPTY && s->upper <= t; };
+  PeekReqs rq;
+  memset(&rq, 0, sizeof(rq));
+  rq.k = k;
+  PeekScanJobs ok_jobs, err_jobs;
+  memset(&ok_jobs, 0, sizeof(ok_jobs));
+  memset(&err_jobs, 0, sizeof(err_jobs));
+  PeekLitSegs segs;
+  memset(&segs, 0, sizeof(segs));
+  bool any = false;
+  u64 n_scan_reqs = 0;  // full-scan requests (each slot of the ok trace's scans is shared by the requests at its as_of)
+  for (uint32_t i = 0; i < k; ++i) {
+    const mzgpu_peek_req& r = reqs[i];
+    mzgpu_peek_result& res = results[i];
+    memset(&res, 0, sizeof(res));
+    rq.err_slot[i] = -1;
+    if (not_ready(ok, r.as_of) || (errs != nullptr && not_ready(errs, r.as_of))) {
+      res.status = MZGPU_PEEK_NOT_READY;
+      continue;
+    }
+    if (since > r.as_of) {
+      res.status = MZGPU_PEEK_ERROR;
+      res.err_kind = MZGPU_PEEK_ERR_SINCE;
+      res.detail[0] = since;
+      res.detail[1] = r.as_of;
+      continue;
+    }
+    any = true;
+    rq.pl[i] = r.plan->dev.as<PeekDevPlan>();
+    rq.as_of[i] = r.as_of;
+    if (errs != nullptr) {  // one error-trace scan per distinct as_of (its slot is numbered below)
+      uint32_t j = 0;
+      while (j < err_jobs.n && err_jobs.as_of[j] != r.as_of) ++j;
+      if (j == err_jobs.n) err_jobs.as_of[err_jobs.n++] = r.as_of;
+      rq.err_slot[i] = (int)j;
+    }
+    if (r.literals == nullptr) {  // one ok-trace scan per distinct as_of, shared by its requests
+      uint32_t j = 0;
+      while (j < ok_jobs.n && ok_jobs.as_of[j] != r.as_of) ++j;
+      if (j == ok_jobs.n) {
+        ok_jobs.slot[j] = k + j;
+        ok_jobs.as_of[ok_jobs.n++] = r.as_of;
+      }
+      rq.reqs[k + j] |= 1ull << i;
+      n_scan_reqs++;
+    } else if (r.n_literals != 0) {
+      segs.slot[segs.n] = i;
+      segs.as_of[segs.n] = r.as_of;
+      segs.start[segs.n + 1] = segs.start[segs.n] + r.n_literals;
+      segs.n++;
+      rq.reqs[i] = 1ull << i;
+    }
+  }
+  rq.err_base = k + ok_jobs.n;
+  for (uint32_t j = 0; j < err_jobs.n; ++j) err_jobs.slot[j] = rq.err_base + j;
+  for (uint32_t i = 0; i < k; ++i)
+    if (rq.err_slot[i] >= 0) rq.err_slot[i] += (int)rq.err_base;
+  if (!any) return MZGPU_OK;
+
+  // 1. gather
+  std::vector<mzgpu_batch*> okb, errb;
+  spine_readable(ok, okb);
+  if (errs != nullptr) spine_readable(errs, errb);
+  std::unique_ptr<TraceView> tv_ok(new TraceView()), tv_err(new TraceView());
+  MZ_TRY(trace_view(ctx, okb, tv_ok.get()));
+  if (errs != nullptr) MZ_TRY(trace_view(ctx, errb, tv_err.get()));
+  mzgpu_buf g;
+  g.ctx = ctx;
+  g.rb = 40;
+  g.len.set(ctx, 0);
+  const u64 ok_rows = peek_rows_ub(okb);
+  const u64 scan_ub = ok_rows * ok_jobs.n + peek_rows_ub(errb) * err_jobs.n;
+  if (scan_ub != 0) {
+    MZ_TRY(buf_reserve(&g, scan_ub, false));
+    Append a;
+    MZ_TRY(buf_begin_append(&g, &a));  // (g is empty: the scans count from 0)
+    MZ_CUDA(ctx, cudaMemsetAsync(a.out_len, 0, 8, ctx->stream));
+    MZ_TRY(mz_peek_scan(ctx, *tv_ok, ok_jobs, g.mem.as<u64>(), g.cap, a.out_len));
+    if (errs != nullptr) MZ_TRY(mz_peek_scan(ctx, *tv_err, err_jobs, g.mem.as<u64>(), g.cap, a.out_len));
+    buf_end_append(&g, a, scan_ub);
+  }
+  if (segs.n != 0) MZ_TRY(peek_literals(ctx, okb, reqs, segs, &g));
+
+  // 2. accumulate, 3. evaluate, 4. finish
+  std::vector<PeekDevResult> hres(k);
+  memset(hres.data(), 0, k * sizeof(PeekDevResult));
+  DevMem pairs, fail, fin, fcons, stage, dres;
+  if (g.ub != 0) {
+    u64 pcap = 0;
+    Lazy4 plen;
+    MZ_TRY(consolidate_dev(ctx, 40, g.mem.p, buf_dlen(&g), g.ub, &pairs, &pcap, &plen));
+    const DLen pn = dlen_of(plen, 0);
+    const u64 p_ub = plen.known ? plen.v[0] : std::min(pcap, g.ub);
+    const u64 n_slots = rq.err_base + err_jobs.n;  // fail[request] and fail[error-trace slot]
+    MZ_TRY(fail.alloc(ctx, n_slots * 8));
+    MZ_CUDA(ctx, cudaMemsetAsync(fail.p, 0xff, n_slots * 8, ctx->stream));
+    // finishing rows: a literal request's pair gives at most one, a scanned pair one per request at its as_of
+    u64 share = 1;
+    for (uint32_t j = 0; j < ok_jobs.n; ++j) share = std::max<u64>(share, __builtin_popcountll(rq.reqs[k + j]));
+    const u64 fin_ub = std::min(p_ub * share, n_scan_reqs * std::min(ok_rows, p_ub) + p_ub);
+    MZ_TRY(fin.alloc(ctx, std::max<u64>(fin_ub, 1) * 72));
+    Lazy4 flen;
+    MZ_TRY(flen.make_pending(ctx));
+    MZ_CUDA(ctx, cudaMemsetAsync(flen.dptr(), 0, 8, ctx->stream));
+    MZ_TRY(mz_peek_eval(ctx, pairs.as<u64>(), pn, p_ub, fin_ub, rq, fin.as<u64>(), flen.dptr(), fail.as<u64>()));
+    flen.mark_written();
+    u64 fcap = 0;
+    Lazy4 fclen;
+    DLen fn = dlen_imm(0);
+    u64 f_ub = 0;
+    if (fin_ub != 0) {
+      MZ_TRY(consolidate_dev(ctx, 72, fin.p, dlen_of(flen, 0), fin_ub, &fcons, &fcap, &fclen));
+      fn = dlen_of(fclen, 0);
+      f_ub = fclen.known ? fclen.v[0] : std::min(fcap, fin_ub);
+    }
+    MZ_TRY(stage.alloc(ctx, std::max<u64>(f_ub, 1) * 40));
+    MZ_TRY(dres.alloc(ctx, k * sizeof(PeekDevResult)));
+    MZ_CUDA(ctx, cudaMemsetAsync(dres.p, 0, k * sizeof(PeekDevResult), ctx->stream));
+    MZ_TRY(mz_peek_finish(ctx, rq, pairs.as<u64>(), fail.as<u64>(), fcons.as<u64>(), fn, stage.as<u64>(),
+                          dres.as<PeekDevResult>()));
+    MZ_TRY(copy_out(ctx, hres.data(), dres.p, k * sizeof(PeekDevResult), MZGPU_MEM_HOST));  // the one wait
+  }
+  for (uint32_t i = 0; i < k; ++i) {
+    if (rq.pl[i] == nullptr) continue;
+    const PeekDevResult& d = hres[i];
+    mzgpu_peek_result& res = results[i];
+    if (d.kind != 0) {
+      res.status = MZGPU_PEEK_ERROR;
+      res.err_kind = (int32_t)d.kind;
+      for (int w = 0; w < 4; ++w) res.detail[w] = d.d[w];
+    } else if (reqs[i].max_rows != 0 && d.n_rows > reqs[i].max_rows) {
+      res.status = MZGPU_PEEK_ERROR;
+      res.err_kind = MZGPU_PEEK_ERR_TOO_LARGE;
+      res.detail[0] = d.n_rows;
+    } else {
+      res.status = MZGPU_PEEK_ROWS;
+      res.n_rows = d.n_rows;
+      if (d.n_rows != 0)
+        MZ_TRY(buf_append_dev(outs[i], (const char*)stage.p + d.lo * 40, dlen_imm(d.n_rows), d.n_rows));
+      ctx->stats.rows_out += d.n_rows;
+    }
+  }
+  return MZGPU_OK;
+}
+
+extern "C" int32_t mzgpu_peek(mzgpu_ctx* ctx, mzgpu_spine* ok, mzgpu_spine* errs, const mzgpu_peek_req* req,
+                              mzgpu_buf* out, mzgpu_peek_result* result) {
+  return mzgpu_peek_many(ctx, ok, errs, 1, req, &out, result);
+}

@@ -13,6 +13,7 @@ pub mod delta_join;
 pub mod exchange;
 pub mod linear_join;
 pub mod mfp;
+pub mod peek;
 pub mod flat_map;
 pub mod reduce;
 pub mod sys;

@@ -94,6 +94,34 @@ pub const P2P_HANDLE_BYTES: usize = 64;
 /// A temporal filter operator (mzgpu_mfp_op), created from an `Mfp` plan.
 pub enum MfpOp {}
 pub enum JoinClosure {}
+pub enum PeekPlan {}
+pub const PEEK_MANY_MAX: u32 = 64;
+pub const PEEK_ROWS: i32 = 0;
+pub const PEEK_NOT_READY: i32 = 1;
+pub const PEEK_ERROR: i32 = 2;
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct Finishing {
+    pub n_order: u32,
+    pub order: [OrderLane; 3],
+    pub limit: i64,
+    pub offset: u64,
+    pub n_project: [u32; 3],
+    pub project: [[Field; 6]; 3],
+}
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct PeekReq {
+    pub plan: *const PeekPlan,
+    pub as_of: u64,
+    pub literals: *const u64,
+    pub n_literals: u64,
+    pub literals_mem: i32,
+    pub max_rows: u64,
+}
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct PeekResult { pub status: i32, pub err_kind: i32, pub n_rows: u64, pub detail: [u64; 4] }
 pub const MFP_MAX_PREDICATES: usize = 4;
 pub const MFP_MAX_TEMPORAL: usize = 4;
 pub const MFP_MAX_OPS: usize = 16;
@@ -298,6 +326,11 @@ extern "C" {
     // join closures: the device MfpPlan as the closure of the probe operators (mzgpu.h)
     pub fn mzgpu_join_closure_new(ctx: *mut Ctx, plan: *const Mfp, map: *const MfpMap, out: *mut *mut JoinClosure) -> i32;
     pub fn mzgpu_join_closure_free(jc: *mut JoinClosure);
+    // index peeks (mzgpu.h)
+    pub fn mzgpu_peek_plan_new(ctx: *mut Ctx, plan: *const Mfp, map: *const MfpMap, fin: *const Finishing, out: *mut *mut PeekPlan) -> i32;
+    pub fn mzgpu_peek_plan_free(p: *mut PeekPlan);
+    pub fn mzgpu_peek_many(ctx: *mut Ctx, ok: *mut Spine, errs: *mut Spine, k: u32, reqs: *const PeekReq, outs: *const *mut Buf, results: *mut PeekResult) -> i32;
+    pub fn mzgpu_peek(ctx: *mut Ctx, ok: *mut Spine, errs: *mut Spine, req: *const PeekReq, out: *mut Buf, result: *mut PeekResult) -> i32;
     pub fn mzgpu_half_join_mfp(ctx: *mut Ctx, stream: *const R32, n: u64, mem: i32, trace: *mut Spine, cmp_mode: i32, jc: *const JoinClosure, consolidate_output: i32, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_half_join_mfp_buf(ctx: *mut Ctx, stream: *mut Buf, trace: *mut Spine, cmp_mode: i32, jc: *const JoinClosure, consolidate_output: i32, out: *mut Buf, errs: *mut Buf) -> i32;
     pub fn mzgpu_half_join_many_mfp(ctx: *mut Ctx, k: u32, streams: *const *mut Buf, traces: *const *mut Spine, cmp_modes: *const i32, jcs: *const *const JoinClosure, outs: *const *mut Buf, errs: *mut Buf) -> i32;
